@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Headline benchmark: clips/sec of one SlowFast-8x8-R50 training step on N B200s (BASELINE.json configs[1]), with the
+"""Headline benchmark: clips/sec of one SlowFast-8x8-R50 training step on N H100s (BASELINE.json configs[1]), with the
 other configs of the metric (MViTv2-S, X3D-M, MaskFeat-S, MaskFeat on MViTv2-B 32x224x224) as secondary legs.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
-    python bench.py --impl reference ...     # the UNMODIFIED reference (baseline/_ref) on the box's host cores
+    python bench.py --impl reference ...     # the UNMODIFIED reference (oracle/_ref) on the box's host cores
 
 A step = zero_grad -> forward (engine kernels) -> loss -> backward (engine kernels) -> [one NCCL all-reduce of the flat
 gradient bucket when N > 1] -> optimizer step, on the recipe's per-GPU batch of synthetic Kinetics-shaped input, random
@@ -66,7 +66,8 @@ def load_peaks():
             p = json.load(f)
         return dict(hbm_gbs=p["hbm_gbs"], tflops_burst=p["bf16_tflops"],
                     tflops_sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback")
+    # no measured peaks: NVIDIA's H100 SXM data sheet (HBM3 bandwidth, dense BF16), an upper bound a card rarely reaches
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 def load_traffic():
@@ -80,7 +81,7 @@ def load_traffic():
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason sampling DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -130,11 +131,11 @@ REF_YAML = {"SLOWFAST_8x8_R50": "Kinetics/SLOWFAST_8x8_R50.yaml", "MVITv2_S_16x4
 
 
 def reference_model(preset: str, overrides=()):
-    """The UNMODIFIED reference module (slowfast.models.build_model on the reference's own yaml) from baseline/_ref (or the
+    """The UNMODIFIED reference module (slowfast.models.build_model on the reference's own yaml) from oracle/_ref (or the
     build container's checkout) through oracle/refshim.py.  Returns (cfg, model) or raises if no reference tree exists."""
     from oracle import refshim
     if not refshim.reference_available():
-        raise RuntimeError("no reference tree (run baseline/install_ref.sh in the build container)")
+        raise RuntimeError("no reference tree (build() copies it into oracle/_ref from a reference checkout)")
     cfg = refshim.load_cfg(REF_YAML[preset], list(overrides))
     return cfg, refshim.build_reference_model(cfg)
 
@@ -178,7 +179,7 @@ def time_reference_cpu(preset: str, batch: int, steps: int, warm: int, budget_s:
 
 def reference_arm(args):
     """``--impl reference``: the reference's OWN CPU implementation of the path (its nn.Conv3d / BatchNorm3d / ... modules,
-    unmodified, from baseline/_ref) on this box's host cores, all the threads the process may use, on the same workload
+    unmodified, from oracle/_ref) on this box's host cores, all the threads the process may use, on the same workload
     (SlowFast-8x8-R50 train step, the same per-step batch); steps are bounded so that the run ends within minutes."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -197,7 +198,7 @@ def reference_arm(args):
                 dtype="f32", data="synthetic", impl="reference",
                 config=dict(workload=leg["what"], per_gpu_batch=args.batch, global_batch=args.batch,
                             parallelism="host CPU", threads=r["threads"],
-                            note="unmodified reference modules (baseline/_ref) on the host cores; fwd + CE + bwd, no "
+                            note="unmodified reference modules (oracle/_ref) on the host cores; fwd + CE + bwd, no "
                                  "optimizer step"),
                 cpu_baseline=dict(value=v, unit="clips/s", cores=r["threads"], kind=kind,
                                   sample=f"{r['steps']} x fwd+bwd of {args.batch} clips through slowfast.models.build_model "
@@ -297,26 +298,53 @@ def build_leg(name: str, nsplit: int, dev, rank: int, batch=None):
     labels = labels.pin_memory()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     meta = torch.Tensor()
+    last = {}   # the model outputs of the latest step (for --dump-outputs)
 
     def step(x, y):
         opt.zero_grad(set_to_none=True)
         if mname == "MaskMViT":
             preds, labs = model([x[0], meta, x[1]])
             loss = sum(F.mse_loss(p, l[0]) * l[1] for p, l in zip(preds, labs))   # losses.py:38-62 MultipleMSELoss
+            last["outputs"] = preds
         else:
-            loss = F.cross_entropy(model(x), y)
+            logits = model(x)
+            loss = F.cross_entropy(logits, y)
+            last["outputs"] = [logits]
         loss.backward()
         if world > 1:
             model.allreduce_gradients()
         opt.step()
+        last["loss"] = loss
         return loss
 
-    return dict(name=name, cfg=cfg, model=model, step=step, host=host, labels=labels, B=B, leg=leg)
+    return dict(name=name, cfg=cfg, model=model, step=step, host=host, labels=labels, B=B, leg=leg, last=last)
 
 
-def measure_leg(L, args, dev, world, barrier, max_over_ranks, clock_index=None):
+PARAM_SAMPLE = 1 << 20   # parameters written by --dump-outputs: a fixed, seeded sample (4 MiB)
+
+
+def dump_outputs(L, out_dir):
+    """Write what the timed step returned last: the model outputs (float32), the loss (float64), and a seeded sample of the
+    parameters the optimizer step produced (float32), as out_dir/<name>.npy.  The same arguments give the same inputs,
+    weights and sample indices, so two builds can be compared array by array."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    last = L["last"]
+    for i, t in enumerate(last["outputs"]):
+        np.save(os.path.join(out_dir, f"output{i}.npy"), t.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "loss.npy"), np.array(float(last["loss"].item()), dtype=np.float64))
+    flat = torch.cat([p.detach().reshape(-1).float() for _, p in L["model"].named_parameters()])
+    n = min(PARAM_SAMPLE, flat.numel())
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n].sort().values
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat.cpu()[idx].numpy())
+    np.save(os.path.join(out_dir, "params_sample_index.npy"), idx.numpy().astype(np.float64))
+
+
+def measure_leg(L, args, dev, world, barrier, max_over_ranks, clock_index=None, dump_dir=None):
     """(1) device-resident clips/s, (2) end-to-end clips/s with pinned H2D + loss read-back inside the timed region,
-    (3) per-class roofline of the implicit-GEMM kernels.  Returns a dict."""
+    (3) per-class roofline of the implicit-GEMM kernels.  Returns a dict.  dump_dir: write the last timed step's outputs
+    there (dump_outputs) before anything else runs."""
     from slowfast_b200 import ops
     step, host, labels_h, B = L["step"], L["host"], L["labels"], L["B"]
     resident = [t.to(dev) for t in host]
@@ -338,6 +366,8 @@ def measure_leg(L, args, dev, world, barrier, max_over_ranks, clock_index=None):
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     launches = ops.launches() - l0
     clocks = sampler.stop() if sampler else None
+    if dump_dir:
+        dump_outputs(L, dump_dir)
     value = B * world * args.steps / (ms_total * 1e-3)
 
     # end to end through the public call with HOST buffers: pinned H2D every step (prefetched on a copy stream, as a
@@ -530,6 +560,9 @@ def main():
                     help="skip timing the reference's own modules (ATen / cuDNN) on this GPU (N=1 only)")
     ap.add_argument("--torch-optim", action="store_true",
                     help="step torch.optim.SGD / AdamW on param.grad instead of the fused flat-bucket optimizer")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed SlowFast steps, write the last step's outputs, loss and a seeded parameter "
+                         "sample to DIR/<name>.npy")
     args = ap.parse_args()
     global TORCH_OPTIM
     TORCH_OPTIM = args.torch_optim
@@ -567,7 +600,8 @@ def main():
     peaks = load_peaks()
     # ---- headline: SlowFast-8x8-R50 ------------------------------------------------------------------------------
     L = build_leg("slowfast", args.nsplit, dev, rank, batch=args.batch)
-    head = measure_leg(L, args, dev, world, barrier, max_over_ranks, clock_index=local if rank == 0 else None)
+    head = measure_leg(L, args, dev, world, barrier, max_over_ranks, clock_index=local if rank == 0 else None,
+                       dump_dir=args.dump_outputs if rank == 0 else None)
     cfg = L["cfg"]
     del L
     torch.cuda.empty_cache()
@@ -579,7 +613,7 @@ def main():
             r = time_reference_cpu("SLOWFAST_8x8_R50", 4, steps=3, warm=1, budget_s=25.0)
             cpu_baseline = dict(value=r["clips_per_s"], unit="clips/s", cores=r["threads"], kind="reference",
                                 sample=f"{r['steps']} x fwd+CE+bwd of {r['batch']} clips through the unmodified reference "
-                                       f"modules (baseline/_ref, fp32 ATen CPU kernels), {r['ms_per_step']:.0f} ms/step")
+                                       f"modules (oracle/_ref, fp32 ATen CPU kernels), {r['ms_per_step']:.0f} ms/step")
         except Exception as e:  # noqa: BLE001
             cpu_baseline = dict(error=repr(e)[:300])
 
@@ -624,7 +658,7 @@ def main():
             config=dict(workload=LEGS["slowfast"]["what"], per_gpu_batch=args.batch, global_batch=args.batch * world,
                         parallelism=f"dp{world}", precision_mode=f"nsplit{args.nsplit}",
                         optimizer="torch.optim on param.grad" if TORCH_OPTIM else "fused SGD-nesterov / AdamW on the flat bucket",
-                        l2_policy="per-step working set (inputs 193 MB + activations > 10 GB) exceeds the 126 MB L2; no flush needed"),
+                        l2_policy="per-step working set (inputs 193 MB + activations > 10 GB) exceeds the 50 MB L2; no flush needed"),
             e2e=head["e2e"], e2e_uint8_input=head["e2e_uint8_input"], gpu_launches=head["gpu_launches"],
             clocks=head["clocks"], roofline=head["roofline"],
             cpu_baseline=cpu_baseline,

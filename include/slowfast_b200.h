@@ -1,5 +1,5 @@
 /*
- * slowfast_b200 — C ABI of the B200-native video-backbone engine.
+ * slowfast_b200 — C ABI of the H100-native video-backbone engine.
  *
  * Drop-in boundary: the reference (facebookresearch/SlowFast) has no native layer; every FLOP of
  * `model(inputs)` / `loss.backward()` behind `slowfast.models.build_model` (slowfast/models/build.py:22)
@@ -24,12 +24,12 @@ extern "C" {
 #endif
 
 const char* sfb_last_error(void);
-/* Library/ABI version and build arch string, e.g. "sm_100a". */
+/* Library/ABI version and build arch string, e.g. "sm_90a". */
 int sfb_abi_version(void);
 const char* sfb_build_arch(void);
 
 /* ------------------------------------------------------------------------------------------------
- * Implicit-GEMM 3-D convolution on tcgen05 tensor cores, TMA im2col operand staging.
+ * Implicit-GEMM 3-D convolution on wgmma tensor cores, TMA im2col operand staging.
  * Replaces nn.Conv3d fprop (resnet_helper.py:332,346,362,485; stem_helper.py:182;
  * video_model_builder.py:147) and, with a transposed/flipped filter matrix and an output view, the
  * autograd dgrad of the same layers (SURVEY.md row a21).  nn.Linear (attention.py:193,195; common.py:20,22;
@@ -504,7 +504,7 @@ int sfb_flat_adamw(const void* chunks, int32_t n_chunks, const float* grad, floa
 
 /* ------------------------------------------------------------------------------------------------
  * Fused pooled-attention forward (MultiScaleAttention.forward, attention.py:355-385; rel-pos bias :64-147):
- * O = softmax(scale * q k^T + bias) v per (clip*head), scores and probabilities kept in TMEM / shared memory.
+ * O = softmax(scale * q k^T + bias) v per (clip*head), scores and probabilities kept in shared memory.
  * q / k / v: split planes [bh, n, 96] (the LayerNorm-ed pooled tensors); rq = q_nocls . [Rh;Rw;Rt]^T [bh*(nq-1), rq_pitch]
  * or NULL (no rel-pos); out fp32 [bh, nq, 96]; p_hi/p_lo (optional): normalised probabilities as planes [bh*nq, p_pitch]
  * (pad columns zero) for the unfused backward; lse (optional) [bh*nq].  Fused for head_dim 96 and an 8x7x7 key grid
@@ -521,22 +521,17 @@ typedef struct sfb_attn_fwd_desc {
   void* p_hi; void* p_lo; int64_t p_pitch;
   float* lse;
   int32_t nsplit;
-  const void* e_sel; /* with rq != NULL: the key selector written once by sfb_attn_fwd_selector (the rel-pos bias is added by
-                        the tensor core as [A | B | C](q) . E(key)^T) */
 } sfb_attn_fwd_desc;
 int32_t sfb_attn_fwd_supported(int32_t nk, int32_t hd, int32_t kt, int32_t kh, int32_t kw);
-int64_t sfb_attn_fwd_selector_bytes(void);
-int sfb_attn_fwd_selector(void* e_sel, int32_t kt, int32_t kh, int32_t kw, void* stream);
-/* First half of the attention backward for the same key grids (attention.py:355-379 through autograd): dP = dO v^T in TMEM,
+/* First half of the attention backward for the same key grids (attention.py:355-379 through autograd): dP = dO v^T in shared memory,
  * dS = P (dP - sum_k P dP) -> split planes [bh*nq, ds_pitch] (operand of the dq = scale dS k and dk = scale dS^T q products, pad
  * columns zero), and the gradient of the decomposed rel-pos bias, dRQ [bh*(nq-1), rq_pitch] (drq == NULL: no bias).  Replaces
- * sfb_gemm_batched (dP) + sfb_softmax_relpos_bwd.  p_hi / p_lo: the planes sfb_attn_fwd wrote (400 columns per row). */
+ * sfb_gemm_batched (dP) + sfb_softmax_relpos_bwd.  p_hi / p_lo: the planes sfb_attn_fwd wrote. */
 typedef struct sfb_attn_bwd_desc {
   const void* do_hi; const void* do_lo; const void* v_hi; const void* v_lo;
   const void* p_hi; const void* p_lo; int64_t p_pitch;
   void* ds_hi; void* ds_lo; int64_t ds_pitch;
   float* drq; int64_t rq_pitch;
-  const void* e_sel;
   int32_t bh, nq, nk, hd;
   int32_t qt, qh, qw, kt, kh, kw;
   int32_t nsplit;

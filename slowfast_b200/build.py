@@ -1,4 +1,4 @@
-"""In-tree build of the native library (nvcc, sm_100a only).
+"""In-tree build of the native library (nvcc, sm_90a only).
 
 The shared object lands next to the sources (``slowfast_b200/csrc/libsfb200.so``) so that it travels with the
 repository snapshot to the GPU box; nothing is installed into site-packages and no JIT cache is used.
@@ -14,16 +14,16 @@ from pathlib import Path
 
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB_NAME = "libsfb200.so"
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
-              "-Xptxas", "-v", "-DSFB_BUILD_ARCH=\"sm_100a\""]
+              "-Xptxas", "-v", "-DSFB_BUILD_ARCH=\"sm_90a\""]
 
 
 def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found (needed to build slowfast_b200's sm_100a kernels)")
+    raise RuntimeError("nvcc not found (needed to build slowfast_b200's sm_90a kernels)")
 
 
 def _digest(paths) -> str:
@@ -40,7 +40,7 @@ def lib_path() -> Path:
 
 
 def build_native(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every ``csrc/*.cu`` for sm_100a and link ``libsfb200.so``. Returns the library path."""
+    """Compile every ``csrc/*.cu`` for sm_90a and link ``libsfb200.so``. Returns the library path."""
     sources = sorted(CSRC.glob("*.cu"))
     headers = sorted(list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h")) +
                      list((CSRC.parent.parent / "include").glob("*.h")))

@@ -1,28 +1,18 @@
-// Fused pooled-attention forward for MViT's MultiScaleAttention (attention.py:355-385): per (clip*head, 128-query tile)
+// Fused pooled attention for MViT's MultiScaleAttention (attention.py:355-385) on wgmma, per (clip*head, 64-query tile):
 //
-//     S = q k^T          tcgen05.mma, accumulator S[128 x 400] lives in TMEM only (never written to HBM)
-//     t = scale*S + rel-pos bias(q, k)   (cal_rel_pos_spatial / _temporal, attention.py:64-147).  The bias is decomposed,
-//                                         bias[q, key] = A[q, kh(key)] + B[q, kw(key)] + C[q, kt(key)], i.e. a rank-22 product
-//                                         [A | B | C][q, 0:22] . E^T with E the one-hot (kh, kw, kt) selector of the key: the 22
-//                                         per-row values are gathered once from RQ = q.[Rh;Rw;Rt]^T, written to shared memory as
-//                                         split planes (divided by scale) and ADDED BY THE TENSOR CORE: two more K = 16 steps
-//                                         per key tile.  The softmax loops then carry no per-column constants.
-//     P = softmax(t)     exact two-pass softmax over the TMEM row block (no online rescaling: the whole key axis is resident)
-//     O = P v            P goes TMEM -> registers -> shared memory (split-bf16 planes, 128-byte-swizzled K-major tiles) and is
-//                        consumed by the second tcgen05.mma straight from there; O accumulates in 96 more TMEM columns
+//   forward   S = q k^T (wgmma 64 x 80 x 16 per key tile, 5 tiles = 400 keys)  -> fp32 score block in shared memory
+//             t = scale*S + rel-pos bias(q, k)  (cal_rel_pos_spatial / _temporal, attention.py:64-147, from RQ = q.[Rh;Rw;Rt]^T)
+//             P = softmax(t)  (exact: the whole key axis is resident), written to global memory as split planes (the
+//                              backward reads them) and staged 64 keys at a time as 128B-swizzled K-major bf16 planes
+//             O = P v   (wgmma 64 x 96 x 16, accumulator in registers; v arrives by TMA as MN-major atoms)
+//   backward  dP = dO v^T (same tile loop as S), dS = P (dP - sum_k P dP) -> split planes, dRQ = the rel-pos bias gradient
 //
-// Why this shape: with POOL_KV_STRIDE_ADAPTIVE the key grid of MViTv2-S is 8 x 7 x 7 in 12 of its 16 blocks, i.e.
-// Nk = 393 <= 400 TMEM columns, so S (400) and O (96) fit the 512 columns of one SM together.  (r2m/r2n versions kept the
-// bias in registers with compile-time column indices: 216 KB of unrolled code, instruction-cache bound.)  Other key
-// grids (Nk = 1569 in blocks 1, 3, 14; MViTv2-B) keep the unfused sequence (gemm_batched -> softmax_relpos -> gemm_batched).
-// The normalised P is also written to global memory as split planes because the (still unfused) backward reads it; the
-// fp32 score tensor, its second read, and the re-read of P by a separate PV GEMM are gone.
-//
-// Warp roles (576 threads, 1 CTA per SM): warp 0 = TMA producer (Q once; K tiles of 80 keys; then V blocks of 64 keys into
-// the same ring), warp 1 = MMA issuer + TMEM owner, warps 2-17 = softmax / epilogue: thread = query row (TMEM lane, quarter =
-// warp % 4) x one of four column groups.  (The first version had 4 softmax warps: correct, but the scalar softmax of a
-// 128 x 400 tile on 128 threads took longer than the unfused kernels it replaced.)
+// Neither S nor dP goes to HBM.  Key grids with Nk <= 400 and head_dim 96 (MViTv2-S: 8 x 7 x 7 keys in 12 of 16 blocks);
+// other grids keep the unfused sequence (sfb_gemm_batched -> sfb_softmax_relpos_* -> sfb_gemm_batched).
+// One warpgroup per CTA: warp-uniform TMA issue by thread 0, every wgmma waited before its shared-memory operands are
+// reused.  The row passes repeat the arithmetic of softmax_relpos_fwd / _bwd (mvit_ops.cu) on the resident block.
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -34,23 +24,38 @@
 
 namespace sfb {
 
-constexpr int AF_KH = 7, AF_KW = 7;
-constexpr int AF_BN = 80;         // keys per QK^T tile (UMMA N)
-constexpr int AF_HD = 96;         // head dim
-constexpr uint32_t AF_QP_BYTES = 16384;   // one [128 x 64] bf16 K-major SW128 tile (Q k-block plane / P k-block plane)
-constexpr uint32_t AF_KT_BYTES = 10240;   // one [80 x 64] bf16 K-major SW128 tile
-constexpr uint32_t AF_VP_BYTES = 16384;   // one V k-block plane: 2 atoms of [64 keys x 64 dims] (MN-major)
+constexpr int AF_BM = 64;          // queries per CTA (one warpgroup, wgmma M)
+constexpr int AF_BN = 80;          // keys per score tile (wgmma N)
+constexpr int AF_NKT = 5;          // score tiles: 400 keys
+constexpr int AF_NK_MAX = AF_BN * AF_NKT;
+constexpr int AF_HD = 96;          // head dim
+constexpr int AF_SP = AF_NK_MAX + 4;                // floats per score row
+constexpr uint32_t AF_QT_BYTES = AF_BM * 128;       // [64 rows x 64 dims] bf16 K-major SW128 tile (q / dO / P k-block)
+constexpr uint32_t AF_KT_BYTES = AF_BN * 128;       // [80 keys x 64 dims] bf16 K-major SW128 tile
+constexpr uint32_t AF_VA_BYTES = 64 * 128;          // [64 keys x 64 dims] MN-major SW128 atom of v
+// shared memory: A operand (2 planes x 2 k-blocks), key tile (2 planes x 2 k-blocks, reused for v: 2 planes x 2 atoms),
+// P staging (2 planes), score block, barriers
+constexpr uint32_t AF_OFF_A = 0;
+constexpr uint32_t AF_OFF_K = AF_OFF_A + 4 * AF_QT_BYTES;
+constexpr uint32_t AF_OFF_P = AF_OFF_K + 4 * AF_KT_BYTES;
+constexpr uint32_t AF_OFF_S = AF_OFF_P + 2 * AF_QT_BYTES;
+constexpr uint32_t AF_OFF_BINS = AF_OFF_S + AF_BM * AF_SP * 4;
+constexpr uint32_t AF_BINS_FLOATS = 256;            // per warp: Lh + Lw + Lt (checked on the host)
+constexpr uint32_t AF_OFF_BAR = AF_OFF_BINS + 4 * AF_BINS_FLOATS * 4;
+constexpr uint32_t AF_SMEM = AF_OFF_BAR + 64 + 1024;
 
-struct AttnFwdParams {
-  CUtensorMap tmQ[2], tmK[2], tmV[2], tmE;
+struct AttnParams {
+  CUtensorMap tmA[2], tmK[2], tmV[2];   // fwd: q, k, v;  bwd: dO, v (as the K-major key operand), unused
   int BH, Nq, Nk, q_tiles;
-  const float* rq; int64_t rq_pitch; int Lh, Lw;
-  int qh, qw;                       // query grid (H, W); T follows from the row index
+  const float* rq; int64_t rq_pitch;    // fwd: RQ [BH*(Nq-1), rq_pitch] or null
+  int qt, qh, qw, kt, kh, kw, Lh, Lw, Lt;
   float rh_q, rh_k, rw_q, rw_k, rt_q, rt_k;
   float scale;
-  float* out;                       // [BH, Nq, 96] fp32
-  __nv_bfloat16* p_hi; __nv_bfloat16* p_lo; int64_t p_pitch;   // [BH * Nq, p_pitch] normalised probabilities (planes)
-  float* lse;                       // [BH * Nq] log-sum-exp of the biased scores (may be null)
+  float* out;                           // fwd: O [BH, Nq, 96]
+  float* lse;                           // fwd: [BH*Nq] or null
+  __nv_bfloat16* p_hi; __nv_bfloat16* p_lo; int64_t p_pitch;     // fwd: written; bwd: read
+  __nv_bfloat16* ds_hi; __nv_bfloat16* ds_lo; int64_t ds_pitch;  // bwd
+  float* drq;                           // bwd: [BH*(Nq-1), rq_pitch] or null
 };
 
 __device__ __forceinline__ void af_tma_3d(void* smem, const CUtensorMap* tm, uint64_t* bar, int32_t c0, int32_t c1, int32_t c2) {
@@ -59,751 +64,293 @@ __device__ __forceinline__ void af_tma_3d(void* smem, const CUtensorMap* tm, uin
       ::"r"(smem_u32(smem)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-
-struct AfSoftmaxCtx {
-  uint32_t s_taddr;
-  float* red_max; float* red_sum;
-  int row, qi, bh, cg;
-  bool valid;
-  uint8_t* qp;
-  uint64_t* p_full; uint64_t* p_empty; uint64_t* o_full;
-};
-
-__device__ __forceinline__ float af_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
+__device__ __forceinline__ void af_put_split(__nv_bfloat16* hi, __nv_bfloat16* lo, int64_t i, float v) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  hi[i] = h;
+  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+}
+__device__ __forceinline__ float af_get_split(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int64_t i) {
+  return __bfloat162float(hi[i]) + (lo ? __bfloat162float(lo[i]) : 0.f);
+}
+__device__ __forceinline__ float af_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ int af_rel_index(int i, int j, float rq, float rk, int nk) {
+  return int(floorf(float(i) * rq - float(j) * rk + float(nk - 1) * rk));
 }
 
-// Softmax + epilogue of one warp (TMEM lane quarter fixed by the caller) for column group cg: 16-column chunks {4*kb + cg}.
-// The accumulator already holds q.k + bias/scale, so a score is raw * scale; exponentials are taken base 2 with
-// scale * log2(e) folded into one FFMA.
-template <int NSPLIT, int KT>
-__device__ __forceinline__ void af_softmax(const AttnFwdParams& p, const AfSoftmaxCtx& c) {
-  constexpr int NK = 1 + KT * AF_KH * AF_KW;
-  constexpr int NKB = (NK + 63) / 64;
-  constexpr uint32_t O_COL = ((NK + AF_BN - 1) / AF_BN) * AF_BN;
-  const int lane = threadIdx.x & 31;
-  const int row = c.row, cg = c.cg;
-  const float sc2 = p.scale * 1.4426950408889634f;
-  // pass 1: row maximum of the raw accumulator over this warp's chunks, then across the four column groups
-  float mx = -INFINITY;
-#pragma unroll 1
-  for (int kb = 0; kb < NKB; ++kb) {
-    const int col0 = (kb * 4 + cg) * 16;
-    if (col0 < NK) {
-      uint32_t v[16];
-      tmem_ld_32x32b_x16(c.s_taddr + uint32_t(col0), v);
-      tmem_ld_wait();
-      if (col0 + 16 <= NK) {
+// S[64 x 400] (fp32, shared) = A[64 x 96] . B[keys x 96]^T for the CTA's query tile; A (q or dO) is loaded here too.
+// `phase` tracks the single TMA barrier.  Keys past Nk read as zero (TMA out-of-bounds fill).
+template <int NSPLIT>
+__device__ __forceinline__ void af_scores(const AttnParams& p, uint8_t* smem, uint64_t* bar, uint32_t& phase, int bh, int q0) {
+  constexpr int NP = NSPLIT == 3 ? 2 : 1;
+  float* S = reinterpret_cast<float*>(smem + AF_OFF_S);
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(bar, NP * 2 * AF_QT_BYTES);
+    for (int pl = 0; pl < NP; ++pl)
+      for (int kb = 0; kb < 2; ++kb)
+        af_tma_3d(smem + AF_OFF_A + (pl * 2 + kb) * AF_QT_BYTES, &p.tmA[pl], bar, kb * 64, q0, bh);
+  }
+  mbar_wait(bar, phase);
+  phase ^= 1;
+  const uint32_t a_base = smem_u32(smem + AF_OFF_A), k_base = smem_u32(smem + AF_OFF_K);
+  for (int t = 0; t < AF_NKT; ++t) {
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(bar, NP * 2 * AF_KT_BYTES);
+      for (int pl = 0; pl < NP; ++pl)
+        for (int kb = 0; kb < 2; ++kb)
+          af_tma_3d(smem + AF_OFF_K + (pl * 2 + kb) * AF_KT_BYTES, &p.tmK[pl], bar, kb * 64, t * AF_BN, bh);
+    }
+    mbar_wait(bar, phase);
+    phase ^= 1;
+    float d[AF_BN / 2];
+    wgmma_fence();
 #pragma unroll
-        for (int e = 0; e < 16; ++e) mx = fmaxf(mx, __uint_as_float(v[e]));
+    for (int ks = 0; ks < AF_HD / 16; ++ks) {
+      const uint32_t off = uint32_t(ks >> 2) * AF_QT_BYTES + uint32_t(ks & 3) * 32u;
+      const uint32_t koff = uint32_t(ks >> 2) * AF_KT_BYTES + uint32_t(ks & 3) * 32u;
+      const uint64_t a_hi = make_smem_desc(a_base + off, 16, 1024, 2);
+      const uint64_t b_hi = make_smem_desc(k_base + koff, 16, 1024, 2);
+      const uint32_t acc = ks != 0;
+      if (NSPLIT == 3) {
+        const uint64_t a_lo = make_smem_desc(a_base + 2 * AF_QT_BYTES + off, 16, 1024, 2);
+        const uint64_t b_lo = make_smem_desc(k_base + 2 * AF_KT_BYTES + koff, 16, 1024, 2);
+        wgmma_m64n80<0, 0>(d, a_lo, b_hi, acc);
+        wgmma_m64n80<0, 0>(d, a_hi, b_lo, 1u);
+        wgmma_m64n80<0, 0>(d, a_hi, b_hi, 1u);
       } else {
-#pragma unroll
-        for (int e = 0; e < 16; ++e)
-          if (col0 + e < NK) mx = fmaxf(mx, __uint_as_float(v[e]));
+        wgmma_m64n80<0, 0>(d, a_hi, b_hi, acc);
       }
     }
-  }
-  c.red_max[cg * 128 + row] = mx;
-  named_bar_sync(1, 512);
-  mx = fmaxf(fmaxf(c.red_max[row], c.red_max[128 + row]), fmaxf(c.red_max[256 + row], c.red_max[384 + row]));
-  const float mxs = mx * sc2;                       // (scale > 0: the maximum commutes with the scaling)
-  // pass 2: sum of exponentials
-  float l = 0.f;
-#pragma unroll 1
-  for (int kb = 0; kb < NKB; ++kb) {
-    const int col0 = (kb * 4 + cg) * 16;
-    if (col0 < NK) {
-      uint32_t v[16];
-      tmem_ld_32x32b_x16(c.s_taddr + uint32_t(col0), v);
-      tmem_ld_wait();
-      if (col0 + 16 <= NK) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) l += af_ex2(fmaf(__uint_as_float(v[e]), sc2, -mxs));
-      } else {
-#pragma unroll
-        for (int e = 0; e < 16; ++e)
-          if (col0 + e < NK) l += af_ex2(fmaf(__uint_as_float(v[e]), sc2, -mxs));
-      }
-    }
-  }
-  c.red_sum[cg * 128 + row] = l;
-  named_bar_sync(1, 512);
-  l = (c.red_sum[row] + c.red_sum[128 + row]) + (c.red_sum[256 + row] + c.red_sum[384 + row]);
-  const float inv = 1.f / l;
-  if (cg == 0 && p.lse && c.valid) p.lse[int64_t(c.bh) * p.Nq + c.qi] = mx * p.scale + __logf(l);
-  // pass 3: normalised probabilities of PV k-block kb (this warp: columns [64 kb + 16 cg, +16)) -> shared-memory A tile
-  // (planes, 128-byte swizzle) + global planes
-  __nv_bfloat16* gp_hi = p.p_hi ? p.p_hi + (int64_t(c.bh) * p.Nq + c.qi) * p.p_pitch : nullptr;
-  __nv_bfloat16* gp_lo = p.p_lo ? p.p_lo + (int64_t(c.bh) * p.Nq + c.qi) * p.p_pitch : nullptr;
-#pragma unroll 1
-  for (int kb = 0; kb < NKB; ++kb) {
-    const int s = kb & 1;
-    mbar_wait(&c.p_empty[s], ((kb >> 1) & 1) ^ 1);
-    uint8_t* pt_hi = c.qp + (s * 2 + 0) * AF_QP_BYTES + row * 128;
-    uint8_t* pt_lo = c.qp + (s * 2 + 1) * AF_QP_BYTES + row * 128;
-    const int col0 = kb * 64 + cg * 16;
-    uint32_t v[16];
-    float pr[16];
-    if (col0 < NK) {                                  // (chunks entirely beyond the last key: zeros, no TMEM read)
-      tmem_ld_32x32b_x16(c.s_taddr + uint32_t(col0), v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int e = 0; e < 16; ++e) pr[e] = (col0 + e < NK) ? af_ex2(fmaf(__uint_as_float(v[e]), sc2, -mxs)) * inv : 0.f;
-    } else {
-#pragma unroll
-      for (int e = 0; e < 16; ++e) pr[e] = 0.f;
-    }
-    // two 16-byte pieces (8 keys each) per plane, 128-byte swizzle: chunk c of row r sits at position c ^ (r & 7)
-#pragma unroll
-    for (int h8 = 0; h8 < 2; ++h8) {
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int w2 = 0; w2 < 4; ++w2) {
-        const float a = pr[h8 * 8 + 2 * w2], b = pr[h8 * 8 + 2 * w2 + 1];
-        const __nv_bfloat16 ah = __float2bfloat16_rn(a), bhh = __float2bfloat16_rn(b);
-        const __nv_bfloat16 al = __float2bfloat16_rn(a - __bfloat162float(ah));
-        const __nv_bfloat16 bl = __float2bfloat16_rn(b - __bfloat162float(bhh));
-        hi[w2] = uint32_t(__bfloat16_as_ushort(ah)) | (uint32_t(__bfloat16_as_ushort(bhh)) << 16);
-        lo[w2] = uint32_t(__bfloat16_as_ushort(al)) | (uint32_t(__bfloat16_as_ushort(bl)) << 16);
-      }
-      const int chunk = cg * 2 + h8;                  // 16-byte chunk index inside the 128-byte row (0..7)
-      const int pos = (chunk ^ (row & 7)) * 16;
-      *reinterpret_cast<uint4*>(pt_hi + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-      if (NSPLIT == 3) *reinterpret_cast<uint4*>(pt_lo + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      const int gcol = col0 + h8 * 8;
-      if (c.valid && gp_hi && gcol < p.p_pitch) {
-        *reinterpret_cast<uint4*>(gp_hi + gcol) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        if (gp_lo) *reinterpret_cast<uint4*>(gp_lo + gcol) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      }
-    }
-    fence_proxy_async_smem();          // generic-proxy writes of this thread -> visible to the tensor core's async proxy
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&c.p_full[s]);
-  }
-  // epilogue: O (already normalised) -> global fp32 [BH, Nq, 96]; 6 chunks of 16 columns over the 4 column groups
-  mbar_wait(c.o_full, 0);
-  tc_fence_after();
-  float* orow = p.out + (int64_t(c.bh) * p.Nq + c.qi) * AF_HD;
-#pragma unroll 1
-  for (int ch = cg; ch < AF_HD / 16; ch += 4) {
-    uint32_t v[16];
-    tmem_ld_32x32b_x16(c.s_taddr + O_COL + uint32_t(ch * 16), v);
-    tmem_ld_wait();
-    if (c.valid) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        reinterpret_cast<float4*>(orow + ch * 16)[j] =
-            make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                        __uint_as_float(v[4 * j + 3]));
-    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_store<AF_BN>(d, AF_BN, S + t * AF_BN, AF_SP);
+    __syncthreads();   // every thread's MMAs have read the key tile before the next load overwrites it
   }
 }
 
-template <int NSPLIT, int KT>
-__global__ void __launch_bounds__(576, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
-  constexpr int NK = 1 + KT * AF_KH * AF_KW;          // 393 keys (cls + grid)
-  constexpr int NKT = (NK + AF_BN - 1) / AF_BN;       // 5 QK^T tiles
-  constexpr int NKB = (NK + 63) / 64;                 // 7 PV k-blocks
-  constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
-  constexpr uint32_t O_COL = NKT * AF_BN;             // 400
-  static_assert(O_COL + AF_HD <= 512, "S and O must fit the 512 TMEM columns");
+template <int NSPLIT>
+__global__ void __launch_bounds__(128, 1) attn_fwd_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // [Q / P union: 4 x 16 KB] [bias tile: 3 planes x 16 KB] [K / V ring: 2 x 50 KB] [barriers]
-  uint8_t* qp = smem;
-  uint8_t* bias_t = smem + 4 * AF_QP_BYTES;
-  uint8_t* ring = bias_t + 3 * AF_QP_BYTES;
-  constexpr uint32_t K_STAGE = 2 * 2 * AF_KT_BYTES + AF_KT_BYTES;   // 2 k-blocks x 2 planes + the selector tile of these keys
-  constexpr uint32_t V_STAGE = 2 * AF_VP_BYTES;       // 2 planes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + 2 * K_STAGE);
-  uint64_t* q_full = bars;            // 1
-  uint64_t* k_full = bars + 1;        // 2
-  uint64_t* k_empty = bars + 3;       // 2
-  uint64_t* s_full = bars + 5;        // 1
-  uint64_t* v_full = bars + 6;        // 2
-  uint64_t* v_empty = bars + 8;       // 2
-  uint64_t* p_full = bars + 10;       // 2
-  uint64_t* p_empty = bars + 12;      // 2
-  uint64_t* o_full = bars + 14;       // 1
-  uint64_t* b_full = bars + 15;       // 1 (bias tile written by the four column-group-0 warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  const bool has_bias = p.rq != nullptr;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int bh = blockIdx.x / p.q_tiles;
-  const int q0 = (blockIdx.x - bh * p.q_tiles) * 128;
-
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + AF_OFF_BAR);
+  float* S = reinterpret_cast<float*>(smem + AF_OFF_S);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int bh = blockIdx.x / p.q_tiles, q0 = (blockIdx.x % p.q_tiles) * AF_BM;
   if (threadIdx.x == 0) {
-    mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], 1);
-      mbar_init(&p_full[s], 16);
-      mbar_init(&p_empty[s], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(o_full, 1);
-    mbar_init(b_full, 4);
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  uint32_t phase = 0;
+  af_scores<NSPLIT>(p, smem, bar, phase, bh, q0);
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------------------------------ TMA producer
-    if (elect_one()) {
-      mbar_expect_tx(q_full, 2 * NP * AF_QP_BYTES);
-      for (int kb = 0; kb < 2; ++kb)
-        for (uint32_t pl = 0; pl < NP; ++pl)
-          af_tma_3d(qp + (kb * 2 + pl) * AF_QP_BYTES, &p.tmQ[pl], q_full, kb * 64, q0, bh);
+  // ---- biased softmax, one warp per row (softmax_relpos_fwd arithmetic); P replaces the scores, zero past Nk
+  const int khw = p.kh * p.kw;
+  for (int rr = warp; rr < AF_BM; rr += 4) {
+    float* s = S + rr * AF_SP;
+    const int q = q0 + rr;
+    if (q >= p.Nq) {
+      for (int k = lane; k < AF_NK_MAX; k += 32) s[k] = 0.f;
+      continue;
     }
-    __syncwarp();
-    for (int t = 0; t < NKT; ++t) {
-      const int s = t & 1;
-      mbar_wait(&k_empty[s], ((t >> 1) & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&k_full[s], 2 * NP * AF_KT_BYTES + (has_bias ? AF_KT_BYTES : 0u));
-        uint8_t* st = ring + s * K_STAGE;
-        for (int kb = 0; kb < 2; ++kb)
-          for (uint32_t pl = 0; pl < NP; ++pl)
-            af_tma_3d(st + (kb * 2 + pl) * AF_KT_BYTES, &p.tmK[pl], &k_full[s], kb * 64, t * AF_BN, bh);
-        if (has_bias) af_tma_3d(st + 4 * AF_KT_BYTES, &p.tmE, &k_full[s], 0, t * AF_BN, 0);
-      }
-      __syncwarp();
+    const int64_t r = int64_t(bh) * p.Nq + q;
+    const float* rq = (p.rq && q > 0) ? p.rq + (int64_t(bh) * (p.Nq - 1) + (q - 1)) * p.rq_pitch : nullptr;
+    int qz = 0, qy = 0, qx = 0;
+    if (q > 0) {
+      int t = q - 1;
+      qx = t % p.qw;
+      t /= p.qw;
+      qy = t % p.qh;
+      qz = t / p.qh;
     }
-    // the V blocks reuse the ring: every QK^T MMA (the last readers of the K tiles) has completed when s_full fires
-    mbar_wait(s_full, 0);
-    for (int kb = 0; kb < NKB; ++kb) {
-      const int s = kb & 1;
-      mbar_wait(&v_empty[s], ((kb >> 1) & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&v_full[s], NP * AF_VP_BYTES);
-        uint8_t* st = ring + s * V_STAGE;
-        for (uint32_t pl = 0; pl < NP; ++pl)
-          for (int j = 0; j < 2; ++j)
-            af_tma_3d(st + pl * AF_VP_BYTES + j * 8192, &p.tmV[pl], &v_full[s], j * 64, kb * 64, bh);
+    const float bh0 = float(qy) * p.rh_q + float(p.kh - 1) * p.rh_k;
+    const float bw0 = float(qx) * p.rw_q + float(p.kw - 1) * p.rw_k;
+    const float bt0 = float(qz) * p.rt_q + float(p.kt - 1) * p.rt_k;
+    float mx = -INFINITY;
+    for (int k = lane; k < p.Nk; k += 32) {
+      float v = s[k] * p.scale;
+      if (rq && k > 0) {
+        const int t = k - 1;
+        const int kz = t / khw;
+        const int rem = t - kz * khw;
+        const int ky = rem / p.kw;
+        const int kx = rem - ky * p.kw;
+        v += rq[int(floorf(bh0 - float(ky) * p.rh_k))] + rq[p.Lh + int(floorf(bw0 - float(kx) * p.rw_k))] +
+             rq[p.Lh + p.Lw + int(floorf(bt0 - float(kz) * p.rt_k))];
       }
-      __syncwarp();
+      s[k] = v;
+      mx = fmaxf(mx, v);
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc_s = make_idesc_bf16(128, AF_BN, 0, 0);
-    const uint32_t idesc_o = make_idesc_bf16(128, AF_HD, 0, 1);
-    mbar_wait(q_full, 0);
-    tc_fence_after();
-    const uint32_t q_base = smem_u32(qp);
-    for (int t = 0; t < NKT; ++t) {
-      const int s = t & 1;
-      mbar_wait(&k_full[s], (t >> 1) & 1);
-      if (has_bias && t == 0) mbar_wait(b_full, 0);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t k_base = smem_u32(ring + s * K_STAGE);
-        const uint32_t d_tmem = tmem_base + uint32_t(t * AF_BN);
 #pragma unroll
-        for (int ks = 0; ks < AF_HD / 16; ++ks) {       // 6 k-steps of 16 over head dim 96 (k-block 0: 4, k-block 1: 2)
-          const int kb = ks >> 2, kk = ks & 3;
-          uint64_t a_d[2], b_d[2];
-          for (uint32_t pl = 0; pl < NP; ++pl) {
-            a_d[pl] = make_smem_desc(q_base + (kb * 2 + pl) * AF_QP_BYTES + kk * 32, 16, 1024, 2);
-            b_d[pl] = make_smem_desc(k_base + (kb * 2 + pl) * AF_KT_BYTES + kk * 32, 16, 1024, 2);
-          }
-          const uint32_t acc = ks != 0 ? 1u : 0u;
-          if (NSPLIT == 3) {
-            umma_bf16(d_tmem, a_d[1], b_d[0], idesc_s, acc);
-            umma_bf16(d_tmem, a_d[0], b_d[1], idesc_s, 1u);
-            umma_bf16(d_tmem, a_d[0], b_d[0], idesc_s, 1u);
-          } else {
-            umma_bf16(d_tmem, a_d[0], b_d[0], idesc_s, acc);
-          }
-        }
-        if (has_bias) {
-          // + [A | B | C]/scale . E^T : 32 K elements (22 used) = 2 k-steps; E is exact in bf16, the row values are split into
-          // three bf16 terms (24 bits: the bias is then as exact as an fp32 add)
-          const uint32_t bt = smem_u32(bias_t), e_base = k_base + 4 * AF_KT_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < 2; ++kk) {
-            const uint64_t e_d = make_smem_desc(e_base + kk * 32, 16, 1024, 2);
-            if (NSPLIT == 3) {
-              umma_bf16(d_tmem, make_smem_desc(bt + 2 * AF_QP_BYTES + kk * 32, 16, 1024, 2), e_d, idesc_s, 1u);
-              umma_bf16(d_tmem, make_smem_desc(bt + AF_QP_BYTES + kk * 32, 16, 1024, 2), e_d, idesc_s, 1u);
-            }
-            umma_bf16(d_tmem, make_smem_desc(bt + kk * 32, 16, 1024, 2), e_d, idesc_s, 1u);
-          }
-        }
-        umma_commit(&k_empty[s]);
-        if (t == NKT - 1) umma_commit(s_full);
-      }
-      __syncwarp();
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    float sum = 0.f;
+    for (int k = lane; k < p.Nk; k += 32) {
+      const float e = expf(s[k] - mx);
+      s[k] = e;
+      sum += e;
     }
-    // O += P_block . V_block
-    const uint32_t o_tmem = tmem_base + O_COL;
-    for (int kb = 0; kb < NKB; ++kb) {
-      const int s = kb & 1;
-      mbar_wait(&v_full[s], (kb >> 1) & 1);
-      mbar_wait(&p_full[s], (kb >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t p_base = smem_u32(qp + s * 2 * AF_QP_BYTES);
-        const uint32_t v_base = smem_u32(ring + s * V_STAGE);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          uint64_t a_d[2], b_d[2];
-          for (uint32_t pl = 0; pl < NP; ++pl) {
-            a_d[pl] = make_smem_desc(p_base + pl * AF_QP_BYTES + ks * 32, 16, 1024, 2);
-            b_d[pl] = make_smem_desc(v_base + pl * AF_VP_BYTES + ks * 2048, 8192, 1024, 2);
-          }
-          const uint32_t acc = (kb | ks) != 0 ? 1u : 0u;
-          if (NSPLIT == 3) {
-            umma_bf16(o_tmem, a_d[1], b_d[0], idesc_o, acc);
-            umma_bf16(o_tmem, a_d[0], b_d[1], idesc_o, 1u);
-            umma_bf16(o_tmem, a_d[0], b_d[0], idesc_o, 1u);
-          } else {
-            umma_bf16(o_tmem, a_d[0], b_d[0], idesc_o, acc);
-          }
-        }
-        umma_commit(&v_empty[s]);
-        umma_commit(&p_empty[s]);
-        if (kb == NKB - 1) umma_commit(o_full);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ------------------------------------------------------------------------------------------ softmax / epilogue
-    // 16 warps: TMEM lane quarter = warp % 4 (hardware rule), column group cg = (warp - 2) / 4 owns the 16-column chunks
-    // {4*kb + cg}: one chunk of every 64-key PV block, 6-7 chunks of the 25 in total.  Row-wise max / sum are combined across
-    // the four column groups of a row through shared memory.
-    const int qw4 = warp & 3;                       // TMEM lane quarter of this warp
-    const int cg = (warp - 2) >> 2;                 // column group 0..3
-    const int row = qw4 * 32 + lane;                // query row inside the tile = TMEM lane
-    const int qi = q0 + row;                        // query index (0 = cls)
-    const bool valid = qi < p.Nq;
-    float* red_max = reinterpret_cast<float*>(bars + 18);      // [4][128]
-    float* red_sum = red_max + 4 * 128;                         // [4][128]
-    if (has_bias && cg == 0) {
-      // per-row bias values A[kh], B[kw], C[kt] gathered once from RQ (cls row / rows past the end: zeros), divided by the
-      // scale and written as the K-major split-plane tile [128 rows x (7 + 7 + KT <= 24) + zero pad to 32]
-      float bv[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) bv[i] = 0.f;
-      if (valid && qi > 0) {
-        int t = qi - 1;
-        const int qx = t % p.qw;
-        t /= p.qw;
-        const int qy = t % p.qh;
-        const int qz = t / p.qh;
-        const float* rq = p.rq + (int64_t(bh) * (p.Nq - 1) + (qi - 1)) * p.rq_pitch;
-        const float bh0 = float(qy) * p.rh_q + float(AF_KH - 1) * p.rh_k;
-        const float bw0 = float(qx) * p.rw_q + float(AF_KW - 1) * p.rw_k;
-        const float bt0 = float(qz) * p.rt_q + float(KT - 1) * p.rt_k;
-        const float is = 1.f / p.scale;
-#pragma unroll
-        for (int i = 0; i < AF_KH; ++i) bv[i] = rq[int(floorf(bh0 - float(i) * p.rh_k))] * is;
-#pragma unroll
-        for (int i = 0; i < AF_KW; ++i) bv[AF_KH + i] = rq[p.Lh + int(floorf(bw0 - float(i) * p.rw_k))] * is;
-#pragma unroll
-        for (int i = 0; i < KT; ++i) bv[AF_KH + AF_KW + i] = rq[p.Lh + p.Lw + int(floorf(bt0 - float(i) * p.rt_k))] * is;
-      }
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t hi[4], lo[4], l2[4];
-#pragma unroll
-        for (int w2 = 0; w2 < 4; ++w2) {
-          const float a = bv[ch * 8 + 2 * w2], b = bv[ch * 8 + 2 * w2 + 1];
-          const __nv_bfloat16 ah = __float2bfloat16_rn(a), bhh = __float2bfloat16_rn(b);
-          const float ar = a - __bfloat162float(ah), br = b - __bfloat162float(bhh);
-          const __nv_bfloat16 al = __float2bfloat16_rn(ar), bl = __float2bfloat16_rn(br);
-          const __nv_bfloat16 a2 = __float2bfloat16_rn(ar - __bfloat162float(al));
-          const __nv_bfloat16 b2 = __float2bfloat16_rn(br - __bfloat162float(bl));
-          hi[w2] = uint32_t(__bfloat16_as_ushort(ah)) | (uint32_t(__bfloat16_as_ushort(bhh)) << 16);
-          lo[w2] = uint32_t(__bfloat16_as_ushort(al)) | (uint32_t(__bfloat16_as_ushort(bl)) << 16);
-          l2[w2] = uint32_t(__bfloat16_as_ushort(a2)) | (uint32_t(__bfloat16_as_ushort(b2)) << 16);
-        }
-        const int pos = row * 128 + ((ch ^ (row & 7)) * 16);
-        *reinterpret_cast<uint4*>(bias_t + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        if (NSPLIT == 3) {
-          *reinterpret_cast<uint4*>(bias_t + AF_QP_BYTES + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-          *reinterpret_cast<uint4*>(bias_t + 2 * AF_QP_BYTES + pos) = make_uint4(l2[0], l2[1], l2[2], l2[3]);
-        }
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(b_full);
-    }
-    mbar_wait(s_full, 0);
-    tc_fence_after();
-    const uint32_t s_taddr = tmem_base + (uint32_t(qw4 * 32) << 16);
-    AfSoftmaxCtx c;
-    c.s_taddr = s_taddr; c.red_max = red_max; c.red_sum = red_sum; c.row = row; c.qi = qi; c.valid = valid; c.bh = bh;
-    c.cg = cg;
-    c.qp = qp; c.p_full = p_full; c.p_empty = p_empty; c.o_full = o_full;
-    af_softmax<NSPLIT, KT>(p, c);
+    sum = af_warp_sum(sum);
+    const float inv = 1.f / sum;
+    for (int k = lane; k < AF_NK_MAX; k += 32) s[k] = k < p.Nk ? s[k] * inv : 0.f;
+    if (p.p_hi)
+      for (int k = lane; k < p.p_pitch; k += 32) af_put_split(p.p_hi, p.p_lo, r * p.p_pitch + k, k < AF_NK_MAX ? s[k] : 0.f);
+    if (p.lse && lane == 0) p.lse[r] = mx + logf(sum);
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  // ---- O = P v over 64-key blocks: P block -> swizzled bf16 planes, v block -> MN-major atoms, wgmma 64 x 96
+  constexpr int NP = NSPLIT == 3 ? 2 : 1;
+  float o[AF_HD / 2];
+  const uint32_t p_base = smem_u32(smem + AF_OFF_P), v_base = smem_u32(smem + AF_OFF_K);
+  const int nkb = (p.Nk + 63) / 64;
+  for (int kb = 0; kb < nkb; ++kb) {
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(bar, NP * 2 * AF_VA_BYTES);
+      for (int pl = 0; pl < NP; ++pl)
+        for (int a = 0; a < 2; ++a)
+          af_tma_3d(smem + AF_OFF_K + (pl * 2 + a) * AF_VA_BYTES, &p.tmV[pl], bar, a * 64, kb * 64, bh);
+    }
+    // element (row r, key c) of a K-major 128B-swizzled [64 x 64] tile: byte r*128 + ((c/8) ^ (r%8))*16 + (c%8)*2
+    for (int i = threadIdx.x; i < AF_BM * 8; i += 128) {
+      const int r = i >> 3, g = i & 7, c0 = kb * 64 + g * 8;
+      uint32_t hw[4], lw[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float x[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) x[e] = (c0 + 2 * j + e) < AF_NK_MAX ? S[r * AF_SP + c0 + 2 * j + e] : 0.f;
+        const __nv_bfloat162 h = __floats2bfloat162_rn(x[0], x[1]);
+        const float2 hf = __bfloat1622float2(h);
+        const __nv_bfloat162 l = __floats2bfloat162_rn(x[0] - hf.x, x[1] - hf.y);
+        hw[j] = *reinterpret_cast<const uint32_t*>(&h);
+        lw[j] = *reinterpret_cast<const uint32_t*>(&l);
+      }
+      const uint32_t off = uint32_t(r) * 128u + uint32_t((g ^ (r & 7)) * 16);
+      *reinterpret_cast<uint4*>(smem + AF_OFF_P + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+      if (NSPLIT == 3) *reinterpret_cast<uint4*>(smem + AF_OFF_P + AF_QT_BYTES + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+    }
+    fence_proxy_async_smem();   // the generic-proxy stores above are read by wgmma (async proxy)
+    __syncthreads();
+    mbar_wait(bar, phase);
+    phase ^= 1;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t a_hi = make_smem_desc(p_base + ks * 32, 16, 1024, 2);
+      const uint64_t b_hi = make_smem_desc(v_base + ks * 2048, AF_VA_BYTES, 1024, 2);
+      const uint32_t acc = (kb | ks) != 0;
+      if (NSPLIT == 3) {
+        const uint64_t a_lo = make_smem_desc(p_base + AF_QT_BYTES + ks * 32, 16, 1024, 2);
+        const uint64_t b_lo = make_smem_desc(v_base + 2 * AF_VA_BYTES + ks * 2048, AF_VA_BYTES, 1024, 2);
+        wgmma_m64n96<0, 1>(o, a_lo, b_hi, acc);
+        wgmma_m64n96<0, 1>(o, a_hi, b_lo, 1u);
+        wgmma_m64n96<0, 1>(o, a_hi, b_hi, 1u);
+      } else {
+        wgmma_m64n96<0, 1>(o, a_hi, b_hi, acc);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncthreads();   // P staging and the v atoms are free for the next block
+  }
+  // O fragments -> [BH, Nq, 96]
+  const int rw = warp * 16 + (lane >> 2), cp = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int q = q0 + rw + 8 * h;
+    if (q < p.Nq) {
+      float* dst = p.out + (int64_t(bh) * p.Nq + q) * AF_HD + cp;
+#pragma unroll
+      for (int j = 0; j < AF_HD / 8; ++j)
+        *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[4 * j + 2 * h], o[4 * j + 2 * h + 1]);
+    }
   }
 }
 
-// ------------------------------------------------------------------------------------------------ backward, first half
-// dS producer: per (clip*head, 128-query tile)
-//     dP = dO v^T                      tcgen05.mma into TMEM columns 0..399 (never written to HBM)
-//     delta = sum_k P dP ;  dS = P (dP - delta)     P from the planes the forward saved, dS -> split planes in HBM (operand of
-//                                                   the dq / dk GEMMs) and in shared memory
-//     d[A | B | C] = dS . E            second tcgen05.mma (the transpose of the forward's bias product): the relative-position
-//                                      gradient of the row's 22 table lookups, scattered into the dRQ row
-// Replaces sfb_gemm_batched (dP, fp32 [BH, Nq, Nk] written and re-read) + sfb_softmax_relpos_bwd.
-struct AttnBwdParams {
-  CUtensorMap tmDO[2], tmV[2], tmE;
-  int BH, Nq, Nk, q_tiles;
-  const __nv_bfloat16* p_hi; const __nv_bfloat16* p_lo; int64_t p_pitch;
-  __nv_bfloat16* ds_hi; __nv_bfloat16* ds_lo; int64_t ds_pitch;
-  float* drq; int64_t rq_pitch; int Lh, Lw;
-  int qh, qw;
-  float rh_q, rh_k, rw_q, rw_k, rt_q, rt_k;
-};
-
-__device__ __forceinline__ void af_unpack8(const uint4& u, float (&f)[8]) {
-  f[0] = __uint_as_float(u.x << 16); f[1] = __uint_as_float(u.x & 0xffff0000u);
-  f[2] = __uint_as_float(u.y << 16); f[3] = __uint_as_float(u.y & 0xffff0000u);
-  f[4] = __uint_as_float(u.z << 16); f[5] = __uint_as_float(u.z & 0xffff0000u);
-  f[6] = __uint_as_float(u.w << 16); f[7] = __uint_as_float(u.w & 0xffff0000u);
-}
-
-template <int NSPLIT, int KT>
-__global__ void __launch_bounds__(576, 1) attn_bwd_ds_kernel(const __grid_constant__ AttnBwdParams p) {
-  constexpr int NK = 1 + KT * AF_KH * AF_KW;
-  constexpr int NKT = (NK + AF_BN - 1) / AF_BN;
-  constexpr int NKB = (NK + 63) / 64;
-  constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
-  constexpr uint32_t O_COL = NKT * AF_BN;             // 400: d[A|B|C] lives in 32 columns behind dP
+template <int NSPLIT>
+__global__ void __launch_bounds__(128, 1) attn_bwd_ds_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // [dO / dS union: 4 x 16 KB] [V tile / E block ring: 2 x 40 KB] [barriers]
-  uint8_t* qp = smem;
-  uint8_t* ring = smem + 4 * AF_QP_BYTES;
-  constexpr uint32_t K_STAGE = 2 * 2 * AF_KT_BYTES;
-  constexpr uint32_t E_STAGE = 8192;                  // one [64 keys x 64] selector block
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + 2 * K_STAGE);
-  uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;
-  uint64_t* k_empty = bars + 3;
-  uint64_t* s_full = bars + 5;
-  uint64_t* e_full = bars + 6;
-  uint64_t* e_empty = bars + 8;
-  uint64_t* p_full = bars + 10;
-  uint64_t* p_empty = bars + 12;
-  uint64_t* o_full = bars + 14;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  const bool has_rel = p.drq != nullptr;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int bh = blockIdx.x / p.q_tiles;
-  const int q0 = (blockIdx.x - bh * p.q_tiles) * 128;
-
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + AF_OFF_BAR);
+  float* S = reinterpret_cast<float*>(smem + AF_OFF_S);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int bh = blockIdx.x / p.q_tiles, q0 = (blockIdx.x % p.q_tiles) * AF_BM;
   if (threadIdx.x == 0) {
-    mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&e_full[s], 1);
-      mbar_init(&e_empty[s], 1);
-      mbar_init(&p_full[s], 16);
-      mbar_init(&p_empty[s], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(o_full, 1);
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  uint32_t phase = 0;
+  af_scores<NSPLIT>(p, smem, bar, phase, bh, q0);   // dP = dO v^T
 
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_expect_tx(q_full, 2 * NP * AF_QP_BYTES);
-      for (int kb = 0; kb < 2; ++kb)
-        for (uint32_t pl = 0; pl < NP; ++pl)
-          af_tma_3d(qp + (kb * 2 + pl) * AF_QP_BYTES, &p.tmDO[pl], q_full, kb * 64, q0, bh);
-    }
-    __syncwarp();
-    for (int t = 0; t < NKT; ++t) {
-      const int s = t & 1;
-      mbar_wait(&k_empty[s], ((t >> 1) & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&k_full[s], 2 * NP * AF_KT_BYTES);
-        uint8_t* st = ring + s * K_STAGE;
-        for (int kb = 0; kb < 2; ++kb)
-          for (uint32_t pl = 0; pl < NP; ++pl)
-            af_tma_3d(st + (kb * 2 + pl) * AF_KT_BYTES, &p.tmV[pl], &k_full[s], kb * 64, t * AF_BN, bh);
-      }
-      __syncwarp();
-    }
-    if (has_rel) {
-      mbar_wait(s_full, 0);              // the V tiles' last readers are done: the ring is free for the selector blocks
-      for (int kb = 0; kb < NKB; ++kb) {
-        const int s = kb & 1;
-        mbar_wait(&e_empty[s], ((kb >> 1) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&e_full[s], E_STAGE);
-          af_tma_3d(ring + s * E_STAGE, &p.tmE, &e_full[s], 0, kb * 64, 0);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc_s = make_idesc_bf16(128, AF_BN, 0, 0);
-    const uint32_t idesc_r = make_idesc_bf16(128, 32, 0, 1);
-    mbar_wait(q_full, 0);
-    tc_fence_after();
-    const uint32_t q_base = smem_u32(qp);
-    for (int t = 0; t < NKT; ++t) {
-      const int s = t & 1;
-      mbar_wait(&k_full[s], (t >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t k_base = smem_u32(ring + s * K_STAGE);
-        const uint32_t d_tmem = tmem_base + uint32_t(t * AF_BN);
-#pragma unroll
-        for (int ks = 0; ks < AF_HD / 16; ++ks) {
-          const int kb = ks >> 2, kk = ks & 3;
-          uint64_t a_d[2], b_d[2];
-          for (uint32_t pl = 0; pl < NP; ++pl) {
-            a_d[pl] = make_smem_desc(q_base + (kb * 2 + pl) * AF_QP_BYTES + kk * 32, 16, 1024, 2);
-            b_d[pl] = make_smem_desc(k_base + (kb * 2 + pl) * AF_KT_BYTES + kk * 32, 16, 1024, 2);
-          }
-          const uint32_t acc = ks != 0 ? 1u : 0u;
-          if (NSPLIT == 3) {
-            umma_bf16(d_tmem, a_d[1], b_d[0], idesc_s, acc);
-            umma_bf16(d_tmem, a_d[0], b_d[1], idesc_s, 1u);
-            umma_bf16(d_tmem, a_d[0], b_d[0], idesc_s, 1u);
-          } else {
-            umma_bf16(d_tmem, a_d[0], b_d[0], idesc_s, acc);
-          }
-        }
-        umma_commit(&k_empty[s]);
-        if (t == NKT - 1) umma_commit(s_full);
-      }
-      __syncwarp();
-    }
-    if (has_rel) {
-      const uint32_t o_tmem = tmem_base + O_COL;
-      for (int kb = 0; kb < NKB; ++kb) {
-        const int s = kb & 1;
-        mbar_wait(&e_full[s], (kb >> 1) & 1);
-        mbar_wait(&p_full[s], (kb >> 1) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t p_base = smem_u32(qp + s * 2 * AF_QP_BYTES);
-          const uint32_t e_base = smem_u32(ring + s * E_STAGE);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t e_d = make_smem_desc(e_base + ks * 2048, 8192, 1024, 2);
-            const uint32_t acc = (kb | ks) != 0 ? 1u : 0u;
-            if (NSPLIT == 3) {
-              umma_bf16(o_tmem, make_smem_desc(p_base + AF_QP_BYTES + ks * 32, 16, 1024, 2), e_d, idesc_r, acc);
-              umma_bf16(o_tmem, make_smem_desc(p_base + ks * 32, 16, 1024, 2), e_d, idesc_r, 1u);
-            } else {
-              umma_bf16(o_tmem, make_smem_desc(p_base + ks * 32, 16, 1024, 2), e_d, idesc_r, acc);
-            }
-          }
-          umma_commit(&e_empty[s]);
-          umma_commit(&p_empty[s]);
-          if (kb == NKB - 1) umma_commit(o_full);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    const int qw4 = warp & 3;
-    const int cg = (warp - 2) >> 2;
-    const int row = qw4 * 32 + lane;
-    const int qi = q0 + row;
-    const bool valid = qi < p.Nq;
-    float* red = reinterpret_cast<float*>(bars + 18);      // [4][128]
-    const int64_t grow = int64_t(bh) * p.Nq + qi;
-    const uint4* ph = reinterpret_cast<const uint4*>(p.p_hi + grow * p.p_pitch);
-    const uint4* plo = reinterpret_cast<const uint4*>(p.p_lo + grow * p.p_pitch);
-    mbar_wait(s_full, 0);
-    tc_fence_after();
-    const uint32_t s_taddr = tmem_base + (uint32_t(qw4 * 32) << 16);
-    // pass 1: delta = sum_k P dP  (pad columns of P are zero)
+  // ---- dS = P (dP - sum_k P dP), dRQ (softmax_relpos_bwd arithmetic), one warp per row
+  const int khw = p.kh * p.kw;
+  const int Ltot = p.Lh + p.Lw + p.Lt;
+  float* bins = reinterpret_cast<float*>(smem + AF_OFF_BINS) + warp * AF_BINS_FLOATS;
+  for (int rr = warp; rr < AF_BM; rr += 4) {
+    const int q = q0 + rr;
+    if (q >= p.Nq) break;
+    float* buf = S + rr * AF_SP;
+    const int64_t r = int64_t(bh) * p.Nq + q;
     float dot = 0.f;
-#pragma unroll 1
-    for (int kb = 0; kb < NKB; ++kb) {
-      const int col0 = (kb * 4 + cg) * 16;
-      if (col0 < NK) {
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(s_taddr + uint32_t(col0), v);
-        float pv[16];
-        if (valid) {
-#pragma unroll
-          for (int h8 = 0; h8 < 2; ++h8) {
-            float a[8];
-            af_unpack8(ph[(col0 >> 3) + h8], a);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) pv[h8 * 8 + e] = a[e];
-            if (NSPLIT == 3) {
-              af_unpack8(plo[(col0 >> 3) + h8], a);
-#pragma unroll
-              for (int e = 0; e < 8; ++e) pv[h8 * 8 + e] += a[e];
-            }
-          }
+    for (int k = lane; k < p.Nk; k += 32) {
+      const float pv = af_get_split(p.p_hi, p.p_lo, r * p.p_pitch + k);
+      dot = fmaf(pv, buf[k], dot);
+    }
+    dot = af_warp_sum(dot);
+    const bool rel = p.drq != nullptr && q > 0;
+    if (rel)
+      for (int j = lane; j < Ltot; j += 32) bins[j] = 0.f;
+    for (int k = lane; k < p.ds_pitch; k += 32) {
+      float ds = 0.f;
+      if (k < p.Nk) {
+        ds = af_get_split(p.p_hi, p.p_lo, r * p.p_pitch + k) * (buf[k] - dot);
+        buf[k] = ds;
+      }
+      af_put_split(p.ds_hi, p.ds_lo, r * p.ds_pitch + k, ds);
+    }
+    __syncwarp();
+    if (rel) {
+      int t = q - 1;
+      const int qx = t % p.qw;
+      t /= p.qw;
+      const int qy = t % p.qh;
+      const int qz = t / p.qh;
+      const float* g = buf + 1;  // key grid [kt][kh][kw] behind the cls column
+      for (int a = lane; a < p.kh + p.kw + p.kt; a += 32) {
+        float sum = 0.f;
+        int bin;
+        if (a < p.kh) {
+          for (int kz = 0; kz < p.kt; ++kz)
+            for (int kx = 0; kx < p.kw; ++kx) sum += g[kz * khw + a * p.kw + kx];
+          bin = af_rel_index(qy, a, p.rh_q, p.rh_k, p.kh);
+        } else if (a < p.kh + p.kw) {
+          const int kx = a - p.kh;
+          for (int kz = 0; kz < p.kt; ++kz)
+            for (int ky = 0; ky < p.kh; ++ky) sum += g[kz * khw + ky * p.kw + kx];
+          bin = p.Lh + af_rel_index(qx, kx, p.rw_q, p.rw_k, p.kw);
         } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) pv[e] = 0.f;
+          const int kz = a - p.kh - p.kw;
+          for (int j = 0; j < khw; ++j) sum += g[kz * khw + j];
+          bin = p.Lh + p.Lw + af_rel_index(qz, kz, p.rt_q, p.rt_k, p.kt);
         }
-        tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < 16; ++e) dot = fmaf(pv[e], __uint_as_float(v[e]), dot);
+        atomicAdd(&bins[bin], sum);
       }
+      __syncwarp();
+      float* o = p.drq + (int64_t(bh) * (p.Nq - 1) + (q - 1)) * p.rq_pitch;
+      for (int j = lane; j < p.rq_pitch; j += 32) o[j] = j < Ltot ? bins[j] : 0.f;
     }
-    red[cg * 128 + row] = dot;
-    named_bar_sync(1, 512);
-    dot = (red[row] + red[128 + row]) + (red[256 + row] + red[384 + row]);
-    // pass 2: dS = P (dP - delta) -> global planes (+ shared-memory planes for the d[A|B|C] product)
-    __nv_bfloat16* gd_hi = p.ds_hi + grow * p.ds_pitch;
-    __nv_bfloat16* gd_lo = p.ds_lo ? p.ds_lo + grow * p.ds_pitch : nullptr;
-#pragma unroll 1
-    for (int kb = 0; kb < NKB; ++kb) {
-      const int s = kb & 1;
-      if (has_rel) mbar_wait(&p_empty[s], ((kb >> 1) & 1) ^ 1);
-      uint8_t* pt_hi = qp + (s * 2 + 0) * AF_QP_BYTES + row * 128;
-      uint8_t* pt_lo = qp + (s * 2 + 1) * AF_QP_BYTES + row * 128;
-      const int col0 = kb * 64 + cg * 16;
-      float ds[16];
-#pragma unroll
-      for (int e = 0; e < 16; ++e) ds[e] = 0.f;
-      if (col0 < NK) {
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(s_taddr + uint32_t(col0), v);
-        float pv[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) pv[e] = 0.f;
-        if (valid) {
-#pragma unroll
-          for (int h8 = 0; h8 < 2; ++h8) {
-            float a[8];
-            af_unpack8(ph[(col0 >> 3) + h8], a);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) pv[h8 * 8 + e] = a[e];
-            if (NSPLIT == 3) {
-              af_unpack8(plo[(col0 >> 3) + h8], a);
-#pragma unroll
-              for (int e = 0; e < 8; ++e) pv[h8 * 8 + e] += a[e];
-            }
-          }
-        }
-        tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < 16; ++e) ds[e] = pv[e] * (__uint_as_float(v[e]) - dot);
-      }
-#pragma unroll
-      for (int h8 = 0; h8 < 2; ++h8) {
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int w2 = 0; w2 < 4; ++w2) {
-          const float a = ds[h8 * 8 + 2 * w2], b = ds[h8 * 8 + 2 * w2 + 1];
-          const __nv_bfloat16 ah = __float2bfloat16_rn(a), bhh = __float2bfloat16_rn(b);
-          const __nv_bfloat16 al = __float2bfloat16_rn(a - __bfloat162float(ah));
-          const __nv_bfloat16 bl = __float2bfloat16_rn(b - __bfloat162float(bhh));
-          hi[w2] = uint32_t(__bfloat16_as_ushort(ah)) | (uint32_t(__bfloat16_as_ushort(bhh)) << 16);
-          lo[w2] = uint32_t(__bfloat16_as_ushort(al)) | (uint32_t(__bfloat16_as_ushort(bl)) << 16);
-        }
-        if (has_rel) {
-          const int pos = ((cg * 2 + h8) ^ (row & 7)) * 16;
-          *reinterpret_cast<uint4*>(pt_hi + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          if (NSPLIT == 3) *reinterpret_cast<uint4*>(pt_lo + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
-        const int gcol = col0 + h8 * 8;
-        if (valid && gcol < p.ds_pitch) {
-          *reinterpret_cast<uint4*>(gd_hi + gcol) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          if (gd_lo) *reinterpret_cast<uint4*>(gd_lo + gcol) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
-      }
-      if (has_rel) {
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[s]);
-      }
-    }
-    // epilogue: the 22 table-lookup gradients of this row -> its dRQ row (zero elsewhere)
-    if (has_rel && cg == 0) {
-      mbar_wait(o_full, 0);
-      tc_fence_after();
-      uint32_t v0[16], v1[16];
-      tmem_ld_32x32b_x16(s_taddr + O_COL, v0);
-      tmem_ld_32x32b_x16(s_taddr + O_COL + 16u, v1);
-      tmem_ld_wait();
-      if (valid && qi > 0) {
-        float* o = p.drq + (int64_t(bh) * (p.Nq - 1) + (qi - 1)) * p.rq_pitch;
-        for (int j = 0; j < int(p.rq_pitch); j += 4) *reinterpret_cast<float4*>(o + j) = make_float4(0.f, 0.f, 0.f, 0.f);
-        int t = qi - 1;
-        const int qx = t % p.qw;
-        t /= p.qw;
-        const int qy = t % p.qh;
-        const int qz = t / p.qh;
-        const float bh0 = float(qy) * p.rh_q + float(AF_KH - 1) * p.rh_k;
-        const float bw0 = float(qx) * p.rw_q + float(AF_KW - 1) * p.rw_k;
-        const float bt0 = float(qz) * p.rt_q + float(KT - 1) * p.rt_k;
-#pragma unroll
-        for (int i = 0; i < AF_KH; ++i) o[int(floorf(bh0 - float(i) * p.rh_k))] = __uint_as_float(v0[i]);
-#pragma unroll
-        for (int i = 0; i < AF_KW; ++i) {
-          const int kap = AF_KH + i;
-          o[p.Lh + int(floorf(bw0 - float(i) * p.rw_k))] = __uint_as_float(kap < 16 ? v0[kap] : v1[kap - 16]);
-        }
-#pragma unroll
-        for (int i = 0; i < KT; ++i) {
-          const int kap = AF_KH + AF_KW + i;
-          o[p.Lh + p.Lw + int(floorf(bt0 - float(i) * p.rt_k))] = __uint_as_float(kap < 16 ? v0[kap] : v1[kap - 16]);
-        }
-      }
-    }
+    __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// E[key j][kappa] (bf16, [400 x 64]): 1 at kappa = kh(j), 7 + kw(j), 14 + kt(j) for the grid keys j >= 1; the cls key and the
-// pad rows are zero
-__global__ void af_selector_kernel(__nv_bfloat16* e, int rows, int kt, int kh, int kw) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= rows * 64) return;
-  const int j = i >> 6, kap = i & 63;
-  float v = 0.f;
-  if (j >= 1 && j < 1 + kt * kh * kw) {
-    const int g = j - 1;
-    const int kx = g % kw, ky = (g / kw) % kh, kz = g / (kw * kh);
-    if (kap == ky || kap == kh + kx || kap == kh + kw + kz) v = 1.f;
-  }
-  e[i] = __float2bfloat16_rn(v);
 }
 
 typedef CUresult (*AfEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// 3-D map over bf16 [batch][rows][cols] (cols contiguous), box = [1][box_rows][64], 128B swizzle, out-of-bounds zero
 static int af_tmap(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint64_t ld, uint64_t bs,
                    uint32_t box_rows) {
   static AfEncodeFn fn = nullptr;
@@ -825,8 +372,31 @@ static int af_tmap(CUtensorMap* out, const void* base, uint64_t cols, uint64_t r
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("sfb_attn_fwd: cuTensorMapEncodeTiled failed (%d)", (int)r);
+    set_error("fused attention: cuTensorMapEncodeTiled failed (%d)", (int)r);
     return -2;
+  }
+  return 0;
+}
+
+static void af_geometry(AttnParams& p, int qt, int qh, int qw, int kt, int kh, int kw) {
+  p.qt = qt; p.qh = qh; p.qw = qw; p.kt = kt; p.kh = kh; p.kw = kw;
+  p.Lh = 2 * std::max(qh, kh) - 1;
+  p.Lw = 2 * std::max(qw, kw) - 1;
+  p.Lt = 2 * std::max(qt, kt) - 1;
+  auto ratio = [](int a, int b) { const float r = float(a) / float(b); return r > 1.f ? r : 1.f; };
+  p.rh_q = ratio(kh, qh); p.rh_k = ratio(qh, kh);
+  p.rw_q = ratio(kw, qw); p.rw_k = ratio(qw, kw);
+  p.rt_q = ratio(kt, qt); p.rt_k = ratio(qt, kt);
+}
+
+template <typename K>
+static int af_launch(K kernel, const AttnParams& p, cudaStream_t stream, const char* what) {
+  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(AF_SMEM));
+  kernel<<<p.BH * p.q_tiles, 128, AF_SMEM, stream>>>(p);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s launch failed: %s (grid=%d smem=%u)", what, cudaGetErrorString(e), p.BH * p.q_tiles, AF_SMEM);
+    return -20;
   }
   return 0;
 }
@@ -837,27 +407,10 @@ using namespace sfb;
 
 extern "C" int32_t sfb_attn_fwd_supported(int32_t nk, int32_t hd, int32_t kt, int32_t kh, int32_t kw) {
   static const bool on = [] { const char* e = getenv("SFB_ATTN_FUSED"); return e ? e[0] != '0' : true; }();
-  return on && hd == AF_HD && kh == AF_KH && kw == AF_KW && kt == 8 && nk == 1 + kt * kh * kw;
-}
-
-extern "C" int64_t sfb_attn_fwd_selector_bytes(void) { return int64_t(400) * 64 * 2; }
-
-extern "C" int sfb_attn_fwd_selector(void* e_sel, int32_t kt, int32_t kh, int32_t kw, void* stream) {
-  if (!e_sel || 1 + kt * kh * kw > 400 || kh + kw + kt > 32) {
-    set_error("sfb_attn_fwd_selector: bad arguments");
-    return -10;
-  }
-  af_selector_kernel<<<(400 * 64 + 255) / 256, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)e_sel, 400, kt, kh, kw);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_attn_fwd_selector launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return on && hd == AF_HD && kh == 7 && kw == 7 && kt == 8 && nk == 1 + kt * kh * kw;
 }
 
 extern "C" int sfb_attn_fwd(const sfb_attn_fwd_desc* d, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
   if (!sfb_attn_fwd_supported(d->nk, d->hd, d->kt, d->kh, d->kw)) {
     set_error("sfb_attn_fwd: only head_dim 96 with an 8x7x7 key grid (Nk = 393) is fused; use the unfused sequence otherwise");
     return -10;
@@ -874,64 +427,27 @@ extern "C" int sfb_attn_fwd(const sfb_attn_fwd_desc* d, void* stream_) {
     set_error("sfb_attn_fwd: p_pitch must be a multiple of 8 and >= nk");
     return -10;
   }
-  AttnFwdParams p;
+  AttnParams p;
   memset(&p, 0, sizeof(p));
   p.BH = d->bh; p.Nq = d->nq; p.Nk = d->nk;
-  p.q_tiles = (d->nq + 127) / 128;
+  p.q_tiles = (d->nq + AF_BM - 1) / AF_BM;
   p.rq = d->rq; p.rq_pitch = d->rq_pitch;
-  p.qh = d->qh; p.qw = d->qw;
-  p.Lh = 2 * std::max(d->qh, d->kh) - 1;
-  p.Lw = 2 * std::max(d->qw, d->kw) - 1;
-  auto ratio = [](int a, int b) { float r = float(a) / float(b); return r > 1.f ? r : 1.f; };
-  p.rh_q = ratio(d->kh, d->qh); p.rh_k = ratio(d->qh, d->kh);
-  p.rw_q = ratio(d->kw, d->qw); p.rw_k = ratio(d->qw, d->kw);
-  p.rt_q = ratio(d->kt, d->qt); p.rt_k = ratio(d->qt, d->kt);
+  af_geometry(p, d->qt, d->qh, d->qw, d->kt, d->kh, d->kw);
   p.scale = d->scale;
-  p.out = d->out; p.p_hi = (__nv_bfloat16*)d->p_hi; p.p_lo = (__nv_bfloat16*)d->p_lo; p.p_pitch = d->p_pitch; p.lse = d->lse;
+  p.out = d->out; p.lse = d->lse;
+  p.p_hi = (__nv_bfloat16*)d->p_hi; p.p_lo = (__nv_bfloat16*)d->p_lo; p.p_pitch = d->p_pitch;
   const int np = d->nsplit == 3 ? 2 : 1;
   for (int pl = 0; pl < np; ++pl) {
-    const void* q = pl ? d->q_lo : d->q_hi;
-    const void* k = pl ? d->k_lo : d->k_hi;
-    const void* v = pl ? d->v_lo : d->v_hi;
-    if (int rc = af_tmap(&p.tmQ[pl], q, AF_HD, d->nq, d->bh, AF_HD, uint64_t(d->nq) * AF_HD, 128)) return rc;
-    if (int rc = af_tmap(&p.tmK[pl], k, AF_HD, d->nk, d->bh, AF_HD, uint64_t(d->nk) * AF_HD, AF_BN)) return rc;
-    if (int rc = af_tmap(&p.tmV[pl], v, AF_HD, d->nk, d->bh, AF_HD, uint64_t(d->nk) * AF_HD, 64)) return rc;
+    if (int rc = af_tmap(&p.tmA[pl], pl ? d->q_lo : d->q_hi, AF_HD, d->nq, d->bh, AF_HD, uint64_t(d->nq) * AF_HD, AF_BM)) return rc;
+    if (int rc = af_tmap(&p.tmK[pl], pl ? d->k_lo : d->k_hi, AF_HD, d->nk, d->bh, AF_HD, uint64_t(d->nk) * AF_HD, AF_BN)) return rc;
+    if (int rc = af_tmap(&p.tmV[pl], pl ? d->v_lo : d->v_hi, AF_HD, d->nk, d->bh, AF_HD, uint64_t(d->nk) * AF_HD, 64)) return rc;
   }
-  if (d->rq) {
-    if (!d->e_sel) {
-      set_error("sfb_attn_fwd: e_sel workspace (sfb_attn_fwd_selector_bytes()) is required with a rel-pos bias");
-      return -10;
-    }
-    if (int rc = af_tmap(&p.tmE, d->e_sel, 64, 400, 1, 64, uint64_t(400) * 64, AF_BN)) return rc;
-  }
-  const uint32_t smem_bytes = 4 * AF_QP_BYTES + 3 * AF_QP_BYTES + 2 * (2 * 2 * AF_KT_BYTES + AF_KT_BYTES) + 256 +
-                              2 * 4 * 128 * 4 + 1024;
-  const int grid = d->bh * p.q_tiles;
-  if (d->nsplit == 3) {
-    static bool a3 = false;
-    if (!a3) {
-      cudaFuncSetAttribute(attn_fwd_kernel<3, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_bytes));
-      a3 = true;
-    }
-    attn_fwd_kernel<3, 8><<<grid, 576, smem_bytes, stream>>>(p);
-  } else {
-    static bool a1 = false;
-    if (!a1) {
-      cudaFuncSetAttribute(attn_fwd_kernel<1, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_bytes));
-      a1 = true;
-    }
-    attn_fwd_kernel<1, 8><<<grid, 576, smem_bytes, stream>>>(p);
-  }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_attn_fwd launch failed: %s (grid=%d smem=%u)", cudaGetErrorString(e), grid, smem_bytes);
-    return -20;
-  }
-  return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  return d->nsplit == 3 ? af_launch(attn_fwd_kernel<3>, p, stream, "sfb_attn_fwd")
+                        : af_launch(attn_fwd_kernel<1>, p, stream, "sfb_attn_fwd");
 }
 
 extern "C" int sfb_attn_bwd_ds(const sfb_attn_bwd_desc* d, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
   if (!sfb_attn_fwd_supported(d->nk, d->hd, d->kt, d->kh, d->kw)) {
     set_error("sfb_attn_bwd_ds: only head_dim 96 with an 8x7x7 key grid (Nk = 393) is fused");
     return -10;
@@ -944,52 +460,26 @@ extern "C" int sfb_attn_bwd_ds(const sfb_attn_bwd_desc* d, void* stream_) {
     set_error("sfb_attn_bwd_ds: null operand pointer");
     return -10;
   }
-  if (d->p_pitch % 8 || d->p_pitch < 400 || d->ds_pitch % 8 || d->ds_pitch < d->nk || (d->drq && (d->rq_pitch % 4 || !d->e_sel))) {
-    set_error("sfb_attn_bwd_ds: P rows must hold 400 columns (pad columns zero), pitches multiples of 8, e_sel set with drq");
+  AttnParams p;
+  memset(&p, 0, sizeof(p));
+  af_geometry(p, d->qt, d->qh, d->qw, d->kt, d->kh, d->kw);
+  if (d->p_pitch % 8 || d->p_pitch < d->nk || d->ds_pitch % 8 || d->ds_pitch < d->nk || (d->drq && d->rq_pitch % 4) ||
+      p.Lh + p.Lw + p.Lt > int(AF_BINS_FLOATS)) {
+    set_error("sfb_attn_bwd_ds: pitches must be multiples of 8 holding nk columns (rq_pitch a multiple of 4), rel-pos tables <= %u",
+              AF_BINS_FLOATS);
     return -10;
   }
-  AttnBwdParams p;
-  memset(&p, 0, sizeof(p));
   p.BH = d->bh; p.Nq = d->nq; p.Nk = d->nk;
-  p.q_tiles = (d->nq + 127) / 128;
-  p.p_hi = (const __nv_bfloat16*)d->p_hi; p.p_lo = (const __nv_bfloat16*)d->p_lo; p.p_pitch = d->p_pitch;
+  p.q_tiles = (d->nq + AF_BM - 1) / AF_BM;
+  p.p_hi = (__nv_bfloat16*)d->p_hi; p.p_lo = d->nsplit == 3 ? (__nv_bfloat16*)d->p_lo : nullptr; p.p_pitch = d->p_pitch;
   p.ds_hi = (__nv_bfloat16*)d->ds_hi; p.ds_lo = (__nv_bfloat16*)d->ds_lo; p.ds_pitch = d->ds_pitch;
   p.drq = d->drq; p.rq_pitch = d->rq_pitch;
-  p.qh = d->qh; p.qw = d->qw;
-  p.Lh = 2 * std::max(d->qh, d->kh) - 1;
-  p.Lw = 2 * std::max(d->qw, d->kw) - 1;
-  auto ratio = [](int a, int b) { float r = float(a) / float(b); return r > 1.f ? r : 1.f; };
-  p.rh_q = ratio(d->kh, d->qh); p.rh_k = ratio(d->qh, d->kh);
-  p.rw_q = ratio(d->kw, d->qw); p.rw_k = ratio(d->qw, d->kw);
-  p.rt_q = ratio(d->kt, d->qt); p.rt_k = ratio(d->qt, d->kt);
   const int np = d->nsplit == 3 ? 2 : 1;
   for (int pl = 0; pl < np; ++pl) {
-    if (int rc = af_tmap(&p.tmDO[pl], pl ? d->do_lo : d->do_hi, AF_HD, d->nq, d->bh, AF_HD, uint64_t(d->nq) * AF_HD, 128)) return rc;
-    if (int rc = af_tmap(&p.tmV[pl], pl ? d->v_lo : d->v_hi, AF_HD, d->nk, d->bh, AF_HD, uint64_t(d->nk) * AF_HD, AF_BN)) return rc;
+    if (int rc = af_tmap(&p.tmA[pl], pl ? d->do_lo : d->do_hi, AF_HD, d->nq, d->bh, AF_HD, uint64_t(d->nq) * AF_HD, AF_BM)) return rc;
+    if (int rc = af_tmap(&p.tmK[pl], pl ? d->v_lo : d->v_hi, AF_HD, d->nk, d->bh, AF_HD, uint64_t(d->nk) * AF_HD, AF_BN)) return rc;
   }
-  if (d->drq)
-    if (int rc = af_tmap(&p.tmE, d->e_sel, 64, 400, 1, 64, uint64_t(400) * 64, 64)) return rc;
-  const uint32_t smem_bytes = 4 * AF_QP_BYTES + 2 * (2 * 2 * AF_KT_BYTES) + 256 + 4 * 128 * 4 + 1024;
-  const int grid = d->bh * p.q_tiles;
-  if (d->nsplit == 3) {
-    static bool a3 = false;
-    if (!a3) {
-      cudaFuncSetAttribute(attn_bwd_ds_kernel<3, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_bytes));
-      a3 = true;
-    }
-    attn_bwd_ds_kernel<3, 8><<<grid, 576, smem_bytes, stream>>>(p);
-  } else {
-    static bool a1 = false;
-    if (!a1) {
-      cudaFuncSetAttribute(attn_bwd_ds_kernel<1, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_bytes));
-      a1 = true;
-    }
-    attn_bwd_ds_kernel<1, 8><<<grid, 576, smem_bytes, stream>>>(p);
-  }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_attn_bwd_ds launch failed: %s (grid=%d smem=%u)", cudaGetErrorString(e), grid, smem_bytes);
-    return -20;
-  }
-  return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  return d->nsplit == 3 ? af_launch(attn_bwd_ds_kernel<3>, p, stream, "sfb_attn_bwd_ds")
+                        : af_launch(attn_bwd_ds_kernel<1>, p, stream, "sfb_attn_bwd_ds");
 }

@@ -19,7 +19,7 @@
 #include "../../include/slowfast_b200.h"
 #include "tmap.h"
 
-// shipped default of the switch (1 once the body is validated and measured faster on the B200; see DESIGN.md)
+// shipped default of the switch
 #ifndef SFB_SIMT_DEFAULT
 #define SFB_SIMT_DEFAULT 1
 #endif
@@ -181,9 +181,9 @@ __global__ void __launch_bounds__(128) conv_direct_kernel(const DirectParams p) 
 
 // 1 = handled here (rc in *rc_out), 0 = not eligible: the caller continues with the tensor-core path
 static int g_simt_enabled = [] { const char* e = getenv("SFB_SIMT_SMALLC"); return e ? int(e[0] == '1') : SFB_SIMT_DEFAULT; }();
-// measured on the B200 (tests/probes/smallc_probe.py, profiles/r2_smallc_probe.md): the fp32 body wins where ONE pixel is a
-// 16-byte TMA request (C_in = 8: 144 -> 80 us for 8->32 1x1x1, 92 -> 58 us for 8->8 1x3x3) and loses from C_in = 16 on
-// (the tensor-core body reaches 2.3-2.8 TB/s there), so the default is C_in <= 8 and <= 1024 MAC per pixel
+// the fp32 body is meant for layers where ONE pixel is a 16-byte TMA request (C_in = 8); from C_in = 16 on the tensor-core
+// body streams its operands at full rate, so the limit is C_in <= 8 and <= 1024 MAC per pixel (tests/probes/smallc_probe.py
+// compares the two)
 static int g_simt_max_macs = [] { const char* e = getenv("SFB_SIMT_MAX_MACS"); return e ? atoi(e) : 1024; }();
 static int g_simt_max_cin = [] { const char* e = getenv("SFB_SIMT_MAX_CIN"); return e ? atoi(e) : 8; }();
 

@@ -1,16 +1,16 @@
-// Implicit-GEMM 3-D convolution for sm_100a.
+// Implicit-GEMM 3-D convolution for sm_90a.
 //
 //   GEMM view: D[M = n*ot*oh*ow, N = cout] = A_im2col[M, K = taps*c] * B[N, K]^T
 //
 // * A is never materialised: each K chunk (one filter tap x CK channels) of a 128-pixel tile is fetched by ONE
 //   TMA im2col load straight into (swizzled) shared memory; padding and the M tail are zero-filled by the unit.
 // * B (filter matrix, K-major) arrives through a tiled TMA load (128B swizzle).
-// * tcgen05.mma (UMMA 128 x BN x 16, bf16 -> fp32) accumulates into TMEM; in parity mode every product is the
+// * wgmma (64 x BN x 16 per warpgroup, bf16 -> fp32) accumulates in registers; in parity mode every product is the
 //   3-term split  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi.
-// * Persistent CTAs, warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM owner),
-//   warps 2..5 = epilogue.  Two TMEM accumulator stages let the epilogue of tile i overlap the main loop of
-//   tile i+1.
-// * Epilogue: TMEM -> registers -> smem transpose -> coalesced fp32 stores through an arbitrary (n,t,h,w)-strided
+// * Persistent CTAs, warp-specialised: warps 0..7 = two MMA warpgroups (rows 0..63 / 64..127 of the tile),
+//   warp 8 = TMA producer, warps 9..16 = epilogue.  The MMA warpgroups hand a finished tile to the epilogue through a
+//   shared-memory accumulator tile and go on with the main loop of the next one.
+// * Epilogue: accumulator tile -> coalesced fp32 stores through an arbitrary (n,t,h,w)-strided
 //   output view (channel-slice "concat in place", strided dgrad scatter), optional accumulate, and per-tile
 //   per-channel (sum, sum^2) partials for train-mode BatchNorm ([2][cout][m_tiles]).
 #include <algorithm>
@@ -29,8 +29,13 @@ constexpr int A_PLANE_BYTES = BLOCK_M * 128;  // 128 pixels x 64 bf16
 constexpr int MAX_STAGES = 8;
 // SFB_CONV_FORCE_IM2COL=1: load tap-free convolutions through the im2col path too (A/B measurements, tests)
 static const bool g_force_im2col = [] { const char* e = getenv("SFB_CONV_FORCE_IM2COL"); return e && e[0] == '1'; }();
-constexpr int EPI_WARPS = 8;                       // two per TMEM lane quarter: the pair splits the tile's 16-column chunks
-constexpr int EPI_STAGE_FLOATS = 32 * 20 + 64;   // per epilogue warp: a [32 rows][16 + 4 pad] fp32 tile + 32 row offsets (int64)
+constexpr int EPI_WARPS = 8;                     // two per 32-row quarter of the tile: the pair splits the tile's 16-column chunks
+constexpr int EPI_STAGE_FLOATS = 64;             // per epilogue warp: 32 row offsets (int64)
+constexpr int MMA_WARPS = 8;                     // two warpgroups of 64 tile rows
+constexpr int PRODUCER_WARP = MMA_WARPS;
+constexpr int EPI_WARP0 = MMA_WARPS + 1;
+constexpr int CONV_THREADS = 32 * (MMA_WARPS + 1 + EPI_WARPS);
+constexpr int BN_MAX = 128;                      // accumulator columns per tile: 64 registers per MMA thread
 
 struct ConvParams {
   CUtensorMap tmA[2];
@@ -46,8 +51,8 @@ struct ConvParams {
   int a_tiled;  // tap-free stride-1 conv: A is the plain [M][C] matrix, loaded with tiled (not im2col) TMA
   uint32_t stage_bytes, chunk_bytes, b_bytes, a_total_bytes, a_plane_bytes;
   uint32_t a_layout, a_sbo, a_lbo;
-  uint32_t tmem_cols;
-  uint32_t off_staging, off_red, off_bars;
+  uint32_t acc_pitch;  // floats per row of the shared-memory accumulator tile
+  uint32_t off_acc, off_staging, off_red, off_bars;
   float* out;
   long long os_n, os_z, os_p, os_q;
   int accumulate;
@@ -59,7 +64,7 @@ struct ConvParams {
 int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out);
 
 template <int NSPLIT>
-__global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
+__global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
@@ -69,33 +74,24 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1) conv_igemm_kernel(cons
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + MAX_STAGES;
   uint64_t* tfull = empty + MAX_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* tempty = tfull + 1;
+  float* acc_tile = reinterpret_cast<float*>(smem + p.off_acc);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 32 * MMA_WARPS);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], EPI_WARPS);
-    }
+    mbar_init(tfull, 32 * MMA_WARPS);
+    mbar_init(tempty, EPI_WARPS);
     fence_mbar_init();
     fence_proxy_async_smem();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int total_tiles = p.m_tiles * p.n_tiles;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
       tma_prefetch_desc(&p.tmA[0]);
@@ -167,78 +163,78 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1) conv_igemm_kernel(cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = make_idesc_bf16(BLOCK_M, uint32_t(p.BN), 0, 0);
+  } else if (warp < MMA_WARPS) {
+    // ------------------------------------------------------------------ MMA warpgroups
+    const int g = warp >> 2;  // tile rows 64g .. 64g+63: 8 core-matrix row groups (SBO apart) further into the A tile
+    const uint32_t a_row_off = uint32_t(g) * 8u * p.a_sbo;
+    float d[BN_MAX / 2];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + uint32_t(acc * p.BN);
+      int held = -1;  // stage whose MMAs may still be reading shared memory
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const int chunk0 = kb * p.cps;
-          const int nch = min(p.cps, p.n_chunks_padded - chunk0);
-          const int ksteps = (nch * p.CK) >> 4;
-          const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t b_base = a_base + p.a_total_bytes;
-          for (int ks = 0; ks < ksteps; ++ks) {
-            uint32_t a_addr;
-            if (p.CK >= 16) {
-              const int k0 = ks * 16;
-              const int chunk = k0 / p.CK;
-              a_addr = a_base + uint32_t(chunk) * p.chunk_bytes + uint32_t(k0 - chunk * p.CK) * 2u;
-            } else {
-              a_addr = a_base + uint32_t(ks * 2) * p.chunk_bytes;
-            }
-            const uint64_t a_hi = make_smem_desc(a_addr, p.a_lbo, p.a_sbo, p.a_layout);
-            const uint64_t b_hi = make_smem_desc(b_base + uint32_t(ks) * 32u, 16, 1024, 2);
-            const uint32_t acc_flag = (kb | ks) != 0 ? 1u : 0u;
-            if (NSPLIT == 3) {
-              const uint64_t a_lo = make_smem_desc(a_addr + p.a_plane_bytes, p.a_lbo, p.a_sbo, p.a_layout);
-              const uint64_t b_lo = make_smem_desc(b_base + p.b_bytes + uint32_t(ks) * 32u, 16, 1024, 2);
-              umma_bf16(d_tmem, a_lo, b_hi, idesc, acc_flag);
-              umma_bf16(d_tmem, a_hi, b_lo, idesc, 1u);
-              umma_bf16(d_tmem, a_hi, b_hi, idesc, 1u);
-            } else {
-              umma_bf16(d_tmem, a_hi, b_hi, idesc, acc_flag);
-            }
+        wgmma_fence();
+        const int chunk0 = kb * p.cps;
+        const int nch = min(p.cps, p.n_chunks_padded - chunk0);
+        const int ksteps = (nch * p.CK) >> 4;
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
+        const uint32_t b_base = a_base + p.a_total_bytes;
+        for (int ks = 0; ks < ksteps; ++ks) {
+          uint32_t a_addr;
+          if (p.CK >= 16) {
+            const int k0 = ks * 16;
+            const int chunk = k0 / p.CK;
+            a_addr = a_base + uint32_t(chunk) * p.chunk_bytes + uint32_t(k0 - chunk * p.CK) * 2u;
+          } else {
+            a_addr = a_base + uint32_t(ks * 2) * p.chunk_bytes;
           }
-          umma_commit(&empty[stage]);                        // smem slot reusable once these MMAs retire
-          if (kb == p.k_blocks - 1) umma_commit(&tfull[acc]);  // accumulator complete
+          a_addr += a_row_off;
+          const uint64_t a_hi = make_smem_desc(a_addr, p.a_lbo, p.a_sbo, p.a_layout);
+          const uint64_t b_hi = make_smem_desc(b_base + uint32_t(ks) * 32u, 16, 1024, 2);
+          const uint32_t acc_flag = (kb | ks) != 0 ? 1u : 0u;
+          if (NSPLIT == 3) {
+            const uint64_t a_lo = make_smem_desc(a_addr + p.a_plane_bytes, p.a_lbo, p.a_sbo, p.a_layout);
+            const uint64_t b_lo = make_smem_desc(b_base + p.b_bytes + uint32_t(ks) * 32u, 16, 1024, 2);
+            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_lo, b_hi, acc_flag);
+            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_hi, b_lo, 1u);
+            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, 1u);
+          } else {
+            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, acc_flag);
+          }
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage can be refilled
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
+      wgmma_wait<0>();
+      mbar_arrive(&empty[held]);
+      mbar_wait(tempty, (it & 1) ^ 1);  // the epilogue has read the previous tile
+      acc_store<BN_MAX>(d, p.BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
+      mbar_arrive(tfull);
     }
   } else {
-    // ------------------------------------------------------------------ epilogue (8 warps: 2 per TMEM lane quarter)
-    // A warp may only read the 32 TMEM lanes of quarter warp % 4; the two warps of a quarter take the even / odd 16-column
-    // chunks of the tile.  (r2: with 4 epilogue warps the memory-bound layers issued one instruction per ~5.7 cycles and
-    // warp - TMEM load -> wait -> shared-memory transpose -> store chains on ONE warp per scheduler, profiles/r2_epilogue_notes.md.)
-    // Per chunk: TMEM -> registers -> [32 rows][16] shared-memory tile -> 8 rows x 64 bytes per store instruction (full
-    // 32-byte sectors; the per-row 16-byte stores of round 1 sent twice the bytes to L2), and the BatchNorm column sums come
-    // out of the same transposed reads.  accumulate = 2 adds with red.global.add (one add per element, no dependent load).
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    float* stg = reinterpret_cast<float*>(smem + p.off_staging) + (warp - 2) * EPI_STAGE_FLOATS;
-    long long* roff_s = reinterpret_cast<long long*>(stg + 32 * 20);
+    // ------------------------------------------------------------------ epilogue (8 warps: 2 per 32-row quarter)
+    // The two warps of a quarter take the even / odd 16-column chunks of the tile.  Per chunk: 8 rows x 64 bytes per store
+    // instruction (full 32-byte sectors) read straight from the accumulator tile, and the BatchNorm column sums come out
+    // of the same reads.  accumulate = 2 adds with red.global.add (one add per element, no dependent load).
+    const int ew = warp - EPI_WARP0;
+    const int q = ew & 3;
+    const int half = ew >> 2;
+    long long* roff_s = reinterpret_cast<long long*>(reinterpret_cast<float*>(smem + p.off_staging) + ew * EPI_STAGE_FLOATS);
     float* red = reinterpret_cast<float*>(smem + p.off_red);  // [2][4][BN][2]
     const int sub = lane >> 2, cq = lane & 3;   // row within a group of 8, 16-byte piece of the chunk's 64-byte row
     const int nchunks = p.BN >> 4;
+    const float* qtile = acc_tile + size_t(q) * 32 * p.acc_pitch;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
       const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
       const int ncol0 = nt * p.BN;
       const int row = mt * BLOCK_M + q * 32 + lane;
@@ -262,37 +258,16 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1) conv_igemm_kernel(cons
 #pragma unroll
       for (int k = 0; k < 4; ++k) ro[k] = roff_s[k * 8 + sub];
 
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(acc * p.BN);
-      if (half >= nchunks) {  // a 16-column tile: the second warp of the pair has nothing to read
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[acc]);
-      }
+      mbar_wait(tfull, it & 1);
       for (int ch = half; ch < nchunks; ch += 2) {
         const int c0 = ch * 16;
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(taddr + uint32_t(c0), v);
-        tmem_ld_wait();
-        if (ch + 2 >= nchunks) {  // this warp's last read of the accumulator: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[acc]);
-        }
-        float4* srow = reinterpret_cast<float4*>(stg + lane * 20);
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          srow[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                __uint_as_float(v[4 * j + 3]));
-        __syncwarp();
         const int limit = min(p.BN, p.Ntot - ncol0) - c0;      // valid columns of this chunk (a multiple of 4)
         const bool cvalid = cq * 4 < limit;
         float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const int r = k * 8 + sub;
-          const float4 y = *reinterpret_cast<const float4*>(stg + r * 20 + cq * 4);
+          const float4 y = *reinterpret_cast<const float4*>(qtile + size_t(r) * p.acc_pitch + c0 + cq * 4);
           s4[0] += y.x; s4[1] += y.y; s4[2] += y.z; s4[3] += y.w;
           q4[0] = fmaf(y.x, y.x, q4[0]); q4[1] = fmaf(y.y, y.y, q4[1]);
           q4[2] = fmaf(y.z, y.z, q4[2]); q4[3] = fmaf(y.w, y.w, q4[3]);
@@ -327,13 +302,14 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1) conv_igemm_kernel(cons
             }
           }
         }
-        __syncwarp();
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(tempty);  // this warp is done with the accumulator tile
       if (p.stats != nullptr) {
         named_bar_sync(1, 32 * EPI_WARPS);
         // the four quarter partials of this tile are in red[acc]; spread the column reduction over the epilogue warps
         const float* rb = red + size_t(acc) * 4 * p.BN * 2;
-        for (int cl = (warp - 2) * 32 + lane; cl < p.BN; cl += 32 * EPI_WARPS) {
+        for (int cl = ew * 32 + lane; cl < p.BN; cl += 32 * EPI_WARPS) {
           const int col = ncol0 + cl;
           if (col < p.Ntot) {
             float s = 0.f, s2 = 0.f;
@@ -351,12 +327,6 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, 1) conv_igemm_kernel(cons
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 static int g_num_sms = 0;
@@ -445,8 +415,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   p.k_blocks = (p.n_chunks_padded + p.cps - 1) / p.cps;
   p.Ntot = d->cout;
   const int n16 = (d->cout + 15) / 16 * 16;
-  const int bn_cap = (d->nsplit == 3) ? 128 : 256;
-  p.BN = std::min(n16, bn_cap);
+  p.BN = std::min(n16, BN_MAX);
   p.n_tiles = (d->cout + p.BN - 1) / p.BN;
   p.m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   p.chunk_bytes = BLOCK_M * p.CK * 2;
@@ -464,33 +433,19 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
     case 16: p.a_layout = 6; p.a_sbo = 256; p.a_lbo = 16; break;
     default: p.a_layout = 0; p.a_sbo = 128; p.a_lbo = p.chunk_bytes; break;
   }
-  uint32_t tc = 32;
-  while (tc < uint32_t(2 * p.BN)) tc <<= 1;
-  p.tmem_cols = tc;
-  const uint32_t tail = EPI_WARPS * EPI_STAGE_FLOATS * 4 + 2 * 4 * p.BN * 2 * 4 + 256;
+  p.acc_pitch = uint32_t(p.BN) + 4;  // 16-byte rows; the 4-float skew spreads the fragment stores over the banks
+  const uint32_t acc_bytes = BLOCK_M * p.acc_pitch * 4;
+  const uint32_t tail = acc_bytes + EPI_WARPS * EPI_STAGE_FLOATS * 4 + 2 * 4 * p.BN * 2 * 4 + 256;
   const uint32_t budget = uint32_t(g_smem_optin) - 1024 - tail;
   p.stages = std::min<int>(MAX_STAGES, budget / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.k_blocks * 4));
-  // Narrow-output / small-K layers (the fast pathway) have tiny tiles whose cost is barrier / TMA latency, not
-  // bandwidth: run 2..3 CTAs per SM (independent pipelines) when shared memory, TMEM (512 columns) and registers
-  // (3 x 192 threads x <= 96 registers) allow it, keeping at least 3 stages per CTA when possible.
-  const int total_tiles_ = p.m_tiles * p.n_tiles;
-  int ctas_per_sm = 1;
-  for (int want = 3; want >= 2; --want) {
-    if (p.tmem_cols * uint32_t(want) > 512u || total_tiles_ < want * g_num_sms) continue;
-    const uint32_t share = (uint32_t(g_smem_optin) + 1024) / uint32_t(want) - 2048;  // per-CTA share of the SM's smem
-    if (share < 1024 + tail + 2 * p.stage_bytes) continue;
-    const int st = int((share - 1024 - tail) / p.stage_bytes);
-    if (st < (want == 3 ? 3 : 2)) continue;
-    p.stages = std::min(p.stages, st);
-    ctas_per_sm = want;
-    break;
-  }
+  const int ctas_per_sm = 1;  // 544 threads x up to 120 registers: one CTA fills the register file
   if (p.stages < 2) {
     set_error("sfb_conv_igemm: not enough shared memory for 2 pipeline stages (stage=%u B)", p.stage_bytes);
     return -11;
   }
-  p.off_staging = p.stages * p.stage_bytes;
+  p.off_acc = p.stages * p.stage_bytes;
+  p.off_staging = p.off_acc + acc_bytes;
   p.off_red = p.off_staging + EPI_WARPS * EPI_STAGE_FLOATS * 4;
   p.off_bars = p.off_red + 2 * 4 * p.BN * 2 * 4;
   const uint32_t smem_bytes = p.off_bars + 256 + 1024;
@@ -545,7 +500,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
       cudaFuncSetAttribute(fns[a], cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
       attr[a] = true;
     }
-    fns[a]<<<grid, 64 + 32 * EPI_WARPS, smem_bytes, stream>>>(p);
+    fns[a]<<<grid, CONV_THREADS, smem_bytes, stream>>>(p);
   }
   e = cudaGetLastError();
   if (e != cudaSuccess) {

@@ -1,4 +1,4 @@
-// Stem convolutions (C_in = 3, stride 2 in W; stem_helper.py:182 ResNetBasicStem, :258 X3DStem) on tcgen05
+// Stem convolutions (C_in = 3, stride 2 in W; stem_helper.py:182 ResNetBasicStem, :258 X3DStem) on wgmma
 // WITHOUT im2col traffic: "W-shift" implicit GEMM.
 //
 // The clip is packed channels-last with the W axis folded by the stride: X'[n, t, h, w', 8] holds pixel pairs
@@ -30,6 +30,11 @@ constexpr int ST_SEG_STRIDE = 2304;   // 136 granules (128 pixels + halo) rounde
 constexpr int ST_SEG_PIX = 136;
 constexpr int ST_WSEG_STRIDE = 1152;  // wgrad: 72 granules (64 pixels + halo)
 constexpr int ST_WSEG_PIX = 72;
+constexpr int ST_MMA_WARPS = 8;   // fprop: two warpgroups of 64 pixels; wgrad: the first warpgroup only (64 co rows)
+constexpr int ST_FPROP_THREADS = 32 * (ST_MMA_WARPS + 1 + 4);
+constexpr int ST_WGRAD_THREADS = 32 * (4 + 1);
+constexpr int ST_BN_MAX = 128;
+constexpr int ST_NPG_MAX = 4;     // wgrad: pairs per CTA, each a <= 32-column accumulator
 
 __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* tm, uint64_t* bar, int32_t c0, int32_t c1,
                                             int32_t c2, int32_t c3, int32_t c4) {
@@ -57,7 +62,7 @@ struct StemParams {
   int cout, BN, w_tiles, m_tiles;
   int stages;
   uint32_t stage_bytes, a_plane_bytes, b_bytes;
-  uint32_t tmem_cols, off_staging, off_red, off_bars;
+  uint32_t acc_pitch, off_acc, off_staging, off_red, off_bars;
   float* out;
   float* stats;
   // wgrad only
@@ -67,40 +72,31 @@ struct StemParams {
 
 // ------------------------------------------------------------------------------------------------ fprop
 template <int NSPLIT>
-__global__ void __launch_bounds__(192, 1) stem_fprop_kernel(const __grid_constant__ StemParams p) {
+__global__ void __launch_bounds__(ST_FPROP_THREADS, 1) stem_fprop_kernel(const __grid_constant__ StemParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + ST_MAX_STAGES;
   uint64_t* tfull = empty + ST_MAX_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* tempty = tfull + 1;
+  float* acc_tile = reinterpret_cast<float*>(smem + p.off_acc);
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 32 * ST_MMA_WARPS);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], 4);
-    }
+    mbar_init(tfull, 32 * ST_MMA_WARPS);
+    mbar_init(tempty, 4);
     fence_mbar_init();
     fence_proxy_async_smem();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
   const int total_tiles = p.m_tiles;
   const int ksteps_per_pair = p.KW / 2;
 
-  if (warp == 0) {
+  if (warp == ST_MMA_WARPS) {
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -135,80 +131,78 @@ __global__ void __launch_bounds__(192, 1) stem_fprop_kernel(const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc_bf16(128, uint32_t(p.BN), 0, 0);
+  } else if (warp < ST_MMA_WARPS) {
+    // MMA warpgroup g: pixels 64g .. 64g+63 of the tile = 8 more 128-byte row groups into each segment
+    const int g = warp >> 2;
+    float d[ST_BN_MAX / 2];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + uint32_t(acc * p.BN);
+      int held = -1;
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const int nq = min(p.pps, p.pairs - kb * p.pps);
-          const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t b_base = a_base + NP * p.a_plane_bytes;
-          int kstep = 0;
-          for (int qq = 0; qq < nq; ++qq) {
-            for (int j = 0; j < ksteps_per_pair; ++j, ++kstep) {
-              // A: rows = pixels 16 B apart (8-row groups 128 B), the two K chunks are taps 2j and 2j+1 = +16 B
-              const uint32_t aa = a_base + qq * ST_SEG_STRIDE + uint32_t(2 * j) * 16u;
-              const uint64_t a_hi = make_smem_desc(aa, 16, 128, 0);
-              const uint64_t b_hi = make_smem_desc(b_base + uint32_t(kstep) * 32u, 16, 1024, 2);
-              const uint32_t acc_flag = (kb | kstep) != 0 ? 1u : 0u;
-              if (NSPLIT == 3) {
-                const uint64_t a_lo = make_smem_desc(aa + p.a_plane_bytes, 16, 128, 0);
-                const uint64_t b_lo = make_smem_desc(b_base + p.b_bytes + uint32_t(kstep) * 32u, 16, 1024, 2);
-                umma_bf16(d_tmem, a_lo, b_hi, idesc, acc_flag);
-                umma_bf16(d_tmem, a_hi, b_lo, idesc, 1u);
-                umma_bf16(d_tmem, a_hi, b_hi, idesc, 1u);
-              } else {
-                umma_bf16(d_tmem, a_hi, b_hi, idesc, acc_flag);
-              }
+        wgmma_fence();
+        const int nq = min(p.pps, p.pairs - kb * p.pps);
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 1024u;
+        const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + NP * p.a_plane_bytes;
+        int kstep = 0;
+        for (int qq = 0; qq < nq; ++qq) {
+          for (int j = 0; j < ksteps_per_pair; ++j, ++kstep) {
+            // A: rows = pixels 16 B apart (8-row groups 128 B), the two K chunks are taps 2j and 2j+1 = +16 B
+            const uint32_t aa = a_base + qq * ST_SEG_STRIDE + uint32_t(2 * j) * 16u;
+            const uint64_t a_hi = make_smem_desc(aa, 16, 128, 0);
+            const uint64_t b_hi = make_smem_desc(b_base + uint32_t(kstep) * 32u, 16, 1024, 2);
+            const uint32_t acc_flag = (kb | kstep) != 0 ? 1u : 0u;
+            if (NSPLIT == 3) {
+              const uint64_t a_lo = make_smem_desc(aa + p.a_plane_bytes, 16, 128, 0);
+              const uint64_t b_lo = make_smem_desc(b_base + p.b_bytes + uint32_t(kstep) * 32u, 16, 1024, 2);
+              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_lo, b_hi, acc_flag);
+              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_hi, b_lo, 1u);
+              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, 1u);
+            } else {
+              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, acc_flag);
             }
           }
-          umma_commit(&empty[stage]);
-          if (kb == p.k_blocks - 1) umma_commit(&tfull[acc]);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
+      wgmma_wait<0>();
+      mbar_arrive(&empty[held]);
+      mbar_wait(tempty, (it & 1) ^ 1);
+      acc_store<ST_BN_MAX>(d, p.BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
+      mbar_arrive(tfull);
     }
   } else {
-    const int q = warp & 3;
+    const int q = warp - (ST_MMA_WARPS + 1);
     float* stg = reinterpret_cast<float*>(smem + p.off_staging) + q * (32 * 33);
     float* red = reinterpret_cast<float*>(smem + p.off_red);
+    const float* arow = acc_tile + size_t(q * 32 + lane) * p.acc_pitch;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
       const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       const int wt = tile % p.w_tiles;
       const int rowi = tile / p.w_tiles;  // (n, ot, oh) flattened
       const int ow = wt * 128 + q * 32 + lane;
       const bool rvalid = ow < p.OW;
       const uint32_t rmask = __ballot_sync(0xffffffffu, rvalid);
       float* red_w = red + ((size_t(acc) * 4 + q) * p.BN) * 2;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(acc * p.BN);
+      mbar_wait(tfull, it & 1);
       for (int c0 = 0; c0 < p.BN; c0 += 32) {
         uint32_t v0[16], v1[16];
-        tmem_ld_32x32b_x16(taddr + uint32_t(c0), v0);
+        acc_ld_x16(arow + c0, v0);
         const bool second = (c0 + 16) < p.BN;
-        if (second) tmem_ld_32x32b_x16(taddr + uint32_t(c0 + 16), v1);
-        tmem_ld_wait();
-        if (c0 + 32 >= p.BN) {
-          tc_fence_before();
+        if (second) acc_ld_x16(arow + c0 + 16, v1);
+        if (c0 + 32 >= p.BN) {  // last read of the accumulator tile: hand it back to the MMA warpgroups
           __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[acc]);
+          if (lane == 0) mbar_arrive(tempty);
         }
         // transpose through shared memory: lane L then holds column c0+L of the warp's 32 pixels, so each store
         // instruction writes one contiguous 128-byte line (pixels of an output row are cout floats apart)
@@ -285,12 +279,6 @@ __global__ void __launch_bounds__(192, 1) stem_fprop_kernel(const __grid_constan
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ wgrad
@@ -300,14 +288,12 @@ __device__ __forceinline__ void st_red_add_v4(float* addr, float a, float b, flo
 }
 
 template <int NSPLIT>
-__global__ void __launch_bounds__(192, 1) stem_wgrad_kernel(const __grid_constant__ StemParams p) {
+__global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const __grid_constant__ StemParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + ST_MAX_STAGES;
-  uint64_t* tfull = empty + ST_MAX_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 1);
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
 
   const int split = blockIdx.x % p.splits;
@@ -321,24 +307,16 @@ __global__ void __launch_bounds__(192, 1) stem_wgrad_kernel(const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 128);
     }
-    mbar_init(tfull, 1);
     fence_mbar_init();
     fence_proxy_async_smem();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t dy_plane = 8192;  // one [64 pos][64 co] box; rows 64..127 of the MMA alias it (LBO = 0)
+  const uint32_t dy_plane = 8192;  // one [64 pos][64 co] box = the 64 rows of the MMA
 
   if (kb1 > kb0 && npairs > 0) {
-    if (warp == 0) {
+    if (warp == 4) {
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
@@ -371,22 +349,24 @@ __global__ void __launch_bounds__(192, 1) stem_wgrad_kernel(const __grid_constan
           phase ^= 1;
         }
       }
-    } else if (warp == 1) {
-      const uint32_t idesc = make_idesc_bf16(128, uint32_t(ncols_pair), 1, 1);
+    } else {
+      // one MMA warpgroup: accumulator of pair j = registers d[16 j ..] (ncols_pair <= 32 columns)
+      float d[ST_NPG_MAX * 16];
       int stage = 0;
       uint32_t phase = 0;
+      int held = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t x_base = a_base + NP * dy_plane;
-          for (int j = 0; j < npairs; ++j) {
-            const uint32_t d_tmem = tmem_base + uint32_t(j * ncols_pair);
+        wgmma_fence();
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
+        const uint32_t x_base = a_base + NP * dy_plane;
+#pragma unroll
+        for (int j = 0; j < ST_NPG_MAX; ++j) {
+          if (j < npairs) {
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks) {
-              // A' = dY (MN-major, 128B swizzle, co atoms aliased); B' = segment: tap atoms 16 B apart, positions
-              // 16 B apart, 8-position groups 128 B apart (no swizzle)
+              // A' = dY (MN-major, 128B swizzle); B' = segment: tap atoms 16 B apart, positions 16 B apart,
+              // 8-position groups 128 B apart (no swizzle)
               const uint64_t a_hi = make_smem_desc(a_base + ks * 2048, 0, 1024, 2);
               const uint64_t b_hi = make_smem_desc(x_base + j * ST_WSEG_STRIDE + ks * 256, 128, 16, 0);
               const uint32_t acc_flag = (kb != kb0 || ks != 0) ? 1u : 0u;
@@ -394,50 +374,48 @@ __global__ void __launch_bounds__(192, 1) stem_wgrad_kernel(const __grid_constan
                 const uint64_t a_lo = make_smem_desc(a_base + dy_plane + ks * 2048, 0, 1024, 2);
                 const uint64_t b_lo =
                     make_smem_desc(x_base + p.a_plane_bytes + j * ST_WSEG_STRIDE + ks * 256, 128, 16, 0);
-                umma_bf16(d_tmem, a_lo, b_hi, idesc, acc_flag);
-                umma_bf16(d_tmem, a_hi, b_lo, idesc, 1u);
-                umma_bf16(d_tmem, a_hi, b_hi, idesc, 1u);
+                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_lo, b_hi, acc_flag);
+                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_hi, b_lo, 1u);
+                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_hi, b_hi, 1u);
               } else {
-                umma_bf16(d_tmem, a_hi, b_hi, idesc, acc_flag);
+                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_hi, b_hi, acc_flag);
               }
             }
           }
-          umma_commit(&empty[stage]);
-          if (kb == kb1 - 1) umma_commit(tfull);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
-    } else {
-      const int q = warp & 3;
-      const int co = q * 32 + lane;
-      mbar_wait(tfull, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16);
-      const int ncols = npairs * ncols_pair;
+      wgmma_wait<0>();
+      // epilogue straight from the fragments: rows co = 16 w + lane/4 (+8), columns 8 c + 2 (lane % 4) (+1)
+      const int co0 = warp * 16 + (lane >> 2);
       const int col_base = pair_base * ncols_pair;
-      for (int c0 = 0; c0 < ncols; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(taddr + uint32_t(c0), v);
-        tmem_ld_wait();
-        if (co < p.cout && co < 64) {
-          float* dst = p.dw + size_t(co) * p.ktot + col_base + c0;
 #pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            st_red_add_v4(dst + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                          __uint_as_float(v[j + 3]));
+      for (int j = 0; j < ST_NPG_MAX; ++j) {
+        if (j < npairs) {
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            if (8 * c < ncols_pair) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int co = co0 + 8 * h;
+                if (co < p.cout) {
+                  float* dst = p.dw + size_t(co) * p.ktot + col_base + j * ncols_pair + 8 * c + 2 * (lane & 3);
+                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[16 * j + 4 * c + 2 * h]),
+                               "f"(d[16 * j + 4 * c + 2 * h + 1]) : "memory");
+                }
+              }
+            }
+          }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
@@ -644,6 +622,10 @@ extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
   p.pps = 64 / (d->kwf * 8);
   p.k_blocks = (p.pairs + p.pps - 1) / p.pps;
   p.BN = (d->cout + 15) / 16 * 16;
+  if (p.BN > ST_BN_MAX) {
+    set_error("sfb_stem_fprop: cout=%d > %d not supported", d->cout, ST_BN_MAX);
+    return -10;
+  }
   p.w_tiles = (d->out_w + 127) / 128;
   p.m_tiles = int(sfb_stem_m_tiles(d));
   p.a_plane_bytes = p.pps * ST_SEG_STRIDE;
@@ -652,13 +634,13 @@ extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
   // B must start 1024-aligned inside the stage for the 128B swizzle
   p.a_plane_bytes = (p.a_plane_bytes + 1023) / 1024 * 1024;
   p.stage_bytes = (p.a_plane_bytes + p.b_bytes) * np;
-  uint32_t tc = 32;
-  while (tc < uint32_t(2 * p.BN)) tc <<= 1;
-  p.tmem_cols = tc;
-  const uint32_t tail = 4 * 32 * 33 * 4 + 2 * 4 * p.BN * 2 * 4 + 256;
+  p.acc_pitch = uint32_t(p.BN) + 4;
+  const uint32_t acc_bytes = 128u * p.acc_pitch * 4u;
+  const uint32_t tail = acc_bytes + 4 * 32 * 33 * 4 + 2 * 4 * p.BN * 2 * 4 + 256;
   p.stages = std::min<int>(ST_MAX_STAGES, (uint32_t(st_smem) - 1024 - tail) / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.k_blocks * 2));
-  p.off_staging = p.stages * p.stage_bytes;
+  p.off_acc = p.stages * p.stage_bytes;
+  p.off_staging = p.off_acc + acc_bytes;
   p.off_red = p.off_staging + 4 * 32 * 33 * 4;
   p.off_bars = p.off_red + 2 * 4 * p.BN * 2 * 4;
   const uint32_t smem_bytes = p.off_bars + 256 + 1024;
@@ -674,11 +656,11 @@ extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
   if (d->nsplit == 3) {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem_fprop_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_fprop_kernel<3><<<grid, 192, smem_bytes, stream>>>(p);
+    stem_fprop_kernel<3><<<grid, ST_FPROP_THREADS, smem_bytes, stream>>>(p);
   } else {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem_fprop_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_fprop_kernel<1><<<grid, 192, smem_bytes, stream>>>(p);
+    stem_fprop_kernel<1><<<grid, ST_FPROP_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -701,8 +683,11 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
   if (rc) return rc;
   const int np = d->nsplit == 3 ? 2 : 1;
   const int ncols_pair = d->kwf * 8;
-  const int col_cap = d->nsplit == 3 ? 128 : 256;
-  p.npg = std::min(p.pairs, col_cap / ncols_pair);
+  if (ncols_pair > 32) {
+    set_error("sfb_stem_wgrad: %d folded W taps > 4 not supported", d->kwf);
+    return -10;
+  }
+  p.npg = std::min(p.pairs, ST_NPG_MAX);
   p.n_groups = (p.pairs + p.npg - 1) / p.npg;
   p.w_chunks = (d->out_w + 63) / 64;
   p.kb_total = d->n * d->out_t * d->out_h * p.w_chunks;
@@ -713,9 +698,6 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
   p.a_plane_bytes = (p.npg * ST_WSEG_STRIDE + 127) / 128 * 128;
   p.stage_bytes = ((8192 + p.a_plane_bytes) * np + 1023) / 1024 * 1024;
   // keep the X planes contiguous after the dY planes: offsets used by the kernel are NP*8192 + pl*a_plane_bytes
-  uint32_t tc = 32;
-  while (tc < uint32_t(p.npg * ncols_pair)) tc <<= 1;
-  p.tmem_cols = tc;
   p.stages = std::min<int>(ST_MAX_STAGES, (uint32_t(st_smem) - 1024 - 256) / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.kb_per_split));
   p.off_bars = p.stages * p.stage_bytes;
@@ -732,11 +714,11 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
   if (d->nsplit == 3) {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_wgrad_kernel<3><<<grid, 192, smem_bytes, stream>>>(p);
+    stem_wgrad_kernel<3><<<grid, ST_WGRAD_THREADS, smem_bytes, stream>>>(p);
   } else {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_wgrad_kernel<1><<<grid, 192, smem_bytes, stream>>>(p);
+    stem_wgrad_kernel<1><<<grid, ST_WGRAD_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

@@ -1,5 +1,5 @@
 // The fast pathway's stem (stem_helper.py:182 ResNetBasicStem with dim_out = 8: Conv3d 3 -> 8, [kt,7,7], stride (1,2,2),
-// pad (kt/2,3,3)) as a "Toeplitz" implicit GEMM on tcgen05.
+// pad (kt/2,3,3)) as a "Toeplitz" implicit GEMM on wgmma.
 //
 // Why: with 8 output channels the W-shift kernels of conv_stem.cu issue 128 x 16 x 16 MMAs whose cost is the 4 KB
 // shared-memory read of the A tile, not the math (measured 1.87 ms fprop, 2.1 ms wgrad per SlowFast step = 11 % of it).
@@ -23,7 +23,7 @@
 // feeds 7 x 6 MMAs (x3 split products).
 //
 // wgrad runs the same operands with the reduction over the row index: dZ[(kt sel, j, co), g*8+s] for the 4 (or 3) H taps
-// of one parity class in TMEM (2 x 64 rows: two T taps share one pass over the clip), then
+// of one parity class in registers (2 x 64 rows: two T taps share one pass over the clip), then
 // dWf[co][kt][kh][kw'][s] = sum_j dZ[(j,co), (j + kw')*8 + s] is folded into the W-shift gradient matrix by atomics.
 #include <algorithm>
 #include <cstdint>
@@ -39,6 +39,8 @@ namespace sfb {
 constexpr int T8_ROWS = 8;     // output rows per tile
 constexpr int T8_SLOTS = 11;   // resident input rows per parity class: 8 + 3
 constexpr int T8_KSTEPS = 6;   // 12 granules of 8 slots = 96 K elements per (kt, kh)
+constexpr int T8_FPROP_THREADS = 32 * (8 + 1);    // two MMA warpgroups (rows 0..63 / 64..127) + producer warp
+constexpr int T8_WGRAD_THREADS = 32 * (16 + 1);   // four MMA warpgroups (row half x tap pair) + producer warp
 
 __device__ __forceinline__ void t8_tma_5d(void* smem, const CUtensorMap* tm, uint64_t* bar, int32_t c0, int32_t c1,
                                           int32_t c2, int32_t c3, int32_t c4) {
@@ -69,36 +71,24 @@ struct Stem8Params {
 
 // ------------------------------------------------------------------------------------------------ fprop
 template <int NSPLIT>
-__global__ void __launch_bounds__(192, 1) stem8_fprop_kernel(const __grid_constant__ Stem8Params p) {
+__global__ void __launch_bounds__(T8_FPROP_THREADS, 1) stem8_fprop_kernel(const __grid_constant__ Stem8Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + 2;
-  uint64_t* tfull = empty + 2;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
   if (threadIdx.x == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 4);
+      mbar_init(&empty[s], 256);
     }
     fence_mbar_init();
     fence_proxy_async_smem();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
@@ -131,134 +121,106 @@ __global__ void __launch_bounds__(192, 1) stem8_fprop_kernel(const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc_bf16(128, 64, 0, 0);
+  } else {
+    // MMA warpgroup g: GEMM rows 64g .. 64g+63 (8 more 128-byte row groups into each array); its warps then store
+    // straight from the fragments: thread = rows 16w + lane/4 (+8), columns 8c + 2(lane%4) (+1) = pixel 7-c, channels
+    const int g = warp >> 2;
+    float* red = reinterpret_cast<float*>(smem + p.off_red);   // [2][8 warps][16]
+    float d[32];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int ot = (tile / p.bands) % p.OT;
+      const int band = tile % p.bands;
+      const int rowg = tile / p.bands;            // (n, ot) flattened
+      const int ot = rowg % p.OT;
       const int kt_lo = max(0, p.pt - ot), kt_hi = min(p.KT, p.T + p.pt - ot);
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + uint32_t(acc * 64);
+      int held = -1;
       for (int kt = kt_lo; kt < kt_hi; ++kt) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t b_base = a_base + p.a_bytes;
-          for (int kh = 0; kh < 7; ++kh) {
-            const int cls = (kh & 1) ^ 1;             // kh even -> odd input rows (class 1)
-            const int so = cls ? (kh >> 1) : ((kh - 1) >> 1);   // slot of output row 0's tap
+        wgmma_fence();
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 1024u;
+        const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + p.a_bytes;
+        for (int kh = 0; kh < 7; ++kh) {
+          const int cls = (kh & 1) ^ 1;             // kh even -> odd input rows (class 1)
+          const int so = cls ? (kh >> 1) : ((kh - 1) >> 1);   // slot of output row 0's tap
 #pragma unroll
-            for (int i = 0; i < T8_KSTEPS; ++i) {
-              const int arr = i < 4 ? 2 * i : 2 * i - 8;
-              const int shift = i < 4 ? 0 : 1;
-              const uint32_t aa = a_base + uint32_t(cls * 8 + arr) * p.ab + uint32_t(so * p.MR + shift) * 16u;
-              const uint32_t bb = b_base + uint32_t(kh * 12 + 1 + 2 * i) * 128u;
-              const uint64_t a_hi = make_smem_desc(aa, p.ab, 128, 0);
-              const uint64_t b_hi = make_smem_desc(bb, 128, 128, 0);
-              const uint32_t acc_flag = (kt != kt_lo || kh != 0 || i != 0) ? 1u : 0u;
-              if (NSPLIT == 3) {
-                const uint64_t a_lo = make_smem_desc(aa + p.a_plane, p.ab, 128, 0);
-                const uint64_t b_lo = make_smem_desc(bb + p.b_plane, 128, 128, 0);
-                umma_bf16(d_tmem, a_lo, b_hi, idesc, acc_flag);
-                umma_bf16(d_tmem, a_hi, b_lo, idesc, 1u);
-                umma_bf16(d_tmem, a_hi, b_hi, idesc, 1u);
-              } else {
-                umma_bf16(d_tmem, a_hi, b_hi, idesc, acc_flag);
-              }
+          for (int i = 0; i < T8_KSTEPS; ++i) {
+            const int arr = i < 4 ? 2 * i : 2 * i - 8;
+            const int shift = i < 4 ? 0 : 1;
+            const uint32_t aa = a_base + uint32_t(cls * 8 + arr) * p.ab + uint32_t(so * p.MR + shift) * 16u;
+            const uint32_t bb = b_base + uint32_t(kh * 12 + 1 + 2 * i) * 128u;
+            const uint64_t a_hi = make_smem_desc(aa, p.ab, 128, 0);
+            const uint64_t b_hi = make_smem_desc(bb, 128, 128, 0);
+            const uint32_t acc_flag = (kt != kt_lo || kh != 0 || i != 0) ? 1u : 0u;
+            if (NSPLIT == 3) {
+              const uint64_t a_lo = make_smem_desc(aa + p.a_plane, p.ab, 128, 0);
+              const uint64_t b_lo = make_smem_desc(bb + p.b_plane, 128, 128, 0);
+              wgmma_m64n64<0, 0>(d, a_lo, b_hi, acc_flag);
+              wgmma_m64n64<0, 0>(d, a_hi, b_lo, 1u);
+              wgmma_m64n64<0, 0>(d, a_hi, b_hi, 1u);
+            } else {
+              wgmma_m64n64<0, 0>(d, a_hi, b_hi, acc_flag);
             }
           }
-          umma_commit(&empty[stage]);
-          if (kt == kt_hi - 1) umma_commit(&tfull[acc]);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == 2) {
           stage = 0;
           phase ^= 1;
         }
       }
-    }
-  } else {
-    const int q = warp & 3;
-    float* red = reinterpret_cast<float*>(smem + p.off_red);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int band = tile % p.bands;
-      const int rowg = tile / p.bands;            // (n, ot) flattened
-      const int rr = q * 32 + lane;
-      const int ohl = rr / p.MR, m = rr - ohl * p.MR;
-      const bool valid = ohl < T8_ROWS && m < p.MR - 1;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(acc * 64);
-      uint32_t v[4][16];
+      wgmma_wait<0>();
+      if (held >= 0) mbar_arrive(&empty[held]);
+      const int cp = 2 * (lane & 3);   // channel pair of this thread
+      float s[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
 #pragma unroll
-      for (int c = 0; c < 4; ++c) tmem_ld_32x32b_x16(taddr + uint32_t(c * 16), v[c]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      float s[8], s2[8];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) s[c] = s2[c] = 0.f;
-      if (valid) {
-        float* dst = p.out + ((static_cast<long long>(rowg) * p.OH + band * T8_ROWS + ohl) * p.OW + 8 * m) * 8;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          // column (7 - j)*8 + co holds pixel 8m + j, channel co
-          const int cb = (7 - j) * 8;
-          float y[8];
+      for (int h = 0; h < 2; ++h) {
+        const int rr = g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        const int ohl = rr / p.MR, m = rr - ohl * p.MR;
+        if (ohl < T8_ROWS && m < p.MR - 1) {
+          float* dst = p.out + ((static_cast<long long>(rowg) * p.OH + band * T8_ROWS + ohl) * p.OW + 8 * m) * 8 + cp;
 #pragma unroll
           for (int c = 0; c < 8; ++c) {
-            y[c] = __uint_as_float(v[(cb + c) >> 4][(cb + c) & 15]);
-            s[c] += y[c];
-            s2[c] = fmaf(y[c], y[c], s2[c]);
+            // column c*8 + co holds pixel 8m + 7 - c, channel co
+            const float y0 = d[4 * c + 2 * h], y1 = d[4 * c + 2 * h + 1];
+            *reinterpret_cast<float2*>(dst + (7 - c) * 8) = make_float2(y0, y1);
+            s[0] += y0; s[1] += y1;
+            s2[0] = fmaf(y0, y0, s2[0]); s2[1] = fmaf(y1, y1, s2[1]);
           }
-          *reinterpret_cast<float4*>(dst + j * 8) = make_float4(y[0], y[1], y[2], y[3]);
-          *reinterpret_cast<float4*>(dst + j * 8 + 4) = make_float4(y[4], y[5], y[6], y[7]);
         }
       }
       if (p.stats != nullptr) {
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
+        for (int c = 0; c < 2; ++c) {
 #pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
+          for (int o = 4; o <= 16; o <<= 1) {
             s[c] += __shfl_xor_sync(0xffffffffu, s[c], o);
             s2[c] += __shfl_xor_sync(0xffffffffu, s2[c], o);
           }
         }
-        float* rw = red + (acc * 4 + q) * 16;
-        if (lane == 0) {
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            rw[c] = s[c];
-            rw[8 + c] = s2[c];
-          }
+        float* rw = red + ((it & 1) * 8 + warp) * 16;
+        if (lane < 4) {
+          rw[cp] = s[0]; rw[cp + 1] = s[1];
+          rw[8 + cp] = s2[0]; rw[8 + cp + 1] = s2[1];
         }
-        named_bar_sync(1, 128);
-        if (q == 0 && lane < 16) {
-          const float* rb = red + acc * 4 * 16;
-          const float tot = rb[lane] + rb[16 + lane] + rb[32 + lane] + rb[48 + lane];
+        named_bar_sync(1, 256);
+        if (warp == 0 && lane < 16) {
+          const float* rb = red + (it & 1) * 8 * 16;
+          float tot = 0.f;
+#pragma unroll
+          for (int w = 0; w < 8; ++w) tot += rb[w * 16 + lane];
           // lane < 8: sum of channel lane; lane >= 8: sum of squares of channel lane - 8   (stats = [2][cout][m_tiles])
           p.stats[size_t(lane) * p.m_tiles + tile] = tot;
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
-  }
 }
+
 
 // ------------------------------------------------------------------------------------------------ wgrad
 __device__ __forceinline__ void t8_red_add_v4(float* addr, float a, float b, float c, float d) {
@@ -269,14 +231,12 @@ __device__ __forceinline__ void t8_red_add_v4(float* addr, float a, float b, flo
 // CTA = (parity class, group of two T taps, split of the (n, input frame, band) steps).  Stage = the class's 8 arrays of
 // the input band + the dY row groups of the two output frames the taps pair this input frame with.
 template <int NSPLIT>
-__global__ void __launch_bounds__(192, 1) stem8_wgrad_kernel(const __grid_constant__ Stem8Params p) {
+__global__ void __launch_bounds__(T8_WGRAD_THREADS, 1) stem8_wgrad_kernel(const __grid_constant__ Stem8Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + 2;
-  uint64_t* tfull = empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 1);
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
   constexpr uint32_t DY_TILE = 16384;   // 128 rows x 128 bytes (120 written by the TMA, the rest stay zero)
 
@@ -310,24 +270,16 @@ __global__ void __launch_bounds__(192, 1) stem8_wgrad_kernel(const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 512);
     }
-    mbar_init(tfull, 1);
     fence_mbar_init();
   }
   fence_proxy_async_smem();
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t x_bytes = NP * 8u * p.ab;       // class arrays, both planes
 
   if (s1 > s0) {
-    if (warp == 0) {
+    if (warp == 16) {
       int stage = 0;
       uint32_t phase = 0;
       for (int step = s0; step < s1; ++step) {
@@ -356,21 +308,24 @@ __global__ void __launch_bounds__(192, 1) stem8_wgrad_kernel(const __grid_consta
           phase ^= 1;
         }
       }
-    } else if (warp == 1) {
-      const uint32_t idesc64 = make_idesc_bf16(128, 64, 1, 1);
-      const uint32_t idesc32 = make_idesc_bf16(128, 32, 1, 1);
+    } else {
+      // MMA warpgroup (g, th): 64-row half g (T tap kta / ktb) and H taps tq = 2 th, 2 th + 1; per tap a 64-column
+      // accumulator (granules 0..7, B0) and a 32-column one (granules 8..11, B1)
+      const int wg = warp >> 2, g = wg & 1, th = wg >> 1;
+      float d0[2][32], d1[2][16];
       int stage = 0;
       uint32_t phase = 0;
+      int held = -1;
       for (int step = s0; step < s1; ++step) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t x_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t dy_base = x_base + x_bytes;
-          const uint32_t lbo_a = has_b ? DY_TILE : 0u;       // second 64-row atom = the other T tap's dY (or an alias)
-          for (int tq = 0; tq < ntaps; ++tq) {
-            // class 1: kh = 2 tq, slot offset tq; class 0: kh = 2 tq + 1, slot offset tq
-            const uint32_t d_tmem = tmem_base + uint32_t(tq * 96);
+        wgmma_fence();
+        const uint32_t x_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
+        const uint32_t lbo_a = has_b ? DY_TILE : 0u;       // second 64-row atom = the other T tap's dY (or an alias)
+        const uint32_t dy_base = x_base + x_bytes + uint32_t(g) * lbo_a;
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int tq = 2 * th + u;   // class 1: kh = 2 tq, slot offset tq; class 0: kh = 2 tq + 1, slot offset tq
+          if (tq < ntaps) {
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks) {
               const uint32_t xa = x_base + uint32_t(tq * p.MR) * 16u + uint32_t(ks) * 256u;
@@ -382,53 +337,51 @@ __global__ void __launch_bounds__(192, 1) stem8_wgrad_kernel(const __grid_consta
                 const uint64_t a_lo = make_smem_desc(dy_base + 2 * DY_TILE + ks * 2048, lbo_a, 1024, 2);
                 const uint64_t b0_lo = make_smem_desc(xa + 8u * p.ab, 128, p.ab, 0);
                 const uint64_t b1_lo = make_smem_desc(xa + 8u * p.ab + 16u, 128, p.ab, 0);
-                umma_bf16(d_tmem, a_lo, b0_hi, idesc64, acc_flag);
-                umma_bf16(d_tmem, a_hi, b0_lo, idesc64, 1u);
-                umma_bf16(d_tmem, a_hi, b0_hi, idesc64, 1u);
-                umma_bf16(d_tmem + 64, a_lo, b1_hi, idesc32, acc_flag);
-                umma_bf16(d_tmem + 64, a_hi, b1_lo, idesc32, 1u);
-                umma_bf16(d_tmem + 64, a_hi, b1_hi, idesc32, 1u);
+                wgmma_m64n64<1, 1>(d0[u], a_lo, b0_hi, acc_flag);
+                wgmma_m64n64<1, 1>(d0[u], a_hi, b0_lo, 1u);
+                wgmma_m64n64<1, 1>(d0[u], a_hi, b0_hi, 1u);
+                wgmma_m64n32<1, 1>(d1[u], a_lo, b1_hi, acc_flag);
+                wgmma_m64n32<1, 1>(d1[u], a_hi, b1_lo, 1u);
+                wgmma_m64n32<1, 1>(d1[u], a_hi, b1_hi, 1u);
               } else {
-                umma_bf16(d_tmem, a_hi, b0_hi, idesc64, acc_flag);
-                umma_bf16(d_tmem + 64, a_hi, b1_hi, idesc32, acc_flag);
+                wgmma_m64n64<1, 1>(d0[u], a_hi, b0_hi, acc_flag);
+                wgmma_m64n32<1, 1>(d1[u], a_hi, b1_hi, acc_flag);
               }
             }
           }
-          umma_commit(&empty[stage]);
-          if (step == s1 - 1) umma_commit(tfull);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == 2) {
           stage = 0;
           phase ^= 1;
         }
       }
-    } else {
-      const int q = warp & 3;
-      const int mu = (q & 1) * 32 + lane;         // row within the 64-row half: (j, co)
-      const int j = mu >> 3, co = mu & 7;
-      const int kt = (q >> 1) ? ktb : kta;
-      mbar_wait(tfull, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16);
-      const bool live = kt < p.KT;
-      for (int tq = 0; tq < ntaps; ++tq) {
-        const int kh = cls ? 2 * tq : 2 * tq + 1;
-        float* dst = p.dwm + size_t(co) * p.kfold + size_t((kt * 7 + kh) * 4) * 8;
+      wgmma_wait<0>();
+      // fragments -> dWf: row mu = (j, co), column granule gi = kw' + j, slots 2 (lane % 4) (+1)
+      const int kt = g ? ktb : kta;
+      if (kt < p.KT) {
+        const int sl = 2 * (lane & 3);
 #pragma unroll
-        for (int c0 = 0; c0 < 96; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(taddr + uint32_t(tq * 96 + c0), v);
-          tmem_ld_wait();
-          if (live) {
+        for (int u = 0; u < 2; ++u) {
+          const int tq = 2 * th + u;
+          if (tq < ntaps) {
+            const int kh = cls ? 2 * tq : 2 * tq + 1;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const int kwp = (c0 >> 3) + h - j;   // folded W tap this granule is for pixel j of the group
-              if (kwp >= 0 && kwp < 4) {
-                t8_red_add_v4(dst + kwp * 8, __uint_as_float(v[h * 8 + 0]), __uint_as_float(v[h * 8 + 1]),
-                              __uint_as_float(v[h * 8 + 2]), __uint_as_float(v[h * 8 + 3]));
-                t8_red_add_v4(dst + kwp * 8 + 4, __uint_as_float(v[h * 8 + 4]), __uint_as_float(v[h * 8 + 5]),
-                              __uint_as_float(v[h * 8 + 6]), __uint_as_float(v[h * 8 + 7]));
+              const int mu = (warp & 3) * 16 + (lane >> 2) + 8 * h;
+              const int j = mu >> 3, co = mu & 7;
+              float* dst = p.dwm + size_t(co) * p.kfold + size_t((kt * 7 + kh) * 4) * 8 + sl;
+#pragma unroll
+              for (int gi = 0; gi < 12; ++gi) {
+                const int kwp = gi - j;   // folded W tap this granule is for pixel j of the group
+                if (kwp >= 0 && kwp < 4) {
+                  const float y0 = gi < 8 ? d0[u][4 * gi + 2 * h] : d1[u][4 * (gi - 8) + 2 * h];
+                  const float y1 = gi < 8 ? d0[u][4 * gi + 2 * h + 1] : d1[u][4 * (gi - 8) + 2 * h + 1];
+                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + kwp * 8), "f"(y0), "f"(y1) : "memory");
+                }
               }
             }
           }
@@ -436,13 +389,8 @@ __global__ void __launch_bounds__(192, 1) stem8_wgrad_kernel(const __grid_consta
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
+
 
 // ------------------------------------------------------------------------------------------------ packing
 // NCTHW fp32 clip -> X''[n][2t + (h&1)][h/2][j][m][8] split planes: granule (j, m) = pixel pair' 8m + j (pair' = pair + 2),
@@ -638,7 +586,7 @@ extern "C" int sfb_stem8_fprop(const sfb_stem_desc* d, void* stream_) {
   p.b_plane = p.zg * 128u;
   p.stage_bytes = (p.a_bytes + np * p.b_plane + 1023u) / 1024u * 1024u;
   p.off_red = 2 * p.stage_bytes;
-  p.off_bars = p.off_red + 2 * 4 * 16 * 4;
+  p.off_bars = p.off_red + 2 * 8 * 16 * 4;
   const uint32_t smem_bytes = p.off_bars + 128 + 1024;
   if (smem_bytes > uint32_t(t8_smem)) {
     set_error("sfb_stem8_fprop: %u bytes of shared memory needed, %d available", smem_bytes, t8_smem);
@@ -656,11 +604,11 @@ extern "C" int sfb_stem8_fprop(const sfb_stem_desc* d, void* stream_) {
   if (d->nsplit == 3) {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem8_fprop_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }
-    stem8_fprop_kernel<3><<<grid, 192, smem_bytes, stream>>>(p);
+    stem8_fprop_kernel<3><<<grid, T8_FPROP_THREADS, smem_bytes, stream>>>(p);
   } else {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem8_fprop_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }
-    stem8_fprop_kernel<1><<<grid, 192, smem_bytes, stream>>>(p);
+    stem8_fprop_kernel<1><<<grid, T8_FPROP_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -714,11 +662,11 @@ extern "C" int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream_) {
   if (d->nsplit == 3) {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem8_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }
-    stem8_wgrad_kernel<3><<<grid, 192, smem_bytes, stream>>>(p);
+    stem8_wgrad_kernel<3><<<grid, T8_WGRAD_THREADS, smem_bytes, stream>>>(p);
   } else {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem8_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }
-    stem8_wgrad_kernel<1><<<grid, 192, smem_bytes, stream>>>(p);
+    stem8_wgrad_kernel<1><<<grid, T8_WGRAD_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

@@ -1,10 +1,10 @@
-// Convolution weight gradient (wgrad) as an implicit GEMM on tcgen05:
+// Convolution weight gradient (wgrad) as an implicit GEMM on wgmma:
 //
 //   dW[co, (tap, ci)] = sum_m dY[m, co] * X_im2col[m, (tap, ci)]        m over n*ot*oh*ow output positions
 //
 // GEMM view: D[M' = co (128 rows), N' = (tap, ci) columns] with the reduction over output positions.  Both
 // operands are "MN-major" for the tensor core (the reduction index is the slow axis of the tiles as they sit in
-// memory), which tcgen05 reads natively through MN-major shared-memory descriptors:
+// memory), which wgmma reads natively through MN-major shared-memory descriptors:
 //   * A' = dY tile  : tiled TMA box [64 positions][64 co]  (two boxes for the 128 co rows)
 //   * B' = X tile   : one TMA im2col load per (tap, channel chunk): [64 positions][CK channels]; consecutive
 //                     chunks form the N' extent of the MMA, so one dY tile is reused by up to 256 dW columns.
@@ -23,6 +23,9 @@ namespace sfb {
 
 constexpr int WG_BLOCK_K = 64;  // output positions per pipeline stage
 constexpr int WG_MAX_STAGES = 8;
+constexpr int WG_MMA_WARPS = 8;   // two warpgroups: co rows 0..63 / 64..127 of the tile
+constexpr int WG_THREADS = 32 * (WG_MMA_WARPS + 1);
+constexpr int WG_BN_MAX = 128;
 
 struct WgradParams {
   CUtensorMap tmX[2];
@@ -41,8 +44,8 @@ struct WgradParams {
   int stages;
   uint32_t stage_bytes, x_chunk_bytes, x_plane_bytes, dy_plane_bytes;
   uint32_t b_layout, b_lbo, b_sbo, b_kstep_bytes;
-  uint32_t tmem_cols;
-  uint32_t off_bars;
+  uint32_t acc_pitch;
+  uint32_t off_acc, off_bars;
   float* dw_out;
 };
 
@@ -52,7 +55,7 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
 }
 
 template <int NSPLIT>
-__global__ void __launch_bounds__(192, 1) conv_wgrad_kernel(const __grid_constant__ WgradParams p) {
+__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_constant__ WgradParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5;
@@ -60,8 +63,7 @@ __global__ void __launch_bounds__(192, 1) conv_wgrad_kernel(const __grid_constan
 
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + WG_MAX_STAGES;
-  uint64_t* tfull = empty + WG_MAX_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 1);
+  float* acc_tile = reinterpret_cast<float*>(smem + p.off_acc);
 
   const int split = blockIdx.x % p.splits;
   const int tile = blockIdx.x / p.splits;
@@ -74,25 +76,17 @@ __global__ void __launch_bounds__(192, 1) conv_wgrad_kernel(const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 32 * WG_MMA_WARPS);
     }
-    mbar_init(tfull, 1);
     fence_mbar_init();
     fence_proxy_async_smem();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int chunk_base = n_tile * p.NG;  // first (tap, channel-chunk) of this N' tile
 
   if (nkb > 0) {
-    if (warp == 0) {
+    if (warp == WG_MMA_WARPS) {
       // ---------------------------------------------------------------- TMA producer
       int stage = 0;
       uint32_t phase = 0;
@@ -155,55 +149,55 @@ __global__ void __launch_bounds__(192, 1) conv_wgrad_kernel(const __grid_constan
           phase ^= 1;
         }
       }
-    } else if (warp == 1) {
-      // ---------------------------------------------------------------- MMA issuer
-      const uint32_t idesc = make_idesc_bf16(128, uint32_t(p.BN), 1, 1);
+    } else {
+      // ---------------------------------------------------------------- MMA warpgroups, then the epilogue
+      const int g = warp >> 2;
+      float d[WG_BN_MAX / 2];
       int stage = 0;
       uint32_t phase = 0;
+      int held = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t b_base = a_base + p.dy_plane_bytes * (NSPLIT == 3 ? 2 : 1);
+        wgmma_fence();
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 8192u;
+        const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + p.dy_plane_bytes * (NSPLIT == 3 ? 2 : 1);
 #pragma unroll
-          for (int ks = 0; ks < WG_BLOCK_K / 16; ++ks) {
-            // A' (dY): MN-major, 128B swizzle; co atoms 8192 B apart, 8-position groups 1024 B apart
-            const uint64_t a_hi = make_smem_desc(a_base + ks * 2048, 8192, 1024, 2);
-            const uint64_t b_hi = make_smem_desc(b_base + ks * p.b_kstep_bytes, p.b_lbo, p.b_sbo, p.b_layout);
-            const uint32_t acc_flag = (kb != kb0 || ks != 0) ? 1u : 0u;
-            if (NSPLIT == 3) {
-              const uint64_t a_lo = make_smem_desc(a_base + p.dy_plane_bytes + ks * 2048, 8192, 1024, 2);
-              const uint64_t b_lo =
-                  make_smem_desc(b_base + p.x_plane_bytes + ks * p.b_kstep_bytes, p.b_lbo, p.b_sbo, p.b_layout);
-              umma_bf16(tmem_base, a_lo, b_hi, idesc, acc_flag);
-              umma_bf16(tmem_base, a_hi, b_lo, idesc, 1u);
-              umma_bf16(tmem_base, a_hi, b_hi, idesc, 1u);
-            } else {
-              umma_bf16(tmem_base, a_hi, b_hi, idesc, acc_flag);
-            }
+        for (int ks = 0; ks < WG_BLOCK_K / 16; ++ks) {
+          // A' (dY): MN-major, 128B swizzle; co atoms 8192 B apart, 8-position groups 1024 B apart
+          const uint64_t a_hi = make_smem_desc(a_base + ks * 2048, 8192, 1024, 2);
+          const uint64_t b_hi = make_smem_desc(b_base + ks * p.b_kstep_bytes, p.b_lbo, p.b_sbo, p.b_layout);
+          const uint32_t acc_flag = (kb != kb0 || ks != 0) ? 1u : 0u;
+          if (NSPLIT == 3) {
+            const uint64_t a_lo = make_smem_desc(a_base + p.dy_plane_bytes + ks * 2048, 8192, 1024, 2);
+            const uint64_t b_lo =
+                make_smem_desc(b_base + p.x_plane_bytes + ks * p.b_kstep_bytes, p.b_lbo, p.b_sbo, p.b_layout);
+            wgmma_bf16<WG_BN_MAX, 1, 1>(d, p.BN, a_lo, b_hi, acc_flag);
+            wgmma_bf16<WG_BN_MAX, 1, 1>(d, p.BN, a_hi, b_lo, 1u);
+            wgmma_bf16<WG_BN_MAX, 1, 1>(d, p.BN, a_hi, b_hi, 1u);
+          } else {
+            wgmma_bf16<WG_BN_MAX, 1, 1>(d, p.BN, a_hi, b_hi, acc_flag);
           }
-          umma_commit(&empty[stage]);
-          if (kb == kb1 - 1) umma_commit(tfull);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
-    } else {
-      // ---------------------------------------------------------------- epilogue: TMEM -> red.add into dW
+      wgmma_wait<0>();
+      acc_store<WG_BN_MAX>(d, p.BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
+      named_bar_sync(1, 32 * WG_MMA_WARPS);
+      // epilogue: red.add into dW; warp w takes co rows 32 (w % 4) .. +31 and every other 16-column chunk
       const int q = warp & 3;
       const int co = co_tile * 128 + q * 32 + lane;
-      mbar_wait(tfull, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16);
+      const float* arow = acc_tile + size_t(q * 32 + lane) * p.acc_pitch;
       const int col_base = chunk_base * p.CK;
-      for (int c0 = 0; c0 < p.BN; c0 += 16) {
+      for (int c0 = (warp >> 2) * 16; c0 < p.BN; c0 += 32) {
         uint32_t v[16];
-        tmem_ld_32x32b_x16(taddr + uint32_t(c0), v);
-        tmem_ld_wait();
+        acc_ld_x16(arow + c0, v);
         if (co < p.cout) {
           float* dst = p.dw_out + size_t(co) * p.ktot + col_base + c0;
 #pragma unroll
@@ -215,13 +209,6 @@ __global__ void __launch_bounds__(192, 1) conv_wgrad_kernel(const __grid_constan
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
@@ -284,8 +271,7 @@ extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
   p.n_chunks = taps * p.cpt;
   p.ktot = taps * d->c;
   p.cout = d->cout;
-  const int bn_cap = d->nsplit == 3 ? 128 : 256;
-  int ng = std::min(p.n_chunks, bn_cap / p.CK);
+  int ng = std::min(p.n_chunks, WG_BN_MAX / p.CK);
   if ((ng * p.CK) % 16) ng += 1;  // CK == 8 with an odd chunk count: pad with a zero chunk
   p.NG = ng;
   p.BN = ng * p.CK;
@@ -308,17 +294,17 @@ extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
     case 16: p.b_layout = 6; p.b_lbo = p.x_chunk_bytes; p.b_sbo = 256; p.b_kstep_bytes = 16 * 32; break;
     default: p.b_layout = 0; p.b_lbo = 128; p.b_sbo = p.x_chunk_bytes; p.b_kstep_bytes = 16 * 16; break;
   }
-  uint32_t tc = 32;
-  while (tc < uint32_t(p.BN)) tc <<= 1;
-  p.tmem_cols = tc;
-  const uint32_t budget = uint32_t(wg_smem_optin) - 1024 - 256;
+  p.acc_pitch = uint32_t(p.BN) + 4;
+  const uint32_t acc_bytes = 128u * p.acc_pitch * 4u;
+  const uint32_t budget = uint32_t(wg_smem_optin) - 1024 - 256 - acc_bytes;
   p.stages = std::min<int>(WG_MAX_STAGES, budget / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.kb_per_split));
   if (p.stages < 2) {
     set_error("sfb_conv_wgrad: not enough shared memory (stage=%u B)", p.stage_bytes);
     return -11;
   }
-  p.off_bars = p.stages * p.stage_bytes;
+  p.off_acc = p.stages * p.stage_bytes;
+  p.off_bars = p.off_acc + acc_bytes;
   const uint32_t smem_bytes = p.off_bars + 256 + 1024;
   p.dw_out = d->dw;
 
@@ -353,14 +339,14 @@ extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
       cudaFuncSetAttribute(conv_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem_optin);
       a3 = true;
     }
-    conv_wgrad_kernel<3><<<grid, 192, smem_bytes, stream>>>(p);
+    conv_wgrad_kernel<3><<<grid, WG_THREADS, smem_bytes, stream>>>(p);
   } else {
     static bool a1 = false;
     if (!a1) {
       cudaFuncSetAttribute(conv_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem_optin);
       a1 = true;
     }
-    conv_wgrad_kernel<1><<<grid, 192, smem_bytes, stream>>>(p);
+    conv_wgrad_kernel<1><<<grid, WG_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

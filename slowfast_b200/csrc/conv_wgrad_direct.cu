@@ -2,7 +2,7 @@
 // 32 -> 8 1x1x1 / 3x1x1, 16 -> 16 1x3x3, the 7x1x1 lateral convolutions; resnet_helper.py:259 BottleneckTransform a / b / c,
 // video_model_builder.py:134 FuseFastToSlow conv_f2s).
 //
-// As a GEMM these are dW[cout <= 32, taps*cin <= 144] reduced over 0.2 - 0.8 M positions: the tcgen05 kernel fills 8 - 32 of
+// As a GEMM these are dW[cout <= 32, taps*cin <= 144] reduced over 0.2 - 0.8 M positions: the wgmma kernel fills 8 - 32 of
 // its 128 accumulator rows and re-reads a 128-row dY tile per 8-channel chunk; measured 237 us for the 8 -> 8 1x3x3 layer
 // whose operands are 51 MB (8 us of HBM time).  Here a WARP owns one job = (tap, 8 input channels, 8 output channels):
 // lane = output position, 64 register accumulators per thread, operands are 16-byte loads (coalesced 512-byte warp rows,
@@ -162,9 +162,8 @@ int wgrad_direct_try(const sfb_wgrad_desc* d, cudaStream_t stream, int* rc_out) 
   const int taps = d->kt * d->kh * d->kw;
   const int64_t M = int64_t(d->n) * d->out_t * d->out_h * d->out_w;
   const int jobs = taps * (d->c / 8) * (d->cout / 8);
-  // narrow layers with many positions only.  Measured on the B200 (profiles/r2q_*): 8 -> 8 1x3x3 72 vs 249 us, 8 -> 8 3x1x1 36 vs
-  // 116, 8 -> 32 57 vs 70, 32 -> 8 102 vs 111, lateral 7x1x1 45 vs 60; 16 -> 16 1x3x3 93 vs 88 and X3D's 8 -> 24 1x3x3 stem
-  // (27 jobs, 3.2 M positions) 1718 vs 953 us: tensor core ahead, excluded (more than 14 jobs)
+  // narrow layers with many positions only (at most 8 channels on one side, at most 14 (tap, 8 x 8 channel block) jobs):
+  // wider layers fill the tensor-core kernel's tiles
   if (d->c * d->cout > 256 || std::min(d->c, d->cout) > 8 || jobs > 14 || M < 32768) return 0;
   if (int64_t(d->n) * d->d * d->h * d->w * d->c_pitch >= (int64_t(1) << 31) || M * d->dy_pitch >= (int64_t(1) << 31)) return 0;
   if (!g_wgd_sms) {

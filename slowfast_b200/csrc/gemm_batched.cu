@@ -1,4 +1,4 @@
-// Batched GEMM on tcgen05 for the attention products of MViT's MultiScaleAttention (attention.py:355-379 and
+// Batched GEMM on wgmma for the attention products of MViT's MultiScaleAttention (attention.py:355-379 and
 // their autograd transposes):
 //
 //     D[b](m, n) (+)= alpha * sum_k A[b](m, k) * B[b](n, k)          b = batch * heads
@@ -9,8 +9,9 @@
 //     O  = P v        A=P  (K)   B=v  (MN)       dq = dS k     A=dS (K)   B=k  (MN)
 //     dv = P^T dO     A=P  (MN)  B=dO (MN)       dk = dS^T q   A=dS (MN)  B=q  (MN)
 // Operands are split-bf16 planes (nsplit 3) or bf16 (nsplit 1), staged by 3-D tiled TMA (128B swizzle; K / row /
-// batch tails zero-filled by the unit), accumulated in TMEM (UMMA 128 x BN x 16), same persistent warp-specialised
-// pipeline as conv_igemm.cu (producer warp / MMA warp / 4 epilogue warps, 2 accumulator stages).
+// batch tails zero-filled by the unit), accumulated in registers (two warpgroups of 64 x BN x 16 wgmma), same persistent
+// warp-specialised pipeline as conv_igemm.cu (two MMA warpgroups / producer warp / 4 epilogue warps reading a
+// shared-memory accumulator tile).
 #include <algorithm>
 #include <cstdint>
 #include <cstdlib>
@@ -25,6 +26,10 @@ namespace sfb {
 constexpr int BG_BLOCK_M = 128;
 constexpr int BG_BLOCK_K = 64;
 constexpr int BG_MAX_STAGES = 8;
+constexpr int BG_MMA_WARPS = 8;
+constexpr int BG_EPI_WARP0 = BG_MMA_WARPS + 1;
+constexpr int BG_THREADS = 32 * (BG_MMA_WARPS + 1 + 4);
+constexpr int BG_BN_MAX = 128;
 
 struct BgemmParams {
   CUtensorMap tmA[2];
@@ -35,8 +40,8 @@ struct BgemmParams {
   int m_tiles, n_tiles, k_blocks;
   int stages;
   uint32_t stage_bytes, a_plane_bytes, b_plane_bytes;
-  uint32_t tmem_cols;
-  uint32_t off_staging, off_bars;
+  uint32_t acc_pitch;
+  uint32_t off_acc, off_bars;
   float* out;
   long long ldd, batch_stride_d;
   float alpha;
@@ -56,7 +61,7 @@ __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* tm, u
 }
 
 template <int NSPLIT>
-__global__ void __launch_bounds__(192, 1) gemm_batched_kernel(const __grid_constant__ BgemmParams p) {
+__global__ void __launch_bounds__(BG_THREADS, 1) gemm_batched_kernel(const __grid_constant__ BgemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5;
@@ -65,36 +70,27 @@ __global__ void __launch_bounds__(192, 1) gemm_batched_kernel(const __grid_const
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + BG_MAX_STAGES;
   uint64_t* tfull = empty + BG_MAX_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* tempty = tfull + 1;
+  float* acc_tile = reinterpret_cast<float*>(smem + p.off_acc);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 32 * BG_MMA_WARPS);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], 4);
-    }
+    mbar_init(tfull, 32 * BG_MMA_WARPS);
+    mbar_init(tempty, 4);
     fence_mbar_init();
     fence_proxy_async_smem();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int tiles_per_batch = p.m_tiles * p.n_tiles;
   const int total_tiles = tiles_per_batch * p.batch;
   const int total_work = total_tiles * p.k_splits;
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
 
-  if (warp == 0) {
+  if (warp == BG_MMA_WARPS) {
     // ------------------------------------------------------------------ TMA producer
     int stage = 0;
     uint32_t phase = 0;
@@ -135,80 +131,84 @@ __global__ void __launch_bounds__(192, 1) gemm_batched_kernel(const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = make_idesc_bf16(BG_BLOCK_M, uint32_t(p.BN), uint32_t(p.a_mn), uint32_t(p.b_mn));
+  } else if (warp < BG_MMA_WARPS) {
+    // ------------------------------------------------------------------ MMA warpgroups (rows 64g .. 64g+63)
+    // Both operand forms put the second 64 rows 8192 B further: the next 64-row MN atom, or 8 more 1024-byte row groups.
+    const int g = warp >> 2;
+    const int mode = p.a_mn * 2 + p.b_mn;
+    float d[BG_BN_MAX / 2];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
     for (int work = blockIdx.x; work < total_work; work += gridDim.x, ++it) {
       const int ksp = work % p.k_splits;
       const int kb0 = ksp * p.kb_per_split, kb1 = min(p.k_blocks, kb0 + p.kb_per_split);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + uint32_t(acc * p.BN);
+      int held = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-          const uint32_t b_base = a_base + NP * p.a_plane_bytes;
+        wgmma_fence();
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 8192u;
+        const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + NP * p.a_plane_bytes;
 #pragma unroll
-          for (int ks = 0; ks < BG_BLOCK_K / 16; ++ks) {
-            uint64_t a_d[2], b_d[2];
-            for (uint32_t pl = 0; pl < NP; ++pl) {
-              const uint32_t aa = a_base + pl * p.a_plane_bytes, bb = b_base + pl * p.b_plane_bytes;
-              a_d[pl] = p.a_mn ? make_smem_desc(aa + ks * 2048, 8192, 1024, 2) : make_smem_desc(aa + ks * 32, 16, 1024, 2);
-              b_d[pl] = p.b_mn ? make_smem_desc(bb + ks * 2048, 8192, 1024, 2) : make_smem_desc(bb + ks * 32, 16, 1024, 2);
-            }
-            const uint32_t acc_flag = ((kb - kb0) | ks) != 0 ? 1u : 0u;
-            if (NSPLIT == 3) {
-              umma_bf16(d_tmem, a_d[1], b_d[0], idesc, acc_flag);
-              umma_bf16(d_tmem, a_d[0], b_d[1], idesc, 1u);
-              umma_bf16(d_tmem, a_d[0], b_d[0], idesc, 1u);
-            } else {
-              umma_bf16(d_tmem, a_d[0], b_d[0], idesc, acc_flag);
+        for (int ks = 0; ks < BG_BLOCK_K / 16; ++ks) {
+          uint64_t a_d[2], b_d[2];
+          for (uint32_t pl = 0; pl < NP; ++pl) {
+            const uint32_t aa = a_base + pl * p.a_plane_bytes, bb = b_base + pl * p.b_plane_bytes;
+            a_d[pl] = p.a_mn ? make_smem_desc(aa + ks * 2048, 8192, 1024, 2) : make_smem_desc(aa + ks * 32, 16, 1024, 2);
+            b_d[pl] = p.b_mn ? make_smem_desc(bb + ks * 2048, 8192, 1024, 2) : make_smem_desc(bb + ks * 32, 16, 1024, 2);
+          }
+          const uint32_t acc_flag = ((kb - kb0) | ks) != 0 ? 1u : 0u;
+          const int nprod = NSPLIT == 3 ? 3 : 1;
+          for (int pr = 0; pr < nprod; ++pr) {
+            // split products: A_lo*B_hi + A_hi*B_lo + A_hi*B_hi
+            const uint64_t ad = (NSPLIT == 3 && pr == 0) ? a_d[1] : a_d[0];
+            const uint64_t bd = (NSPLIT == 3 && pr == 1) ? b_d[1] : b_d[0];
+            const uint32_t af = pr == 0 ? acc_flag : 1u;
+            switch (mode) {
+              case 0: wgmma_bf16<BG_BN_MAX, 0, 0>(d, p.BN, ad, bd, af); break;
+              case 1: wgmma_bf16<BG_BN_MAX, 0, 1>(d, p.BN, ad, bd, af); break;
+              case 2: wgmma_bf16<BG_BN_MAX, 1, 0>(d, p.BN, ad, bd, af); break;
+              default: wgmma_bf16<BG_BN_MAX, 1, 1>(d, p.BN, ad, bd, af); break;
             }
           }
-          umma_commit(&empty[stage]);
-          if (kb == kb1 - 1) umma_commit(&tfull[acc]);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0) mbar_arrive(&empty[held]);
+        held = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
+      wgmma_wait<0>();
+      mbar_arrive(&empty[held]);
+      mbar_wait(tempty, (it & 1) ^ 1);
+      acc_store<BG_BN_MAX>(d, p.BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
+      mbar_arrive(tfull);
     }
   } else {
     // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;
+    const int q = warp - BG_EPI_WARP0;
+    const float* arow = acc_tile + size_t(q * 32 + lane) * p.acc_pitch;
     int it = 0;
     for (int work = blockIdx.x; work < total_work; work += gridDim.x, ++it) {
       const int tile = work / p.k_splits;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       const int b = tile / tiles_per_batch;
       const int r = tile - b * tiles_per_batch;
       const int mt = r / p.n_tiles, nt = r - mt * p.n_tiles;
       const int row0 = mt * BG_BLOCK_M + q * 32;
       const int ncol0 = nt * p.BN;
       float* obase = p.out + size_t(b) * p.batch_stride_d;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(acc * p.BN);
+      mbar_wait(tfull, it & 1);
       for (int c0 = 0; c0 < p.BN; c0 += 32) {
         uint32_t v0[16], v1[16];
-        tmem_ld_32x32b_x16(taddr + uint32_t(c0), v0);
+        acc_ld_x16(arow + c0, v0);
         const bool second = (c0 + 16) < p.BN;
-        if (second) tmem_ld_32x32b_x16(taddr + uint32_t(c0 + 16), v1);
-        tmem_ld_wait();
-        if (c0 + 32 >= p.BN) {
-          tc_fence_before();
+        if (second) acc_ld_x16(arow + c0 + 16, v1);
+        if (c0 + 32 >= p.BN) {  // last read of the accumulator tile: hand it back to the MMA warpgroups
           __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[acc]);
+          if (lane == 0) mbar_arrive(tempty);
         }
         float x[32];
 #pragma unroll
@@ -246,12 +246,6 @@ __global__ void __launch_bounds__(192, 1) gemm_batched_kernel(const __grid_const
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 typedef CUresult (*EncodeTiledFn3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -332,8 +326,7 @@ extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
   p.a_mn = d->a_mn_major ? 1 : 0;
   p.b_mn = d->b_mn_major ? 1 : 0;
   const int n16 = (d->n + 15) / 16 * 16;
-  const int bn_cap = d->nsplit == 3 ? 128 : 256;
-  p.BN = std::min(n16, bn_cap);
+  p.BN = std::min(n16, BG_BN_MAX);
   p.n_atoms = (p.BN + 63) / 64;
   p.m_tiles = (d->m + BG_BLOCK_M - 1) / BG_BLOCK_M;
   p.n_tiles = (d->n + p.BN - 1) / p.BN;
@@ -342,10 +335,9 @@ extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
   p.b_plane_bytes = p.b_mn ? uint32_t(p.n_atoms) * 8192u : uint32_t((p.BN + 7) / 8 * 8) * 128u;
   p.b_plane_bytes = (p.b_plane_bytes + 1023) / 1024 * 1024;
   p.stage_bytes = (p.a_plane_bytes + p.b_plane_bytes) * np;
-  uint32_t tc = 32;
-  while (tc < uint32_t(2 * p.BN)) tc <<= 1;
-  p.tmem_cols = tc;
-  const uint32_t tail = 4 * 32 * 33 * 4 + 256;
+  p.acc_pitch = uint32_t(p.BN) + 4;
+  const uint32_t acc_bytes = uint32_t(BG_BLOCK_M) * p.acc_pitch * 4u;
+  const uint32_t tail = acc_bytes + 256;
   const uint32_t budget = uint32_t(bg_smem) - 1024 - tail;
   p.stages = std::min<int>(BG_MAX_STAGES, budget / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.k_blocks * 4));
@@ -353,8 +345,8 @@ extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
     set_error("sfb_gemm_batched: not enough shared memory (stage=%u B)", p.stage_bytes);
     return -11;
   }
-  p.off_staging = p.stages * p.stage_bytes;
-  p.off_bars = p.off_staging + 4 * 32 * 33 * 4;
+  p.off_acc = p.stages * p.stage_bytes;
+  p.off_bars = p.off_acc + acc_bytes;
   const uint32_t smem_bytes = p.off_bars + 256 + 1024;
   p.out = d->out;
   p.ldd = d->ldd;
@@ -395,14 +387,14 @@ extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
       cudaFuncSetAttribute(gemm_batched_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bg_smem);
       a3 = true;
     }
-    gemm_batched_kernel<3><<<grid, 192, smem_bytes, stream>>>(p);
+    gemm_batched_kernel<3><<<grid, BG_THREADS, smem_bytes, stream>>>(p);
   } else {
     static bool a1 = false;
     if (!a1) {
       cudaFuncSetAttribute(gemm_batched_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bg_smem);
       a1 = true;
     }
-    gemm_batched_kernel<1><<<grid, 192, smem_bytes, stream>>>(p);
+    gemm_batched_kernel<1><<<grid, BG_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

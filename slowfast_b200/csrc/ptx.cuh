@@ -1,10 +1,12 @@
-// Thin inline-PTX wrappers for the sm_100a features the engine uses:
-// mbarrier, TMA (tiled + im2col), tcgen05 (TMEM alloc, UMMA, commit, TMEM loads).
+// Thin inline-PTX wrappers for the sm_90a features the engine uses:
+// mbarrier, TMA (tiled + im2col), wgmma ordering (the MMA instructions themselves are in wgmma.cuh).
 // Everything here is a 1:1 spelling of a PTX instruction; no policy lives in this file.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
 #include <cuda_runtime.h>
+
+#include "wgmma.cuh"
 
 namespace sfb {
 
@@ -93,74 +95,55 @@ __device__ __forceinline__ void tma_load_im2col_5d(void* smem, const CUtensorMap
       : "memory");
 }
 
-// ----------------------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 operands, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      " .reg .pred p;\n"
-      " setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued UMMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 bit, 16 consecutive columns: thread i of the warp receives row (lane base + i).
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+// ----------------------------------------------------------------------------- wgmma
+// Ordering of register accesses against the asynchronous warpgroup MMAs (all 128 threads of the warpgroup execute these).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
 // ----------------------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (sm_100 format): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
-// version=1 [46,48) | layout type [61,64) (0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B).
+// Shared-memory matrix descriptor (sm_90 format): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
+// layout type [62,64) (0 none, 1 = 128B swizzle, 2 = 64B, 3 = 32B).  The callers pass the layout as 0 / 2 / 4 / 6,
+// i.e. the same field shifted one bit down ([61,64)).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
                                                    uint32_t layout_type) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout_type & 7) << 61;
+  d |= static_cast<uint64_t>(layout_type & 6) << 61;
   return d;
 }
-// Instruction descriptor for kind::f16 with bf16 A/B, fp32 D.
-// c_format=F32 (1) at [4,6); a_format=BF16 (1) at [7,10); b_format at [10,13); a_major bit 15; b_major bit 16
-// (0 = K-major, 1 = MN-major); N>>3 at [17,23); M>>4 at [24,29).
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(uint32_t m, uint32_t n, uint32_t a_mn_major,
-                                                             uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) |
-         ((m >> 4) << 24);
+
+// ----------------------------------------------------------------------------- accumulator tile hand-off
+// The MMA warpgroups keep a [64 x n] fp32 accumulator in registers (wgmma fragment layout, wgmma.cuh); the epilogue warps
+// read it from a row-major shared-memory tile of `pitch` floats per row.  acc_store writes the calling warpgroup's
+// fragment to rows [0, 64) of `tile`; every thread of the warpgroup calls it.
+template <int MAXN>
+__device__ __forceinline__ void acc_store(const float* d, int n, float* tile, int pitch) {
+  const int t = threadIdx.x & 127;
+  const int r = (t >> 5) * 16 + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < MAXN / 8; ++j) {
+    if (8 * j < n) {
+      *reinterpret_cast<float2*>(tile + r * pitch + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+      *reinterpret_cast<float2*>(tile + (r + 8) * pitch + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+  }
+}
+// 16 consecutive columns of one row of an accumulator tile (16-byte aligned).
+__device__ __forceinline__ void acc_ld_x16(const float* src, uint32_t (&v)[16]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float4 x = reinterpret_cast<const float4*>(src)[j];
+    v[4 * j] = __float_as_uint(x.x);
+    v[4 * j + 1] = __float_as_uint(x.y);
+    v[4 * j + 2] = __float_as_uint(x.z);
+    v[4 * j + 3] = __float_as_uint(x.w);
+  }
 }
 
 // named barrier among a subset of warps

@@ -8,7 +8,7 @@ engine's own backward kernels and parameter gradients land in ``param.grad`` (an
 Building blocks:
   * ``Storage``/``Act``  - channels-last split-bf16 activation storage (+ lazily allocated fp32 gradient) and a
                            channel-slice view of it ("concat in place").
-  * ``ConvBN``           - conv (tcgen05 implicit GEMM) + train/eval BatchNorm statistics; backward = BN backward,
+  * ``ConvBN``           - conv (wgmma implicit GEMM) + train/eval BatchNorm statistics; backward = BN backward,
                            wgrad, dgrad (strided dgrad via ``conv_plan``).
   * ``Ctx``              - per-model buffer cache, scratch, flat gradient buffer, launch bookkeeping.
 """
@@ -254,12 +254,11 @@ RMW_DGRAD = os.environ.get("SFB_RMW_DGRAD", "0") != "0"
 ATOMIC_DGRAD = os.environ.get("SFB_ATOMIC_DGRAD", "1") != "0"
 # fast-pathway stem weight gradient on the fp32 pipes (csrc/conv_stem.cu, stem_wgrad_direct); 0 = tensor-core W-shift path
 DIRECT_STEM_WGRAD = os.environ.get("SFB_DIRECT_STEM_WGRAD", "1") != "0"
-# Toeplitz tcgen05 kernels for the 8-channel (fast pathway) stem, csrc/conv_stem8.cu: "0" = W-shift fprop + SIMT wgrad of r1
+# Toeplitz wgmma kernels for the 8-channel (fast pathway) stem, csrc/conv_stem8.cu: "0" = W-shift fprop + SIMT wgrad of r1
 STEM_T8 = os.environ.get("SFB_STEM_T8", "1") != "0"
 STEM_T8_WGRAD = os.environ.get("SFB_STEM_T8_WGRAD", "1") != "0"
-# one filter-packing launch per phase (ops.PackPlan) instead of one per layer.  Validated on the B200 (SlowFast / X3D goldens
-# and gentle-fixture gradients pass with SFB_BATCHED_PACK=1) but it buys nothing under CUDA-graph replay (34.77 vs 34.79
-# ms/step: the ~250 tiny pack kernels were already hidden), so it stays opt-in; it matters for eager (graph-less) runs.
+# one filter-packing launch per phase (ops.PackPlan) instead of one per layer.  Under CUDA-graph replay the ~250 tiny pack
+# kernels are already hidden, so it stays opt-in; it matters for eager (graph-less) runs.
 BATCHED_PACK = os.environ.get("SFB_BATCHED_PACK", "0") != "0"
 
 

@@ -91,7 +91,7 @@ class AttnFwdDesc(C.Structure):
         ("bh", C.c_int32), ("nq", C.c_int32), ("nk", C.c_int32), ("hd", C.c_int32),
         ("qt", C.c_int32), ("qh", C.c_int32), ("qw", C.c_int32), ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
         ("scale", C.c_float), ("out", C.c_void_p), ("p_hi", C.c_void_p), ("p_lo", C.c_void_p), ("p_pitch", C.c_int64),
-        ("lse", C.c_void_p), ("nsplit", C.c_int32), ("e_sel", C.c_void_p),
+        ("lse", C.c_void_p), ("nsplit", C.c_int32),
     ]
 
 
@@ -102,7 +102,7 @@ class AttnBwdDesc(C.Structure):
         ("do_hi", C.c_void_p), ("do_lo", C.c_void_p), ("v_hi", C.c_void_p), ("v_lo", C.c_void_p),
         ("p_hi", C.c_void_p), ("p_lo", C.c_void_p), ("p_pitch", C.c_int64),
         ("ds_hi", C.c_void_p), ("ds_lo", C.c_void_p), ("ds_pitch", C.c_int64),
-        ("drq", C.c_void_p), ("rq_pitch", C.c_int64), ("e_sel", C.c_void_p),
+        ("drq", C.c_void_p), ("rq_pitch", C.c_int64),
         ("bh", C.c_int32), ("nq", C.c_int32), ("nk", C.c_int32), ("hd", C.c_int32),
         ("qt", C.c_int32), ("qh", C.c_int32), ("qw", C.c_int32), ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
         ("nsplit", C.c_int32),
@@ -367,8 +367,6 @@ _SIGNATURES = [
     ("sfb_attn_fwd_supported", C.c_int32, [C.c_int32] * 5),
     ("sfb_attn_fwd", C.c_int, [C.POINTER(AttnFwdDesc), C.c_void_p]),
     ("sfb_attn_bwd_ds", C.c_int, [C.POINTER(AttnBwdDesc), C.c_void_p]),
-    ("sfb_attn_fwd_selector_bytes", C.c_int64, []),
-    ("sfb_attn_fwd_selector", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_clip_normalize_pack", C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                           C.c_int32, C.c_void_p, C.c_void_p]),
     ("sfb_allreduce_flat", C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p]),
@@ -397,7 +395,7 @@ def load() -> C.CDLL:
     path = Path(lib_path())
     if not path.exists():
         raise NativeLibraryError(
-            f"{path} is missing: build it with `python -m slowfast_b200.build` (nvcc, sm_100a). "
+            f"{path} is missing: build it with `python -m slowfast_b200.build` (nvcc, sm_90a). "
             "slowfast_b200 has no CPU fallback.")
     lib = C.CDLL(str(path))
     for name, res, args in _SIGNATURES:

@@ -1,4 +1,4 @@
-"""MaskFeat pre-training wrapper (slowfast/models/masked.py:25 MaskMViT) on the B200 engine.
+"""MaskFeat pre-training wrapper (slowfast/models/masked.py:25 MaskMViT) on the engine.
 
 ``MaskMViT`` = the MViTv2 encoder with (a) masked patch tokens replaced by a learned ``mask_token`` right after the
 patch embedding (masked.py:551-565), (b) no final norm / classification head but an ``MSSeparateHead`` (LayerNorm +
@@ -7,7 +7,7 @@ targets computed from the input frames (operators.py:79 HOGLayerC, masked.py:254
 ``(preds, labels)`` exactly like the reference so that ``MultipleMSELoss`` (losses.py:25) consumes it unchanged.
 
 Execution: the encoder is ``B200MViT``'s program; the wrapper adds the masked token assembly, the prediction head
-(LayerNorm over all token rows -> split planes -> tcgen05 GEMM 768 -> 108, run for every token so the program is
+(LayerNorm over all token rows -> split planes -> wgmma GEMM 768 -> 108, run for every token so the program is
 static and CUDA-graph capturable; the boolean row selection ``pred[mask]`` happens on the result, row-wise identical
 to selecting first) and the HOG target kernel (csrc/maskfeat.cu).
 

@@ -1,12 +1,12 @@
-"""MViTv2 (video_model_builder.py:806 MViT; attention.py MultiScaleBlock / MultiScaleAttention) on the B200 engine.
+"""MViTv2 (video_model_builder.py:806 MViT; attention.py MultiScaleBlock / MultiScaleAttention) on the engine.
 
 Module tree, parameter names and initialisation mirror the reference (patch_embed.proj, cls_token, blocks.{i}.norm1 /
 attn.{qkv,proj,pool_{q,k,v},norm_{q,k,v},rel_pos_{h,w,t}} / norm2 / mlp.{fc1,fc2} / proj, norm, head.projection).
 Execution:
-  * every Linear (qkv, proj, fc1, fc2, block proj) and the patch embedding run on the tcgen05 implicit-GEMM kernel;
+  * every Linear (qkv, proj, fc1, fc2, block proj) and the patch embedding run on the wgmma implicit-GEMM kernel;
     their wgrad / dgrad on the same kernels as the conv nets;
   * pooled attention: depthwise pooling convs read the fused-qkv GEMM output in place (no permute/contiguous copies),
-    QK^T / PV and the four backward products are batched tcgen05 GEMMs in all operand-major combinations, the
+    QK^T / PV and the four backward products are batched wgmma GEMMs in all operand-major combinations, the
     decomposed relative-position bias is ONE extra GEMM of q against the concatenated [Rh;Rw;Rt] tables plus an
     index lookup inside the softmax kernel (SURVEY.md section 7.6: identical to cal_rel_pos_spatial/_temporal);
   * LayerNorm, GELU, residual/bias/stochastic-depth combines, max-pool skip are fused row kernels.
@@ -166,10 +166,12 @@ class TransformerHeadModule(Namespace):
         self.act_func = act_func
 
 
-# fused pooled-attention forward (csrc/attn_fused.cu); SFB_ATTN_FUSED=0 keeps the unfused sequence everywhere
-ATTN_FUSED = os.environ.get("SFB_ATTN_FUSED", "1") != "0"
-# fused first half of the attention backward (dP in TMEM -> dS planes + dRQ); SFB_ATTN_FUSED_BWD=0 = dP GEMM + softmax_relpos_bwd
-ATTN_FUSED_BWD = os.environ.get("SFB_ATTN_FUSED_BWD", "1") != "0"
+# fused pooled attention (csrc/attn_fused.cu), opt-in with SFB_ATTN_FUSED=1 / SFB_ATTN_FUSED_BWD=1: on one H100 (400 W) the
+# MViTv2-S step runs 59.0 clips/s with it and 67.3 with the unfused sequence (gemm_batched -> softmax_relpos -> gemm_batched),
+# because the fused kernel is not yet tuned (one warpgroup per CTA, loads not overlapped with the MMAs)
+ATTN_FUSED = os.environ.get("SFB_ATTN_FUSED", "0") != "0"
+# fused first half of the attention backward (dP in shared memory -> dS planes + dRQ); 0 = dP GEMM + softmax_relpos_bwd
+ATTN_FUSED_BWD = os.environ.get("SFB_ATTN_FUSED_BWD", "0") != "0"
 
 
 def _ptr(t):
@@ -515,7 +517,7 @@ class B200MViT(nn.Module):
         Nq, Nk = Lq + 1, Lk + 1
         Nkp = ops.pad8(Nk)
         BH = B * Hn
-        # fused path (csrc/attn_fused.cu): S, the rel-pos bias, the softmax and P.V in ONE kernel with the scores in TMEM,
+        # fused path (csrc/attn_fused.cu): S, the rel-pos bias, the softmax and P.V in ONE kernel with the scores in shared memory,
         # for the geometry it covers (head_dim 96, 8x7x7 key grid: 12 of MViTv2-S's 16 blocks); else the unfused sequence
         fused = bool(ATTN_FUSED and lib.sfb_attn_fwd_supported(Nk, hd, *k_thw))
         S = None
@@ -567,13 +569,6 @@ class B200MViT(nn.Module):
             fd.out = O.data_ptr()
             fd.p_hi, fd.p_lo, fd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp   # (the unfused backward reads P)
             fd.nsplit = ctx.nsplit
-            if rq is not None:
-                # key selector of the decomposed rel-pos bias (added by the tensor core); constant, rewritten per block
-                # so that it is part of every captured program
-                esel = ctx.buf(("attn.esel",) + tuple(k_thw), (int(lib.sfb_attn_fwd_selector_bytes()) // 2,), BF16)
-                L.check(lib.sfb_attn_fwd_selector(esel.data_ptr(), *k_thw, _st()), "sfb_attn_fwd_selector")
-                ops._count()
-                fd.e_sel = esel.data_ptr()
             L.check(lib.sfb_attn_fwd(C.byref(fd), _st()), "sfb_attn_fwd")
             ops._count()
         else:
@@ -742,16 +737,13 @@ class B200MViT(nn.Module):
         Ltp = sv["Ltp"]
         drq = ctx.scratch("attn.RQ", BH * Lq * Ltp, F32).view(BH * Lq, Ltp) if Ltp else None
         if sv["fused"] and ATTN_FUSED_BWD and Nkp == 400:
-            # dP = dO v^T stays in TMEM; dS planes and dRQ come out of one kernel (csrc/attn_fused.cu)
+            # dP = dO v^T stays in shared memory; dS planes and dRQ come out of one kernel (csrc/attn_fused.cu)
             bd = L.AttnBwdDesc()
             bd.do_hi, bd.do_lo = dO.hi_ptr(), dO.lo_ptr()
             bd.v_hi, bd.v_lo = pl["v"].hi_ptr(), pl["v"].lo_ptr()
             bd.p_hi, bd.p_lo, bd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
             bd.ds_hi, bd.ds_lo, bd.ds_pitch = dS.hi_ptr(), dS.lo_ptr(), Nkp
             bd.drq, bd.rq_pitch = _ptr(drq), Ltp
-            if drq is not None:
-                esel = ctx.buf(("attn.esel",) + tuple(k_thw), (int(lib.sfb_attn_fwd_selector_bytes()) // 2,), BF16)
-                bd.e_sel = esel.data_ptr()      # written by this step's forward
             bd.bh, bd.nq, bd.nk, bd.hd = BH, Nq, Nk, hd
             bd.qt, bd.qh, bd.qw = q_thw
             bd.kt, bd.kh, bd.kw = k_thw

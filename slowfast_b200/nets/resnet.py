@@ -1,4 +1,4 @@
-"""SlowFast / ResNet (C2D, I3D, Slow) video backbones on the B200 engine.
+"""SlowFast / ResNet (C2D, I3D, Slow) video backbones on the engine.
 
 Mirrors the reference's module tree and parameter names (slowfast/models/video_model_builder.py:173 SlowFast,
 :445 ResNet; resnet_helper.py:259 BottleneckTransform, :395 ResBlock, :524 ResStage; stem_helper.py:20,127;

@@ -1,6 +1,6 @@
-"""Single-pathway ResNet video models (C2D / I3D / Slow; video_model_builder.py:445 ResNet) on the B200 engine.
+"""Single-pathway ResNet video models (C2D / I3D / Slow; video_model_builder.py:445 ResNet) on the engine.
 
-Same building blocks as ``B200SlowFast`` (W-shift stem, tcgen05 bottleneck blocks, fused BN/ReLU/residual passes),
+Same building blocks as ``B200SlowFast`` (W-shift stem, wgmma bottleneck blocks, fused BN/ReLU/residual passes),
 plus the temporal max-pool the c2d / i3d archs insert after res2 (``pathway0_pool``, _POOL1 :100-103).
 """
 from __future__ import annotations

@@ -1,12 +1,12 @@
 """X3D (video_model_builder.py:664 X3D; resnet_helper.py:122 X3DTransform; stem_helper.py:204 X3DStem;
-operators.py:14 SE; head_helper.py:352 X3DHead) on the B200 engine.
+operators.py:14 SE; head_helper.py:352 X3DHead) on the engine.
 
 Module tree and parameter names mirror the reference (``s1.pathway0_stem.{conv_xy,conv,bn}``,
 ``s{2..5}.pathway0_res{i}.{branch1,branch1_bn,branch2.{a,a_bn,b,b_bn,se.fc1,se.fc2,c,c_bn}}``,
 ``head.{conv_5,conv_5_bn,lin_5,projection}``), so checkpoints, the optimizer's parameter grouping and
 ``build_model`` work unchanged.  Execution:
 
-  stem   : conv_xy 1x3x3 (tcgen05 implicit GEMM, C_in padded 3->8) -> channelwise 5x1x1 conv with the BatchNorm
+  stem   : conv_xy 1x3x3 (wgmma implicit GEMM, C_in padded 3->8) -> channelwise 5x1x1 conv with the BatchNorm
            partials in its epilogue -> fused BN+ReLU
   block  : a (1x1x1 GEMM + BN stats) -> BN+ReLU -> channelwise 3x3x3 (+ BN partials per sample tile, which also
            ARE the SE average pool) -> [SE FCs, one block per sample] -> BN*gate -> Swish -> c (1x1x1 GEMM + BN)

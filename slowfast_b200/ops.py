@@ -512,6 +512,8 @@ def stem_m_tiles(x: Planes, g: StemGeom) -> int:
 
 def stem_fprop(x: Planes, f: FilterMat, g: StemGeom, out: torch.Tensor, stats: Optional[torch.Tensor],
                nsplit: int = 3) -> None:
+    """W-shift stem forward (csrc/conv_stem.cu): up to 128 output channels (one accumulator tile of 128 columns); the
+    stems of the supported models have 8, 24 or 64."""
     lib = L.load()
     d = _stem_desc(x, g, nsplit)
     d.f_hi, d.f_lo = f.hi.data_ptr(), _ptr(f.lo)
@@ -521,6 +523,8 @@ def stem_fprop(x: Planes, f: FilterMat, g: StemGeom, out: torch.Tensor, stats: O
 
 
 def stem_wgrad(x: Planes, dy: Planes, g: StemGeom, dwm: torch.Tensor, nsplit: int = 3) -> None:
+    """W-shift stem weight gradient (csrc/conv_stem.cu): up to 64 output channels and 4 folded W taps (filters up to 7
+    wide at stride 2)."""
     lib = L.load()
     assert dy.pitch == dy.c == g.cout
     d = _stem_desc(x, g, nsplit)

@@ -29,7 +29,7 @@ def main():
         cnt[n] += 1
     tot = sum(agg.values())
     print(f"# {title}\n")
-    print(f"Command (B200 box): `{cmd}`")
+    print(f"Command: `{cmd}`")
     print("Per-launch times under ncu are serialised and cold-cache: compare SHARES, not absolutes.\n")
     print(f"Total device time of the step: {tot / 1e6:.1f} ms over {len(body)} launches.\n")
     print("| kernel | launches | total us | share | avg us |\n|---|---:|---:|---:|---:|")

@@ -54,7 +54,7 @@ for which in ("slowfast", "mvit", "x3d"):
 json.dump(summary, open(f"{dst}_summary.json", "w"), indent=1)
 open(f"{dst}.md", "w").write(
     "# Round 2 - DRAM traffic per kernel class (ncu `dram__bytes_read.sum`, `dram__bytes_write.sum`, `gpu__time_duration.sum`)\n\n"
-    "Command (B200 box, per model): `ncu --profile-from-start off --metrics gpu__time_duration.sum,dram__bytes_read.sum,"
+    "Command (per model): `ncu --profile-from-start off --metrics gpu__time_duration.sum,dram__bytes_read.sum,"
     "dram__bytes_write.sum --clock-control none --csv --log-file ... python tests/probes/ncu_step.py <model>` - one eager train step "
     "(fwd + CE + bwd) after two warm-up steps, parity mode, recipe batch.  Times under ncu are serialised and cold-cache: compare "
     "shares; the DRAM byte counts are what `bench.py`'s `roofline.traffic` reports (bytes per launch of the dominant class).\n\n"

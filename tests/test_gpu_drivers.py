@@ -6,7 +6,7 @@ drivers on the same synthetic clips.
 What runs unmodified: build_model (+ .cuda(), + the DDP wrap for NUM_GPUS 2), construct_optimizer (BN / zero-WD parameter
 grouping by module type), the loaders, train_epoch (autocast context, GradScaler, grad-norm clipping, LR policy, meters),
 save_checkpoint / load_test_checkpoint (state_dict key parity), eval_epoch, perform_test (multi-view ensembling).
-Reference tree: baseline/_ref (see baseline/install_ref.sh) through oracle/refshim.py; tests skip when it is absent.
+Reference tree: oracle/_ref (copied by build(), oracle/install_ref.py) through oracle/refshim.py; tests skip when it is absent.
 """
 import os
 import tempfile
@@ -39,7 +39,7 @@ def _restore_stock_registry():
 def _harness():
     import driver_harness as H
     if H.setup_reference() is None:
-        pytest.skip("no reference tree on this box (run baseline/install_ref.sh in the build container)")
+        pytest.skip("no reference tree: build() copies it into oracle/_ref from a reference checkout")
     return H
 
 
@@ -119,7 +119,7 @@ def test_two_gpu_ddp_through_build_model(engine, cuda_device):
     """NUM_GPUS 2: build_model wraps the module in DistributedDataParallel (build.py:66-76); the engine's single autograd
     node hands every parameter gradient to DDP's reducer.  Compared with the stock model under the same DDP driver."""
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     H = _harness()
     import torch.multiprocessing as mp
     recs = {}

@@ -87,7 +87,7 @@ def test_conv_fprop(case, nsplit, cuda_device):
 
 
 ACC_CASES = [
-    # n, t, h, w, cin, cout, k, stride, pad   (both epilogue variants of the tcgen05 kernel, and the SIMT body)
+    # n, t, h, w, cin, cout, k, stride, pad   (both epilogue variants of the wgmma kernel, and the SIMT body)
     (2, 4, 14, 14, 64, 256, (1, 1, 1), (1, 1, 1), (0, 0, 0)),     # short K: line-coalesced epilogue
     (1, 2, 14, 14, 256, 64, (1, 3, 3), (1, 1, 1), (0, 1, 1)),     # K = 2304: direct per-row stores
     (2, 4, 28, 28, 8, 32, (1, 1, 1), (1, 1, 1), (0, 0, 0)),       # C_in = 8: fp32 SIMT body
@@ -431,7 +431,7 @@ def test_stem_wshift_fprop_wgrad(case, nsplit, cuda_device):
 
 
 def test_gemm_batched_all_layouts(cuda_device):
-    """Batched tcgen05 GEMM in the four operand-major combinations the attention products need."""
+    """Batched wgmma GEMM in the four operand-major combinations the attention products need."""
     ops = _ops()
     from slowfast_b200 import lib as L
     import ctypes as C

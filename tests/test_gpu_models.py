@@ -14,10 +14,13 @@ Tolerances
     median < 0.2 and max < 0.5 vs the oracle, cosine > 0.9.  (Each backward kernel is checked on its own to 2e-5 in
     tests/test_gpu_kernels.py, where no mask can flip.)
 """
+import json
 import os
 
 import pytest
 import torch
+
+from oracle.golden_cfg import engine_cfg as _cfg_for
 
 pytestmark = pytest.mark.gpu
 
@@ -25,13 +28,6 @@ GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 TOL = 1e-3
 # parameter-gradient norms (see module docstring)
 GRAD_TOL = 0.15
-
-
-PRESET = {"Kinetics/SLOWFAST_8x8_R50.yaml": "SLOWFAST_8x8_R50", "Kinetics/C2D_8x8_R50.yaml": "C2D_8x8_R50",
-          "Kinetics/SLOW_8x8_R50.yaml": "SLOW_8x8_R50", "Kinetics/I3D_8x8_R50.yaml": "I3D_8x8_R50",
-          "Kinetics/MVITv2_S_16x4.yaml": "MVITv2_S_16x4", "Kinetics/MVITv2_B_32x3.yaml": "MVITv2_B_32x3",
-          "Kinetics/X3D_M.yaml": "X3D_M",
-          "masked_ssl/k400_MVITv2_S_16x4_MaskFeat_PT.yaml": "MVITv2_S_16x4_MaskFeat_PT"}
 
 
 def sample_idx(numel: int, k: int = 256) -> torch.Tensor:
@@ -53,19 +49,6 @@ def _model_class(cfg):
     return B200ResNet
 
 
-def _cfg_for(gold, nsplit=3):
-    from slowfast_b200.config import get_cfg
-    preset = PRESET[gold["yaml"]]
-    if gold["case"].startswith("maskfeat_b"):   # composed config (BASELINE config 5, SURVEY.md section 3.5)
-        preset = "MVITv2_B_32x3_MaskFeat_PT"
-    cfg = get_cfg(preset, B200={"NSPLIT": nsplit})
-    ov = gold["overrides"]
-    for k, v in zip(ov[0::2], ov[1::2]):
-        sec, key = k.split(".")
-        if sec == "AUG":
-            continue  # loader-side keys (mask window) are not read by the model
-        cfg[sec][key] = v
-    return cfg
 
 
 def _run_engine(cfg, state, inputs, dlogits, dev):
@@ -110,8 +93,8 @@ def test_model_matches_reference_golden(name, cuda_device):
     # filter / shifted tap shows up as O(1) here even when the norm happens to agree
     heads = sorted(v[1] for v in errs.values())
     print(f"{name}: leading-element error / RMS: median {heads[len(heads) // 2]:.2e}, max {heads[-1]:.2e}")
-    # (measured on the B200: median 0.07-0.12, max 0.2-0.5 on these deliberately chaotic fixtures, where ReLU mask flips put
-    # ~8 % rel-L2 into every gradient of ANY two implementations; a layout error gives a median of ~1.4)
+    # (these fixtures are deliberately chaotic: ReLU mask flips put ~8 % rel-L2 into every gradient of ANY two
+    # implementations; a layout error gives a median of ~1.4)
     assert heads[len(heads) // 2] < 0.25 and heads[-1] < 1.5, (heads[len(heads) // 2], heads[-1])
     if "grad_samples" in gold:
         # element-wise: 256 evenly spaced elements of EVERY parameter gradient against the reference's fp32 values, held
@@ -463,5 +446,11 @@ def test_fast_mode_is_in_the_reference_bf16_autocast_error_class(family, cuda_de
               f"{e_grad:.2e} (reference {r_grad:.2e})")
         bound_log, bound_grad = max(2 * r_log, 1e-3), max(2 * r_grad, 1e-3)
     else:
-        print(f"{family}: fast mode logits rel-L2 {e_log:.2e}, median gradient rel-L2 {e_grad:.2e} (no reference tree here)")
+        # the reference's CUDA bf16-autocast run on an H100, stored by oracle/make_fast_mode_bounds.py --device cuda
+        with open(os.path.join(GOLDEN, "fast_mode_reference_error.json")) as f:
+            ref = json.load(f)[family]
+        r_log, r_grad = ref["logits_rel_l2"], ref["median_grad_rel_l2"]
+        print(f"{family}: fast mode logits rel-L2 {e_log:.2e} (stored reference bf16 autocast {r_log:.2e}); median "
+              f"gradient rel-L2 {e_grad:.2e} (reference {r_grad:.2e})")
+        bound_log, bound_grad = max(2 * r_log, 1e-3), max(2 * r_grad, 1e-3)
     assert e_log < bound_log and e_grad < bound_grad, (e_log, bound_log, e_grad, bound_grad)

@@ -347,9 +347,9 @@ def test_device_input_pipeline_matches_reference_host_functions(arch, reverse, c
 @pytest.mark.parametrize("q_thw,bh,rel,nsplit", [((8, 7, 7), 2, True, 3), ((8, 14, 14), 3, True, 3), ((8, 28, 28), 1, True, 3),
                                                   ((8, 14, 14), 2, False, 3), ((8, 14, 14), 2, True, 1)])
 def test_fused_attention_forward(q_thw, bh, rel, nsplit, cuda_device):
-    """sfb_attn_fwd (csrc/attn_fused.cu): O = softmax(scale q k^T + rel-pos bias) v with the scores kept in TMEM, for the
+    """sfb_attn_fwd (csrc/attn_fused.cu): O = softmax(scale q k^T + rel-pos bias) v with the scores kept in shared memory, for the
     8x7x7 key grid (Nk = 393), against fp64 on the operand values the kernel saw (split planes); also the normalised P planes
-    it leaves for the backward and the log-sum-exp.  Tile tails (Nq = 393, 1569, 6273 are not multiples of 128), cls row /
+    it leaves for the backward and the log-sum-exp.  Tile tails (Nq = 393, 1569, 6273 are not multiples of 64), cls row /
     column without bias, and the no-rel-pos variant are covered."""
     from slowfast_b200 import lib as L
     lib, dev = L.load(), cuda_device
@@ -399,9 +399,6 @@ def test_fused_attention_forward(q_thw, bh, rel, nsplit, cuda_device):
     d.scale = hd ** -0.5
     d.out, d.p_hi, d.p_lo, d.p_pitch, d.lse = out.data_ptr(), p_hi.data_ptr(), (p_lo.data_ptr() if nsplit == 3 else None), Nkp, lse.data_ptr()
     d.nsplit = nsplit
-    e_sel = torch.empty(int(lib.sfb_attn_fwd_selector_bytes()) // 2, dtype=torch.bfloat16, device=dev)
-    L.check(lib.sfb_attn_fwd_selector(e_sel.data_ptr(), kt, kh, kw, _st()), "sfb_attn_fwd_selector")
-    d.e_sel = e_sel.data_ptr()
     L.check(lib.sfb_attn_fwd(C.byref(d), _st()), "sfb_attn_fwd")
     torch.cuda.synchronize()
     # fp64 reference on the plane values
@@ -429,8 +426,8 @@ def test_fused_attention_forward(q_thw, bh, rel, nsplit, cuda_device):
 @pytest.mark.parametrize("q_thw,bh,rel,nsplit", [((8, 7, 7), 2, True, 3), ((8, 14, 14), 3, True, 3), ((8, 28, 28), 1, True, 3),
                                                   ((8, 14, 14), 2, False, 3), ((8, 14, 14), 2, True, 1)])
 def test_fused_attention_backward_ds(q_thw, bh, rel, nsplit, cuda_device):
-    """sfb_attn_bwd_ds (csrc/attn_fused.cu): dP = dO v^T in TMEM, dS = P (dP - sum_k P dP) as planes, and the gradient of the
-    decomposed rel-pos bias dRQ (the transpose of the forward's selector product on the tensor core), against fp64 on the
+    """sfb_attn_bwd_ds (csrc/attn_fused.cu): dP = dO v^T in shared memory, dS = P (dP - sum_k P dP) as planes, and the gradient of the
+    decomposed rel-pos bias dRQ, against fp64 on the
     operand values the kernel saw."""
     from slowfast_b200 import lib as L
     lib, dev = L.load(), cuda_device
@@ -470,9 +467,6 @@ def test_fused_attention_backward_ds(q_thw, bh, rel, nsplit, cuda_device):
     d.p_hi, d.p_lo, d.p_pitch = ph.data_ptr(), plo.data_ptr(), Nkp
     d.ds_hi, d.ds_lo, d.ds_pitch = ds_hi.data_ptr(), (ds_lo.data_ptr() if nsplit == 3 else None), Nkp
     d.drq, d.rq_pitch = (drq.data_ptr() if rel else None), Ltp
-    e_sel = torch.empty(int(lib.sfb_attn_fwd_selector_bytes()) // 2, dtype=torch.bfloat16, device=dev)
-    L.check(lib.sfb_attn_fwd_selector(e_sel.data_ptr(), kt, kh, kw, _st()), "sfb_attn_fwd_selector")
-    d.e_sel = e_sel.data_ptr()
     d.bh, d.nq, d.nk, d.hd = bh, Nq, Nk, hd
     d.qt, d.qh, d.qw = q_thw
     d.kt, d.kh, d.kw = k_thw
