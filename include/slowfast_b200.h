@@ -558,6 +558,27 @@ int sfb_clip_normalize_pack(const uint8_t* frames, int32_t b, int32_t t, int32_t
  * ---------------------------------------------------------------------------------------------- */
 int sfb_allreduce_flat(float* buf, int64_t count, void* nccl_comm, int32_t average, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Non-local block (nonlocal_helper.py:103-144, placed by resnet_helper.py:687-722).  The convolutions, the pooling, the
+ * affinity products and the softmax run on sfb_conv_igemm / sfb_conv_wgrad, sfb_maxpool3d_*, sfb_gemm_batched and
+ * sfb_softmax_relpos_* (rq = NULL); these are the block's remaining pieces.
+ * ---------------------------------------------------------------------------------------------- */
+/* fp32 [rows, c] (row pitch x_pitch, any column offset folded into x) + optional bias[c] -> split-bf16 planes
+ * [rows, c_out] (row pitch o_pitch), columns [c, c_out) zero; lo may be NULL.  The bias add of conv_theta / conv_phi /
+ * conv_g (:107-114, all four convs have bias=True) fused into the operand packing; without a bias it packs the d x d
+ * matrix of the dot_product path and the gradients. */
+int sfb_bias_split(const float* x, int64_t rows, int32_t c, int64_t x_pitch, const float* bias, void* hi, void* lo,
+                   int64_t o_pitch, int32_t c_out, void* stream);
+/* BatchNorm behind a conv with a bias (conv_out -> bn, :142-143), run after sfb_bn_finalize on the bias-free conv output:
+ * training: running_mean += momentum * bias (the batch mean of the biased output; normalisation is unchanged);
+ * eval: shift += scale * bias and save_mean -= bias. */
+int sfb_bn_conv_bias(const float* bias, int32_t c, float momentum, int32_t training, float* running_mean,
+                     const float* scale, float* shift, float* save_mean, void* stream);
+/* planes [rows, c] (row pitch `pitch`) -> fp32 hi + lo (row pitch out_pitch): the BN-input gradient of conv_out, whose
+ * column sum is the gradient of conv_out's bias. */
+int sfb_planes_to_f32(const void* hi, const void* lo, int64_t rows, int32_t c, int64_t pitch, float* out,
+                      int64_t out_pitch, void* stream);
+
 /* Narrow layers (C_in, C_out <= 64, taps*C_in*C_out <= max_macs) of sfb_conv_igemm on the fp32 pipes (csrc/conv_direct.cu)
  * instead of the tensor-core body: same descriptor, same results layout.  max_macs <= 0 keeps the current threshold. */
 int sfb_set_simt_smallc(int32_t enabled, int32_t max_macs);

@@ -216,6 +216,24 @@ _PRESETS = {
         "RNG_SEED": 0,
     },
 }
+# Non-local recipes (Wang et al., arXiv:1711.07971): the same backbones with Non-local blocks after res3 blocks 1, 3 and
+# res4 blocks 1, 3, 5 (slow pathway only for SlowFast); NONLOCAL.POOL keeps its default [1, 2, 2]
+_NLN_R50 = {"LOCATION": [[[]], [[1, 3]], [[1, 3, 5]], [[]]], "GROUP": [[1], [1], [1], [1]]}
+_PRESETS.update({
+    # configs/Kinetics/C2D_NLN_8x8_R50.yaml
+    "C2D_NLN_8x8_R50": dict(copy.deepcopy(_PRESETS["C2D_8x8_R50"]), NONLOCAL=dict(_NLN_R50, INSTANTIATION="softmax")),
+    # configs/Kinetics/I3D_NLN_8x8_R50.yaml
+    "I3D_NLN_8x8_R50": dict(copy.deepcopy(_PRESETS["I3D_8x8_R50"]), NONLOCAL=dict(_NLN_R50, INSTANTIATION="softmax")),
+    # configs/Kinetics/SLOW_NLN_8x8_R50.yaml
+    "SLOW_NLN_8x8_R50": dict(copy.deepcopy(_PRESETS["SLOW_8x8_R50"]),
+                             NONLOCAL=dict(_NLN_R50, INSTANTIATION="dot_product")),
+    # configs/Kinetics/SLOWFAST_NLN_8x8_R50.yaml (FUSION_KERNEL_SZ 5, not the 7 of SLOWFAST_8x8_R50.yaml)
+    "SLOWFAST_NLN_8x8_R50": dict(
+        copy.deepcopy(_PRESETS["SLOWFAST_8x8_R50"]),
+        SLOWFAST={"ALPHA": 4, "BETA_INV": 8, "FUSION_CONV_CHANNEL_RATIO": 2, "FUSION_KERNEL_SZ": 5},
+        NONLOCAL={"LOCATION": [[[], []], [[1, 3], []], [[1, 3, 5], []], [[], []]],
+                  "GROUP": [[1, 1], [1, 1], [1, 1], [1, 1]], "INSTANTIATION": "dot_product"}),
+})
 
 
 def get_cfg(preset: str | None = None, **overrides) -> Cfg:

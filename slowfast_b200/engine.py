@@ -267,15 +267,20 @@ def _t3(v) -> Tuple[int, int, int]:
 
 
 class ConvBN:
-    """nn.Conv3d (bias-free) followed by nn.BatchNorm3d, executed by the library's kernels.
+    """nn.Conv3d followed by nn.BatchNorm3d (or by nothing: ``bn=None``), executed by the library's kernels.
 
     The torch modules are parameter containers only (their ``forward`` is never called); they keep the reference's
-    ``state_dict`` names and ``_NormBase`` identity (optimizer.py:41-56, checkpoint.py, precise-BN)."""
+    ``state_dict`` names and ``_NormBase`` identity (optimizer.py:41-56, checkpoint.py, precise-BN).
 
-    def __init__(self, name: str, conv: nn.Conv3d, bn: nn.BatchNorm3d, ctx: Ctx):
-        assert conv.bias is None and conv.groups == 1 and _t3(conv.dilation) == (1, 1, 1), \
-            f"{name}: only dense, bias-free, undilated Conv3d is on this path"
+    A conv bias (the Non-local block's conv_out) never enters the conv output ``y``: train-mode batch statistics cancel
+    it, so it only moves the BN's running mean, the eval-mode shift and its own gradient (the column sum of the BN-input
+    gradient).  Without a BN the caller adds it (``ops.bias_split``) and computes its gradient."""
+
+    def __init__(self, name: str, conv: nn.Conv3d, bn: Optional[nn.BatchNorm3d], ctx: Ctx):
+        assert conv.groups == 1 and _t3(conv.dilation) == (1, 1, 1), \
+            f"{name}: only dense, undilated Conv3d is on this path"
         self.name, self.conv, self.bn, self.ctx = name, conv, bn, ctx
+        self.bias = conv.bias
         assert bn is None or bn.momentum is not None, \
             f"{name}: BatchNorm momentum=None (cumulative moving average) is not on the engine path"
         self.k, self.stride, self.pad = _t3(conv.kernel_size), _t3(conv.stride), _t3(conv.padding)
@@ -322,6 +327,9 @@ class ConvBN:
         ops.bn_finalize(stats, m_tiles, c, x.n * ot * oh * ow, bn.weight, bn.bias, bn.running_mean, bn.running_var,
                         bn.momentum if bn.momentum is not None else 0.1, bn.eps, ctx.training, self.scale,
                         self.shift, self.mean, self.invstd)
+        if self.bias is not None:
+            ops.bn_conv_bias(self.bias, c, bn.momentum if bn.momentum is not None else 0.1, ctx.training,
+                             bn.running_mean, self.scale, self.shift, self.mean)
         return y
 
     # ---------------------------------------------------------------------------------- backward
@@ -339,6 +347,12 @@ class ConvBN:
                    ctx.grad_of(bn.bias), dy, partials, coef, training=ctx.training, dres=dres,
                    dres_accumulate=dres_accumulate, c_valid=self.cout,
                    mask_affine=(self.scale, self.shift) if mask_from_y else None)
+        if self.bias is not None:
+            rows = n * ot * oh * ow
+            dyf = ctx.scratch("bias.dy", rows * c, F32).view(rows, c)
+            ops.planes_to_f32(dy, ops.f32view(dyf))
+            part = ctx.scratch("colsum.part", ops.colsum_blocks(rows) * self.cout, F32)
+            ops.colsum(dyf, rows, self.cout, ctx.grad_of(self.bias), part, pitch=c)
         self.wgrad(dy)
         if x_act is not None:
             self.dgrad(dy, x_act)

@@ -380,6 +380,12 @@ _SIGNATURES = [
     ("sfb_flat_adamw", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_int64, C.c_void_p]),
     ("sfb_hog_targets", C.c_int, [C.c_void_p] + [C.c_int32] * 9 + [C.c_void_p, C.c_void_p]),
+    ("sfb_bias_split", C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_int64, C.c_int32, C.c_void_p]),
+    ("sfb_bn_conv_bias", C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p]),
+    ("sfb_planes_to_f32", C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,
+                                    C.c_void_p]),
 ]
 
 

@@ -307,12 +307,8 @@ class B200MViT(nn.Module):
         return Planes(s.hi, s.lo, 1, 1, 1, rows, c, 0)
 
     def _colsum(self, src: torch.Tensor, rows, c, out: torch.Tensor, pitch=None, accumulate=False):
-        lib = L.load()
-        nb = lib.sfb_rowslab_blocks(rows)
-        part = self.ctx.scratch("colsum.part", nb * c, F32)
-        L.check(lib.sfb_colsum(src.data_ptr(), pitch or c, rows, c, out.data_ptr(), 1 if accumulate else 0,
-                               part.data_ptr(), _st()), "sfb_colsum")
-        ops._count(2)
+        part = self.ctx.scratch("colsum.part", ops.colsum_blocks(rows) * c, F32)
+        ops.colsum(src, rows, c, out, part, pitch=pitch, accumulate=accumulate)
 
     def _ln_fwd(self, x: torch.Tensor, x_pitch, rows, c, ln: nn.LayerNorm, out: Optional[Planes], out_f32, mean, rstd):
         lib = L.load()
@@ -336,15 +332,8 @@ class B200MViT(nn.Module):
     def _bgemm(self, a: Planes, a_shape, a_mn, b: Planes, b_shape, b_mn, m, n, k, batch, out, ldd, alpha=1.0,
                accumulate=False):
         """a_shape / b_shape = (pitch, batch_stride) in elements of the storage as laid out in memory."""
-        lib = L.load()
-        d = L.BgemmDesc()
-        d.a_hi, d.a_lo, d.lda, d.batch_stride_a, d.a_mn_major = a.hi_ptr(), a.lo_ptr(), a_shape[0], a_shape[1], int(a_mn)
-        d.b_hi, d.b_lo, d.ldb, d.batch_stride_b, d.b_mn_major = b.hi_ptr(), b.lo_ptr(), b_shape[0], b_shape[1], int(b_mn)
-        d.m, d.n, d.k, d.batch = m, n, k, batch
-        d.out, d.ldd, d.batch_stride_d = out.data_ptr(), ldd, m * ldd
-        d.alpha, d.accumulate, d.nsplit = alpha, 1 if accumulate else 0, self.ctx.nsplit
-        L.check(lib.sfb_gemm_batched(C.byref(d), _st()), "sfb_gemm_batched")
-        ops._count()
+        ops.gemm_batched(a, a_shape, a_mn, b, b_shape, b_mn, m, n, k, batch, out, ldd, alpha=alpha, accumulate=accumulate,
+                         nsplit=self.ctx.nsplit)
 
     # ================================================================================== forward program
     def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:

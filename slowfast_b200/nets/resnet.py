@@ -22,6 +22,7 @@ import torch.nn as nn
 from .. import ops
 from ..config import nsplit_of
 from ..engine import Act, ConvBN, Ctx, ModelFunction, Namespace, StemConvBN, bump_num_batches_tracked
+from ..ops import F32, Planes
 
 # depth -> blocks per stage (video_model_builder.py:38)
 STAGE_DEPTH = {18: (2, 2, 2, 2), 50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
@@ -152,14 +153,179 @@ class ResBlockModule(Namespace):
         u["a"].bwd(xa.grad_view(), xa.planes, x)
 
 
+NONLOCAL_INSTANTIATIONS = ("softmax", "dot_product")
+
+
+class NonlocalModule(Namespace):
+    """Non-local block (nonlocal_helper.py:10-144): conv_theta, conv_phi, conv_g, conv_out (1x1x1, bias=True), bn (+ pool)
+    and the engine program of one block, including the temporal group fold of resnet_helper.py:704-722.
+
+      theta = conv_theta(x);  xp = maxpool(x);  phi, g = conv_phi(xp), conv_g(xp)        (biases added while packing)
+      softmax     : O = softmax(d^-0.5 theta phi^T) g    S / P: [n*G, Nq, pad8(Nk)], kept for the backward
+      dot_product : O = (1/Nk) theta (phi^T g)           reassociated: the Nq x Nk matrix is never formed
+      out = x + bn(conv_out(O))                           no ReLU; one BN-apply pass with the residual
+
+    Channels-last, the fold of T into the batch ([n, T, ...] -> [n*G, T/G, ...]) is the same memory, so every kernel
+    simply runs on that view."""
+
+    def __init__(self, name, dim, dim_inner, pool_size, instantiation, group, ctx: Ctx, eps=1e-5, mmt=0.1):
+        super().__init__()
+        if instantiation not in NONLOCAL_INSTANTIATIONS:
+            raise NotImplementedError(f"Unknown norm type {instantiation}")
+        self.conv_theta = nn.Conv3d(dim, dim_inner, kernel_size=1, stride=1, padding=0)
+        self.conv_phi = nn.Conv3d(dim, dim_inner, kernel_size=1, stride=1, padding=0)
+        self.conv_g = nn.Conv3d(dim, dim_inner, kernel_size=1, stride=1, padding=0)
+        self.conv_out = nn.Conv3d(dim_inner, dim, kernel_size=1, stride=1, padding=0)
+        self.conv_out.zero_init = False
+        self.bn = nn.BatchNorm3d(dim, eps=eps, momentum=mmt)
+        self.bn.transform_final_bn = True
+        self.use_pool = pool_size is not None and any(s > 1 for s in pool_size)
+        self.pool_size = tuple(int(s) for s in pool_size) if pool_size is not None else None
+        if self.use_pool:
+            self.pool = nn.MaxPool3d(kernel_size=list(pool_size), stride=list(pool_size), padding=[0, 0, 0])
+        assert dim % 8 == 0 and dim_inner % 8 == 0, "Non-local widths must be multiples of 8"
+        self.instantiation = instantiation
+        self.dim, self.dim_inner, self.group = dim, dim_inner, int(group)
+        self._n = name
+        self._ctx = ctx
+        object.__setattr__(self, "_units", None)
+
+    def units(self):
+        if self._units is None:
+            n, ctx = self._n, self._ctx
+            u = {"theta": ConvBN(n + ".theta", self.conv_theta, None, ctx),
+                 "phi": ConvBN(n + ".phi", self.conv_phi, None, ctx),
+                 "g": ConvBN(n + ".g", self.conv_g, None, ctx),
+                 "out": ConvBN(n + ".out", self.conv_out, self.bn, ctx)}
+            object.__setattr__(self, "_units", u)
+        return self._units
+
+    def run_forward(self, x: Act, out: Act) -> None:
+        ctx, u, nm = self._ctx, self.units(), self._n
+        n, t, h, w = x.dims
+        c, d, grp = x.c, self.dim_inner, self.group
+        if t % grp:
+            raise ValueError(f"{nm}: NONLOCAL.GROUP {grp} does not divide the {t} frames of the block's input")
+        ng, tg = n * grp, t // grp
+        nq = tg * h * w
+        xg = Planes(x.s.hi, x.s.lo, ng, tg, h, w, c, x.c0)  # the group fold: a view of the same memory
+        th = Act(ctx.storage((nm, "theta"), n, t, h, w, d))
+        ops.bias_split(ops.f32view(u["theta"].fprop(x.planes)), self.conv_theta.bias, th.planes)
+        argmax = None
+        if self.use_pool:
+            k = self.pool_size
+            od = (tg // k[0], h // k[1], w // k[2])
+            if min(od) < 1:
+                raise ValueError(f"{nm}: pool {k} larger than the (grouped) input {(tg, h, w)}")
+            src = Act(ctx.storage((nm, "xp"), ng, *od, c))
+            argmax = ctx.buf((nm, "argmax"), (ng, *od, c), torch.uint8)
+            ops.maxpool3d_fwd(xg, src.planes, argmax, k, k, (0, 0, 0))
+        else:
+            src = x
+        sn, st, sh, sw = src.dims
+        nk = sn * st * sh * sw // ng
+        ph = Act(ctx.storage((nm, "phi"), sn, st, sh, sw, d))
+        gg = Act(ctx.storage((nm, "g"), sn, st, sh, sw, d))
+        ops.bias_split(ops.f32view(u["phi"].fprop(src.planes)), self.conv_phi.bias, ph.planes)
+        ops.bias_split(ops.f32view(u["g"].fprop(src.planes)), self.conv_g.bias, gg.planes)
+        o = ctx.scratch("nl.O", ng * nq * d, F32).view(ng * nq, d)
+        nsplit = ctx.nsplit
+        if self.instantiation == "softmax":
+            nkp = ops.pad8(nk)
+            s = ctx.scratch("nl.S", ng * nq * nkp, F32).view(ng * nq, nkp)
+            ops.gemm_batched(th.planes, (d, nq * d), False, ph.planes, (d, nk * d), False, nq, nk, d, ng, s, nkp,
+                             alpha=d ** -0.5, nsplit=nsplit)
+            ps = ctx.storage((nm, "P"), 1, 1, 1, ng * nq, nkp)
+            aux = Planes(ps.hi, ps.lo, 1, 1, 1, ng * nq, nkp, 0)
+            ops.row_softmax_planes(s, nkp, aux, ng, nq, nk)
+            # O = P g   (g MN-major: memory [n*G][Nk][d])
+            ops.gemm_batched(aux, (nkp, nq * nkp), False, gg.planes, (d, nk * d), True, nq, d, nk, ng, o, d, nsplit=nsplit)
+        else:
+            # M = phi^T g (d x d per batch entry), O = (1/Nk) theta M
+            mf = ctx.scratch("nl.M", ng * d * d, F32).view(ng * d, d)
+            ops.gemm_batched(ph.planes, (d, nk * d), True, gg.planes, (d, nk * d), True, d, d, nk, ng, mf, d,
+                             nsplit=nsplit)
+            ms = ctx.storage((nm, "M"), 1, 1, 1, ng * d, d)
+            aux = Planes(ms.hi, ms.lo, 1, 1, 1, ng * d, d, 0)
+            ops.bias_split(ops.f32view(mf), None, aux)
+            ops.gemm_batched(th.planes, (d, nq * d), False, aux, (d, d * d), True, nq, d, d, ng, o, d, alpha=1.0 / nk,
+                             nsplit=nsplit)
+        oa = Act(ctx.storage((nm, "O"), n, t, h, w, d))
+        ops.bias_split(ops.f32view(o), None, oa.planes)
+        yo = u["out"].fprop(oa.planes)
+        ops.bn_apply(ops.f32view(yo), u["out"].scale, u["out"].shift, out.planes, relu=False, res=x.planes)
+        object.__setattr__(self, "_saved", (x, out, xg, th, src, argmax, ph, gg, aux, oa, ng, nq, nk))
+
+    def run_backward(self) -> None:
+        """Consumes out.grad, accumulates into x.grad and writes every parameter gradient of the block."""
+        ctx, u = self._ctx, self.units()
+        x, out, xg, th, src, argmax, ph, gg, aux, oa, ng, nq, nk = self._saved
+        d, nsplit = self.dim_inner, ctx.nsplit
+        # identity path + conv_out: dres = dout (no ReLU), dO = conv_out dgrad of the BN-input gradient
+        acc = x.s.grad_written
+        u["out"].bwd(out.grad_view(), None, oa, dres=x.grad_view(), dres_accumulate=acc)
+        x.s.grad_written = True
+        do = ctx.scratch_planes("nl.dO", 1, 1, 1, ng * nq, d)
+        ops.bias_split(ops.f32view(oa.s.grad.view(ng * nq, d)), None, do)
+        dth = ctx.scratch("nl.dth", ng * nq * d, F32).view(ng * nq, d)
+        dph = ctx.scratch("nl.dphi", ng * nk * d, F32).view(ng * nk, d)
+        dg = ctx.scratch("nl.dg", ng * nk * d, F32).view(ng * nk, d)
+        if self.instantiation == "softmax":
+            nkp = aux.pitch
+            dp = ctx.scratch("nl.S", ng * nq * nkp, F32).view(ng * nq, nkp)
+            ops.gemm_batched(do, (d, nq * d), False, gg.planes, (d, nk * d), False, nq, nk, d, ng, dp, nkp, nsplit=nsplit)
+            ds = ctx.scratch_planes("nl.dS", 1, 1, 1, ng * nq, nkp)
+            ops.row_softmax_planes_bwd(aux, dp, nkp, ds, ng, nq, nk)
+            a = d ** -0.5
+            # d theta = a dS phi;  d phi = a dS^T theta;  dg = P^T dO
+            ops.gemm_batched(ds, (nkp, nq * nkp), False, ph.planes, (d, nk * d), True, nq, d, nk, ng, dth, d, alpha=a,
+                             nsplit=nsplit)
+            ops.gemm_batched(ds, (nkp, nq * nkp), True, th.planes, (d, nq * d), True, nk, d, nq, ng, dph, d, alpha=a,
+                             nsplit=nsplit)
+            ops.gemm_batched(aux, (nkp, nq * nkp), True, do, (d, nq * d), True, nk, d, nq, ng, dg, d, nsplit=nsplit)
+        else:
+            s = 1.0 / nk
+            # d theta = s dO M^T;  dM = s theta^T dO;  d phi = g dM^T;  dg = phi dM
+            ops.gemm_batched(do, (d, nq * d), False, aux, (d, d * d), False, nq, d, d, ng, dth, d, alpha=s, nsplit=nsplit)
+            dmf = ctx.scratch("nl.M", ng * d * d, F32).view(ng * d, d)
+            ops.gemm_batched(th.planes, (d, nq * d), True, do, (d, nq * d), True, d, d, nq, ng, dmf, d, alpha=s,
+                             nsplit=nsplit)
+            dm = ctx.scratch_planes("nl.dM", 1, 1, 1, ng * d, d)
+            ops.bias_split(ops.f32view(dmf), None, dm)
+            ops.gemm_batched(gg.planes, (d, nk * d), False, dm, (d, d * d), False, nk, d, d, ng, dph, d, nsplit=nsplit)
+            ops.gemm_batched(ph.planes, (d, nk * d), False, dm, (d, d * d), True, nk, d, d, ng, dg, d, nsplit=nsplit)
+        for conv, gm in ((self.conv_theta, dth), (self.conv_phi, dph), (self.conv_g, dg)):
+            part = ctx.scratch("colsum.part", ops.colsum_blocks(gm.shape[0]) * d, F32)
+            ops.colsum(gm, gm.shape[0], d, ctx.grad_of(conv.bias), part)
+        n, t, h, w = x.dims
+        dthp = ctx.scratch_planes("nl.dthp", n, t, h, w, d)
+        dphp = ctx.scratch_planes("nl.dphip", *src.dims, d)
+        dgp = ctx.scratch_planes("nl.dgp", *src.dims, d)
+        ops.bias_split(ops.f32view(dth), None, dthp)
+        ops.bias_split(ops.f32view(dph), None, dphp)
+        ops.bias_split(ops.f32view(dg), None, dgp)
+        u["theta"].wgrad(dthp)
+        u["theta"].dgrad(dthp, x)
+        u["phi"].wgrad(dphp)
+        u["g"].wgrad(dgp)
+        u["phi"].dgrad(dphp, src)
+        u["g"].dgrad(dgp, src)
+        if self.use_pool:
+            k = self.pool_size
+            ops.maxpool3d_bwd(src.grad_view(), argmax, xg, src.dims[1:], x.grad_view(), k, k, (0, 0, 0), accumulate=True)
+
+
 class StageModule(Namespace):
-    """ResStage container: pathway{p}_res{i} blocks."""
+    """ResStage container: pathway{p}_res{i} blocks, each optionally followed by pathway{p}_nonlocal{i}
+    (resnet_helper.py:666-695)."""
 
     def __init__(self, name, dim_in, dim_out, dim_inner, temp_kernel_sizes, stride, num_blocks, num_block_temp_kernel,
-                 stride_1x1, ctx: Ctx):
+                 stride_1x1, ctx: Ctx, nonlocal_inds=None, nonlocal_pool=None, nonlocal_group=None,
+                 instantiation="softmax"):
         super().__init__()
         self.num_pathways = len(num_blocks)
         self.num_blocks = list(num_blocks)
+        nonlocal_inds = nonlocal_inds or [[] for _ in num_blocks]
         for p in range(self.num_pathways):
             tks = (temp_kernel_sizes[p] * num_blocks[p])[:num_block_temp_kernel[p]] + \
                 [1] * (num_blocks[p] - num_block_temp_kernel[p])
@@ -167,9 +333,33 @@ class StageModule(Namespace):
                 blk = ResBlockModule(f"{name}.pathway{p}_res{i}", dim_in[p] if i == 0 else dim_out[p], dim_out[p],
                                      tks[i], stride[p] if i == 0 else 1, dim_inner[p], stride_1x1, ctx)
                 self.add_module(f"pathway{p}_res{i}", blk)
+                if i in nonlocal_inds[p]:
+                    nln = NonlocalModule(f"{name}.pathway{p}_nonlocal{i}", dim_out[p], dim_out[p] // 2, nonlocal_pool[p],
+                                         instantiation, nonlocal_group[p], ctx)
+                    self.add_module(f"pathway{p}_nonlocal{i}", nln)
 
     def blocks(self, p) -> List[ResBlockModule]:
         return [getattr(self, f"pathway{p}_res{i}") for i in range(self.num_blocks[p])]
+
+    def nonlocal_after(self, p, i) -> Optional[NonlocalModule]:
+        return getattr(self, f"pathway{p}_nonlocal{i}", None)
+
+    def run_block_forward(self, p, i, x: Act, out: Act, key) -> None:
+        """pathway{p}_res{i} (+ its Non-local block) from x into out; ``key`` names the intermediate storage."""
+        blk, nln = self.blocks(p)[i], self.nonlocal_after(p, i)
+        if nln is None:
+            blk.run_forward(x, out)
+            return
+        n, t, h, w = out.dims
+        mid = Act(blk._ctx.storage(key + ("nl_in",), n, t, h, w, out.c))
+        blk.run_forward(x, mid)
+        nln.run_forward(mid, out)
+
+    def run_block_backward(self, p, i) -> None:
+        nln = self.nonlocal_after(p, i)
+        if nln is not None:
+            nln.run_backward()
+        self.blocks(p)[i].run_backward()
 
 
 class BasicHeadModule(Namespace):
@@ -200,6 +390,8 @@ def init_resnet_weights(model: nn.Module, fc_init_std, zero_init_final_bn, zero_
                 m.weight.data.zero_()
             else:
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
+                if m.bias is not None:  # (the Non-local convs; c2_msra_fill zeroes the bias)
+                    m.bias.data.zero_()
         elif isinstance(m, (nn.BatchNorm3d, nn.BatchNorm2d, nn.BatchNorm1d)):
             zero = getattr(m, "transform_final_bn", False) and zero_init_final_bn
             if m.weight is not None:
@@ -231,7 +423,6 @@ class _VideoResNetBase(nn.Module):
         assert cfg.RESNET.TRANS_FUNC == "bottleneck_transform"
         assert cfg.RESNET.NUM_GROUPS == 1
         assert not cfg.DETECTION.ENABLE, "RoI head is out of scope"
-        assert all(len(l) == 0 for st in cfg.NONLOCAL.LOCATION for l in st), "Nonlocal blocks are out of scope"
         assert all(d == 1 for st in cfg.RESNET.SPATIAL_DILATIONS for d in st)
         assert float(cfg.MODEL.DROPCONNECT_RATE) == 0.0 or True  # drop-connect is a no-op in the reference (§3.3)
 
@@ -383,7 +574,9 @@ class B200SlowFast(_VideoResNetBase):
                 f"s{i + 2}", dim_in=[prev + prev // out_dim_ratio, prev // beta_inv], dim_out=[wd, wd // beta_inv],
                 dim_inner=[dim_inner * (2 ** i), dim_inner * (2 ** i) // beta_inv], temp_kernel_sizes=tk[i + 1],
                 stride=cfg.RESNET.SPATIAL_STRIDES[i], num_blocks=[dp] * 2,
-                num_block_temp_kernel=cfg.RESNET.NUM_BLOCK_TEMP_KERNEL[i], stride_1x1=cfg.RESNET.STRIDE_1X1, ctx=ctx)
+                num_block_temp_kernel=cfg.RESNET.NUM_BLOCK_TEMP_KERNEL[i], stride_1x1=cfg.RESNET.STRIDE_1X1, ctx=ctx,
+                nonlocal_inds=cfg.NONLOCAL.LOCATION[i], nonlocal_pool=cfg.NONLOCAL.POOL[i],
+                nonlocal_group=cfg.NONLOCAL.GROUP[i], instantiation=cfg.NONLOCAL.INSTANTIATION)
             self.add_module(f"s{i + 2}", st)
             if i < 3:
                 self.add_module(f"s{i + 2}_fuse", FuseModule(wd // beta_inv, ratio, fk, alpha))
@@ -461,7 +654,7 @@ class B200SlowFast(_VideoResNetBase):
                     else:
                         full = None
                         out = Act(ctx.storage((f"s{i}", p, bi), n, t, h, w, cout))
-                    blk.run_forward(x, out)
+                    stage.run_block_forward(p, bi, x, out, (f"s{i}", p, bi))
                     x = full if full is not None else out
                 outs.append(x)
             slow, fast = outs
@@ -496,8 +689,8 @@ class B200SlowFast(_VideoResNetBase):
                 fast, out = self._fuse_saved[i]
                 u[f"fuse{i}"].bwd(out.grad_view(), out.planes, fast)
             for p in (0, 1):
-                for blk in reversed(stage.blocks(p)):
-                    blk.run_backward()
+                for bi in reversed(range(stage.num_blocks[p])):
+                    stage.run_block_backward(p, bi)
         fast, out = self._fuse_saved[1]
         u["fuse1"].bwd(out.grad_view(), out.planes, fast)
         self._stem_backward(0, u["stem0"])

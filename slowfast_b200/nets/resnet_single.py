@@ -42,7 +42,9 @@ class B200ResNet(_VideoResNetBase):
             st = StageModule(f"s{i + 2}", dim_in=[prev], dim_out=[wd], dim_inner=[dim_inner * (2 ** i)],
                              temp_kernel_sizes=tk[i + 1], stride=cfg.RESNET.SPATIAL_STRIDES[i], num_blocks=[dp],
                              num_block_temp_kernel=cfg.RESNET.NUM_BLOCK_TEMP_KERNEL[i],
-                             stride_1x1=cfg.RESNET.STRIDE_1X1, ctx=ctx)
+                             stride_1x1=cfg.RESNET.STRIDE_1X1, ctx=ctx, nonlocal_inds=cfg.NONLOCAL.LOCATION[i],
+                             nonlocal_pool=cfg.NONLOCAL.POOL[i], nonlocal_group=cfg.NONLOCAL.GROUP[i],
+                             instantiation=cfg.NONLOCAL.INSTANTIATION)
             self.add_module(f"s{i + 2}", st)
             if i == 0:
                 self.add_module("pathway0_pool", nn.MaxPool3d(kernel_size=list(self._pool1), stride=list(self._pool1),
@@ -92,7 +94,7 @@ class B200ResNet(_VideoResNetBase):
             for bi, blk in enumerate(stage.blocks(0)):
                 tt, hh, ww = blk.out_dims(*cur.dims[1:])
                 out = Act(ctx.storage((f"s{i}", 0, bi), n, tt, hh, ww, blk._dim_out))
-                blk.run_forward(cur, out)
+                stage.run_block_forward(0, bi, cur, out, (f"s{i}", 0, bi))
                 cur = out
             if i == 2 and self._pool1 != (1, 1, 1):
                 k = self._pool1
@@ -123,8 +125,9 @@ class B200ResNet(_VideoResNetBase):
                 ops.maxpool3d_bwd(pooled.grad_view(), argmax, src.planes, pooled.dims[1:], src.grad_view(), k, k,
                                   (0, 0, 0))
                 src.s.grad_written = True
-            for blk in reversed(getattr(self, f"s{i}").blocks(0)):
-                blk.run_backward()
+            stage: StageModule = getattr(self, f"s{i}")
+            for bi in reversed(range(stage.num_blocks[0])):
+                stage.run_block_backward(0, bi)
         self._stem_backward(0, u["stem0"])
         ctx.end_phase()
         return [ctx.grad_of(p) for p in params]

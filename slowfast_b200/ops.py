@@ -617,6 +617,91 @@ def stem8_wgrad(x: Planes, dy: Planes, g: StemGeom, dwm: torch.Tensor, nsplit: i
     _count()
 
 
+# ------------------------------------------------------------------------------------------------ row / batched-GEMM pieces
+def colsum_blocks(rows: int) -> int:
+    """Row slabs of ``colsum``'s partial sums (first extent of its ``partials`` scratch)."""
+    return int(L.load().sfb_rowslab_blocks(rows))
+
+
+def colsum(src: torch.Tensor, rows: int, c: int, out: torch.Tensor, partials: torch.Tensor, pitch: Optional[int] = None,
+           accumulate: bool = False) -> None:
+    """out[c] (= or +=) column sums of the fp32 matrix src[rows, c] (row pitch ``pitch``): bias gradients.
+    ``partials``: fp32 scratch of at least colsum_blocks(rows) * c elements."""
+    lib = L.load()
+    assert partials.numel() >= colsum_blocks(rows) * c
+    L.check(lib.sfb_colsum(src.data_ptr(), pitch or c, rows, c, out.data_ptr(), 1 if accumulate else 0,
+                           partials.data_ptr(), _stream()), "sfb_colsum")
+    _count(2)
+
+
+def gemm_batched(a: Planes, a_shape, a_mn: bool, b: Planes, b_shape, b_mn: bool, m: int, n: int, k: int, batch: int,
+                 out: torch.Tensor, ldd: int, alpha: float = 1.0, accumulate: bool = False, nsplit: int = 3) -> None:
+    """out[b](m, n) (+)= alpha * sum_k A[b](m, k) * B[b](n, k) (csrc/gemm_batched.cu); a_shape / b_shape = (pitch,
+    batch stride) in elements of the operand planes as laid out in memory, *_mn: operand stored MN-major."""
+    lib = L.load()
+    d = L.BgemmDesc()
+    d.a_hi, d.a_lo, d.lda, d.batch_stride_a, d.a_mn_major = a.hi_ptr(), a.lo_ptr(), a_shape[0], a_shape[1], int(a_mn)
+    d.b_hi, d.b_lo, d.ldb, d.batch_stride_b, d.b_mn_major = b.hi_ptr(), b.lo_ptr(), b_shape[0], b_shape[1], int(b_mn)
+    d.m, d.n, d.k, d.batch = m, n, k, batch
+    d.out, d.ldd, d.batch_stride_d = out.data_ptr(), ldd, m * ldd
+    d.alpha, d.accumulate, d.nsplit = alpha, 1 if accumulate else 0, nsplit
+    L.check(lib.sfb_gemm_batched(C.byref(d), _stream()), "sfb_gemm_batched")
+    _count()
+
+
+def row_softmax_planes(s: torch.Tensor, s_pitch: int, p: Planes, batch: int, nq: int, nk: int) -> None:
+    """P = softmax over the nk keys of every row of S [batch * nq, s_pitch] -> planes (pad columns zero): the
+    softmax_relpos kernel without a bias."""
+    lib = L.load()
+    d = L.SoftmaxDesc()
+    d.s, d.s_pitch = s.data_ptr(), s_pitch
+    d.p_hi, d.p_lo, d.p_pitch = p.hi_ptr(), p.lo_ptr(), p.pitch
+    d.bh, d.nq, d.nk = batch, nq, nk
+    d.qt = d.qh = d.qw = d.kt = d.kh = d.kw = 1
+    L.check(lib.sfb_softmax_relpos_fwd(C.byref(d), _stream()), "sfb_softmax_relpos_fwd")
+    _count()
+
+
+def row_softmax_planes_bwd(p: Planes, dp: torch.Tensor, dp_pitch: int, ds: Planes, batch: int, nq: int, nk: int) -> None:
+    """dS = P * (dP - sum_k P dP) -> planes (pad columns zero)."""
+    lib = L.load()
+    d = L.SoftmaxDesc()
+    d.p_hi, d.p_lo, d.p_pitch = p.hi_ptr(), p.lo_ptr(), p.pitch
+    d.dp, d.dp_pitch = dp.data_ptr(), dp_pitch
+    d.ds_hi, d.ds_lo, d.ds_pitch = ds.hi_ptr(), ds.lo_ptr(), ds.pitch
+    d.bh, d.nq, d.nk = batch, nq, nk
+    d.qt = d.qh = d.qw = d.kt = d.kh = d.kw = 1
+    L.check(lib.sfb_softmax_relpos_bwd(C.byref(d), _stream()), "sfb_softmax_relpos_bwd")
+    _count()
+
+
+def bias_split(x: F32View, bias: Optional[torch.Tensor], out: Planes) -> None:
+    """planes[rows, out.c] = x[rows, x.c] (+ bias), columns past x.c zero (csrc/nonlocal.cu)."""
+    lib = L.load()
+    assert x.rows == out.rows and x.c <= out.c
+    assert bias is None or (bias.is_contiguous() and bias.numel() == x.c)
+    L.check(lib.sfb_bias_split(x.ptr(), x.rows, x.c, x.pitch, _ptr(bias), out.hi_ptr(), out.lo_ptr(), out.pitch, out.c,
+                               _stream()), "sfb_bias_split")
+    _count()
+
+
+def bn_conv_bias(bias: torch.Tensor, c: int, momentum: float, training: bool, running_mean, scale, shift,
+                 save_mean) -> None:
+    """Fold a conv bias into the BatchNorm that follows it, after ``bn_finalize`` (csrc/nonlocal.cu)."""
+    lib = L.load()
+    L.check(lib.sfb_bn_conv_bias(bias.data_ptr(), c, momentum, 1 if training else 0, _ptr(running_mean), _ptr(scale),
+                                 _ptr(shift), _ptr(save_mean), _stream()), "sfb_bn_conv_bias")
+    _count()
+
+
+def planes_to_f32(x: Planes, out: F32View) -> None:
+    lib = L.load()
+    assert out.rows == x.rows and out.c == x.c
+    L.check(lib.sfb_planes_to_f32(x.hi_ptr(), x.lo_ptr(), x.rows, x.c, x.pitch, out.ptr(), out.pitch, _stream()),
+            "sfb_planes_to_f32")
+    _count()
+
+
 # ------------------------------------------------------------------------------------------------ generic max pool
 def _pool3d_desc(x: Planes, out_dims, k, s, p):
     d = L.Pool3dDesc()
