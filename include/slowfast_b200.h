@@ -144,7 +144,24 @@ int sfb_filter_unpack_grad(const float* dwm, float* dw, int32_t cout, int32_t ci
 int sfb_bn_finalize(const float* partials, int32_t m_tiles, int32_t c, int64_t count, const float* gamma,
                     const float* beta, float* running_mean, float* running_var, float momentum, float eps,
                     int32_t training, float* scale, float* shift, float* save_mean, float* save_invstd,
-                    void* stream);
+                    int32_t affine_c, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * SubBatchNorm3d (batchnorm_helper.py:40-112; BN.NORM_TYPE sub_batchnorm, multigrid's long cycle).  In training,
+ * x.view(n // S, C*S, t, h, w) -> split_bn puts clip k in split s = k % S, and its channel c is split_bn channel s*C + c.
+ * Every split-aware entry takes (splits, rows_per_clip): row r of a channels-last activation belongs to clip
+ * r / rows_per_clip, so to split (r / rows_per_clip) % splits, and uses row s of the [splits][C] coefficient tables.
+ * splits <= 1 is the plain BatchNorm path, unchanged.
+ *
+ * Statistics: one pass over the conv output y (the conv runs with stats = NULL) writes [2][S*C][tiles] partials,
+ * tiles = sfb_bn_split_stats_tiles(rows, rows_per_clip, S, C), no block straddling a clip.  sfb_bn_finalize then reduces
+ * them as S*C channels (count rows / S) against split_bn's running statistics, with affine_c = C so that every split
+ * reads the container's shared gamma / beta; scale / shift / save_mean / save_invstd come out as [S][C] tables.
+ * affine_c <= 0 means c (one affine per channel).
+ * ---------------------------------------------------------------------------------------------- */
+int32_t sfb_bn_split_stats_tiles(int64_t rows, int64_t rows_per_clip, int32_t splits, int32_t c);
+int sfb_bn_split_stats(const float* y, int64_t y_pitch, int64_t rows, int32_t c, int32_t splits, int64_t rows_per_clip,
+                       float* partials, void* stream);
 
 /* out = act( y*scale + shift [+ y2*scale2 + shift2] [+ residual planes] ) written as split planes.
  * Covers BN+ReLU (a_bn/b_bn), the block tail relu(x + c_bn(..)) and relu(branch1_bn(..) + c_bn(..))
@@ -156,6 +173,7 @@ typedef struct sfb_bn_apply_desc {
   const void* res_hi; const void* res_lo; int64_t res_pitch;                    /* optional identity residual */
   void* out_hi; void* out_lo; int64_t out_pitch;
   int64_t rows; int32_t c; int32_t relu;
+  int32_t splits; int64_t rows_per_clip; /* splits > 1: scale/shift (and scale2/shift2) are [splits][c] tables */
 } sfb_bn_apply_desc;
 int sfb_bn_apply(const sfb_bn_apply_desc* d, void* stream);
 
@@ -172,15 +190,19 @@ typedef struct sfb_bn_bwd_desc {
   int32_t training;
   void* dy_hi; void* dy_lo; int64_t dy_pitch;
   float* dres; int64_t dres_pitch; int32_t dres_accumulate;
-  float* partials; /* scratch [sfb_bn_bwd_blocks(rows,c)][2][c] */
-  float* coef;     /* scratch [3][c] */
+  float* partials; /* scratch [sfb_bn_bwd_blocks(rows, c, splits, rows_per_clip)][2][c] */
+  float* coef;     /* scratch [3][splits][c] */
   int64_t rows; int32_t c;
   int32_t c_valid; /* channels >= c_valid (> 0) are padding: zero coefficients, no parameter-gradient writes */
   /* alternative to mask_hi when the post-ReLU planes were never materialised (X3D: fused into the channelwise conv):
    * the ReLU mask is recomputed as y*mask_scale + mask_shift > 0 (the forward BN affine) */
   const float* mask_scale; const float* mask_shift;
+  /* splits > 1: mean / invstd / mask_scale / mask_shift are [splits][c] tables; the sums are reduced per (split,
+   * channel) with no reduce block mixing splits, dy uses its split's statistics, and dgamma / dbeta are the sums over
+   * all splits (gamma is shared) */
+  int32_t splits; int64_t rows_per_clip;
 } sfb_bn_bwd_desc;
-int32_t sfb_bn_bwd_blocks(int64_t rows, int32_t c);
+int32_t sfb_bn_bwd_blocks(int64_t rows, int32_t c, int32_t splits, int64_t rows_per_clip);
 int sfb_bn_bwd(const sfb_bn_bwd_desc* d, void* stream);
 
 /* Stem tail: BN -> ReLU -> MaxPool3d [1,kh,kw] stride [1,sh,sw] pad [0,ph,pw] (stem_helper.py:190-201), fused;
@@ -192,6 +214,7 @@ typedef struct sfb_pool_desc {
   uint8_t* argmax;
   const float* dout; int64_t dout_pitch; /* backward: gradient w.r.t. the pooled output */
   float* dz;                              /* backward: gradient w.r.t. relu(bn(y)), dense [n,t,h,w,c] */
+  int32_t splits;                         /* forward, > 1: scale / shift are [splits][c] tables, clip n uses row n % splits */
 } sfb_pool_desc;
 int sfb_bn_relu_maxpool_fwd(const sfb_pool_desc* d, void* stream);
 int sfb_bn_relu_maxpool_bwd(const sfb_pool_desc* d, void* stream);
@@ -571,9 +594,10 @@ int sfb_bias_split(const float* x, int64_t rows, int32_t c, int64_t x_pitch, con
                    int64_t o_pitch, int32_t c_out, void* stream);
 /* BatchNorm behind a conv with a bias (conv_out -> bn, :142-143), run after sfb_bn_finalize on the bias-free conv output:
  * training: running_mean += momentum * bias (the batch mean of the biased output; normalisation is unchanged);
- * eval: shift += scale * bias and save_mean -= bias. */
+ * eval: shift += scale * bias and save_mean -= bias.  splits > 1 (training only): running_mean is split_bn's
+ * [splits][c] and every split moves by momentum * bias. */
 int sfb_bn_conv_bias(const float* bias, int32_t c, float momentum, int32_t training, float* running_mean,
-                     const float* scale, float* shift, float* save_mean, void* stream);
+                     const float* scale, float* shift, float* save_mean, int32_t splits, void* stream);
 /* planes [rows, c] (row pitch `pitch`) -> fp32 hi + lo (row pitch out_pitch): the BN-input gradient of conv_out, whose
  * column sum is the gradient of conv_out's bias. */
 int sfb_planes_to_f32(const void* hi, const void* lo, int64_t rows, int32_t c, int64_t pitch, float* out,

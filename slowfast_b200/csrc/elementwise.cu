@@ -201,8 +201,9 @@ __global__ void filter_unpack_grad_kernel(const float* __restrict__ dwm, float* 
 // Merge the conv epilogue's per-tile (sum, sum^2) partials in fp64, produce the affine (scale, shift) the apply
 // kernel uses, save (mean, invstd) for backward and update the running statistics exactly like
 // torch.nn.BatchNorm3d in train mode (biased variance for normalisation, unbiased for running_var).
+// affine_c: period of gamma / beta.  SubBatchNorm3d finalizes its S*C split_bn channels against ONE shared [C] affine.
 __global__ void __launch_bounds__(256) bn_finalize_kernel(const float* __restrict__ partials, int m_tiles, int c,
-                                                          double count, const float* __restrict__ gamma,
+                                                          int affine_c, double count, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, float* __restrict__ running_mean,
                                                           float* __restrict__ running_var, float momentum, float eps,
                                                           int training, float* __restrict__ scale,
@@ -246,14 +247,89 @@ __global__ void __launch_bounds__(256) bn_finalize_kernel(const float* __restric
     mean_f = running_mean[ch];
     invstd_f = float(1.0 / sqrt(double(running_var[ch]) + double(eps)));
   }
-  const float g = gamma ? gamma[ch] : 1.f, b = beta ? beta[ch] : 0.f;
+  const int ca = ch % affine_c;
+  const float g = gamma ? gamma[ca] : 1.f, b = beta ? beta[ca] : 0.f;
   scale[ch] = g * invstd_f;
   shift[ch] = b - mean_f * g * invstd_f;
   if (save_mean) save_mean[ch] = mean_f;
   if (save_invstd) save_invstd[ch] = invstd_f;
 }
 
+// Training statistics of SubBatchNorm3d (batchnorm_helper.py:101-106, x.view(n // S, C*S, t, h, w)): clip k of the
+// batch is in split s = k % S and its channel c is split_bn channel s*C + c.  Every block sums one chunk of rows of ONE
+// clip, so no partial mixes splits (the conv epilogue's 128-row tiles cross clip boundaries); the partials are laid out
+// [2][S*C][blocks_per_split] (column = (k / S) * chunks + chunk), so sfb_bn_finalize reduces them as S*C channels.
+// Rows per block: 8 per row lane, at least 128 (the tile height of the conv epilogue's partials).  256 threads cover
+// min(C/8, 256) channel groups, so a narrow layer has many row lanes: C = 8 (the fast stem) takes 2048-row chunks.
+__host__ __device__ inline int64_t split_stats_chunk(int c) {
+  const int cg = c / 8;
+  const int lanes_r = 256 / (cg < 256 ? cg : 256);
+  return lanes_r * 8 > 128 ? lanes_r * 8 : 128;
+}
+struct SplitStatsParams {
+  const float* y; int64_t y_pitch;
+  int64_t rows_per_clip; int64_t chunk_rows;
+  int c, splits, chunks, blocks_per_split;
+  float* partials;
+};
+__global__ void __launch_bounds__(256) bn_split_stats_kernel(const SplitStatsParams p) {
+  extern __shared__ float sm[];  // [blockDim.x][16]
+  const int cg = p.c / 8;
+  const int lanes_c = cg < int(blockDim.x) ? cg : int(blockDim.x);
+  const int lanes_r = blockDim.x / lanes_c;
+  const int lc = threadIdx.x % lanes_c;
+  const int lr = threadIdx.x / lanes_c;
+  const int64_t clip = blockIdx.x / p.chunks;
+  const int j = int(blockIdx.x % p.chunks);
+  const int s = int(clip % p.splits);
+  const int col = int(clip / p.splits) * p.chunks + j;
+  const int64_t r0 = clip * p.rows_per_clip + j * p.chunk_rows;
+  const int64_t r1 = min(r0 + p.chunk_rows, (clip + 1) * p.rows_per_clip);
+  const int64_t sq = int64_t(p.splits) * p.c * p.blocks_per_split;  // start of the sum-of-squares half
+  for (int g0 = 0; g0 < cg; g0 += lanes_c) {
+    const int g = g0 + lc;
+    float s1[8], s2[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s1[k] = s2[k] = 0.f;
+    if (g < cg && lr < lanes_r) {
+      for (int64_t r = r0 + lr; r < r1; r += lanes_r) {
+        float v[8];
+        load8(p.y + r * p.y_pitch + g * 8, v);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          s1[k] += v[k];
+          s2[k] = fmaf(v[k], v[k], s2[k]);
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      sm[threadIdx.x * 16 + k] = s1[k];
+      sm[threadIdx.x * 16 + 8 + k] = s2[k];
+    }
+    __syncthreads();
+    if (lr == 0 && g < cg) {
+      for (int q = 1; q < lanes_r; ++q) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          s1[k] += sm[(q * lanes_c + lc) * 16 + k];
+          s2[k] += sm[(q * lanes_c + lc) * 16 + 8 + k];
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int64_t ch = int64_t(s) * p.c + g * 8 + k;
+        p.partials[ch * p.blocks_per_split + col] = s1[k];
+        p.partials[sq + ch * p.blocks_per_split + col] = s2[k];
+      }
+    }
+    __syncthreads();
+  }
+}
+
 // out = act( y*scale + shift  [+ y2*scale2 + shift2]  [+ (r_hi + r_lo)] ), written as split planes
+// splits > 1 (SubBatchNorm3d in training): the coefficient vectors are [splits][c] tables and row r uses row
+// (r / rows_per_clip) % splits of them.
 struct BnApplyParams {
   const float* y; int64_t y_pitch;
   const float* scale; const float* shift;
@@ -262,7 +338,11 @@ struct BnApplyParams {
   const __nv_bfloat16* r_hi; const __nv_bfloat16* r_lo; int64_t r_pitch;
   __nv_bfloat16* o_hi; __nv_bfloat16* o_lo; int64_t o_pitch;
   int64_t rows; int c; int relu;
+  int splits; int64_t rows_per_clip;
 };
+__device__ __forceinline__ int split_of_row(int64_t r, int64_t rows_per_clip, int splits) {
+  return int((r / rows_per_clip) % splits);
+}
 // Thread mapping of the BatchNorm elementwise passes: a thread owns ONE 8-channel group (its per-channel coefficients are
 // loaded once, outside the row loop - ncu r2c showed the L1 at 71 % busy re-reading five coefficient vectors per item) and
 // walks rows; consecutive lanes = consecutive channel groups (contiguous 32-byte pieces of a row), remaining lanes = rows.
@@ -288,7 +368,21 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const BnApplyParams p) {
       load8(p.scale2 + c, sc2);
       load8(p.shift2 + c, sh2);
     }
+    int cur = 0;  // coefficient row held in registers
     for (int64_t r = int64_t(blockIdx.x) * L.lanes_r + L.lr; r < p.rows; r += int64_t(gridDim.x) * L.lanes_r) {
+      if (p.splits > 1) {
+        const int s = split_of_row(r, p.rows_per_clip, p.splits);
+        if (s != cur) {
+          cur = s;
+          const int64_t o = int64_t(s) * p.c + c;
+          load8(p.scale + o, sc);
+          load8(p.shift + o, sh);
+          if (p.y2) {
+            load8(p.scale2 + o, sc2);
+            load8(p.shift2 + o, sh2);
+          }
+        }
+      }
       float v[8];
       load8(p.y + r * p.y_pitch + c, v);
 #pragma unroll
@@ -325,6 +419,9 @@ struct BnBwdReduceParams {
   int64_t rows; int c;
   float* partials;  // [gridDim.x][2][c]
   const float* mask_scale; const float* mask_shift;  // alternative ReLU mask: y*scale + shift > 0 (no planes kept)
+  // splits > 1: mean / invstd / mask_scale / mask_shift are [splits][c] tables and every block reduces a slab of ONE
+  // clip (blocks_per_clip slabs per clip), so its partial row belongs to split (blockIdx.x / blocks_per_clip) % splits
+  int splits; int64_t rows_per_clip; int blocks_per_clip;
 };
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdReduceParams p) {
   extern __shared__ float sm[];  // [blockDim.x][16]
@@ -334,9 +431,18 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdReducePar
   const int lanes_r = blockDim.x / lanes_c;
   const int lc = threadIdx.x % lanes_c;
   const int lr = threadIdx.x / lanes_c;
-  const int64_t rows_per_block = (p.rows + gridDim.x - 1) / gridDim.x;
-  const int64_t r0 = blockIdx.x * rows_per_block;
-  const int64_t r1 = (r0 + rows_per_block < p.rows) ? r0 + rows_per_block : p.rows;
+  int64_t r0, r1, coff = 0;
+  if (p.splits > 1) {
+    const int64_t clip = blockIdx.x / p.blocks_per_clip;
+    const int64_t rpb = (p.rows_per_clip + p.blocks_per_clip - 1) / p.blocks_per_clip;
+    r0 = clip * p.rows_per_clip + (blockIdx.x % p.blocks_per_clip) * rpb;
+    r1 = min(r0 + rpb, (clip + 1) * p.rows_per_clip);
+    coff = (clip % p.splits) * p.c;
+  } else {
+    const int64_t rows_per_block = (p.rows + gridDim.x - 1) / gridDim.x;
+    r0 = blockIdx.x * rows_per_block;
+    r1 = (r0 + rows_per_block < p.rows) ? r0 + rows_per_block : p.rows;
+  }
   for (int g0 = 0; g0 < cg; g0 += lanes_c) {
     const int g = g0 + lc;
     float s1[8], s2[8];
@@ -345,11 +451,11 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdReducePar
     if (g < cg && lr < lanes_r) {
       const int c = g * 8;
       float mu[8], is[8], msc[8], msh[8];
-      load8(p.mean + c, mu);
-      load8(p.invstd + c, is);
+      load8(p.mean + coff + c, mu);
+      load8(p.invstd + coff + c, is);
       if (p.mask_scale) {
-        load8(p.mask_scale + c, msc);
-        load8(p.mask_shift + c, msh);
+        load8(p.mask_scale + coff + c, msc);
+        load8(p.mask_shift + coff + c, msh);
       }
       for (int64_t r = r0 + lr; r < r1; r += lanes_r) {
         float d[8], yv[8];
@@ -396,43 +502,59 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdReducePar
 // merge partials -> dgamma (+=), dbeta (+=) and the two per-channel coefficients of pass 2:
 //   dy = a * dz - b - xhat * cc     with a = gamma*invstd, b = a*S1/M, cc = a*S2/M
 // In eval mode (training == 0) the statistics are constants: dy = a * dz.
+// splits > 1: the sums are taken per (split, channel) over that split's blocks (see bn_bwd_reduce_kernel), the
+// coefficients become [3][splits][c] and count is the rows of one split; gamma is shared, so dgamma / dbeta are the sums
+// over all splits.
 __global__ void __launch_bounds__(64) bn_bwd_finalize_kernel(const float* __restrict__ partials, int nblocks, int c,
                                                              double count, const float* __restrict__ gamma,
                                                              const float* __restrict__ invstd,
                                                              float* __restrict__ dgamma, float* __restrict__ dbeta,
                                                              int accumulate, int training,
-                                                             float* __restrict__ coef /* [3][c] */, int c_valid) {
+                                                             float* __restrict__ coef /* [3][splits][c] */, int c_valid,
+                                                             int splits, int blocks_per_clip) {
   // one 64-thread block per channel: the row-slab partials are merged in fp64 with a fixed (deterministic) tree
   __shared__ double sm1[64], sm2[64];
   const int ch = blockIdx.x;
+  const int sc = splits * c;
   if (ch >= c_valid) {  // padding channel: its activations and gradients are exact zeros
-    if (threadIdx.x == 0) coef[ch] = coef[c + ch] = coef[2 * c + ch] = 0.f;
+    if (threadIdx.x == 0)
+      for (int s = 0; s < splits; ++s) coef[s * c + ch] = coef[sc + s * c + ch] = coef[2 * sc + s * c + ch] = 0.f;
     return;
   }
-  double s1 = 0.0, s2 = 0.0;
-  for (int b = threadIdx.x; b < nblocks; b += 64) {
-    s1 += double(partials[size_t(b) * 2 * c + ch]);
-    s2 += double(partials[size_t(b) * 2 * c + c + ch]);
-  }
-  sm1[threadIdx.x] = s1;
-  sm2[threadIdx.x] = s2;
-  __syncthreads();
-  for (int o = 32; o > 0; o >>= 1) {
-    if (threadIdx.x < o) {
-      sm1[threadIdx.x] += sm1[threadIdx.x + o];
-      sm2[threadIdx.x] += sm2[threadIdx.x + o];
+  const int nb_split = nblocks / splits;
+  double t1 = 0.0, t2 = 0.0;
+  for (int s = 0; s < splits; ++s) {
+    double s1 = 0.0, s2 = 0.0;
+    for (int i = threadIdx.x; i < nb_split; i += 64) {
+      const int b = splits > 1 ? ((i / blocks_per_clip) * splits + s) * blocks_per_clip + i % blocks_per_clip : i;
+      s1 += double(partials[size_t(b) * 2 * c + ch]);
+      s2 += double(partials[size_t(b) * 2 * c + c + ch]);
     }
+    sm1[threadIdx.x] = s1;
+    sm2[threadIdx.x] = s2;
     __syncthreads();
+    for (int o = 32; o > 0; o >>= 1) {
+      if (threadIdx.x < o) {
+        sm1[threadIdx.x] += sm1[threadIdx.x + o];
+        sm2[threadIdx.x] += sm2[threadIdx.x + o];
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+      s1 = sm1[0];
+      s2 = sm2[0];
+      t1 += s1;
+      t2 += s2;
+      const double a = double(gamma ? gamma[ch] : 1.f) * double(invstd[s * c + ch]);
+      coef[s * c + ch] = float(a);
+      coef[sc + s * c + ch] = training ? float(a * s1 / count) : 0.f;
+      coef[2 * sc + s * c + ch] = training ? float(a * s2 / count) : 0.f;
+    }
+    __syncthreads();  // sm1 / sm2 are refilled by the next split
   }
   if (threadIdx.x != 0) return;
-  s1 = sm1[0];
-  s2 = sm2[0];
-  if (dgamma) dgamma[ch] = accumulate ? dgamma[ch] + float(s2) : float(s2);
-  if (dbeta) dbeta[ch] = accumulate ? dbeta[ch] + float(s1) : float(s1);
-  const double a = double(gamma ? gamma[ch] : 1.f) * double(invstd[ch]);
-  coef[ch] = float(a);
-  coef[c + ch] = training ? float(a * s1 / count) : 0.f;
-  coef[2 * c + ch] = training ? float(a * s2 / count) : 0.f;
+  if (dgamma) dgamma[ch] = accumulate ? dgamma[ch] + float(t2) : float(t2);
+  if (dbeta) dbeta[ch] = accumulate ? dbeta[ch] + float(t1) : float(t1);
 }
 
 // pass 2: dy = a*dz - b - xhat*cc  -> split planes for the dgrad / wgrad GEMMs; optionally also emits
@@ -446,6 +568,26 @@ struct BnBwdApplyParams {
   float* dres; int64_t dres_pitch; int dres_accumulate;
   int64_t rows; int c;
   const float* mask_scale; const float* mask_shift;
+  int splits; int64_t rows_per_clip;  // splits > 1: [splits][c] statistics / mask tables, [3][splits][c] coefficients
+};
+struct BnBwdCoef {
+  float mu[8], ca[8], cb[8], k1[8], msc[8], msh[8];
+  // dy = ca*dz - cb - (y - mu)*is*cc  =  ca*dz - (y - mu)*k1 - cb   with k1 = is*cc
+  __device__ __forceinline__ void load(const BnBwdApplyParams& p, int s, int c) {
+    const int64_t o = int64_t(s) * p.c + c, sc = int64_t(p.splits > 1 ? p.splits : 1) * p.c;
+    float is[8], cc[8];
+    load8(p.mean + o, mu);
+    load8(p.invstd + o, is);
+    load8(p.coef + o, ca);
+    load8(p.coef + sc + o, cb);
+    load8(p.coef + 2 * sc + o, cc);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) k1[j] = is[j] * cc[j];
+    if (p.mask_scale) {
+      load8(p.mask_scale + o, msc);
+      load8(p.mask_shift + o, msh);
+    }
+  }
 };
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const BnBwdApplyParams p) {
   const int cg = p.c / 8;
@@ -453,23 +595,18 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const BnBwdApplyParam
   if (L.lr >= L.lanes_r) return;
   for (int g = L.lc; g < cg; g += L.lanes_c) {
     const int c = g * 8;
-    // dy = ca*dz - cb - (y - mu)*is*cc  =  ca*dz - (y - mu)*k1 - cb   with k1 = is*cc  (per-channel, loaded once)
-    float mu[8], ca[8], cb[8], k1[8], msc[8], msh[8];
-    {
-      float is[8], cc[8];
-      load8(p.mean + c, mu);
-      load8(p.invstd + c, is);
-      load8(p.coef + c, ca);
-      load8(p.coef + p.c + c, cb);
-      load8(p.coef + 2 * p.c + c, cc);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) k1[j] = is[j] * cc[j];
-    }
-    if (p.mask_scale) {
-      load8(p.mask_scale + c, msc);
-      load8(p.mask_shift + c, msh);
-    }
+    BnBwdCoef k;  // per-channel coefficients, loaded once per split change
+    k.load(p, 0, c);
+    float (&mu)[8] = k.mu, (&ca)[8] = k.ca, (&cb)[8] = k.cb, (&k1)[8] = k.k1, (&msc)[8] = k.msc, (&msh)[8] = k.msh;
+    int cur = 0;
     for (int64_t r = int64_t(blockIdx.x) * L.lanes_r + L.lr; r < p.rows; r += int64_t(gridDim.x) * L.lanes_r) {
+      if (p.splits > 1) {
+        const int s = split_of_row(r, p.rows_per_clip, p.splits);
+        if (s != cur) {
+          cur = s;
+          k.load(p, s, c);
+        }
+      }
       float d[8], yv[8];
       load8(p.dout + r * p.dout_pitch + c, d);
       load8(p.y + r * p.y_pitch + c, yv);
@@ -513,8 +650,10 @@ struct PoolParams {
   uint8_t* argmax;
   // backward
   const float* dout; int64_t dout_pitch; float* dz;
+  int splits;  // > 1: scale / shift are [splits][c] tables, clip n uses row n % splits
 };
-__global__ void bn_relu_maxpool_fwd_kernel(const PoolParams p) {
+// (4 blocks of 256 per SM, the occupancy this memory-bound pass had before the split index was added: <= 64 registers)
+__global__ void __launch_bounds__(256, 4) bn_relu_maxpool_fwd_kernel(const PoolParams p) {
   const int cg = p.c / 8;
   const int64_t items = int64_t(p.n) * p.t * p.oh * p.ow * cg;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
@@ -527,8 +666,9 @@ __global__ void bn_relu_maxpool_fwd_kernel(const PoolParams p) {
     const int c = g * 8;
     float sc[8], sh[8], best[8];
     uint8_t arg[8];
-    load8(p.scale + c, sc);
-    load8(p.shift + c, sh);
+    const int64_t co = p.splits > 1 ? int64_t((nt / p.t) % p.splits) * p.c + c : c;
+    load8(p.scale + co, sc);
+    load8(p.shift + co, sh);
 #pragma unroll
     for (int j = 0; j < 8; ++j) { best[j] = -INFINITY; arg[j] = 255; }
     for (int ky = 0; ky < p.kh; ++ky) {
@@ -682,15 +822,58 @@ extern "C" int sfb_filter_unpack_grad(const float* dwm, float* dw, int32_t cout,
 extern "C" int sfb_bn_finalize(const float* partials, int32_t m_tiles, int32_t c, int64_t count, const float* gamma,
                                const float* beta, float* running_mean, float* running_var, float momentum, float eps,
                                int32_t training, float* scale, float* shift, float* save_mean, float* save_invstd,
-                               void* stream) {
+                               int32_t affine_c, void* stream) {
   if (!training && (!running_mean || !running_var)) {
     set_error("sfb_bn_finalize: eval mode needs running statistics");
     return -10;
   }
-  bn_finalize_kernel<<<c, 256, 0, (cudaStream_t)stream>>>(partials, m_tiles, c, double(count), gamma,
+  if (affine_c <= 0) affine_c = c;
+  if (c % affine_c) {
+    set_error("sfb_bn_finalize: affine period %d does not divide c=%d", affine_c, c);
+    return -10;
+  }
+  bn_finalize_kernel<<<c, 256, 0, (cudaStream_t)stream>>>(partials, m_tiles, c, affine_c, double(count), gamma,
                                                                        beta, running_mean, running_var, momentum, eps,
                                                                        training, scale, shift, save_mean, save_invstd);
   SFB_LAUNCH_CHECK("sfb_bn_finalize");
+  return 0;
+}
+
+static int split_geometry_ok(const char* who, int64_t rows, int32_t splits, int64_t rows_per_clip) {
+  if (splits <= 1) return 1;
+  if (rows_per_clip <= 0 || rows % rows_per_clip || (rows / rows_per_clip) % splits) {
+    set_error("%s: %lld rows are not whole clips of %lld rows in a multiple of %d splits", who, (long long)rows,
+              (long long)rows_per_clip, splits);
+    return 0;
+  }
+  return 1;
+}
+
+extern "C" int32_t sfb_bn_split_stats_tiles(int64_t rows, int64_t rows_per_clip, int32_t splits, int32_t c) {
+  if (rows_per_clip <= 0 || splits <= 0 || c < 8) return 0;
+  const int64_t chunk = split_stats_chunk(c);
+  const int64_t chunks = (rows_per_clip + chunk - 1) / chunk;
+  return int32_t(rows / rows_per_clip / splits * chunks);
+}
+
+extern "C" int sfb_bn_split_stats(const float* y, int64_t y_pitch, int64_t rows, int32_t c, int32_t splits,
+                                  int64_t rows_per_clip, float* partials, void* stream) {
+  if (c % 8 || y_pitch % 4 || splits < 1 || rows_per_clip <= 0 || rows % rows_per_clip ||
+      (rows / rows_per_clip) % splits) {
+    set_error("sfb_bn_split_stats: c=%d (a multiple of 8), %lld rows in clips of %lld rows, %d splits", c,
+              (long long)rows, (long long)rows_per_clip, splits);
+    return -10;
+  }
+  SplitStatsParams p;
+  p.y = y; p.y_pitch = y_pitch; p.rows_per_clip = rows_per_clip; p.chunk_rows = split_stats_chunk(c);
+  p.c = c; p.splits = splits;
+  p.chunks = int((rows_per_clip + p.chunk_rows - 1) / p.chunk_rows);
+  p.blocks_per_split = sfb_bn_split_stats_tiles(rows, rows_per_clip, splits, c);
+  p.partials = partials;
+  const int64_t blocks = rows / rows_per_clip * p.chunks;
+  if (blocks == 0) return 0;
+  bn_split_stats_kernel<<<unsigned(blocks), 256, 256 * 16 * sizeof(float), (cudaStream_t)stream>>>(p);
+  SFB_LAUNCH_CHECK("sfb_bn_split_stats");
   return 0;
 }
 
@@ -699,12 +882,14 @@ extern "C" int sfb_bn_apply(const sfb_bn_apply_desc* d, void* stream) {
     set_error("sfb_bn_apply: c=%d must be a multiple of 8", d->c);
     return -10;
   }
+  if (!split_geometry_ok("sfb_bn_apply", d->rows, d->splits, d->rows_per_clip)) return -10;
   BnApplyParams p;
   p.y = d->y; p.y_pitch = d->y_pitch; p.scale = d->scale; p.shift = d->shift;
   p.y2 = d->y2; p.y2_pitch = d->y2_pitch; p.scale2 = d->scale2; p.shift2 = d->shift2;
   p.r_hi = (const bf16*)d->res_hi; p.r_lo = (const bf16*)d->res_lo; p.r_pitch = d->res_pitch;
   p.o_hi = (bf16*)d->out_hi; p.o_lo = (bf16*)d->out_lo; p.o_pitch = d->out_pitch;
   p.rows = d->rows; p.c = d->c; p.relu = d->relu;
+  p.splits = d->splits > 1 ? d->splits : 1; p.rows_per_clip = d->rows_per_clip;
   const int64_t items = d->rows * (d->c / 8);
   if (items == 0) return 0;
   bn_apply_kernel<<<rowlane_grid(d->rows, d->c / 8, 256), 256, 0, (cudaStream_t)stream>>>(p);
@@ -712,15 +897,30 @@ extern "C" int sfb_bn_apply(const sfb_bn_apply_desc* d, void* stream) {
   return 0;
 }
 
-extern "C" int32_t sfb_bn_bwd_blocks(int64_t rows, int32_t c) {
+static int64_t bn_bwd_slabs(int64_t rows) {
   // enough row slabs to fill the machine; at least 16 rows per slab (ncu r2c: 64-row slabs gave 196 blocks = 16 % active
   // warps on a 12.5 k-row layer)
   int64_t b = (rows + 15) / 16;
   const int64_t cap = int64_t(ew_sms()) * 4;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
+  return b;
+}
+
+// slabs per clip of the split reduce: about as many blocks in all as the unsplit reduce, none straddling a clip
+static int32_t bn_bwd_blocks_per_clip(int64_t rows, int64_t rows_per_clip) {
+  const int64_t clips = rows / rows_per_clip;
+  int64_t per = (bn_bwd_slabs(rows) + clips - 1) / clips;
+  const int64_t most = (rows_per_clip + 15) / 16;
+  if (per > most) per = most;
+  return int32_t(per < 1 ? 1 : per);
+}
+
+extern "C" int32_t sfb_bn_bwd_blocks(int64_t rows, int32_t c, int32_t splits, int64_t rows_per_clip) {
   (void)c;
-  return int32_t(b);
+  if (splits > 1 && rows_per_clip > 0)
+    return int32_t(rows / rows_per_clip * bn_bwd_blocks_per_clip(rows, rows_per_clip));
+  return int32_t(bn_bwd_slabs(rows));
 }
 
 extern "C" int sfb_bn_bwd(const sfb_bn_bwd_desc* d, void* stream_) {
@@ -729,19 +929,23 @@ extern "C" int sfb_bn_bwd(const sfb_bn_bwd_desc* d, void* stream_) {
     set_error("sfb_bn_bwd: c=%d must be a multiple of 8", d->c);
     return -10;
   }
-  const int nblocks = sfb_bn_bwd_blocks(d->rows, d->c);
+  if (!split_geometry_ok("sfb_bn_bwd", d->rows, d->splits, d->rows_per_clip)) return -10;
+  const int splits = d->splits > 1 ? d->splits : 1;
+  const int nblocks = sfb_bn_bwd_blocks(d->rows, d->c, splits, d->rows_per_clip);
+  const int bpc = splits > 1 ? bn_bwd_blocks_per_clip(d->rows, d->rows_per_clip) : 1;
   BnBwdReduceParams r;
   r.dout = d->dout; r.dout_pitch = d->dout_pitch;
   r.mask = (const bf16*)d->mask_hi; r.mask_pitch = d->mask_pitch;
   r.mask_scale = d->mask_scale; r.mask_shift = d->mask_shift;
   r.y = d->y; r.y_pitch = d->y_pitch; r.mean = d->mean; r.invstd = d->invstd;
   r.rows = d->rows; r.c = d->c; r.partials = d->partials;
+  r.splits = splits; r.rows_per_clip = d->rows_per_clip; r.blocks_per_clip = bpc;
   bn_bwd_reduce_kernel<<<nblocks, 256, 256 * 16 * sizeof(float), stream>>>(r);
   SFB_LAUNCH_CHECK("sfb_bn_bwd(reduce)");
-  bn_bwd_finalize_kernel<<<d->c, 64, 0, stream>>>(d->partials, nblocks, d->c, double(d->rows), d->gamma,
+  bn_bwd_finalize_kernel<<<d->c, 64, 0, stream>>>(d->partials, nblocks, d->c, double(d->rows / splits), d->gamma,
                                                                  d->invstd, d->dgamma, d->dbeta, d->accumulate_param_grads,
                                                                  d->training, d->coef,
-                                                                 d->c_valid > 0 ? d->c_valid : d->c);
+                                                                 d->c_valid > 0 ? d->c_valid : d->c, splits, bpc);
   SFB_LAUNCH_CHECK("sfb_bn_bwd(finalize)");
   BnBwdApplyParams a;
   a.dout = d->dout; a.dout_pitch = d->dout_pitch;
@@ -751,6 +955,7 @@ extern "C" int sfb_bn_bwd(const sfb_bn_bwd_desc* d, void* stream_) {
   a.dy_hi = (bf16*)d->dy_hi; a.dy_lo = (bf16*)d->dy_lo; a.dy_pitch = d->dy_pitch;
   a.dres = d->dres; a.dres_pitch = d->dres_pitch; a.dres_accumulate = d->dres_accumulate;
   a.rows = d->rows; a.c = d->c;
+  a.splits = splits; a.rows_per_clip = d->rows_per_clip;
   const int64_t items = d->rows * (d->c / 8);
   bn_bwd_apply_kernel<<<rowlane_grid(d->rows, d->c / 8, 256), 256, 0, stream>>>(a);
   SFB_LAUNCH_CHECK("sfb_bn_bwd(apply)");
@@ -768,6 +973,11 @@ extern "C" int sfb_bn_relu_maxpool_fwd(const sfb_pool_desc* d, void* stream) {
   p.n = d->n; p.t = d->t; p.h = d->h; p.w = d->w; p.c = d->c; p.oh = d->oh; p.ow = d->ow;
   p.kh = d->kh; p.kw = d->kw; p.sh = d->sh; p.sw = d->sw; p.ph = d->ph; p.pw = d->pw;
   p.o_hi = (bf16*)d->out_hi; p.o_lo = (bf16*)d->out_lo; p.o_pitch = d->out_pitch; p.argmax = d->argmax;
+  p.splits = d->splits > 1 ? d->splits : 1;
+  if (d->n % p.splits) {
+    set_error("sfb_bn_relu_maxpool_fwd: batch %d is not a multiple of %d splits", d->n, p.splits);
+    return -10;
+  }
   const int64_t items = int64_t(d->n) * d->t * d->oh * d->ow * (d->c / 8);
   bn_relu_maxpool_fwd_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
   SFB_LAUNCH_CHECK("sfb_bn_relu_maxpool_fwd");

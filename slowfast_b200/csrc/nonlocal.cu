@@ -53,14 +53,16 @@ __global__ void bias_split_kernel(const float* __restrict__ x, int64_t rows, int
 // BatchNorm behind a biased conv, z = y + b with y the bias-free conv output the statistics were taken from:
 //   train: the batch mean of z is mean(y) + b  -> running_mean += momentum * b (normalised output unchanged)
 //   eval : (y + b - rm) * scale + beta         -> shift += scale * b, save_mean = rm - b (what the backward centres y by)
+// splits > 1 (SubBatchNorm3d in training): running_mean is split_bn's [splits][c]; every split's mean moves by b.
 __global__ void bn_conv_bias_kernel(const float* __restrict__ bias, int c, float momentum, int training,
                                     float* __restrict__ running_mean, const float* __restrict__ scale,
-                                    float* __restrict__ shift, float* __restrict__ save_mean) {
+                                    float* __restrict__ shift, float* __restrict__ save_mean, int splits) {
   const int ch = blockIdx.x * blockDim.x + threadIdx.x;
   if (ch >= c) return;
   const float b = bias[ch];
   if (training) {
-    if (running_mean) running_mean[ch] += momentum * b;
+    if (running_mean)
+      for (int s = 0; s < splits; ++s) running_mean[s * c + ch] += momentum * b;
   } else {
     shift[ch] += scale[ch] * b;
     if (save_mean) save_mean[ch] -= b;
@@ -103,13 +105,14 @@ extern "C" int sfb_bias_split(const float* x, int64_t rows, int32_t c, int64_t x
 }
 
 extern "C" int sfb_bn_conv_bias(const float* bias, int32_t c, float momentum, int32_t training, float* running_mean,
-                                const float* scale, float* shift, float* save_mean, void* stream) {
+                                const float* scale, float* shift, float* save_mean, int32_t splits, void* stream) {
   if (!bias || (!training && (!scale || !shift))) {
     set_error("sfb_bn_conv_bias: null bias, or eval mode without scale / shift");
     return -10;
   }
+  if (!training) splits = 1;  // eval uses the single BN's statistics
   bn_conv_bias_kernel<<<(c + 255) / 256, 256, 0, (cudaStream_t)stream>>>(bias, c, momentum, training, running_mean, scale,
-                                                                         shift, save_mean);
+                                                                         shift, save_mean, splits > 1 ? splits : 1);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error("sfb_bn_conv_bias launch failed: %s", cudaGetErrorString(e));

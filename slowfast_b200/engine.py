@@ -23,6 +23,7 @@ import torch.nn as nn
 from . import ops
 from .conv_plan import dgrad_out_view, dgrad_plan
 from .ops import F32, F32View, Planes
+from .subbn import is_sub_bn
 
 
 class Storage:
@@ -274,15 +275,23 @@ class ConvBN:
 
     A conv bias (the Non-local block's conv_out) never enters the conv output ``y``: train-mode batch statistics cancel
     it, so it only moves the BN's running mean, the eval-mode shift and its own gradient (the column sum of the BN-input
-    gradient).  Without a BN the caller adds it (``ops.bias_split``) and computes its gradient."""
+    gradient).  Without a BN the caller adds it (``ops.bias_split``) and computes its gradient.
 
-    def __init__(self, name: str, conv: nn.Conv3d, bn: Optional[nn.BatchNorm3d], ctx: Ctx):
+    ``bn`` may be a sub-batch BN container (subbn.py): gamma / beta are the container's; a training pass takes its
+    statistics per split (``bn_split_stats``) into ``split_bn`` and emits [S][C] coefficient tables, which every
+    apply / backward kernel indexes by the split of the row's clip (``split_kw``); eval is the plain path on ``bn``."""
+
+    def __init__(self, name: str, conv: nn.Conv3d, bn: Optional[nn.Module], ctx: Ctx):
         assert conv.groups == 1 and _t3(conv.dilation) == (1, 1, 1), \
             f"{name}: only dense, undilated Conv3d is on this path"
         self.name, self.conv, self.bn, self.ctx = name, conv, bn, ctx
         self.bias = conv.bias
-        assert bn is None or bn.momentum is not None, \
+        self.sub = bn is not None and is_sub_bn(bn)
+        assert bn is None or self._stats_bn(True).momentum is not None, \
             f"{name}: BatchNorm momentum=None (cumulative moving average) is not on the engine path"
+        assert not self.sub or (bn.affine and conv.out_channels % 8 == 0), \
+            f"{name}: sub-batch BN needs an affine container and a multiple of 8 channels"
+        self.splits, self.rows_per_clip = 1, 0
         self.k, self.stride, self.pad = _t3(conv.kernel_size), _t3(conv.stride), _t3(conv.padding)
         self.cin, self.cout = conv.in_channels, conv.out_channels
         self.cin_pad = ops.pad8(self.cin)
@@ -299,6 +308,38 @@ class ConvBN:
     def out_dims(self, t, h, w):
         return tuple(ops.conv_out_size(i, k, s, p) for i, k, s, p in zip((t, h, w), self.k, self.stride, self.pad))
 
+    def _stats_bn(self, training: bool) -> nn.Module:
+        """The BatchNorm whose running statistics this pass uses: split_bn (training) / bn (eval) of a sub-batch BN."""
+        if not self.sub:
+            return self.bn
+        return self.bn.split_bn if training else self.bn.bn
+
+    @property
+    def split_kw(self) -> dict:
+        """Split geometry of the last forward, for the kernels that apply this unit's coefficients."""
+        return {"splits": self.splits, "rows_per_clip": self.rows_per_clip}
+
+    def _bn_forward(self, y: torch.Tensor, stats: Optional[torch.Tensor], m_tiles: int, cp: int, zero: bool) -> None:
+        """Finalize the BN of conv output ``y`` [n, t, h, w, cp]: scale / shift / mean / invstd ([splits][cp] tables
+        under sub-batch BN training; there the conv ran without epilogue statistics and they are taken here)."""
+        ctx, bn, c, s = self.ctx, self.bn, self.cout, self.splits
+        rows = y.numel() // y.shape[-1]
+        if s > 1:
+            m_tiles = ops.bn_split_stats_tiles(rows, self.rows_per_clip, s, c)
+            stats = ctx.buf((self.name, "stats.split"), (2, s * c, m_tiles))
+            ops.bn_split_stats(ops.f32view(y), s, self.rows_per_clip, stats)
+        self.scale = ctx.buf((self.name, "scale"), (s * cp,), zero=zero)
+        self.shift = ctx.buf((self.name, "shift"), (s * cp,), zero=zero)
+        self.mean = ctx.buf((self.name, "mean"), (s * cp,), zero=zero)
+        self.invstd = ctx.buf((self.name, "invstd"), (s * cp,), zero=zero)
+        sbn = self._stats_bn(ctx.training)
+        momentum = sbn.momentum if sbn.momentum is not None else 0.1
+        ops.bn_finalize(stats, m_tiles, s * c, rows // s, bn.weight, bn.bias, sbn.running_mean, sbn.running_var,
+                        momentum, sbn.eps, ctx.training, self.scale, self.shift, self.mean, self.invstd, affine_c=c)
+        if self.bias is not None:
+            ops.bn_conv_bias(self.bias, c, momentum, ctx.training, sbn.running_mean, self.scale, self.shift, self.mean,
+                             splits=s)
+
     def fprop(self, x: Planes) -> torch.Tensor:
         """y = conv(x) (fp32, dense channels-last) + BN statistics -> self.scale/self.shift."""
         ctx = self.ctx
@@ -312,24 +353,18 @@ class ConvBN:
         c, cp = self.cout, self.cout_pad
         y = ctx.buf((self.name, "y"), (x.n, ot, oh, ow, cp))
         m_tiles = ops.conv_m_tiles(x.n, geom)
-        stats = ctx.buf((self.name, "stats"), (2, c, m_tiles)) if (ctx.training and self.bn is not None) else None
+        self.splits = self.bn.num_splits if (self.sub and ctx.training) else 1
+        self.rows_per_clip = ot * oh * ow
+        # (sub-batch BN: the epilogue's 128-row tiles cross clips, so the statistics are a separate pass)
+        stats = ctx.buf((self.name, "stats"), (2, c, m_tiles)) \
+            if (ctx.training and self.bn is not None and self.splits == 1) else None
         # (the epilogue stores whole float4 groups: columns [c, cp) receive the zero accumulators of filter rows
         # the TMA box reads out of bounds)
         ops.conv_igemm(x, fm, geom, y, (ot * oh * ow * cp, oh * ow * cp, ow * cp, cp), stats=stats, nsplit=ctx.nsplit)
         self.x, self.geom, self.y = x, geom, y
         if self.bn is None:
             return y
-        self.scale = ctx.buf((self.name, "scale"), (cp,), zero=True)
-        self.shift = ctx.buf((self.name, "shift"), (cp,), zero=True)
-        self.mean = ctx.buf((self.name, "mean"), (cp,), zero=True)
-        self.invstd = ctx.buf((self.name, "invstd"), (cp,), zero=True)
-        bn = self.bn
-        ops.bn_finalize(stats, m_tiles, c, x.n * ot * oh * ow, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                        bn.momentum if bn.momentum is not None else 0.1, bn.eps, ctx.training, self.scale,
-                        self.shift, self.mean, self.invstd)
-        if self.bias is not None:
-            ops.bn_conv_bias(self.bias, c, bn.momentum if bn.momentum is not None else 0.1, ctx.training,
-                             bn.running_mean, self.scale, self.shift, self.mean)
+        self._bn_forward(y, stats, m_tiles, cp, zero=True)
         return y
 
     # ---------------------------------------------------------------------------------- backward
@@ -346,7 +381,7 @@ class ConvBN:
         ops.bn_bwd(dout, mask, ops.f32view(self.y), self.mean, self.invstd, bn.weight, ctx.grad_of(bn.weight),
                    ctx.grad_of(bn.bias), dy, partials, coef, training=ctx.training, dres=dres,
                    dres_accumulate=dres_accumulate, c_valid=self.cout,
-                   mask_affine=(self.scale, self.shift) if mask_from_y else None)
+                   mask_affine=(self.scale, self.shift) if mask_from_y else None, **self.split_kw)
         if self.bias is not None:
             rows = n * ot * oh * ow
             dyf = ctx.scratch("bias.dy", rows * c, F32).view(rows, c)
@@ -358,9 +393,9 @@ class ConvBN:
             self.dgrad(dy, x_act)
 
     def _bwd_scratch(self, rows, c):
-        nb = ops.L.load().sfb_bn_bwd_blocks(rows, c)
+        nb = ops.bn_bwd_blocks(rows, c, self.splits, self.rows_per_clip)
         return (self.ctx.scratch("bnb.partials", nb * 2 * c, F32).view(nb, 2, c),
-                self.ctx.scratch("bnb.coef", 3 * c, F32).view(3, c))
+                self.ctx.scratch("bnb.coef", 3 * self.splits * c, F32).view(3, self.splits * c))
 
     def wgrad(self, dy: Planes) -> None:
         ctx = self.ctx
@@ -445,6 +480,8 @@ class StemConvBN(ConvBN):
     def fprop(self, x: Planes) -> torch.Tensor:
         ctx, g = self.ctx, self.g
         c = self.cout
+        self.splits = self.bn.num_splits if (self.sub and ctx.training) else 1
+        want_stats = ctx.training and self.splits == 1  # (sub-batch BN: statistics in a separate pass)
         if self.t8:
             n, t, h, w = x.n, x.t // 2, x.h * 2, (x.w // 8 - 1) * 16
             ot, oh, ow = g.out_dims(t, h, w)
@@ -453,7 +490,7 @@ class StemConvBN(ConvBN):
             ops.stem8_filter_fold(self.conv.weight, f, flo)
             y = ctx.buf((self.name, "y"), (n, ot, oh, ow, c))
             m_tiles = ops.stem8_m_tiles(x, g)
-            stats = ctx.buf((self.name, "stats8"), (2, c, m_tiles)) if ctx.training else None
+            stats = ctx.buf((self.name, "stats8"), (2, c, m_tiles)) if want_stats else None
             ops.stem8_fprop(x, f, flo, g, y, stats, nsplit=ctx.nsplit)
         else:
             n = x.n
@@ -464,16 +501,10 @@ class StemConvBN(ConvBN):
             ops.stem_filter_fold(self.conv.weight, g, fm)
             y = ctx.buf((self.name, "y"), (n, ot, oh, ow, c))
             m_tiles = ops.stem_m_tiles(x, g)
-            stats = ctx.buf((self.name, "stats"), (2, c, m_tiles)) if ctx.training else None
+            stats = ctx.buf((self.name, "stats"), (2, c, m_tiles)) if want_stats else None
             ops.stem_fprop(x, fm, g, y, stats, nsplit=ctx.nsplit)
-        self.scale = ctx.buf((self.name, "scale"), (c,))
-        self.shift = ctx.buf((self.name, "shift"), (c,))
-        self.mean = ctx.buf((self.name, "mean"), (c,))
-        self.invstd = ctx.buf((self.name, "invstd"), (c,))
-        bn = self.bn
-        ops.bn_finalize(stats, m_tiles, c, n * ot * oh * ow, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                        bn.momentum if bn.momentum is not None else 0.1, bn.eps, ctx.training, self.scale,
-                        self.shift, self.mean, self.invstd)
+        self.rows_per_clip = ot * oh * ow
+        self._bn_forward(y, stats, m_tiles, c, zero=False)
         self.x, self.y = x, y
         return y
 

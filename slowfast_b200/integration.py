@@ -36,7 +36,12 @@ def register(replace: bool = False):
     """Register the engine models in the reference's MODEL_REGISTRY. Returns the list of names now served by the
     engine."""
     from slowfast.models.build import MODEL_REGISTRY  # the reference's registry object
+    from slowfast.models.batchnorm_helper import SubBatchNorm3d
+    from . import subbn
 
+    # BN.NORM_TYPE sub_batchnorm: build the reference's own container class (only its parameters and buffers are used,
+    # never its forward), so that the unmodified misc.aggregate_sub_bn_stats - an isinstance check - finds it
+    subbn.SUB_BN_CLASS = SubBatchNorm3d
     served = []
     for ref_name, spec in ENGINE_CLASSES.items():
         cls = _resolve(spec)

@@ -63,6 +63,7 @@ class BnApplyDesc(C.Structure):
         ("res_hi", C.c_void_p), ("res_lo", C.c_void_p), ("res_pitch", C.c_int64),
         ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("out_pitch", C.c_int64),
         ("rows", C.c_int64), ("c", C.c_int32), ("relu", C.c_int32),
+        ("splits", C.c_int32), ("rows_per_clip", C.c_int64),
     ]
 
 
@@ -79,6 +80,7 @@ class BnBwdDesc(C.Structure):
         ("partials", C.c_void_p), ("coef", C.c_void_p),
         ("rows", C.c_int64), ("c", C.c_int32), ("c_valid", C.c_int32),
         ("mask_scale", C.c_void_p), ("mask_shift", C.c_void_p),
+        ("splits", C.c_int32), ("rows_per_clip", C.c_int64),
     ]
 
 
@@ -125,6 +127,7 @@ class PoolDesc(C.Structure):
         ("argmax", C.c_void_p),
         ("dout", C.c_void_p), ("dout_pitch", C.c_int64),
         ("dz", C.c_void_p),
+        ("splits", C.c_int32),
     ]
 
 
@@ -282,9 +285,12 @@ _SIGNATURES = [
                                          C.c_int32, C.c_void_p]),
     ("sfb_bn_finalize", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_float, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                  C.c_void_p, C.c_void_p]),
+                                  C.c_void_p, C.c_int32, C.c_void_p]),
+    ("sfb_bn_split_stats_tiles", C.c_int32, [C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
+    ("sfb_bn_split_stats", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_void_p,
+                                     C.c_void_p]),
     ("sfb_bn_apply", C.c_int, [C.POINTER(BnApplyDesc), C.c_void_p]),
-    ("sfb_bn_bwd_blocks", C.c_int32, [C.c_int64, C.c_int32]),
+    ("sfb_bn_bwd_blocks", C.c_int32, [C.c_int64, C.c_int32, C.c_int32, C.c_int64]),
     ("sfb_bn_bwd", C.c_int, [C.POINTER(BnBwdDesc), C.c_void_p]),
     ("sfb_bn_relu_maxpool_fwd", C.c_int, [C.POINTER(PoolDesc), C.c_void_p]),
     ("sfb_bn_relu_maxpool_bwd", C.c_int, [C.POINTER(PoolDesc), C.c_void_p]),
@@ -383,7 +389,7 @@ _SIGNATURES = [
     ("sfb_bias_split", C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_int32, C.c_void_p]),
     ("sfb_bn_conv_bias", C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_void_p]),
+                                   C.c_void_p, C.c_int32, C.c_void_p]),
     ("sfb_planes_to_f32", C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,
                                     C.c_void_p]),
 ]

@@ -23,6 +23,7 @@ from .. import ops
 from ..config import nsplit_of
 from ..engine import Act, ConvBN, Ctx, ModelFunction, Namespace, StemConvBN, bump_num_batches_tracked
 from ..ops import F32, Planes
+from ..subbn import is_sub_bn, norm_factory, num_splits_of
 
 # depth -> blocks per stage (video_model_builder.py:38)
 STAGE_DEPTH = {18: (2, 2, 2, 2), 50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
@@ -48,12 +49,15 @@ def _conv(cin, cout, k, stride, pad):
 
 
 class StemModule(Namespace):
-    """ResNetBasicStem parameter container: conv, bn (+ inert relu / pool_layer)."""
+    """ResNetBasicStem parameter container: conv, bn (+ inert relu / pool_layer).
 
-    def __init__(self, cin, cout, k, stride, pad, eps, mmt):
+    ``norm`` (here and in every container below) builds the BN modules: nn.BatchNorm3d, or the sub-batch BN container
+    of ``subbn.norm_factory``."""
+
+    def __init__(self, cin, cout, k, stride, pad, eps, mmt, norm=nn.BatchNorm3d):
         super().__init__()
         self.conv = _conv(cin, cout, k, stride, pad)
-        self.bn = nn.BatchNorm3d(cout, eps=eps, momentum=mmt)
+        self.bn = norm(num_features=cout, eps=eps, momentum=mmt)
         self.relu = nn.ReLU(True)
         self.pool_layer = nn.MaxPool3d(kernel_size=[1, 3, 3], stride=[1, 2, 2], padding=[0, 1, 1])
 
@@ -61,40 +65,41 @@ class StemModule(Namespace):
 class FuseModule(Namespace):
     """FuseFastToSlow parameter container: conv_f2s, bn."""
 
-    def __init__(self, dim_in, ratio, kernel, alpha, eps=1e-5, mmt=0.1):
+    def __init__(self, dim_in, ratio, kernel, alpha, eps=1e-5, mmt=0.1, norm=nn.BatchNorm3d):
         super().__init__()
         self.conv_f2s = _conv(dim_in, dim_in * ratio, (kernel, 1, 1), (alpha, 1, 1), (kernel // 2, 0, 0))
-        self.bn = nn.BatchNorm3d(dim_in * ratio, eps=eps, momentum=mmt)
+        self.bn = norm(num_features=dim_in * ratio, eps=eps, momentum=mmt)
         self.relu = nn.ReLU(True)
 
 
 class BottleneckModule(Namespace):
     """BottleneckTransform parameter container: a, a_bn, b, b_bn, c, c_bn."""
 
-    def __init__(self, dim_in, dim_out, temp_k, stride, dim_inner, stride_1x1, eps, mmt):
+    def __init__(self, dim_in, dim_out, temp_k, stride, dim_inner, stride_1x1, eps, mmt, norm=nn.BatchNorm3d):
         super().__init__()
         s1, s3 = (stride, 1) if stride_1x1 else (1, stride)
         self.a = _conv(dim_in, dim_inner, (temp_k, 1, 1), (1, s1, s1), (temp_k // 2, 0, 0))
-        self.a_bn = nn.BatchNorm3d(dim_inner, eps=eps, momentum=mmt)
+        self.a_bn = norm(num_features=dim_inner, eps=eps, momentum=mmt)
         self.a_relu = nn.ReLU(True)
         self.b = _conv(dim_inner, dim_inner, (1, 3, 3), (1, s3, s3), (0, 1, 1))
-        self.b_bn = nn.BatchNorm3d(dim_inner, eps=eps, momentum=mmt)
+        self.b_bn = norm(num_features=dim_inner, eps=eps, momentum=mmt)
         self.b_relu = nn.ReLU(True)
         self.c = _conv(dim_inner, dim_out, (1, 1, 1), (1, 1, 1), (0, 0, 0))
         self.c.final_conv = True
-        self.c_bn = nn.BatchNorm3d(dim_out, eps=eps, momentum=mmt)
+        self.c_bn = norm(num_features=dim_out, eps=eps, momentum=mmt)
         self.c_bn.transform_final_bn = True
 
 
 class ResBlockModule(Namespace):
     """ResBlock parameter container (+ engine program of one bottleneck block)."""
 
-    def __init__(self, name, dim_in, dim_out, temp_k, stride, dim_inner, stride_1x1, ctx: Ctx, eps=1e-5, mmt=0.1):
+    def __init__(self, name, dim_in, dim_out, temp_k, stride, dim_inner, stride_1x1, ctx: Ctx, eps=1e-5, mmt=0.1,
+                 norm=nn.BatchNorm3d):
         super().__init__()
         if dim_in != dim_out or stride != 1:
             self.branch1 = _conv(dim_in, dim_out, (1, 1, 1), (1, stride, stride), (0, 0, 0))
-            self.branch1_bn = nn.BatchNorm3d(dim_out, eps=eps, momentum=mmt)
-        self.branch2 = BottleneckModule(dim_in, dim_out, temp_k, stride, dim_inner, stride_1x1, eps, mmt)
+            self.branch1_bn = norm(num_features=dim_out, eps=eps, momentum=mmt)
+        self.branch2 = BottleneckModule(dim_in, dim_out, temp_k, stride, dim_inner, stride_1x1, eps, mmt, norm)
         self.relu = nn.ReLU(True)
         self._n = name
         self._ctx = ctx
@@ -123,17 +128,18 @@ class ResBlockModule(Namespace):
         n, t, h, w = x.dims
         ya = u["a"].fprop(x.planes)
         xa = Act(ctx.storage((nm, "xa"), *ya.shape))
-        ops.bn_apply(ops.f32view(ya), u["a"].scale, u["a"].shift, xa.planes, relu=True)
+        ops.bn_apply(ops.f32view(ya), u["a"].scale, u["a"].shift, xa.planes, relu=True, **u["a"].split_kw)
         yb = u["b"].fprop(xa.planes)
         xb = Act(ctx.storage((nm, "xb"), *yb.shape))
-        ops.bn_apply(ops.f32view(yb), u["b"].scale, u["b"].shift, xb.planes, relu=True)
+        ops.bn_apply(ops.f32view(yb), u["b"].scale, u["b"].shift, xb.planes, relu=True, **u["b"].split_kw)
         yc = u["c"].fprop(xb.planes)
         if "s" in u:
             ys = u["s"].fprop(x.planes)
             ops.bn_apply(ops.f32view(yc), u["c"].scale, u["c"].shift, out.planes, relu=True, y2=ops.f32view(ys),
-                         scale2=u["s"].scale, shift2=u["s"].shift)
+                         scale2=u["s"].scale, shift2=u["s"].shift, **u["c"].split_kw)
         else:
-            ops.bn_apply(ops.f32view(yc), u["c"].scale, u["c"].shift, out.planes, relu=True, res=x.planes)
+            ops.bn_apply(ops.f32view(yc), u["c"].scale, u["c"].shift, out.planes, relu=True, res=x.planes,
+                         **u["c"].split_kw)
         object.__setattr__(self, "_saved", (x, xa, xb, out))
 
     def run_backward(self) -> None:
@@ -168,7 +174,8 @@ class NonlocalModule(Namespace):
     Channels-last, the fold of T into the batch ([n, T, ...] -> [n*G, T/G, ...]) is the same memory, so every kernel
     simply runs on that view."""
 
-    def __init__(self, name, dim, dim_inner, pool_size, instantiation, group, ctx: Ctx, eps=1e-5, mmt=0.1):
+    def __init__(self, name, dim, dim_inner, pool_size, instantiation, group, ctx: Ctx, eps=1e-5, mmt=0.1,
+                 norm=nn.BatchNorm3d):
         super().__init__()
         if instantiation not in NONLOCAL_INSTANTIATIONS:
             raise NotImplementedError(f"Unknown norm type {instantiation}")
@@ -177,7 +184,7 @@ class NonlocalModule(Namespace):
         self.conv_g = nn.Conv3d(dim, dim_inner, kernel_size=1, stride=1, padding=0)
         self.conv_out = nn.Conv3d(dim_inner, dim, kernel_size=1, stride=1, padding=0)
         self.conv_out.zero_init = False
-        self.bn = nn.BatchNorm3d(dim, eps=eps, momentum=mmt)
+        self.bn = norm(num_features=dim, eps=eps, momentum=mmt)
         self.bn.transform_final_bn = True
         self.use_pool = pool_size is not None and any(s > 1 for s in pool_size)
         self.pool_size = tuple(int(s) for s in pool_size) if pool_size is not None else None
@@ -253,7 +260,8 @@ class NonlocalModule(Namespace):
         oa = Act(ctx.storage((nm, "O"), n, t, h, w, d))
         ops.bias_split(ops.f32view(o), None, oa.planes)
         yo = u["out"].fprop(oa.planes)
-        ops.bn_apply(ops.f32view(yo), u["out"].scale, u["out"].shift, out.planes, relu=False, res=x.planes)
+        ops.bn_apply(ops.f32view(yo), u["out"].scale, u["out"].shift, out.planes, relu=False, res=x.planes,
+                     **u["out"].split_kw)
         object.__setattr__(self, "_saved", (x, out, xg, th, src, argmax, ph, gg, aux, oa, ng, nq, nk))
 
     def run_backward(self) -> None:
@@ -321,7 +329,7 @@ class StageModule(Namespace):
 
     def __init__(self, name, dim_in, dim_out, dim_inner, temp_kernel_sizes, stride, num_blocks, num_block_temp_kernel,
                  stride_1x1, ctx: Ctx, nonlocal_inds=None, nonlocal_pool=None, nonlocal_group=None,
-                 instantiation="softmax"):
+                 instantiation="softmax", norm=nn.BatchNorm3d):
         super().__init__()
         self.num_pathways = len(num_blocks)
         self.num_blocks = list(num_blocks)
@@ -331,11 +339,11 @@ class StageModule(Namespace):
                 [1] * (num_blocks[p] - num_block_temp_kernel[p])
             for i in range(num_blocks[p]):
                 blk = ResBlockModule(f"{name}.pathway{p}_res{i}", dim_in[p] if i == 0 else dim_out[p], dim_out[p],
-                                     tks[i], stride[p] if i == 0 else 1, dim_inner[p], stride_1x1, ctx)
+                                     tks[i], stride[p] if i == 0 else 1, dim_inner[p], stride_1x1, ctx, norm=norm)
                 self.add_module(f"pathway{p}_res{i}", blk)
                 if i in nonlocal_inds[p]:
                     nln = NonlocalModule(f"{name}.pathway{p}_nonlocal{i}", dim_out[p], dim_out[p] // 2, nonlocal_pool[p],
-                                         instantiation, nonlocal_group[p], ctx)
+                                         instantiation, nonlocal_group[p], ctx, norm=norm)
                     self.add_module(f"pathway{p}_nonlocal{i}", nln)
 
     def blocks(self, p) -> List[ResBlockModule]:
@@ -413,13 +421,17 @@ class _VideoResNetBase(nn.Module):
     graph_warmup = 2
     # W-shift stem kernels (csrc/conv_stem.cu); False = generic im2col path (kept for A/B checks)
     wshift_stem = True
+    # splits of the training batch (BN.NUM_SPLITS under sub_batchnorm; set by _check_cfg)
+    _bn_splits = 1
 
     def _init_graph_state(self):
         object.__setattr__(self, "_graphs", {})
         object.__setattr__(self, "_graph_seen", {})
 
     def _check_cfg(self, cfg):
-        assert cfg.BN.NORM_TYPE == "batchnorm", "only BN.NORM_TYPE=batchnorm is on the engine path (SURVEY §2 #9)"
+        # BN.NORM_TYPE: batchnorm or sub_batchnorm (multigrid's long cycle); norm_factory rejects the others
+        self._norm = norm_factory(cfg)
+        self._bn_splits = num_splits_of(cfg)
         assert cfg.RESNET.TRANS_FUNC == "bottleneck_transform"
         assert cfg.RESNET.NUM_GROUPS == 1
         assert not cfg.DETECTION.ENABLE, "RoI head is out of scope"
@@ -431,11 +443,20 @@ class _VideoResNetBase(nn.Module):
         assert bboxes is None, "detection is out of scope of the engine"
         x = list(x[:])
         assert len(x) == self.num_pathways, f"Input tensor does not contain {self.num_pathways} pathway"
+        if self.training and self._bn_splits > 1 and x[0].shape[0] % self._bn_splits:
+            raise ValueError(f"sub_batchnorm: BN.NUM_SPLITS {self._bn_splits} does not divide the batch size "
+                             f"{x[0].shape[0]} (every split takes batch / NUM_SPLITS clips)")
         params = [p for p in self.parameters()]
         return ModelFunction.apply(self, len(x), *x, *params)
 
     def _all_bns(self):
+        """Every nn.BatchNorm3d, both BNs of a sub-batch BN included (fvcore's precise-BN sees them all too)."""
         return [m for m in self.modules() if isinstance(m, nn.BatchNorm3d)]
+
+    def _train_bns(self):
+        """The BNs a training forward runs: a sub-batch BN runs its split_bn only, never its eval ``bn``."""
+        skip = {id(m.bn) for m in self.modules() if is_sub_bn(m)}
+        return [m for m in self._all_bns() if id(m) not in skip]
 
     def allreduce_gradients(self, group=None) -> None:
         """Data-parallel exchange step (SURVEY.md §8e): ONE NCCL all-reduce (average) over the flat gradient
@@ -458,7 +479,8 @@ class _VideoResNetBase(nn.Module):
         y = unit.fprop(xin.planes)
         _, ot, oh, ow, co = y.shape
         argmax = ctx.buf(("stem.argmax", p), (n, ot, out.dims[2], out.dims[3], co), torch.uint8)
-        ops.bn_relu_maxpool_fwd(y, unit.scale, unit.shift, out.planes, argmax, (3, 3), (2, 2), (1, 1))
+        ops.bn_relu_maxpool_fwd(y, unit.scale, unit.shift, out.planes, argmax, (3, 3), (2, 2), (1, 1),
+                                splits=unit.splits)
         self._stem_saved[p] = (xin, argmax, out)
 
     def _stem_backward(self, p: int, unit: ConvBN) -> None:
@@ -560,12 +582,13 @@ class B200SlowFast(_VideoResNetBase):
         assert POOL1[cfg.MODEL.ARCH] == [[1, 1, 1], [1, 1, 1]]
         cin = cfg.DATA.INPUT_CHANNEL_NUM
 
+        norm = self._norm
         self.s1 = Namespace()
         self.s1.add_module("pathway0_stem", StemModule(cin[0], wpg, tk[0][0] + [7, 7], (1, 2, 2),
-                                                       (tk[0][0][0] // 2, 3, 3), 1e-5, 0.1))
+                                                       (tk[0][0][0] // 2, 3, 3), 1e-5, 0.1, norm))
         self.s1.add_module("pathway1_stem", StemModule(cin[1], wpg // beta_inv, tk[0][1] + [7, 7], (1, 2, 2),
-                                                       (tk[0][1][0] // 2, 3, 3), 1e-5, 0.1))
-        self.s1_fuse = FuseModule(wpg // beta_inv, ratio, fk, alpha)
+                                                       (tk[0][1][0] // 2, 3, 3), 1e-5, 0.1, norm))
+        self.s1_fuse = FuseModule(wpg // beta_inv, ratio, fk, alpha, norm=norm)
         widths = [wpg * 4, wpg * 8, wpg * 16, wpg * 32]
         depths = [d2, d3, d4, d5]
         prev = wpg
@@ -576,10 +599,10 @@ class B200SlowFast(_VideoResNetBase):
                 stride=cfg.RESNET.SPATIAL_STRIDES[i], num_blocks=[dp] * 2,
                 num_block_temp_kernel=cfg.RESNET.NUM_BLOCK_TEMP_KERNEL[i], stride_1x1=cfg.RESNET.STRIDE_1X1, ctx=ctx,
                 nonlocal_inds=cfg.NONLOCAL.LOCATION[i], nonlocal_pool=cfg.NONLOCAL.POOL[i],
-                nonlocal_group=cfg.NONLOCAL.GROUP[i], instantiation=cfg.NONLOCAL.INSTANTIATION)
+                nonlocal_group=cfg.NONLOCAL.GROUP[i], instantiation=cfg.NONLOCAL.INSTANTIATION, norm=norm)
             self.add_module(f"s{i + 2}", st)
             if i < 3:
-                self.add_module(f"s{i + 2}_fuse", FuseModule(wd // beta_inv, ratio, fk, alpha))
+                self.add_module(f"s{i + 2}_fuse", FuseModule(wd // beta_inv, ratio, fk, alpha, norm=norm))
             if i == 0:
                 for p in range(2):
                     self.add_module(f"pathway{p}_pool", nn.Identity())
@@ -664,7 +687,7 @@ class B200SlowFast(_VideoResNetBase):
             trace.append((slow, fast, cs))
         self._trace = trace
         if ctx.training:
-            bump_num_batches_tracked(self._all_bns())
+            bump_num_batches_tracked(self._train_bns())
         out = self._head_forward([slow, fast])
         ctx.end_phase()
         return out
@@ -672,7 +695,7 @@ class B200SlowFast(_VideoResNetBase):
     def _fuse_forward(self, i: int, fast: Act, out: Act) -> None:
         unit = self._engine_units()[f"fuse{i}"]
         y = unit.fprop(fast.planes)
-        ops.bn_apply(ops.f32view(y), unit.scale, unit.shift, out.planes, relu=True)
+        ops.bn_apply(ops.f32view(y), unit.scale, unit.shift, out.planes, relu=True, **unit.split_kw)
         self.__dict__.setdefault("_fuse_saved", {})[i] = (fast, out)
 
     # ------------------------------------------------------------------ backward program

@@ -35,7 +35,7 @@ class B200ResNet(_VideoResNetBase):
         cin = cfg.DATA.INPUT_CHANNEL_NUM
         self.s1 = Namespace()
         self.s1.add_module("pathway0_stem", StemModule(cin[0], wpg, tk[0][0] + [7, 7], (1, 2, 2),
-                                                       (tk[0][0][0] // 2, 3, 3), 1e-5, 0.1))
+                                                       (tk[0][0][0] // 2, 3, 3), 1e-5, 0.1, self._norm))
         widths = [wpg * 4, wpg * 8, wpg * 16, wpg * 32]
         prev = wpg
         for i, (wd, dp) in enumerate(zip(widths, (d2, d3, d4, d5))):
@@ -44,7 +44,7 @@ class B200ResNet(_VideoResNetBase):
                              num_block_temp_kernel=cfg.RESNET.NUM_BLOCK_TEMP_KERNEL[i],
                              stride_1x1=cfg.RESNET.STRIDE_1X1, ctx=ctx, nonlocal_inds=cfg.NONLOCAL.LOCATION[i],
                              nonlocal_pool=cfg.NONLOCAL.POOL[i], nonlocal_group=cfg.NONLOCAL.GROUP[i],
-                             instantiation=cfg.NONLOCAL.INSTANTIATION)
+                             instantiation=cfg.NONLOCAL.INSTANTIATION, norm=self._norm)
             self.add_module(f"s{i + 2}", st)
             if i == 0:
                 self.add_module("pathway0_pool", nn.MaxPool3d(kernel_size=list(self._pool1), stride=list(self._pool1),
@@ -106,7 +106,7 @@ class B200ResNet(_VideoResNetBase):
                 self._pool_saved = (cur, pooled, argmax, k)
                 cur = pooled
         if ctx.training:
-            bump_num_batches_tracked(self._all_bns())
+            bump_num_batches_tracked(self._train_bns())
         out = self._head_forward([cur])
         ctx.end_phase()
         return out

@@ -270,18 +270,40 @@ def conv_wgrad(x: Planes, dy: Planes, geom: ConvGeom, dwm: torch.Tensor, nsplit:
 
 # ------------------------------------------------------------------------------------------------ batch norm
 def bn_finalize(partials: Optional[torch.Tensor], m_tiles: int, c: int, count: int, gamma, beta, running_mean,
-                running_var, momentum: float, eps: float, training: bool, scale, shift, save_mean, save_invstd):
+                running_var, momentum: float, eps: float, training: bool, scale, shift, save_mean, save_invstd,
+                affine_c: int = 0):
+    """``affine_c``: period of gamma / beta (sub-batch BN: ``c`` = S*C split channels share one [C] affine)."""
     lib = L.load()
     L.check(lib.sfb_bn_finalize(_ptr(partials), m_tiles, c, count, _ptr(gamma), _ptr(beta), _ptr(running_mean),
                                 _ptr(running_var), momentum, eps, 1 if training else 0, scale.data_ptr(),
-                                shift.data_ptr(), _ptr(save_mean), _ptr(save_invstd), _stream()), "sfb_bn_finalize")
+                                shift.data_ptr(), _ptr(save_mean), _ptr(save_invstd), affine_c, _stream()),
+            "sfb_bn_finalize")
+    _count()
+
+
+def bn_split_stats_tiles(rows: int, rows_per_clip: int, splits: int, c: int) -> int:
+    """Partial columns per split channel that ``bn_split_stats`` writes for a ``c``-channel activation."""
+    return L.load().sfb_bn_split_stats_tiles(rows, rows_per_clip, splits, c)
+
+
+def bn_split_stats(y: F32View, splits: int, rows_per_clip: int, partials: torch.Tensor) -> None:
+    """Sub-batch BN training statistics of y: partials [2][splits*c][bn_split_stats_tiles(...)] for ``bn_finalize``
+    over ``splits*c`` channels (clip k is split k % splits)."""
+    lib = L.load()
+    tiles = bn_split_stats_tiles(y.rows, rows_per_clip, splits, y.c)
+    assert partials.dtype == F32 and partials.numel() >= 2 * splits * y.c * tiles
+    L.check(lib.sfb_bn_split_stats(y.ptr(), y.pitch, y.rows, y.c, splits, rows_per_clip, partials.data_ptr(),
+                                   _stream()), "sfb_bn_split_stats")
     _count()
 
 
 def bn_apply(y: F32View, scale, shift, out: Planes, relu: bool, y2: Optional[F32View] = None, scale2=None,
-             shift2=None, res: Optional[Planes] = None) -> None:
+             shift2=None, res: Optional[Planes] = None, splits: int = 1, rows_per_clip: int = 0) -> None:
+    """``splits`` > 1: scale / shift (scale2 / shift2) are [splits][c] tables, row r uses row
+    (r // rows_per_clip) % splits."""
     lib = L.load()
     d = L.BnApplyDesc()
+    d.splits, d.rows_per_clip = splits, rows_per_clip
     d.y, d.y_pitch, d.scale, d.shift = y.ptr(), y.pitch, scale.data_ptr(), shift.data_ptr()
     if y2 is not None:
         d.y2, d.y2_pitch, d.scale2, d.shift2 = y2.ptr(), y2.pitch, scale2.data_ptr(), shift2.data_ptr()
@@ -295,21 +317,26 @@ def bn_apply(y: F32View, scale, shift, out: Planes, relu: bool, y2: Optional[F32
     _count()
 
 
-def bn_bwd_scratch(rows: int, c: int, device):
-    lib = L.load()
-    nb = lib.sfb_bn_bwd_blocks(rows, c)
-    return (torch.empty((nb, 2, c), dtype=F32, device=device), torch.empty((3, c), dtype=F32, device=device))
+def bn_bwd_blocks(rows: int, c: int, splits: int = 1, rows_per_clip: int = 0) -> int:
+    return L.load().sfb_bn_bwd_blocks(rows, c, splits, rows_per_clip)
+
+
+def bn_bwd_scratch(rows: int, c: int, device, splits: int = 1, rows_per_clip: int = 0):
+    nb = bn_bwd_blocks(rows, c, splits, rows_per_clip)
+    return (torch.empty((nb, 2, c), dtype=F32, device=device), torch.empty((3, splits * c), dtype=F32, device=device))
 
 
 def bn_bwd(dout: F32View, mask: Optional[Planes], y: F32View, mean, invstd, gamma, dgamma, dbeta, dy: Planes,
            partials, coef, training: bool = True, accumulate_param_grads: bool = False,
            dres: Optional[F32View] = None, dres_accumulate: bool = False, c_valid: int = 0,
-           mask_affine=None) -> None:
+           mask_affine=None, splits: int = 1, rows_per_clip: int = 0) -> None:
     """``mask``: post-ReLU planes (ReLU mask = planes > 0) or None; ``mask_affine`` = (scale, shift): recompute the
-    mask as y*scale + shift > 0 instead (used when the activation was never materialised)."""
+    mask as y*scale + shift > 0 instead (used when the activation was never materialised).  ``splits`` > 1: mean /
+    invstd (and mask_affine) are [splits][c] tables of sub-batch BN, clip k of the batch being split k % splits."""
     lib = L.load()
     d = L.BnBwdDesc()
     d.c_valid = c_valid
+    d.splits, d.rows_per_clip = splits, rows_per_clip
     if mask_affine is not None:
         assert mask is None
         d.mask_scale, d.mask_shift = mask_affine[0].data_ptr(), mask_affine[1].data_ptr()
@@ -340,10 +367,13 @@ def _pool_desc(n, t, h, w, c, oh, ow, k, s, p):
     return d
 
 
-def bn_relu_maxpool_fwd(y: torch.Tensor, scale, shift, out: Planes, argmax: torch.Tensor, k, s, p) -> None:
+def bn_relu_maxpool_fwd(y: torch.Tensor, scale, shift, out: Planes, argmax: torch.Tensor, k, s, p,
+                        splits: int = 1) -> None:
+    """``splits`` > 1: scale / shift are [splits][c] tables, clip n uses row n % splits."""
     lib = L.load()
     n, t, h, w, c = y.shape
     d = _pool_desc(n, t, h, w, c, out.h, out.w, k, s, p)
+    d.splits = splits
     d.y, d.scale, d.shift = y.data_ptr(), scale.data_ptr(), shift.data_ptr()
     d.out_hi, d.out_lo, d.out_pitch = out.hi_ptr(), out.lo_ptr(), out.pitch
     d.argmax = argmax.data_ptr()
@@ -686,11 +716,12 @@ def bias_split(x: F32View, bias: Optional[torch.Tensor], out: Planes) -> None:
 
 
 def bn_conv_bias(bias: torch.Tensor, c: int, momentum: float, training: bool, running_mean, scale, shift,
-                 save_mean) -> None:
-    """Fold a conv bias into the BatchNorm that follows it, after ``bn_finalize`` (csrc/nonlocal.cu)."""
+                 save_mean, splits: int = 1) -> None:
+    """Fold a conv bias into the BatchNorm that follows it, after ``bn_finalize`` (csrc/nonlocal.cu).  ``splits`` > 1:
+    running_mean is a sub-batch BN's [splits][c] split_bn statistics (training)."""
     lib = L.load()
     L.check(lib.sfb_bn_conv_bias(bias.data_ptr(), c, momentum, 1 if training else 0, _ptr(running_mean), _ptr(scale),
-                                 _ptr(shift), _ptr(save_mean), _stream()), "sfb_bn_conv_bias")
+                                 _ptr(shift), _ptr(save_mean), splits, _stream()), "sfb_bn_conv_bias")
     _count()
 
 
