@@ -309,7 +309,7 @@ int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream);
  * :293, MultiScaleBlock.forward :491; common.py Mlp :26; stem_helper.py PatchEmbed :315).  Tokens are
  * [B, N = 1 + T*H*W, C] fp32 with the cls token first; GEMM operands are split-bf16 planes.
  * ---------------------------------------------------------------------------------------------- */
-/* nn.LayerNorm(eps) over the last dim (C <= 768): planes and/or fp32 output, saves mean / rstd per row. */
+/* nn.LayerNorm(eps) over the last dim (C <= 1280): planes and/or fp32 output, saves mean / rstd per row. */
 int sfb_layernorm_fwd(const float* x, int64_t x_pitch, int64_t rows, int32_t c, const float* gamma, const float* beta,
                       float eps, void* o_hi, void* o_lo, float* o_f32, int64_t o_pitch, float* mean, float* rstd,
                       void* stream);
@@ -323,11 +323,31 @@ int sfb_layernorm_bwd(const float* dy, int64_t dy_pitch, const float* x, int64_t
 /* out[c] (= or +=) column sums of src[rows, c] (bias gradients); partials scratch [sfb_rowslab_blocks(rows)][c]. */
 int sfb_colsum(const float* src, int64_t pitch, int64_t rows, int32_t c, float* out, int32_t accumulate, float* partials,
                void* stream);
-/* x[b,0,:] = cls; x[b,1+l,:] = y[b,l,:] + bias   (PatchEmbed output + cls token, video_model_builder.py:1180-1186) */
-int sfb_tokens_assemble(const float* y, const float* bias, const float* cls, int32_t b, int32_t l, int32_t c, float* x,
-                        void* stream);
+/* x[b,0,:] = cls; x[b,1+l,:] = y[b,l,:] + bias   (PatchEmbed output + cls token, video_model_builder.py:1180-1186).
+ * With separable absolute positions (all three tables non-null, hw = H*W of the token grid, l = T*hw):
+ * x[b,0,:] = cls + pos_class; x[b,1+t*hw+s,:] = (y + bias) + (pos_spatial[s] + pos_temporal[t]).  Null tables run the
+ * plain assembly. */
+int sfb_tokens_assemble(const float* y, const float* bias, const float* cls, const float* pos_spatial,
+                        const float* pos_temporal, const float* pos_class, int32_t b, int32_t l, int32_t hw, int32_t c,
+                        float* x, void* stream);
 int sfb_tokens_split_grad(const float* dx, int32_t b, int32_t l, int32_t c, void* dy_hi, void* dy_lo, float* dy_f32,
                           void* stream);
+/* Slab count of the segmented row sums below: their `partials` scratch is [groups][sfb_segment_slabs(groups, rows)][c]
+ * (groups = t for sfb_pos_embed_sep_bwd with rows = hw; groups = b for sfb_token_mean_fwd with rows = n - 1). */
+int32_t sfb_segment_slabs(int32_t groups, int32_t seg_rows);
+/* Gradients of the separable position tables from the token gradient dx [b, 1 + t*hw, c] (all "="):
+ * dps[s] = sum_b sum_t dx[b,1+t*hw+s]; dpt[t] = sum_b sum_s dx[b,1+t*hw+s]; dpc = sum_b dx[b,0].  Fixed-order sums, no
+ * atomics: the result is a function of the input bits. */
+int sfb_pos_embed_sep_bwd(const float* dx, int32_t b, int32_t t, int32_t hw, int32_t c, float* dps, float* dpt,
+                          float* dpc, float* partials, void* stream);
+/* Mean-token readout (USE_MEAN_POOLING, video_model_builder.py:1231-1234): out[b] = mean of x[b, 1..n-1] ([b, n, c] ->
+ * [b, c]), deterministic; the backward writes dx[b,0] = 0 and dx[b,1+l] = dmean[b] / (n-1). */
+int sfb_token_mean_fwd(const float* x, int32_t b, int32_t n, int32_t c, float* out, float* partials, void* stream);
+int sfb_token_mean_bwd(const float* dmean, int32_t b, int32_t n, int32_t c, float* dx, void* stream);
+/* Non-overlapping patch embedding input (Conv3d with stride == kernel, no padding): NCTHW fp32 clip -> split-bf16 rows
+ * [b * (t/kt)(h/kh)(w/kw), cin*kt*kh*kw], columns in Conv3d's weight-flatten order (cin, kt, kh, kw); K % 8 == 0. */
+int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt, int32_t kh,
+                 int32_t kw, void* hi, void* lo, void* stream);
 /* attention_pool with the depthwise Conv3d (groups = head_dim, weight shared by the heads, padding k/2):
  * src = fused-qkv GEMM output [B, 1+L, src_pitch] (+bias on real tokens), out = [B, heads, 1+L', hd] fp32. */
 typedef struct sfb_dwpool_desc {

@@ -216,6 +216,46 @@ _PRESETS = {
         "RNG_SEED": 0,
     },
 }
+_MVIT_B_POOL = {"DIM_MUL": [[1, 2.0], [3, 2.0], [14, 2.0]], "HEAD_MUL": [[1, 2.0], [3, 2.0], [14, 2.0]],
+                 "POOL_KVQ_KERNEL": [3, 3, 3], "POOL_KV_STRIDE_ADAPTIVE": [1, 8, 8]}
+_PRESETS.update({
+    # configs/Kinetics/MVIT_B_16x4_CONV.yaml (MViTv1-B: separable absolute positions, cls readout)
+    "MVIT_B_16x4_CONV": {
+        "DATA": {"NUM_FRAMES": 16, "TRAIN_CROP_SIZE": 224, "TEST_CROP_SIZE": 224, "INPUT_CHANNEL_NUM": [3]},
+        "MVIT": dict(_MVIT_B_POOL, ZERO_DECAY_POS_CLS=False, SEP_POS_EMBED=True, DEPTH=16, NUM_HEADS=1, EMBED_DIM=96,
+                     PATCH_KERNEL=[3, 7, 7], PATCH_STRIDE=[2, 4, 4], PATCH_PADDING=[1, 3, 3], MLP_RATIO=4.0,
+                     QKV_BIAS=True, DROPPATH_RATE=0.2, NORM="layernorm", MODE="conv", CLS_EMBED_ON=True,
+                     POOL_Q_STRIDE=[[1, 1, 2, 2], [3, 1, 2, 2], [14, 1, 2, 2]], DROPOUT_RATE=0.0),
+        "MODEL": {"NUM_CLASSES": 400, "ARCH": "mvit", "MODEL_NAME": "MViT", "DROPOUT_RATE": 0.5},
+        "TRAIN": {"BATCH_SIZE": 16},
+        "RNG_SEED": 0,
+    },
+    # configs/masked_ssl/k400_VIT_B_16x4_FT.yaml (ViT-B: 2x16x16 patches, separable positions, mean readout)
+    "VIT_B_16x4_FT": {
+        "DATA": {"NUM_FRAMES": 16, "TRAIN_CROP_SIZE": 224, "TEST_CROP_SIZE": 224, "INPUT_CHANNEL_NUM": [3]},
+        "MVIT": {"ZERO_DECAY_POS_CLS": False, "SEP_POS_EMBED": True, "PATCH_KERNEL": [2, 16, 16],
+                 "PATCH_STRIDE": [2, 16, 16], "PATCH_PADDING": [0, 0, 0], "EMBED_DIM": 768, "NUM_HEADS": 12,
+                 "MLP_RATIO": 4.0, "QKV_BIAS": True, "NORM": "layernorm", "DEPTH": 12, "MODE": "conv",
+                 "DROPPATH_RATE": 0.1, "LAYER_SCALE_INIT_VALUE": 0.0, "USE_MEAN_POOLING": True,
+                 "HEAD_INIT_SCALE": 0.001},
+        "MODEL": {"NUM_CLASSES": 400, "ARCH": "mvit", "MODEL_NAME": "MViT", "DROPOUT_RATE": 0.3},
+        "TRAIN": {"BATCH_SIZE": 1},
+        "RNG_SEED": 0,
+    },
+    # configs/masked_ssl/k400_MVITv2_S_16x4_FT.yaml (MaskFeat fine-tuning: MViTv2-S with the mean readout)
+    "MVITv2_S_16x4_FT": {
+        "DATA": {"NUM_FRAMES": 16, "TRAIN_CROP_SIZE": 224, "TEST_CROP_SIZE": 224, "INPUT_CHANNEL_NUM": [3]},
+        "MVIT": dict(_MVIT_B_POOL, DEPTH=16, NUM_HEADS=1, EMBED_DIM=96, PATCH_KERNEL=[3, 7, 7], PATCH_STRIDE=[2, 4, 4],
+                     PATCH_PADDING=[1, 3, 3], ZERO_DECAY_POS_CLS=False, QKV_BIAS=True,
+                     POOL_Q_STRIDE=[[i, 1, 2, 2] if i in (1, 3, 14) else [i, 1, 1, 1] for i in range(16)],
+                     CLS_EMBED_ON=True, USE_ABS_POS=False, SEP_POS_EMBED=True, REL_POS_SPATIAL=True,
+                     REL_POS_TEMPORAL=True, RESIDUAL_POOLING=True, MODE="conv", DROPPATH_RATE=0.1,
+                     LAYER_SCALE_INIT_VALUE=0.0, USE_MEAN_POOLING=True, HEAD_INIT_SCALE=0.001),
+        "MODEL": {"NUM_CLASSES": 400, "ARCH": "mvit", "MODEL_NAME": "MViT", "DROPOUT_RATE": 0.0},
+        "TRAIN": {"BATCH_SIZE": 16},
+        "RNG_SEED": 0,
+    },
+})
 # Non-local recipes (Wang et al., arXiv:1711.07971): the same backbones with Non-local blocks after res3 blocks 1, 3 and
 # res4 blocks 1, 3, 5 (slow pathway only for SlowFast); NONLOCAL.POOL keeps its default [1, 2, 2]
 _NLN_R50 = {"LOCATION": [[[]], [[1, 3]], [[1, 3, 5]], [[]]], "GROUP": [[1], [1], [1], [1]]}

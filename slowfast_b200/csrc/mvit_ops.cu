@@ -49,8 +49,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // ------------------------------------------------------------------------------------------- LayerNorm
 // One warp per row (C <= 1024).  y = (x - mean) * rstd * gamma + beta -> split planes and/or fp32.
-constexpr int LN_MAX_PER_LANE = 24;  // C <= 768
-// NPL = elements per lane (c <= 32*NPL): instantiated for 3 / 6 / 12 / 24 so that narrow rows (c = 96: the first
+constexpr int LN_MAX_PER_LANE = 40;  // C <= 1280 (ViT-H)
+// NPL = elements per lane (c <= 32*NPL): instantiated for 3 / 6 / 12 / 24 / 32 / 40 so that narrow rows (c = 96: the first
 // MViT stages, the per-head pooling norms) do not pay for 24 predicated-off iterations per row
 template <int NPL>
 __global__ void __launch_bounds__(256) ln_fwd_kernel(const float* __restrict__ x, int64_t x_pitch, int64_t rows, int c,
@@ -157,6 +157,74 @@ __global__ void __launch_bounds__(256) ln_bwd_kernel(const float* __restrict__ d
     partials[(size_t(blockIdx.x) * 2 + which) * c + ch] = s;
   }
 }
+// Rows wider than 768 (ViT-L 1024, MViTv2-L's last stage 1152, ViT-H 1280): the same arithmetic, but a row's dy / x are
+// read twice from global memory (L1 / L2) instead of being held in registers, and the per-block dgamma / dbeta merge runs
+// in 256-channel chunks, so the kernel keeps its registers (no spills) and 16 KB of static shared memory.
+template <int NPL>
+__global__ void __launch_bounds__(256) ln_bwd_wide_kernel(const float* __restrict__ dy, int64_t dy_pitch,
+                                                          const float* __restrict__ x, int64_t x_pitch, int64_t rows,
+                                                          int c, const float* __restrict__ gamma,
+                                                          const float* __restrict__ mean, const float* __restrict__ rstd,
+                                                          float* __restrict__ dx, int64_t dx_pitch, int dx_accumulate,
+                                                          float* __restrict__ partials /* [grid][2][c] */) {
+  static_assert(NPL % 8 == 0, "chunked merge: 8 lane slots = 256 channels per chunk");
+  __shared__ float sm[8][2][256];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int64_t warp = (blockIdx.x * int64_t(blockDim.x) + threadIdx.x) >> 5;
+  const int64_t nwarps = (int64_t(gridDim.x) * blockDim.x) >> 5;
+  float dg[NPL], db[NPL];
+#pragma unroll
+  for (int i = 0; i < NPL; ++i) dg[i] = db[i] = 0.f;
+  for (int64_t r = warp; r < rows; r += nwarps) {
+    const float mu = mean[r], rs = rstd[r];
+    const float* dyr = dy + r * dy_pitch;
+    const float* xr = x + r * x_pitch;
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < NPL; ++i) {
+      const int j = lane + 32 * i;
+      const bool ok = j < c;
+      const float d = ok ? dyr[j] : 0.f;
+      const float xh = ok ? (xr[j] - mu) * rs : 0.f;
+      const float g = d * (ok ? gamma[j] : 0.f);
+      s1 += g;
+      s2 = fmaf(g, xh, s2);
+      dg[i] = fmaf(d, xh, dg[i]);
+      db[i] += d;
+    }
+    s1 = warp_sum(s1) / float(c);
+    s2 = warp_sum(s2) / float(c);
+#pragma unroll
+    for (int i = 0; i < NPL; ++i) {
+      const int j = lane + 32 * i;
+      if (j < c) {
+        const float xh = (xr[j] - mu) * rs;
+        const float v = rs * (dyr[j] * gamma[j] - s1 - xh * s2);
+        float* o = dx + r * dx_pitch + j;
+        *o = dx_accumulate ? *o + v : v;
+      }
+    }
+  }
+#pragma unroll
+  for (int i0 = 0; i0 < NPL; i0 += 8) {
+    const int c0 = 32 * i0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      sm[wid][0][lane + 32 * i] = dg[i0 + i];
+      sm[wid][1][lane + 32 * i] = db[i0 + i];
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < 2 * 256; j += blockDim.x) {
+      const int which = j >> 8, ch = j & 255;
+      if (c0 + ch < c) {
+        float s = 0.f;
+        for (int w = 0; w < 8; ++w) s += sm[w][which][ch];
+        partials[(size_t(blockIdx.x) * 2 + which) * c + c0 + ch] = s;
+      }
+    }
+    __syncthreads();
+  }
+}
 // ------------------------------------------------------------------------------------------- column sums (bias grads)
 // partials[block][c] = sum over the block's row slab of src[rows, c]
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ src, int64_t pitch, int64_t rows, int c,
@@ -219,15 +287,121 @@ __global__ void __launch_bounds__(256) colsum4_kernel(const float* __restrict__ 
 
 // ------------------------------------------------------------------------------------------- token assembly
 // x[b, 0, :] = cls;  x[b, 1 + l, :] = y[b, l, :] + bias      (patch embedding output -> token sequence)
+// with separable absolute positions (ps != null): x[b, 0, :] = cls + pc;  x[b, 1 + t*hw + s, :] = (y + bias) + (ps[s] + pt[t]),
+// the reference's order (the position table is summed first, then added: video_model_builder.py:1189-1199)
 __global__ void tokens_assemble_kernel(const float* __restrict__ y, const float* __restrict__ bias,
-                                       const float* __restrict__ cls, int b, int l, int c, float* __restrict__ x) {
+                                       const float* __restrict__ cls, const float* __restrict__ ps,
+                                       const float* __restrict__ pt, const float* __restrict__ pc, int b, int l, int hw,
+                                       int c, float* __restrict__ x) {
   const int64_t items = int64_t(b) * (l + 1) * c;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int ch = int(i % c);
     const int64_t t = i / c;
     const int n = int(t % (l + 1));
     const int64_t bb = t / (l + 1);
-    x[i] = n == 0 ? cls[ch] : y[(bb * l + n - 1) * c + ch] + bias[ch];
+    if (!ps) {
+      x[i] = n == 0 ? cls[ch] : y[(bb * l + n - 1) * c + ch] + bias[ch];
+    } else if (n == 0) {
+      x[i] = cls[ch] + pc[ch];
+    } else {
+      const int m = n - 1;
+      x[i] = (y[(bb * l + m) * c + ch] + bias[ch]) + (ps[int64_t(m % hw) * c + ch] + pt[int64_t(m / hw) * c + ch]);
+    }
+  }
+}
+// ------------------------------------------------------------------------------------------- separable position grads
+// Deterministic: every output element is a fixed-order sum (no atomics), so CUDA-graph replay reproduces eager bitwise.
+// dps[s, :] = sum_b sum_t dx[b, 1 + t*hw + s, :] and dpc[:] = sum_b dx[b, 0, :]: one thread per output element
+__global__ void pos_sep_bwd_spatial_kernel(const float* __restrict__ dx, int b, int t, int hw, int c,
+                                           float* __restrict__ dps, float* __restrict__ dpc) {
+  const int64_t n = 1 + int64_t(t) * hw;
+  const int64_t items = int64_t(hw + 1) * c;
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
+    const int ch = int(i % c);
+    const int s = int(i / c);
+    float acc = 0.f;
+    if (s == hw) {
+      for (int bb = 0; bb < b; ++bb) acc += dx[bb * n * c + ch];
+      dpc[ch] = acc;
+    } else {
+      for (int bb = 0; bb < b; ++bb) {
+        const float* p = dx + (bb * n + 1 + s) * c + ch;
+        for (int tt = 0; tt < t; ++tt) acc += p[int64_t(tt) * hw * c];
+      }
+      dps[int64_t(s) * c + ch] = acc;
+    }
+  }
+}
+// Segmented row sums (the temporal position gradient and the mean-token readout):
+//   partials[g][slab][ch] = sum_{o < n_outer} sum_{r in slab} src[(o * outer_stride + g * group_stride + r) * c + ch]
+// grid (slabs, groups); fixed order inside a block, so the result depends on the shape only
+__global__ void segment_rowsum_partial_kernel(const float* __restrict__ src, int c, int n_outer, int64_t outer_stride,
+                                              int64_t group_stride, int seg_rows, float* __restrict__ partials) {
+  const int g = blockIdx.y, slab = blockIdx.x, nslab = gridDim.x;
+  const int rps = (seg_rows + nslab - 1) / nslab;
+  const int r0 = slab * rps, r1 = min(seg_rows, r0 + rps);
+  for (int ch = threadIdx.x; ch < c; ch += blockDim.x) {
+    float s0 = 0.f, s1 = 0.f;  // two independent chains
+    for (int o = 0; o < n_outer; ++o) {
+      const float* p = src + (o * outer_stride + g * group_stride) * c + ch;
+      int r = r0;
+      for (; r + 1 < r1; r += 2) {
+        s0 += p[int64_t(r) * c];
+        s1 += p[int64_t(r + 1) * c];
+      }
+      if (r < r1) s0 += p[int64_t(r) * c];
+    }
+    partials[(int64_t(g) * nslab + slab) * c + ch] = s0 + s1;
+  }
+}
+// out[g][ch] = scale * sum_slab partials[g][slab][ch]   (fp64, slab order)
+__global__ void segment_rowsum_merge_kernel(const float* __restrict__ partials, int nslab, int groups, int c, float scale,
+                                            float* __restrict__ out) {
+  const int64_t items = int64_t(groups) * c;
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
+    const int ch = int(i % c);
+    const int64_t g = i / c;
+    double s = 0.0;
+    for (int k = 0; k < nslab; ++k) s += double(partials[(g * nslab + k) * c + ch]);
+    out[i] = float(s) * scale;
+  }
+}
+// mean readout backward: dx[b, 0, :] = 0;  dx[b, 1 + l, :] = dmean[b, :] * scale
+__global__ void token_mean_bwd_kernel(const float* __restrict__ dmean, int b, int n, int c, float scale,
+                                      float* __restrict__ dx) {
+  const int64_t items = int64_t(b) * n * c;
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
+    const int ch = int(i % c);
+    const int64_t t = i / c;
+    const int r = int(t % n);
+    dx[i] = r == 0 ? 0.f : dmean[(t / n) * c + ch] * scale;
+  }
+}
+// ------------------------------------------------------------------------------------------- non-overlapping patches
+// stride == kernel, no padding: NCTHW clip -> split rows [b * L, cin*kt*kh*kw], row (b, ot, oh, ow), column
+// (ci, dt, dy, dx) in Conv3d's weight-flatten order, so the patch embedding is one plain [E, K] GEMM
+__global__ void patchify_kernel(const float* __restrict__ x, int b, int cin, int T, int H, int W, int kt, int kh, int kw,
+                                int ot, int oh, int ow, __nv_bfloat16* hi, __nv_bfloat16* lo) {
+  const int K = cin * kt * kh * kw;
+  const int64_t L = int64_t(ot) * oh * ow;
+  const int64_t items = int64_t(b) * L * K;
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
+    int k = int(i % K);
+    const int64_t row = i / K;
+    const int dx_ = k % kw;
+    k /= kw;
+    const int dy_ = k % kh;
+    k /= kh;
+    const int dt_ = k % kt;
+    const int ci = k / kt;
+    int64_t l = row % L;
+    const int64_t bb = row / L;
+    const int px = int(l % ow);
+    l /= ow;
+    const int py = int(l % oh);
+    const int pz = int(l / oh);
+    const float v = x[(((bb * cin + ci) * T + pz * kt + dt_) * int64_t(H) + py * kh + dy_) * W + px * kw + dx_];
+    put_split(hi, lo, i, v);
   }
 }
 // backward: dy[b, l, :] planes = dx[b, 1 + l, :];  dcls partial / dbias via colsum on the caller side
@@ -810,7 +984,11 @@ extern "C" int sfb_layernorm_fwd(const float* x, int64_t x_pitch, int64_t rows, 
                                                                          (bf*)o_lo, o_f32, o_pitch, mean, rstd);
   else if (c <= 384) ln_fwd_kernel<12><<<mv_grid(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, rows, c, gamma, beta, eps, (bf*)o_hi,
                                                                          (bf*)o_lo, o_f32, o_pitch, mean, rstd);
-  else ln_fwd_kernel<24><<<mv_grid(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, rows, c, gamma, beta, eps, (bf*)o_hi,
+  else if (c <= 768) ln_fwd_kernel<24><<<mv_grid(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, rows, c, gamma, beta, eps, (bf*)o_hi,
+                                                                         (bf*)o_lo, o_f32, o_pitch, mean, rstd);
+  else if (c <= 1024) ln_fwd_kernel<32><<<mv_grid(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, rows, c, gamma, beta, eps, (bf*)o_hi,
+                                                                         (bf*)o_lo, o_f32, o_pitch, mean, rstd);
+  else ln_fwd_kernel<40><<<mv_grid(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, rows, c, gamma, beta, eps, (bf*)o_hi,
                                                                          (bf*)o_lo, o_f32, o_pitch, mean, rstd);
   SFB_MV_CHECK("sfb_layernorm_fwd");
   return 0;
@@ -854,8 +1032,12 @@ extern "C" int sfb_layernorm_bwd(const float* dy, int64_t dy_pitch, const float*
                                                                         rstd, dx, dx_pitch, dx_accumulate, partials);
   else if (c <= 384) ln_bwd_kernel<12><<<nb, 256, size_t(8) * 2 * c * sizeof(float), stream>>>(dy, dy_pitch, x, x_pitch, rows, c, gamma, mean,
                                                                         rstd, dx, dx_pitch, dx_accumulate, partials);
-  else ln_bwd_kernel<24><<<nb, 256, size_t(8) * 2 * c * sizeof(float), stream>>>(dy, dy_pitch, x, x_pitch, rows, c, gamma, mean,
+  else if (c <= 768) ln_bwd_kernel<24><<<nb, 256, size_t(8) * 2 * c * sizeof(float), stream>>>(dy, dy_pitch, x, x_pitch, rows, c, gamma, mean,
                                                                         rstd, dx, dx_pitch, dx_accumulate, partials);
+  else if (c <= 1024) ln_bwd_wide_kernel<32><<<nb, 256, 0, stream>>>(dy, dy_pitch, x, x_pitch, rows, c, gamma, mean, rstd, dx,
+                                                                    dx_pitch, dx_accumulate, partials);
+  else ln_bwd_wide_kernel<40><<<nb, 256, 0, stream>>>(dy, dy_pitch, x, x_pitch, rows, c, gamma, mean, rstd, dx, dx_pitch,
+                                                     dx_accumulate, partials);
   SFB_MV_CHECK("sfb_layernorm_bwd");
   partial_merge2_kernel<<<dim3(c, 2), 64, 0, stream>>>(partials, nb, 2, c, dgamma, dbeta, param_accumulate);
   SFB_MV_CHECK("sfb_layernorm_bwd(merge)");
@@ -874,11 +1056,80 @@ extern "C" int sfb_colsum(const float* src, int64_t pitch, int64_t rows, int32_t
   SFB_MV_CHECK("sfb_colsum(merge)");
   return 0;
 }
-extern "C" int sfb_tokens_assemble(const float* y, const float* bias, const float* cls, int32_t b, int32_t l, int32_t c,
-                                   float* x, void* stream) {
+extern "C" int sfb_tokens_assemble(const float* y, const float* bias, const float* cls, const float* pos_spatial,
+                                   const float* pos_temporal, const float* pos_class, int32_t b, int32_t l, int32_t hw,
+                                   int32_t c, float* x, void* stream) {
+  const bool any = pos_spatial || pos_temporal || pos_class;
+  if (any && !(pos_spatial && pos_temporal && pos_class && hw > 0 && l % hw == 0)) {
+    set_error("sfb_tokens_assemble: positions need all three tables and hw=%d dividing l=%d", hw, l);
+    return -10;
+  }
   const int64_t items = int64_t(b) * (l + 1) * c;
-  tokens_assemble_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(y, bias, cls, b, l, c, x);
+  tokens_assemble_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(
+      y, bias, cls, pos_spatial, pos_temporal, pos_class, b, l, any ? hw : 1, c, x);
   SFB_MV_CHECK("sfb_tokens_assemble");
+  return 0;
+}
+extern "C" int32_t sfb_segment_slabs(int32_t groups, int32_t seg_rows) {
+  // about two blocks per SM over all groups, and at least 8 rows per slab
+  int32_t s = (296 + groups - 1) / std::max(groups, 1);
+  s = std::min(s, (seg_rows + 7) / 8);
+  return std::max(s, 1);
+}
+static int segment_rowsum(const float* src, int c, int n_outer, int64_t outer_stride, int64_t group_stride, int seg_rows,
+                          int groups, float scale, float* out, float* partials, cudaStream_t stream) {
+  const int nslab = sfb_segment_slabs(groups, seg_rows);
+  const int threads = std::min(256, (c + 31) / 32 * 32);
+  segment_rowsum_partial_kernel<<<dim3(nslab, groups), threads, 0, stream>>>(src, c, n_outer, outer_stride, group_stride,
+                                                                             seg_rows, partials);
+  SFB_MV_CHECK("segment_rowsum");
+  segment_rowsum_merge_kernel<<<mv_grid(int64_t(groups) * c, 256), 256, 0, stream>>>(partials, nslab, groups, c, scale,
+                                                                                    out);
+  SFB_MV_CHECK("segment_rowsum(merge)");
+  return 0;
+}
+extern "C" int sfb_pos_embed_sep_bwd(const float* dx, int32_t b, int32_t t, int32_t hw, int32_t c, float* dps, float* dpt,
+                                     float* dpc, float* partials, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (b < 1 || t < 1 || hw < 1 || c < 1) {
+    set_error("sfb_pos_embed_sep_bwd: b=%d t=%d hw=%d c=%d", b, t, hw, c);
+    return -10;
+  }
+  pos_sep_bwd_spatial_kernel<<<mv_grid(int64_t(hw + 1) * c, 256), 256, 0, stream>>>(dx, b, t, hw, c, dps, dpc);
+  SFB_MV_CHECK("sfb_pos_embed_sep_bwd");
+  const int64_t n = 1 + int64_t(t) * hw;
+  return segment_rowsum(dx + c, c, b, n, hw, hw, t, 1.f, dpt, partials, stream);
+}
+extern "C" int sfb_token_mean_fwd(const float* x, int32_t b, int32_t n, int32_t c, float* out, float* partials,
+                                  void* stream) {
+  if (b < 1 || n < 2 || c < 1) {
+    set_error("sfb_token_mean_fwd: b=%d n=%d c=%d (needs a token besides cls)", b, n, c);
+    return -10;
+  }
+  return segment_rowsum(x + c, c, 1, 0, n, n - 1, b, 1.f / float(n - 1), out, partials, (cudaStream_t)stream);
+}
+extern "C" int sfb_token_mean_bwd(const float* dmean, int32_t b, int32_t n, int32_t c, float* dx, void* stream) {
+  if (b < 1 || n < 2 || c < 1) {
+    set_error("sfb_token_mean_bwd: b=%d n=%d c=%d (needs a token besides cls)", b, n, c);
+    return -10;
+  }
+  token_mean_bwd_kernel<<<mv_grid(int64_t(b) * n * c, 256), 256, 0, (cudaStream_t)stream>>>(dmean, b, n, c,
+                                                                                           1.f / float(n - 1), dx);
+  SFB_MV_CHECK("sfb_token_mean_bwd");
+  return 0;
+}
+extern "C" int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt, int32_t kh,
+                            int32_t kw, void* hi, void* lo, void* stream) {
+  if (kt < 1 || kh < 1 || kw < 1 || t < kt || h < kh || w < kw || (cin * kt * kh * kw) % 8 != 0) {
+    set_error("sfb_patchify: kernel %dx%dx%d over %dx%dx%d with %d channels (K must be a multiple of 8)", kt, kh, kw, t,
+              h, w, cin);
+    return -10;
+  }
+  const int ot = t / kt, oh = h / kh, ow = w / kw;
+  const int64_t items = int64_t(b) * ot * oh * ow * cin * kt * kh * kw;
+  patchify_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, b, cin, t, h, w, kt, kh, kw, ot, oh, ow,
+                                                                         (bf*)hi, (bf*)lo);
+  SFB_MV_CHECK("sfb_patchify");
   return 0;
 }
 extern "C" int sfb_tokens_split_grad(const float* dx, int32_t b, int32_t l, int32_t c, void* dy_hi, void* dy_lo,

@@ -317,8 +317,13 @@ _SIGNATURES = [
     ("sfb_rowslab_blocks", C.c_int32, [C.c_int64]),
     ("sfb_layernorm_bwd", C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     ("sfb_colsum", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
-    ("sfb_tokens_assemble", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    ("sfb_tokens_assemble", C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]),
     ("sfb_tokens_split_grad", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("sfb_segment_slabs", C.c_int32, [C.c_int32, C.c_int32]),
+    ("sfb_pos_embed_sep_bwd", C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 5),
+    ("sfb_token_mean_fwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
+    ("sfb_token_mean_bwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 2),
+    ("sfb_patchify", C.c_int, [C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p] * 3),
     ("sfb_dwpool_fwd", C.c_int, [C.POINTER(DwPoolDesc), C.c_void_p]),
     ("sfb_dwpool_wgrad_blocks", C.c_int32, [C.POINTER(DwPoolDesc)]),
     ("sfb_dwpool_bwd", C.c_int, [C.POINTER(DwPoolDesc), C.c_void_p, C.c_int32, C.c_void_p]),

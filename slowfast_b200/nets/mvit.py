@@ -10,8 +10,10 @@ Execution:
     decomposed relative-position bias is ONE extra GEMM of q against the concatenated [Rh;Rw;Rt] tables plus an
     index lookup inside the softmax kernel (SURVEY.md section 7.6: identical to cal_rel_pos_spatial/_temporal);
   * LayerNorm, GELU, residual/bias/stochastic-depth combines, max-pool skip are fused row kernels.
-Scope: the MViTv2 configuration family of the reference's Kinetics configs (cls token on, no absolute position
-embedding, conv pooling, pool_first False, DIM_MUL_IN_ATT True).
+Scope: the MViTv2 configuration family of the reference's Kinetics configs (cls token on, conv pooling, pool_first False,
+both DIM_MUL_IN_ATT modes), MViTv1 and ViT with separable absolute position tables (SEP_POS_EMBED) added in the token
+assembly, and the mean-token readout (USE_MEAN_POOLING) of the MaskFeat fine-tuning recipes.  A patch embedding with
+stride == kernel and no padding (ViT's 2x16x16) is packed into rows and runs as one plain GEMM.
 """
 from __future__ import annotations
 
@@ -192,13 +194,14 @@ class B200MViT(nn.Module):
         super().__init__()
         mv = cfg.MVIT
         assert cfg.DATA.TRAIN_CROP_SIZE == cfg.DATA.TEST_CROP_SIZE
-        assert mv.MODE == "conv" and mv.CLS_EMBED_ON and not mv.USE_ABS_POS and not mv.POOL_FIRST
-        assert not mv.SEPARATE_QKV and not mv.NORM_STEM and not mv.USE_MEAN_POOLING
-        assert not mv.PATCH_2D and not mv.REV.ENABLE and not cfg.DETECTION.ENABLE and mv.NORM == "layernorm"
-        assert float(mv.LAYER_SCALE_INIT_VALUE) == 0.0 and float(mv.DROPOUT_RATE) == 0.0
+        assert mv.MODE == "conv" and not mv.POOL_FIRST
+        assert not mv.SEPARATE_QKV and not mv.NORM_STEM
+        assert not cfg.DETECTION.ENABLE and mv.NORM == "layernorm"
+        assert float(mv.LAYER_SCALE_INIT_VALUE) == 0.0
+        self.specs = block_specs(cfg)
+        self._reject_unsupported(cfg, self.specs)
         self.cfg = cfg
         self.ctx = Ctx(nsplit_of(cfg))
-        self.specs = block_specs(cfg)
         self.patch_stride = list(mv.PATCH_STRIDE)
         self.T = cfg.DATA.NUM_FRAMES // self.patch_stride[0]
         self.H = cfg.DATA.TRAIN_CROP_SIZE // self.patch_stride[1]
@@ -206,9 +209,19 @@ class B200MViT(nn.Module):
         self.num_classes = cfg.MODEL.NUM_CLASSES
         self.residual_pooling = bool(mv.RESIDUAL_POOLING)
         self.dim_mul_in_att = bool(mv.DIM_MUL_IN_ATT)
-        self.patch_embed = PatchEmbedModule(cfg.DATA.INPUT_CHANNEL_NUM[0], mv.EMBED_DIM, mv.PATCH_KERNEL, mv.PATCH_STRIDE,
-                                            mv.PATCH_PADDING)
+        self.use_abs_pos = bool(mv.USE_ABS_POS)
+        self.use_mean_pooling = bool(mv.USE_MEAN_POOLING)
+        cin = cfg.DATA.INPUT_CHANNEL_NUM[0]
+        # non-overlapping patches (ViT's 2x16x16) are packed into rows and run as one plain GEMM; overlapping ones
+        # (MViT's 3x7x7 / stride 2x4x4) take the implicit-GEMM convolution
+        self.patchify = (list(mv.PATCH_KERNEL) == list(mv.PATCH_STRIDE) and not any(mv.PATCH_PADDING)
+                         and cin * math.prod(mv.PATCH_KERNEL) % 8 == 0)
+        self.patch_embed = PatchEmbedModule(cin, mv.EMBED_DIM, mv.PATCH_KERNEL, mv.PATCH_STRIDE, mv.PATCH_PADDING)
         self.cls_token = nn.Parameter(torch.zeros(1, 1, mv.EMBED_DIM))
+        if self.use_abs_pos:  # video_model_builder.py:892-901 (zeros: no RNG draw here)
+            self.pos_embed_spatial = nn.Parameter(torch.zeros(1, self.H * self.W, mv.EMBED_DIM))
+            self.pos_embed_temporal = nn.Parameter(torch.zeros(1, self.T, mv.EMBED_DIM))
+            self.pos_embed_class = nn.Parameter(torch.zeros(1, 1, mv.EMBED_DIM))
         self.blocks = nn.ModuleList()
         for spec in self.specs:
             self.blocks.append(BlockModule(spec, mv.MLP_RATIO, mv.QKV_BIAS, mv.REL_POS_SPATIAL, mv.REL_POS_TEMPORAL,
@@ -216,6 +229,10 @@ class B200MViT(nn.Module):
         embed = self.specs[-1]["dim_out"]
         self.norm = nn.LayerNorm(embed, eps=1e-6)
         self.head = TransformerHeadModule(embed, self.num_classes, cfg.MODEL.DROPOUT_RATE, cfg.MODEL.HEAD_ACT)
+        if self.use_abs_pos:  # drawn after the head and before cls_token, as the reference does (:1057-1077)
+            nn.init.trunc_normal_(self.pos_embed_spatial, std=0.02)
+            nn.init.trunc_normal_(self.pos_embed_temporal, std=0.02)
+            nn.init.trunc_normal_(self.pos_embed_class, std=0.02)
         nn.init.trunc_normal_(self.cls_token, std=0.02)
         self.apply(self._init_weights)
         self.head.projection.weight.data.mul_(mv.HEAD_INIT_SCALE)
@@ -229,6 +246,29 @@ class B200MViT(nn.Module):
             self.cuda_graphs = bool(b200["CUDA_GRAPH"])
         self._seed = int(getattr(cfg, "RNG_SEED", 0))
         object.__setattr__(self, "_saved", None)
+
+    @staticmethod
+    def _reject_unsupported(cfg, specs):
+        """Configurations the reference builds but the engine program does not run fail here, naming the option."""
+        mv = cfg.MVIT
+        bad = [
+            (not mv.CLS_EMBED_ON, "MVIT.CLS_EMBED_ON False (the engine's token layout keeps the cls token first)"),
+            (float(mv.DROPOUT_RATE) != 0.0, "MVIT.DROPOUT_RATE > 0 (position / attention / MLP dropout)"),
+            (bool(mv.PATCH_2D), "MVIT.PATCH_2D (2-D image patch embedding)"),
+            (bool(mv.REV.ENABLE), "MVIT.REV.ENABLE (reversible MViT)"),
+            (bool(mv.USE_ABS_POS) and not mv.SEP_POS_EMBED,
+             "MVIT.USE_ABS_POS with SEP_POS_EMBED False (a joint pos_embed table)"),
+            (bool(mv.USE_FIXED_SINCOS_POS), "MVIT.USE_FIXED_SINCOS_POS (fixed sin-cos position table)"),
+        ]
+        for i, s in enumerate(specs):
+            for name, k, st in (("q", s["kq"], s["sq"]), ("kv", s["kkv"], s["skv"])):
+                # dwpool_bwd's weight gradient accumulates at most 3 taps per axis (csrc/mvit_ops.cu)
+                bad.append((_is_pool(k, st) and max(k) > 3,
+                            f"block {i} {name} pooling kernel {list(k)} (more than 3 taps per axis; set "
+                            f"MVIT.POOL_KVQ_KERNEL, e.g. [3, 3, 3])"))
+        for cond, what in bad:
+            if cond:
+                raise NotImplementedError(f"{what} is not on the engine path")
 
     @staticmethod
     def _init_weights(m):
@@ -245,6 +285,8 @@ class B200MViT(nn.Module):
     def no_weight_decay(self):
         names = []
         if self.cfg.MVIT.ZERO_DECAY_POS_CLS:
+            if self.use_abs_pos:
+                names.extend(["pos_embed_spatial", "pos_embed_temporal", "pos_embed_class"])
             if self.cfg.MVIT.REL_POS_SPATIAL:
                 names.extend(["rel_pos_h", "rel_pos_w", "rel_pos_hw"])
             if self.cfg.MVIT.REL_POS_TEMPORAL:
@@ -267,12 +309,15 @@ class B200MViT(nn.Module):
     # ================================================================================== helpers
     def _lin_fwd(self, key, lin: nn.Linear, x: Planes) -> torch.Tensor:
         """y[rows, out] = x[rows, in] . W^T  (no bias; consumers add it)."""
+        return self._mat_fwd(key, lin.weight, x)
+
+    def _mat_fwd(self, key, weight: torch.Tensor, x: Planes) -> torch.Tensor:
         ctx = self.ctx
-        out_f, in_f = lin.weight.shape
+        out_f, in_f = weight.shape
         f = ctx.scratch("lin.f.hi", out_f * in_f, BF16).view(out_f, in_f)
         flo = ctx.scratch("lin.f.lo", out_f * in_f, BF16).view(out_f, in_f) if ctx.nsplit == 3 else None
         fm = ops.FilterMat(f, flo, out_f, 1, in_f)
-        ops.filter_pack(lin.weight, fm)
+        ops.filter_pack(weight, fm)
         rows = x.rows
         y = ctx.buf(key, (rows, out_f))
         ops.conv_igemm(x, fm, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 0), (x.t, x.h, x.w)), y,
@@ -347,22 +392,35 @@ class B200MViT(nn.Module):
         pe = self.patch_embed.proj
         # ---- patch embedding: clip -> [B, L, 96] (+bias, cls) -------------------------------------------------
         n, cin, t, h, w = x.shape
-        xin = ctx.storage(("pe.in",), n, t, h, w, 8)
-        xin_p = Planes(xin.hi, xin.lo, n, t, h, w, 8, 0)
-        ops.input_pack(x.contiguous().float(), xin_p)
         k3, s3, p3 = tuple(pe.kernel_size), tuple(pe.stride), tuple(pe.padding)
-        taps = k3[0] * k3[1] * k3[2]
         E = pe.out_channels
-        f = ctx.buf(("pe.f.hi",), (E, taps * 8), BF16)
-        flo = ctx.buf(("pe.f.lo",), (E, taps * 8), BF16) if ctx.nsplit == 3 else None
-        fm = ops.FilterMat(f, flo, E, taps, 8)
-        ops.filter_pack(pe.weight, fm)
-        geom = ops.fprop_geom(xin_p, k3, s3, p3)
-        T, H, W = geom.out
-        assert (T, H, W) == (self.T, self.H, self.W), ((T, H, W), (self.T, self.H, self.W))
-        Lt = T * H * W
-        ype = ctx.buf(("pe.y",), (B, Lt, E))
-        ops.conv_igemm(xin_p, fm, geom, ype, (Lt * E, H * W * E, W * E, E), nsplit=ctx.nsplit)
+        if self.patchify:
+            # stride == kernel: the clip packs into [B*L, cin*kt*kh*kw] rows and the weight is a plain [E, K] matrix
+            T, H, W = t // k3[0], h // k3[1], w // k3[2]
+            assert (T, H, W) == (self.T, self.H, self.W), ((T, H, W), (self.T, self.H, self.W))
+            Lt = T * H * W
+            K = cin * math.prod(k3)
+            xin_p = self._rows_planes(("pe.rows",), B * Lt, K)
+            L.check(lib.sfb_patchify(x.contiguous().float().data_ptr(), n, cin, t, h, w, *k3, xin_p.hi_ptr(),
+                                     xin_p.lo_ptr(), _st()), "sfb_patchify")
+            ops._count()
+            geom = None
+            ype = self._mat_fwd(("pe.y",), pe.weight.view(E, K), xin_p)
+        else:
+            xin = ctx.storage(("pe.in",), n, t, h, w, 8)
+            xin_p = Planes(xin.hi, xin.lo, n, t, h, w, 8, 0)
+            ops.input_pack(x.contiguous().float(), xin_p)
+            taps = k3[0] * k3[1] * k3[2]
+            f = ctx.buf(("pe.f.hi",), (E, taps * 8), BF16)
+            flo = ctx.buf(("pe.f.lo",), (E, taps * 8), BF16) if ctx.nsplit == 3 else None
+            fm = ops.FilterMat(f, flo, E, taps, 8)
+            ops.filter_pack(pe.weight, fm)
+            geom = ops.fprop_geom(xin_p, k3, s3, p3)
+            T, H, W = geom.out
+            assert (T, H, W) == (self.T, self.H, self.W), ((T, H, W), (self.T, self.H, self.W))
+            Lt = T * H * W
+            ype = ctx.buf(("pe.y",), (B, Lt, E))
+            ops.conv_igemm(xin_p, fm, geom, ype, (Lt * E, H * W * E, W * E, E), nsplit=ctx.nsplit)
         x0 = ctx.buf(("x", 0), (B, Lt + 1, E))
         self._tokens_assemble(ype, x0, B, Lt, E, inputs)
         # ---- stochastic depth scales ---------------------------------------------------------------------------
@@ -391,10 +449,13 @@ class B200MViT(nn.Module):
 
     # ---- hooks the MaskFeat wrapper overrides -------------------------------------------------------------------
     def _tokens_assemble(self, ype, x0, B, Lt, E, inputs) -> None:
-        """[cls ; patch embedding + bias] (video_model_builder.py:1166-1181)."""
+        """[cls ; patch embedding + bias] (+ separable positions) (video_model_builder.py:1166-1199)."""
         pe = self.patch_embed.proj
-        L.check(L.load().sfb_tokens_assemble(ype.data_ptr(), pe.bias.data_ptr(), self.cls_token.data_ptr(), B, Lt, E,
-                                             x0.data_ptr(), _st()), "sfb_tokens_assemble")
+        pos = [None] * 3
+        if self.use_abs_pos:
+            pos = [p.data_ptr() for p in (self.pos_embed_spatial, self.pos_embed_temporal, self.pos_embed_class)]
+        L.check(L.load().sfb_tokens_assemble(ype.data_ptr(), pe.bias.data_ptr(), self.cls_token.data_ptr(), *pos, B, Lt,
+                                             self.H * self.W, E, x0.data_ptr(), _st()), "sfb_tokens_assemble")
         ops._count()
 
     def _tokens_split_grad(self, dx, B, Lt, E):
@@ -408,12 +469,22 @@ class B200MViT(nn.Module):
         return dyp, dyf
 
     def _final_forward(self, cur: torch.Tensor, thw, B) -> torch.Tensor:
-        """Final LayerNorm on the cls rows + TransformerBasicHead (video_model_builder.py:1200-1215)."""
+        """Final LayerNorm on the cls rows, or on the mean of the other tokens (USE_MEAN_POOLING), + TransformerBasicHead
+        (video_model_builder.py:1230-1242)."""
         ctx = self.ctx
         Nf, Cf = cur.shape[1], cur.shape[2]
+        if self.use_mean_pooling:
+            lib = L.load()
+            ln_in, ln_pitch = ctx.buf(("final.pool",), (B, Cf)), Cf
+            part = ctx.scratch("final.pool.part", B * lib.sfb_segment_slabs(B, Nf - 1) * Cf, F32)
+            L.check(lib.sfb_token_mean_fwd(cur.data_ptr(), B, Nf, Cf, ln_in.data_ptr(), part.data_ptr(), _st()),
+                    "sfb_token_mean_fwd")
+            ops._count(2)
+        else:
+            ln_in, ln_pitch = cur, Nf * Cf
         cls_n = ctx.buf(("final.cls",), (B, Cf))
         fmean, frstd = ctx.buf(("final.mean",), (B,)), ctx.buf(("final.rstd",), (B,))
-        self._ln_fwd(cur, Nf * Cf, B, Cf, self.norm, None, cls_n, fmean, frstd)
+        self._ln_fwd(ln_in, ln_pitch, B, Cf, self.norm, None, cls_n, fmean, frstd)
         head = self.head
         feat = cls_n
         mask = None
@@ -428,15 +499,16 @@ class B200MViT(nn.Module):
         ops.small_linear_fwd(feat, head.projection.weight, head.projection.bias, logits)
         if not ctx.training and head.act_func == "softmax":
             ops.row_softmax(logits)
-        self._saved["final"] = (cur, fmean, frstd, feat, mask)
+        self._saved["final"] = (cur, ln_in, ln_pitch, fmean, frstd, feat, mask)
         return logits
 
     def _final_backward(self, dlogits: torch.Tensor) -> torch.Tensor:
-        """Returns the gradient w.r.t. the block stack output [B, Nf, Cf] (zero except the cls rows)."""
+        """Returns the gradient w.r.t. the block stack output [B, Nf, Cf] (zero except the cls rows, or zero on the cls
+        rows under USE_MEAN_POOLING)."""
         ctx = self.ctx
         sv = self._saved
         B = sv["B"]
-        cur, fmean, frstd, feat, mask = sv["final"]
+        cur, ln_in, ln_pitch, fmean, frstd, feat, mask = sv["final"]
         Nf, Cf = cur.shape[1], cur.shape[2]
         head = self.head
         dfeat = ctx.buf(("head.dfeat",), (B, Cf))
@@ -445,6 +517,13 @@ class B200MViT(nn.Module):
         if mask is not None:
             ops.dropout_bwd(dfeat, mask, head.dropout_rate)
         dx = ctx.scratch("dx.a", B * Nf * Cf, F32).view(B, Nf, Cf)
+        if self.use_mean_pooling:
+            dpool = ctx.scratch("final.dpool", B * Cf, F32).view(B, Cf)
+            self._ln_bwd(dfeat, Cf, ln_in, ln_pitch, B, Cf, self.norm, fmean, frstd, dpool, Cf, False)
+            L.check(L.load().sfb_token_mean_bwd(dpool.data_ptr(), B, Nf, Cf, dx.data_ptr(), _st()),
+                    "sfb_token_mean_bwd")
+            ops._count()
+            return dx
         ops.zero_f32(ops.f32view(dx.view(B * Nf, Cf)))
         self._ln_bwd(dfeat, Cf, cur, Nf * Cf, B, Cf, self.norm, fmean, frstd, dx, Nf * Cf, False)
         return dx
@@ -649,9 +728,23 @@ class B200MViT(nn.Module):
         Lt = T * H * W
         pe = self.patch_embed.proj
         E = pe.out_channels
+        if self.use_abs_pos:
+            part = ctx.scratch("pos.part", T * lib.sfb_segment_slabs(T, H * W) * E, F32)
+            L.check(lib.sfb_pos_embed_sep_bwd(dx.data_ptr(), B, T, H * W, E, ctx.grad_of(self.pos_embed_spatial).data_ptr(),
+                                              ctx.grad_of(self.pos_embed_temporal).data_ptr(),
+                                              ctx.grad_of(self.pos_embed_class).data_ptr(), part.data_ptr(), _st()),
+                    "sfb_pos_embed_sep_bwd")
+            ops._count(3)
         dyp, dyf = self._tokens_split_grad(dx, B, Lt, E)
         self._colsum(dyf, B * Lt, E, ctx.grad_of(pe.bias))
         self._colsum(dx, B, E, ctx.grad_of(self.cls_token).view(E), pitch=(Lt + 1) * E)
+        if self.patchify:
+            xr = sv["xin"]
+            gw = ctx.grad_of(pe.weight).view(E, xr.c)
+            ops.zero_f32(ops.f32view(gw))
+            ops.conv_wgrad(xr, dyp, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 0), (xr.t, xr.h, xr.w)), gw,
+                           nsplit=ctx.nsplit)
+            return [ctx.grad_of(p) for p in params]
         taps = math.prod(pe.kernel_size)
         dwm = ctx.scratch("pe.dwm", E * taps * 8, F32).view(E, taps * 8)
         ops.zero_f32(ops.f32view(dwm))
