@@ -93,7 +93,7 @@ typedef struct sfb_wgrad_desc {
 
 int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream);
 /* Layers with c*cout <= 512 and >= 32768 output positions (the fast pathway's narrow stages) take an fp32 SIMT body inside
- * sfb_conv_wgrad (csrc/conv_wgrad_direct.cu); enabled = 0 keeps every layer on the tensor-core kernel (A/B tests). */
+ * sfb_conv_wgrad (csrc/conv_wgrad_direct.cu); enabled = 0 keeps every layer on the tensor-core kernel (the tests' reference for the SIMT body). */
 int sfb_set_wgrad_direct(int32_t enabled);
 
 /* Zero-fill a [rows, c] fp32 view (row pitch in elements) on the stream (gradient accumulators). */
@@ -121,17 +121,6 @@ int sfb_input_pack(const float* x, int32_t n, int32_t c, int32_t t, int32_t h, i
  * cols_pad >= inner channel count (zero padded). */
 int sfb_filter_pack(const float* w, int32_t cout, int32_t cin, int32_t taps_total, const int32_t* tapmap,
                     int32_t ntaps, int32_t transpose, int32_t cols_pad, void* hi, void* lo, void* stream);
-/* The same packing for MANY filters in one launch (one per phase of a step instead of one per layer).  `jobs_device`
- * is an array in DEVICE memory, sorted by first_block; job k owns grid blocks [first_block, first_block + n_blocks).
- * ntaps <= 32 (larger tap counts - the stems - keep using sfb_filter_pack). */
-typedef struct sfb_pack_job {
-  const float* w; void* hi; void* lo;
-  int32_t cout, cin, taps_total, ntaps, transpose, cols_pad;
-  int32_t first_block, n_blocks;
-  int16_t tapmap[32];
-} sfb_pack_job;
-int32_t sfb_pack_job_size(void);
-int sfb_filter_pack_multi(const sfb_pack_job* jobs_device, int32_t njobs, int32_t total_blocks, void* stream);
 /* wgrad matrix [cout][taps][cin_pad] fp32 -> parameter-gradient layout [cout][cin][taps] (= or +=). */
 int sfb_filter_unpack_grad(const float* dwm, float* dw, int32_t cout, int32_t cin, int32_t taps, int32_t cin_pad,
                            int32_t accumulate, void* stream);
@@ -546,43 +535,6 @@ int sfb_flat_adamw(const void* chunks, int32_t n_chunks, const float* grad, floa
                    int64_t step, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused pooled-attention forward (MultiScaleAttention.forward, attention.py:355-385; rel-pos bias :64-147):
- * O = softmax(scale * q k^T + bias) v per (clip*head), scores and probabilities kept in shared memory.
- * q / k / v: split planes [bh, n, 96] (the LayerNorm-ed pooled tensors); rq = q_nocls . [Rh;Rw;Rt]^T [bh*(nq-1), rq_pitch]
- * or NULL (no rel-pos); out fp32 [bh, nq, 96]; p_hi/p_lo (optional): normalised probabilities as planes [bh*nq, p_pitch]
- * (pad columns zero) for the unfused backward; lse (optional) [bh*nq].  Fused for head_dim 96 and an 8x7x7 key grid
- * (nk = 393: the pooled K/V of 12 of MViTv2-S's 16 blocks) - sfb_attn_fwd_supported() says whether a geometry is; the
- * unfused sequence sfb_gemm_batched -> sfb_softmax_relpos_fwd -> sfb_gemm_batched covers the rest.
- * ---------------------------------------------------------------------------------------------- */
-typedef struct sfb_attn_fwd_desc {
-  const void* q_hi; const void* q_lo; const void* k_hi; const void* k_lo; const void* v_hi; const void* v_lo;
-  const float* rq; int64_t rq_pitch;
-  int32_t bh, nq, nk, hd;
-  int32_t qt, qh, qw, kt, kh, kw;
-  float scale;
-  float* out;
-  void* p_hi; void* p_lo; int64_t p_pitch;
-  float* lse;
-  int32_t nsplit;
-} sfb_attn_fwd_desc;
-int32_t sfb_attn_fwd_supported(int32_t nk, int32_t hd, int32_t kt, int32_t kh, int32_t kw);
-/* First half of the attention backward for the same key grids (attention.py:355-379 through autograd): dP = dO v^T in shared memory,
- * dS = P (dP - sum_k P dP) -> split planes [bh*nq, ds_pitch] (operand of the dq = scale dS k and dk = scale dS^T q products, pad
- * columns zero), and the gradient of the decomposed rel-pos bias, dRQ [bh*(nq-1), rq_pitch] (drq == NULL: no bias).  Replaces
- * sfb_gemm_batched (dP) + sfb_softmax_relpos_bwd.  p_hi / p_lo: the planes sfb_attn_fwd wrote. */
-typedef struct sfb_attn_bwd_desc {
-  const void* do_hi; const void* do_lo; const void* v_hi; const void* v_lo;
-  const void* p_hi; const void* p_lo; int64_t p_pitch;
-  void* ds_hi; void* ds_lo; int64_t ds_pitch;
-  float* drq; int64_t rq_pitch;
-  int32_t bh, nq, nk, hd;
-  int32_t qt, qh, qw, kt, kh, kw;
-  int32_t nsplit;
-} sfb_attn_bwd_desc;
-int sfb_attn_bwd_ds(const sfb_attn_bwd_desc* d, void* stream);
-int sfb_attn_fwd(const sfb_attn_fwd_desc* d, void* stream);
-
-/* ------------------------------------------------------------------------------------------------
  * Device-side input pipeline head (SURVEY.md section 8f-3): uint8 clip [b, t, h, w, 3] (decoder layout) ->
  * fp32 NCTHW [b, 3, t_out, h, w] = (x / 255 - mean[c]) / std[c] at the frames frame_idx[0..t_out) (NULL = all frames).
  * Replaces, on the host side of the reference: tensor_normalize (datasets/utils.py:278-297), the THWC -> CTHW permute
@@ -622,13 +574,6 @@ int sfb_bn_conv_bias(const float* bias, int32_t c, float momentum, int32_t train
  * column sum is the gradient of conv_out's bias. */
 int sfb_planes_to_f32(const void* hi, const void* lo, int64_t rows, int32_t c, int64_t pitch, float* out,
                       int64_t out_pitch, void* stream);
-
-/* Narrow layers (C_in, C_out <= 64, taps*C_in*C_out <= max_macs) of sfb_conv_igemm on the fp32 pipes (csrc/conv_direct.cu)
- * instead of the tensor-core body: same descriptor, same results layout.  max_macs <= 0 keeps the current threshold. */
-int sfb_set_simt_smallc(int32_t enabled, int32_t max_macs);
-
-/* A/B switch of the shared-memory-ring channelwise 3x3x3 kernels (csrc/x3d_ops.cu "v3"); 1 = on (default). */
-int sfb_set_dw3(int32_t enabled);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,6 @@
 // Direct (fp32 SIMT) convolution for SMALL channel counts - an alternative body of sfb_conv_igemm (same descriptor,
-// same packed filter planes, same output view and BatchNorm-partial layout), selected by sfb_conv_igemm when
-// SFB_SIMT_SMALLC=1 and the layer is narrow.
+// same packed filter planes, same output view and BatchNorm-partial layout), selected by sfb_conv_igemm when the layer
+// is narrow.
 //
 // Why: the fast pathway's first stages (8..32 channels, 0.8 M pixels per layer) are bound by the TMA unit's per-pixel
 // request rate on the tensor-core path (profiles/r1c_conv_igemm_notes.md: 113 us for 128 MB), while their arithmetic is
@@ -10,19 +10,13 @@
 // feeds 4 output channels, broadcast across the warp) and writes its fp32 output row.  One block = 128 pixels = one
 // "m-tile", so the per-tile BatchNorm partials have exactly the layout the tensor-core kernel produces.
 //
-// Selection: sfb_set_simt_smallc(enabled, max_macs) at run time (tests / A-B probes), initial value from the environment
-// (SFB_SIMT_SMALLC = 0 | 1, SFB_SIMT_MAX_MACS); layers with C_in, C_out <= 64 and taps*C_in*C_out <= max_macs take this body.
+// Selection (conv_direct_try): C_in <= 8, C_out <= 64, taps*C_in*C_out <= 1024 and the staged filter within 96 KiB of
+// shared memory.
 #include <cstdint>
-#include <cstdlib>
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
 #include "tmap.h"
-
-// shipped default of the switch
-#ifndef SFB_SIMT_DEFAULT
-#define SFB_SIMT_DEFAULT 1
-#endif
 
 namespace sfb {
 
@@ -179,29 +173,17 @@ __global__ void __launch_bounds__(128) conv_direct_kernel(const DirectParams p) 
   }
 }
 
-// 1 = handled here (rc in *rc_out), 0 = not eligible: the caller continues with the tensor-core path
-static int g_simt_enabled = [] { const char* e = getenv("SFB_SIMT_SMALLC"); return e ? int(e[0] == '1') : SFB_SIMT_DEFAULT; }();
-// the fp32 body is meant for layers where ONE pixel is a 16-byte TMA request (C_in = 8); from C_in = 16 on the tensor-core
-// body streams its operands at full rate, so the limit is C_in <= 8 and <= 1024 MAC per pixel (tests/probes/smallc_probe.py
-// compares the two)
-static int g_simt_max_macs = [] { const char* e = getenv("SFB_SIMT_MAX_MACS"); return e ? atoi(e) : 1024; }();
-static int g_simt_max_cin = [] { const char* e = getenv("SFB_SIMT_MAX_CIN"); return e ? atoi(e) : 8; }();
-
-void conv_direct_configure(int enabled, int max_macs) {
-  g_simt_enabled = enabled;
-  if (max_macs > 0) g_simt_max_macs = max_macs;
-}
-
+// 1 = handled here (rc in *rc_out), 0 = not eligible: the caller continues with the tensor-core path.
+// The fp32 body is meant for layers where ONE pixel is a 16-byte TMA request (C_in = 8); from C_in = 16 on the tensor-core
+// body streams its operands at full rate, so the limit is C_in <= 8 and <= 1024 MAC per pixel.
 int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out) {
-  if (!g_simt_enabled) return 0;
   const int taps = d->kt * d->kh * d->kw;
   const int64_t macs = int64_t(taps) * d->c * d->cout;
   int coutp = 8;
   while (coutp < d->cout) coutp <<= 1;
   const size_t smem = (size_t(taps) * d->c * coutp + size_t(8) * coutp + size_t(128) * (coutp + 1)) * sizeof(float) +
                       128 * sizeof(long long) + 8;
-  if (d->c > 64 || d->cout > 64 || macs > g_simt_max_macs || smem > 96 * 1024) return 0;
-  if (d->c > g_simt_max_cin && g_simt_max_macs <= 4096) return 0;  // (probe runs lift both limits through max_macs)
+  if (d->c > 8 || d->cout > 64 || macs > 1024 || smem > 96 * 1024) return 0;
   DirectParams p;
   p.a_hi = (const __nv_bfloat16*)d->a_hi; p.a_lo = (const __nv_bfloat16*)d->a_lo; p.c_pitch = d->c_pitch;
   p.b_hi = (const __nv_bfloat16*)d->b_hi; p.b_lo = (const __nv_bfloat16*)d->b_lo;
@@ -242,8 +224,3 @@ int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out) {
 }
 
 }  // namespace sfb
-
-extern "C" int sfb_set_simt_smallc(int32_t enabled, int32_t max_macs) {
-  sfb::conv_direct_configure(enabled, max_macs);
-  return 0;
-}

@@ -15,7 +15,6 @@
 //   per-channel (sum, sum^2) partials for train-mode BatchNorm ([2][cout][m_tiles]).
 #include <algorithm>
 #include <cstdint>
-#include <cstdlib>
 #include <cstdio>
 
 #include "../../include/slowfast_b200.h"
@@ -27,8 +26,6 @@ namespace sfb {
 constexpr int BLOCK_M = 128;
 constexpr int A_PLANE_BYTES = BLOCK_M * 128;  // 128 pixels x 64 bf16
 constexpr int MAX_STAGES = 8;
-// SFB_CONV_FORCE_IM2COL=1: load tap-free convolutions through the im2col path too (A/B measurements, tests)
-static const bool g_force_im2col = [] { const char* e = getenv("SFB_CONV_FORCE_IM2COL"); return e && e[0] == '1'; }();
 constexpr int EPI_WARPS = 8;                     // two per 32-row quarter of the tile: the pair splits the tile's 16-column chunks
 constexpr int EPI_STAGE_FLOATS = 64;             // per epilogue warp: 32 row offsets (int64)
 constexpr int MMA_WARPS = 8;                     // two warpgroups of 64 tile rows
@@ -60,7 +57,7 @@ struct ConvParams {
   float* stats;
 };
 
-// csrc/conv_direct.cu: opt-in fp32 SIMT body for narrow layers (SFB_SIMT_SMALLC=1); returns 1 when it handled the call
+// csrc/conv_direct.cu: fp32 SIMT body for narrow layers (C_in <= 8); returns 1 when it handled the call
 int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out);
 
 template <int NSPLIT>
@@ -465,7 +462,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
                         d->low_t + (d->out_t - 1) * d->str_t + 1 - d->d};
   const SwizzleBytes aswz = p.CK == 64 ? SWZ_128 : p.CK == 32 ? SWZ_64 : p.CK == 16 ? SWZ_32 : SWZ_NONE;
   p.a_tiled = (taps == 1 && d->str_w == 1 && d->str_h == 1 && d->str_t == 1 && d->low_w == 0 && d->low_h == 0 &&
-               d->low_t == 0 && d->out_w == d->w && d->out_h == d->h && d->out_t == d->d && !g_force_im2col)
+               d->low_t == 0 && d->out_w == d->w && d->out_h == d->h && d->out_t == d->d)
                   ? 1 : 0;
   int rc;
   if (p.a_tiled)

@@ -313,12 +313,8 @@ extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
   const int upper[3] = {d->low_w + (d->out_w - 1) * d->str_w + 1 - d->w, d->low_h + (d->out_h - 1) * d->str_h + 1 - d->h,
                         d->low_t + (d->out_t - 1) * d->str_t + 1 - d->d};
   const SwizzleBytes xswz = p.CK == 64 ? SWZ_128 : p.CK == 32 ? SWZ_64 : p.CK == 16 ? SWZ_32 : SWZ_NONE;
-  {
-    const char* e = getenv("SFB_CONV_FORCE_IM2COL");
-    const bool force = e && e[0] == '1';
-    p.x_tiled = (taps == 1 && d->str_w == 1 && d->str_h == 1 && d->str_t == 1 && d->low_w == 0 && d->low_h == 0 &&
-                 d->low_t == 0 && d->out_w == d->w && d->out_h == d->h && d->out_t == d->d && !force) ? 1 : 0;
-  }
+  p.x_tiled = (taps == 1 && d->str_w == 1 && d->str_h == 1 && d->str_t == 1 && d->low_w == 0 && d->low_h == 0 &&
+               d->low_t == 0 && d->out_w == d->w && d->out_h == d->h && d->out_t == d->d) ? 1 : 0;
   int rc;
   for (int pl = 0; pl < ns; ++pl) {
     if (p.x_tiled)

@@ -151,38 +151,6 @@ __global__ void filter_pack_kernel(const __grid_constant__ FilterPackParams p) {
   }
 }
 
-// All filter matrices of one phase (forward, or backward) in ONE launch: jobs[] lives in device memory, every job owns
-// the contiguous block range [first_block, first_block + n_blocks) of the grid (jobs sorted by first_block).
-__global__ void filter_pack_multi_kernel(const sfb_pack_job* __restrict__ jobs, int njobs) {
-  int lo = 0, hi = njobs - 1;
-  while (lo < hi) {  // last job whose first_block <= blockIdx.x
-    const int mid = (lo + hi + 1) >> 1;
-    if (jobs[mid].first_block <= int(blockIdx.x)) lo = mid; else hi = mid - 1;
-  }
-  const sfb_pack_job& jb = jobs[lo];
-  const int rows = jb.transpose ? jb.cin : jb.cout;
-  const int cols = jb.transpose ? jb.cout : jb.cin;
-  const int64_t items = int64_t(rows) * jb.ntaps * jb.cols_pad;
-  const int lb = int(blockIdx.x) - jb.first_block;
-  __nv_bfloat16* hi_p = reinterpret_cast<__nv_bfloat16*>(jb.hi);
-  __nv_bfloat16* lo_p = reinterpret_cast<__nv_bfloat16*>(jb.lo);
-  for (int64_t i = int64_t(lb) * blockDim.x + threadIdx.x; i < items; i += int64_t(jb.n_blocks) * blockDim.x) {
-    const int cc = int(i % jb.cols_pad);
-    const int64_t t = i / jb.cols_pad;
-    const int j = int(t % jb.ntaps);
-    const int r = int(t / jb.ntaps);
-    float v = 0.f;
-    if (cc < cols) {
-      const int co = jb.transpose ? cc : r;
-      const int ci = jb.transpose ? r : cc;
-      v = jb.w[(int64_t(co) * jb.cin + ci) * jb.taps_total + jb.tapmap[j]];
-    }
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    hi_p[i] = h;
-    if (lo_p) lo_p[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-  }
-}
-
 // wgrad matrix [cout][taps][cin_pad] (fp32) -> parameter-gradient layout [cout][cin][taps]
 __global__ void filter_unpack_grad_kernel(const float* __restrict__ dwm, float* __restrict__ dw, int cout, int cin,
                                           int taps, int cin_pad, int accumulate) {
@@ -795,18 +763,6 @@ extern "C" int sfb_filter_pack(const float* w, int32_t cout, int32_t cin, int32_
   const int64_t items = int64_t(p.rows) * ntaps * cols_pad;
   filter_pack_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
   SFB_LAUNCH_CHECK("sfb_filter_pack");
-  return 0;
-}
-
-extern "C" int32_t sfb_pack_job_size(void) { return int32_t(sizeof(sfb_pack_job)); }
-extern "C" int sfb_filter_pack_multi(const sfb_pack_job* jobs_device, int32_t njobs, int32_t total_blocks,
-                                     void* stream) {
-  if (njobs < 1 || total_blocks < njobs) {
-    set_error("sfb_filter_pack_multi: njobs=%d total_blocks=%d", njobs, total_blocks);
-    return -10;
-  }
-  filter_pack_multi_kernel<<<total_blocks, 256, 0, (cudaStream_t)stream>>>(jobs_device, njobs);
-  SFB_LAUNCH_CHECK("sfb_filter_pack_multi");
   return 0;
 }
 

@@ -370,8 +370,7 @@ extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
   // zeroed here unless the caller accumulates): at least 8 k-blocks (512 reduction elements) per split
   p.k_splits = 1;
   p.kb_per_split = p.k_blocks;
-  static const bool splitk_on = [] { const char* e = getenv("SFB_BGEMM_SPLITK"); return e ? e[0] != '0' : true; }();
-  if (splitk_on && total_tiles * 2 <= bg_sms && p.k_blocks >= 32 && d->ldd == d->n && d->batch_stride_d == int64_t(d->m) * d->ldd) {
+  if (total_tiles * 2 <= bg_sms && p.k_blocks >= 32 && d->ldd == d->n && d->batch_stride_d == int64_t(d->m) * d->ldd) {
     int want = std::min(bg_sms / total_tiles, p.k_blocks / 8);
     if (want > 1) {
       p.kb_per_split = (p.k_blocks + want - 1) / want;

@@ -1148,9 +1148,8 @@ int dw3_run_strided(int mode, const float* x, int64_t x_pitch, int64_t x_so, int
                     const float* dy, int64_t dy_pitch, int64_t dy_so, int64_t dy_si, float* dw, int n_outer, int n_inner,
                     int T, int H, int W, int C, cudaStream_t st);
 }
-static int g_dwpool_ring = [] { const char* e = getenv("SFB_DWPOOL_RING"); return e ? int(e[0] != '0') : 1; }();
 static bool dwpool_ring_ok(const sfb_dwpool_desc* d) {
-  return g_dwpool_ring && d->has_pool && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 1 && d->sw == 1 &&
+  return d->has_pool && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 1 && d->sw == 1 &&
          d->t >= 2 && d->h % 7 == 0 && d->w_ % 7 == 0 && d->ot == d->t && d->oh == d->h && d->ow == d->w_ && d->hd % 4 == 0 &&
          d->src_pitch % 4 == 0 && d->src_c0 % 4 == 0;
 }

@@ -331,8 +331,8 @@ __device__ __forceinline__ float dw2_in(const Dw2Params& p, const float* ptr, fl
   return v;
 }
 
-template <int KT, int KH, int KW, int S, int OTT, int OHT, int OWT, int MAXT = 512, int MINB = 1>
-__global__ void __launch_bounds__(MAXT, MINB) dw2_conv_kernel(const Dw2Params p) {
+template <int KT, int KH, int KW, int S, int OTT, int OHT, int OWT>
+__global__ void __launch_bounds__(512, 1) dw2_conv_kernel(const Dw2Params p) {
   constexpr int IT = OTT - 1 + KT, IH = (OHT - 1) * S + KH, IW = (OWT - 1) * S + KW, TAPS = KT * KH * KW;
   extern __shared__ float red[];  // [SP][2][C]
   const int C = p.C;
@@ -1338,19 +1338,16 @@ static int dw2_cfg(const sfb_dwconv_desc* d) {
   if (d->kt == 5 && d->kh == 1 && d->kw == 1 && d->sh == 1 && d->sw == 1) return 2;
   return -1;
 }
-static const int kDw2Tile[4][3] = {{1, 2, 4}, {1, 1, 4}, {4, 1, 1}, {1, 1, 4}};
-// cfg 3 = cfg 0's layers with a 1x1x4 micro-tile in <= 256-thread blocks at 3 blocks / SM (more warps in flight)
-static const bool g_dw2_small = [] { const char* e = getenv("SFB_DW2_SMALL"); return e && e[0] == '1'; }();
-static int dw2_conv_cfg(int cfg, int c) { return (cfg == 0 && g_dw2_small && c <= 256) ? 3 : cfg; }
-static int dw2_budget(int cfg) { return cfg == 3 ? 256 : 512; }
-static int dw2_sp(int c, int cfg = 0) { return std::max(1, dw2_budget(cfg) / c); }
+static const int kDw2Tile[3][3] = {{1, 2, 4}, {1, 1, 4}, {4, 1, 1}};
+// spatial lanes of a block: 512 threads over the channels
+static int dw2_sp(int c) { return std::max(1, 512 / c); }
 // forward tiling: micro-tiles per sample, tiles (= blocks = BatchNorm partial columns) per sample
 static void dw2_fwd_tiling(int n, int ot, int oh, int ow, int c, int cfg, Dw2Params& p) {
   p.mt_t = (ot + kDw2Tile[cfg][0] - 1) / kDw2Tile[cfg][0];
   p.mt_h = (oh + kDw2Tile[cfg][1] - 1) / kDw2Tile[cfg][1];
   p.mt_w = (ow + kDw2Tile[cfg][2] - 1) / kDw2Tile[cfg][2];
   p.MT = p.mt_t * p.mt_h * p.mt_w;
-  const int sp = dw2_sp(c, cfg);
+  const int sp = dw2_sp(c);
   int want = (148 * 8 + n - 1) / n;
   const int maxt = (p.MT + sp - 1) / sp;
   if (want > maxt) want = maxt;
@@ -1377,12 +1374,11 @@ static void dw2_block_split(Dw2Params& p, int c, int* blocks) {
   *blocks = int((p.total_mts + p.mts_per_block - 1) / p.mts_per_block);
 }
 // v3 (shared-memory ring) eligibility: 3x3x3, stride 1, padding 1, fp32 input, H and W multiples of 7.  tile = 14x14 or 7x7
-static int g_dw3_enabled = [] { const char* e = getenv("SFB_DW3"); return e ? int(e[0] != '0') : 1; }();
 // `samples` x `c` decide between 14x14 tiles (31 % halo) and 7x7 tiles (65 % halo, 4x the blocks): the big tile only when it
 // still yields two blocks per SM (ncu r2h: 48-block launches at 255 GB/s on the 14x14 stages of MViT)
 static int dw3_tile(int t, int h, int w, int ot, int oh, int ow, int kt, int kh, int kw, int st, int sh, int sw, int pt,
                     int ph, int pw, bool f32, int samples, int c, bool wgrad = false) {
-  if (!g_dw3_enabled || !f32 || kt != 3 || kh != 3 || kw != 3 || st != 1 || sh != 1 || sw != 1 || pt != 1 || ph != 1 ||
+  if (!f32 || kt != 3 || kh != 3 || kw != 3 || st != 1 || sh != 1 || sw != 1 || pt != 1 || ph != 1 ||
       pw != 1 || ot != t || oh != h || ow != w || t < 2)
     return 0;
   if (h % 14 == 0 && w % 14 == 0) {
@@ -1443,7 +1439,7 @@ static int dw3_launch(int tile, bool wgrad, Dw2Params& p, cudaStream_t st, int s
 
 // stride (1,2,2) eligibility: 3x3x3, padding 1, fp32 input, even input extents, output extents multiples of 7
 static bool dw3_s2_ok(const sfb_dwconv_desc* d) {
-  return g_dw3_enabled && d->x_f32 != nullptr && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 2 &&
+  return d->x_f32 != nullptr && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 2 &&
          d->sw == 2 && d->pt == 1 && d->ph == 1 && d->pw == 1 && d->ot == d->t && d->h == 2 * d->oh && d->w_ == 2 * d->ow &&
          d->oh % 7 == 0 && d->ow % 7 == 0 && d->t >= 2;
 }
@@ -1476,13 +1472,11 @@ static int dw2_launch_conv(int cfg, const Dw2Params& p, int threads, size_t smem
   static bool attr = false;
   if (!attr) {
     dw2_optin(dw2_conv_kernel<3, 3, 3, 1, 1, 2, 4>);
-    dw2_optin(dw2_conv_kernel<3, 3, 3, 1, 1, 1, 4, 256, 3>);
     dw2_optin(dw2_conv_kernel<3, 3, 3, 2, 1, 1, 4>);
     dw2_optin(dw2_conv_kernel<5, 1, 1, 1, 4, 1, 1>);
     attr = true;
   }
   if (cfg == 0) dw2_conv_kernel<3, 3, 3, 1, 1, 2, 4><<<p.m_tiles, threads, smem, st>>>(p);
-  else if (cfg == 3) dw2_conv_kernel<3, 3, 3, 1, 1, 1, 4, 256, 3><<<p.m_tiles, threads, smem, st>>>(p);
   else if (cfg == 1) dw2_conv_kernel<3, 3, 3, 2, 1, 1, 4><<<p.m_tiles, threads, smem, st>>>(p);
   else dw2_conv_kernel<5, 1, 1, 1, 4, 1, 1><<<p.m_tiles, threads, smem, st>>>(p);
   SFB_X3_CHECK("sfb_dwconv (v2 conv)");
@@ -1517,7 +1511,7 @@ extern "C" int32_t sfb_dwconv_tiles_per_sample(const sfb_dwconv_desc* d) {
   if (cfg == 1 && dw3_s2_ok(d)) return (d->oh / 7) * (d->ow / 7);
   if (cfg >= 0) {
     Dw2Params p;
-    dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, dw2_conv_cfg(cfg, d->c), p);
+    dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg, p);
     return p.tiles_per_sample;
   }
   return dw_tiles_per_sample(d->n, int64_t(d->ot) * d->oh * d->ow);
@@ -1544,11 +1538,10 @@ extern "C" int sfb_dwconv_fwd(const sfb_dwconv_desc* d, void* stream) {
   if (cfg2 >= 0) {
     Dw2Params q;
     dw2_common(q, d);
-    const int ccfg = dw2_conv_cfg(cfg2, d->c);
-    dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, ccfg, q);
+    dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg2, q);
     q.y = d->y; q.y_pitch = d->y_pitch; q.stats = d->stats;
-    const int sp = dw2_sp(d->c, ccfg);
-    return dw2_launch_conv(ccfg, q, sp * d->c, size_t(sp) * 2 * d->c * sizeof(float), (cudaStream_t)stream);
+    const int sp = dw2_sp(d->c);
+    return dw2_launch_conv(cfg2, q, sp * d->c, size_t(sp) * 2 * d->c * sizeof(float), (cudaStream_t)stream);
   }
   if (d->in_scale != nullptr) {
     set_error("sfb_dwconv_fwd: the fused input transform needs an fp32 input and a 3x3x3 / 5x1x1 filter");
@@ -1630,10 +1623,8 @@ extern "C" int sfb_dwconv_bwd(const sfb_dwconv_desc* d, float* dw, void* stream)
           if (int rc = dw3_launch(t3, false, q, st)) return rc;
           return 0;
         }
-        const int ccfg = dw2_conv_cfg(cfg2, d->c);
-        const int csp = dw2_sp(d->c, ccfg);
-        dw2_fwd_tiling(d->n, d->t, d->h, d->w_, d->c, ccfg, q);
-        if (int rc = dw2_launch_conv(ccfg, q, csp * d->c, size_t(csp) * 2 * d->c * sizeof(float), st)) return rc;
+        dw2_fwd_tiling(d->n, d->t, d->h, d->w_, d->c, cfg2, q);
+        if (int rc = dw2_launch_conv(cfg2, q, threads, size_t(sp) * 2 * d->c * sizeof(float), st)) return rc;
       }
     }
     return 0;
@@ -1731,10 +1722,5 @@ extern "C" int sfb_relu_fwd(float* x, int64_t n, void* stream) {
 extern "C" int sfb_relu_bwd(float* dx, const float* y, int64_t n, void* stream) {
   relu_bwd_kernel<<<x3_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(dx, y, n);
   SFB_X3_CHECK("sfb_relu_bwd");
-  return 0;
-}
-
-extern "C" int sfb_set_dw3(int32_t enabled) {
-  sfb::g_dw3_enabled = enabled;
   return 0;
 }

@@ -14,7 +14,6 @@ Building blocks:
 """
 from __future__ import annotations
 
-import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -104,10 +103,6 @@ class Ctx:
         self.flat_grad: Optional[torch.Tensor] = None
         self.grad_slots: Dict[int, torch.Tensor] = {}  # id(param) -> view into flat_grad
         self.training = True
-        # batched filter packing (opt-in): one plan per phase, recorded on the first pass
-        self.pack_plans: Dict[str, ops.PackPlan] = {}
-        self._pack_phase: Optional[str] = None
-        self._pack_recording = False
 
     # arenas -------------------------------------------------------------------------------------------
     def use_arena(self, key) -> "Arena":
@@ -129,41 +124,6 @@ class Ctx:
         self.arena = a
         self._bufs, self._storages, self._scratch = a.bufs, a.storages, a.scratch
         return a
-
-    # batched filter packing --------------------------------------------------------------------------
-    def begin_phase(self, phase: str) -> None:
-        """Called by the model at the start of its forward / backward program."""
-        if not BATCHED_PACK:
-            return
-        self._pack_phase = phase
-        phase = (phase, self.arena.key)
-        self._pack_phase = phase
-        plan = self.pack_plans.get(phase)
-        if plan is not None and plan.ready and plan.signature() == plan._sig:
-            plan.launch()              # every filter of this phase is packed now
-            self._pack_recording = False
-        else:
-            self.pack_plans[phase] = ops.PackPlan()
-            self._pack_recording = True
-
-    def end_phase(self) -> None:
-        if not BATCHED_PACK or self._pack_phase is None:
-            return
-        if self._pack_recording:
-            plan = self.pack_plans[self._pack_phase]
-            if plan.jobs:
-                plan.finalize(self.device)
-        self._pack_phase, self._pack_recording = None, False
-
-    def pack(self, w: torch.Tensor, fm, tapmap=None, transpose: bool = False) -> None:
-        """Filter packing of one layer: immediate (default), or part of the phase's batched launch."""
-        if BATCHED_PACK and self._pack_phase is not None:
-            if not self._pack_recording:
-                if fm.ntaps <= 32:
-                    return             # already packed by begin_phase's launch (static program: same jobs every pass)
-            else:
-                self.pack_plans[self._pack_phase].record(w, fm, tapmap, transpose)
-        ops.filter_pack(w, fm, tapmap=tapmap, transpose=transpose)
 
     # persistent named buffers -------------------------------------------------------------------
     def buf(self, key: Tuple, shape: Sequence[int], dtype=F32, zero: bool = False) -> torch.Tensor:
@@ -244,23 +204,6 @@ def allreduce_flat_gradients(flat: torch.Tensor, params: Sequence[nn.Parameter],
         n = p.numel()
         if p.grad is None or p.grad.data_ptr() != flat.data_ptr() + flat.element_size() * off:
             p.grad = flat[off:off + n].view_as(p)
-
-
-# Second and later data-gradient contributions to one tensor: read-modify-write in the GEMM epilogue (coalesced since
-# the epilogue stores whole 128-byte lines) instead of a scratch tensor + add pass.  Measured SLOWER (the dependent
-# load-add-store chain is latency-bound with 4 epilogue warps: 50.2 vs 37.9 ms/step), so it is opt-in: SFB_RMW_DGRAD=1.
-RMW_DGRAD = os.environ.get("SFB_RMW_DGRAD", "0") != "0"
-# r2: the same accumulation with `red.global.add.v4.f32` (no load, no dependent chain): every element still receives exactly one
-# add per launch, so the result equals the scratch + add pass bit for bit; SFB_ATOMIC_DGRAD=0 = scratch tensor + add pass.
-ATOMIC_DGRAD = os.environ.get("SFB_ATOMIC_DGRAD", "1") != "0"
-# fast-pathway stem weight gradient on the fp32 pipes (csrc/conv_stem.cu, stem_wgrad_direct); 0 = tensor-core W-shift path
-DIRECT_STEM_WGRAD = os.environ.get("SFB_DIRECT_STEM_WGRAD", "1") != "0"
-# Toeplitz wgmma kernels for the 8-channel (fast pathway) stem, csrc/conv_stem8.cu: "0" = W-shift fprop + SIMT wgrad of r1
-STEM_T8 = os.environ.get("SFB_STEM_T8", "1") != "0"
-STEM_T8_WGRAD = os.environ.get("SFB_STEM_T8_WGRAD", "1") != "0"
-# one filter-packing launch per phase (ops.PackPlan) instead of one per layer.  Under CUDA-graph replay the ~250 tiny pack
-# kernels are already hidden, so it stays opt-in; it matters for eager (graph-less) runs.
-BATCHED_PACK = os.environ.get("SFB_BATCHED_PACK", "0") != "0"
 
 
 def _t3(v) -> Tuple[int, int, int]:
@@ -349,7 +292,7 @@ class ConvBN:
         f = ctx.buf((self.name, "f.hi"), (self.cout, self.taps * self.cin_pad), torch.bfloat16)
         flo = ctx.buf((self.name, "f.lo"), f.shape, torch.bfloat16) if ctx.nsplit == 3 else None
         fm = ops.FilterMat(f, flo, self.cout, self.taps, self.cin_pad)
-        ctx.pack(self.conv.weight, fm)
+        ops.filter_pack(self.conv.weight, fm)
         c, cp = self.cout, self.cout_pad
         y = ctx.buf((self.name, "y"), (x.n, ot, oh, ow, cp))
         m_tiles = ops.conv_m_tiles(x.n, geom)
@@ -411,41 +354,27 @@ class ConvBN:
             ops.filter_unpack_grad(dwm, gw, self.cin_pad, accumulate=False)
 
     def dgrad(self, dy: Planes, x_act: Act) -> None:
-        """Data gradient into x_act's gradient storage.  The first contribution is stored directly; later ones go
-        through a scratch tensor of the same geometry and are merged by one coalesced add pass (a read-modify-write
-        GEMM epilogue would touch 32 different cache lines per instruction)."""
+        """Data gradient into x_act's gradient storage.  The first contribution is stored directly; later ones are
+        added in the GEMM epilogue with vector float reductions (``accumulate=2``): every element receives exactly one
+        add per launch, and positions no tap reaches keep their value."""
         ctx = self.ctx
-        n, t, h, w, pitch = x_act.s.shape
+        _, t, h, w, pitch = x_act.s.shape
         plan = dgrad_plan((t, h, w), self.k, self.stride, self.pad)
         acc = x_act.s.grad_written
-        rmw = acc and (RMW_DGRAD or ATOMIC_DGRAD)  # (positions no tap reaches simply keep their value)
-        acc_mode = (2 if ATOMIC_DGRAD and not RMW_DGRAD else 1) if rmw else 0
-        if acc and not rmw:
-            g = ctx.scratch("dgrad.tmp", n * t * h * w * pitch, F32).view(n, t, h, w, pitch)
-            view = F32View(g, n * t * h * w, x_act.c, pitch, x_act.c0)
-        else:
-            g = x_act.s.ensure_grad()
-            view = x_act.grad_view()
-        if plan.needs_zero_fill and not rmw:
-            ops.zero_f32(view)
-        for i, sub in enumerate(plan.subs):
+        g = x_act.s.ensure_grad()
+        if plan.needs_zero_fill and not acc:
+            ops.zero_f32(x_act.grad_view())
+        for sub in plan.subs:
             ntap = len(sub.tapmap)
             cp = ops.pad8(self.cout)
-            if BATCHED_PACK:  # the batched launch packs ahead of time: every (layer, sub-problem) owns its buffers
-                f = ctx.buf((self.name, "dgf.hi", i), (self.cin, ntap * cp), torch.bfloat16)
-                flo = ctx.buf((self.name, "dgf.lo", i), (self.cin, ntap * cp), torch.bfloat16) \
-                    if ctx.nsplit == 3 else None
-            else:
-                f = ctx.scratch("dgf.hi", self.cin * ntap * cp, torch.bfloat16).view(self.cin, ntap * cp)
-                flo = ctx.scratch("dgf.lo", self.cin * ntap * cp, torch.bfloat16).view(self.cin, ntap * cp) \
-                    if ctx.nsplit == 3 else None
+            f = ctx.scratch("dgf.hi", self.cin * ntap * cp, torch.bfloat16).view(self.cin, ntap * cp)
+            flo = ctx.scratch("dgf.lo", self.cin * ntap * cp, torch.bfloat16).view(self.cin, ntap * cp) \
+                if ctx.nsplit == 3 else None
             fm = ops.FilterMat(f, flo, self.cin, ntap, cp)
-            ctx.pack(self.conv.weight, fm, tapmap=sub.tapmap, transpose=True)
+            ops.filter_pack(self.conv.weight, fm, tapmap=sub.tapmap, transpose=True)
             off, strides = dgrad_out_view((t, h, w), self.stride, sub, pitch, x_act.c0)
             ops.conv_igemm(dy, fm, ops.ConvGeom(sub.k, (1, 1, 1), sub.low, sub.out), g, strides, out_offset=off,
-                           accumulate=acc_mode, nsplit=ctx.nsplit)
-        if acc and not rmw:
-            ops.add_f32(x_act.grad_view(), view)
+                           accumulate=2 if acc else 0, nsplit=ctx.nsplit)
         x_act.s.grad_written = True
 
 
@@ -467,7 +396,7 @@ class StemConvBN(ConvBN):
         n, c, t, h, w = x.shape
         self.x_f32 = x.contiguous().float()  # kept for the direct weight-gradient kernel (narrow stems)
         # 8 output channels: one GEMM row = 8 output pixels (Toeplitz operands, csrc/conv_stem8.cu) when the extent allows
-        self.t8 = bool(STEM_T8 and self.cout == 8 and
+        self.t8 = bool(self.cout == 8 and
                        ops.stem8_supported(self.cin, self.cout, self.k, self.stride, self.pad, t, h, w))
         if self.t8:
             xin = Act(self.ctx.storage((key, "t8"), *ops.stem8_plane_dims(n, t, h, w)))
@@ -510,18 +439,18 @@ class StemConvBN(ConvBN):
 
     def wgrad(self, dy: Planes) -> None:
         ctx, g = self.ctx, self.g
-        if self.t8 and STEM_T8_WGRAD and dy.pitch == 8:
+        if self.t8 and dy.pitch == 8:
             dwm = ctx.scratch("dwm", self.cout * g.kfold, F32).view(self.cout, g.kfold)
             ops.zero_f32(ops.f32view(dwm))
             ops.stem8_wgrad(self.x, dy, g, dwm, nsplit=ctx.nsplit)
             ops.stem_filter_unfold_grad(dwm, ctx.grad_of(self.conv.weight), g)
             return
-        if (DIRECT_STEM_WGRAD and self.cout == 8 and self.cin == 3 and self.stride == (1, 2, 2) and self.pad[2] <= 4
+        if (self.cout == 8 and self.cin == 3 and self.stride == (1, 2, 2) and self.pad[2] <= 4
                 and self.cin * self.taps <= 768 and dy.pitch == 8):
             # 8 output channels fill 8 of the 128 UMMA rows: the fp32 SIMT kernel is ~3x faster and exact
             ops.stem_wgrad_direct(self.x_f32, dy, self.k, self.stride, self.pad, ctx.grad_of(self.conv.weight))
             return
-        assert not self.t8, "the W-shift weight gradient needs the W-shift clip layout (SFB_STEM_T8_WGRAD=0 needs the direct kernel)"
+        assert not self.t8, "the W-shift weight gradient needs the W-shift clip layout"
         dwm = ctx.scratch("dwm", self.cout * g.kfold, F32).view(self.cout, g.kfold)
         ops.zero_f32(ops.f32view(dwm))
         ops.stem_wgrad(self.x, dy, g, dwm, nsplit=ctx.nsplit)

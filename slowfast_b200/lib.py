@@ -84,33 +84,6 @@ class BnBwdDesc(C.Structure):
     ]
 
 
-class AttnFwdDesc(C.Structure):
-    """Mirror of ``sfb_attn_fwd_desc``."""
-
-    _fields_ = [
-        ("q_hi", C.c_void_p), ("q_lo", C.c_void_p), ("k_hi", C.c_void_p), ("k_lo", C.c_void_p), ("v_hi", C.c_void_p),
-        ("v_lo", C.c_void_p), ("rq", C.c_void_p), ("rq_pitch", C.c_int64),
-        ("bh", C.c_int32), ("nq", C.c_int32), ("nk", C.c_int32), ("hd", C.c_int32),
-        ("qt", C.c_int32), ("qh", C.c_int32), ("qw", C.c_int32), ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
-        ("scale", C.c_float), ("out", C.c_void_p), ("p_hi", C.c_void_p), ("p_lo", C.c_void_p), ("p_pitch", C.c_int64),
-        ("lse", C.c_void_p), ("nsplit", C.c_int32),
-    ]
-
-
-class AttnBwdDesc(C.Structure):
-    """Mirror of ``sfb_attn_bwd_desc``."""
-
-    _fields_ = [
-        ("do_hi", C.c_void_p), ("do_lo", C.c_void_p), ("v_hi", C.c_void_p), ("v_lo", C.c_void_p),
-        ("p_hi", C.c_void_p), ("p_lo", C.c_void_p), ("p_pitch", C.c_int64),
-        ("ds_hi", C.c_void_p), ("ds_lo", C.c_void_p), ("ds_pitch", C.c_int64),
-        ("drq", C.c_void_p), ("rq_pitch", C.c_int64),
-        ("bh", C.c_int32), ("nq", C.c_int32), ("nk", C.c_int32), ("hd", C.c_int32),
-        ("qt", C.c_int32), ("qh", C.c_int32), ("qw", C.c_int32), ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
-        ("nsplit", C.c_int32),
-    ]
-
-
 class OptChunk(C.Structure):
     """Mirror of ``sfb_opt_chunk``."""
 
@@ -256,16 +229,6 @@ class SeDesc(C.Structure):
     ]
 
 
-class PackJob(C.Structure):
-    _fields_ = [
-        ("w", C.c_void_p), ("hi", C.c_void_p), ("lo", C.c_void_p),
-        ("cout", C.c_int32), ("cin", C.c_int32), ("taps_total", C.c_int32), ("ntaps", C.c_int32),
-        ("transpose", C.c_int32), ("cols_pad", C.c_int32),
-        ("first_block", C.c_int32), ("n_blocks", C.c_int32),
-        ("tapmap", C.c_int16 * 32),
-    ]
-
-
 _SIGNATURES = [
     ("sfb_last_error", C.c_char_p, []),
     ("sfb_abi_version", C.c_int, []),
@@ -352,8 +315,6 @@ _SIGNATURES = [
                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_row_softmax", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_droppath_scales", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
-    ("sfb_pack_job_size", C.c_int32, []),
-    ("sfb_filter_pack_multi", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_stem_wgrad_direct", C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p] + [C.c_int32] * 10 +
      [C.c_void_p, C.c_void_p]),
     ("sfb_dwconv_m_tiles", C.c_int32, [C.POINTER(DwConvDesc)]),
@@ -375,14 +336,9 @@ _SIGNATURES = [
     ("sfb_rows_unpad_bias", C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_void_p]),
     ("sfb_rows_pad_split", C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3),
-    ("sfb_attn_fwd_supported", C.c_int32, [C.c_int32] * 5),
-    ("sfb_attn_fwd", C.c_int, [C.POINTER(AttnFwdDesc), C.c_void_p]),
-    ("sfb_attn_bwd_ds", C.c_int, [C.POINTER(AttnBwdDesc), C.c_void_p]),
     ("sfb_clip_normalize_pack", C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                           C.c_int32, C.c_void_p, C.c_void_p]),
     ("sfb_allreduce_flat", C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p]),
-    ("sfb_set_simt_smallc", C.c_int, [C.c_int32, C.c_int32]),
-    ("sfb_set_dw3", C.c_int, [C.c_int32]),
     ("sfb_opt_chunk_size", C.c_int32, []),
     ("sfb_flat_sumsq_blocks", C.c_int32, []),
     ("sfb_flat_sumsq", C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),

@@ -19,7 +19,6 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 from typing import List, Optional
 
 import torch
@@ -166,14 +165,6 @@ class TransformerHeadModule(Namespace):
         self.projection = nn.Linear(dim_in, num_classes, bias=True)
         self.dropout_rate = dropout_rate
         self.act_func = act_func
-
-
-# fused pooled attention (csrc/attn_fused.cu), opt-in with SFB_ATTN_FUSED=1 / SFB_ATTN_FUSED_BWD=1: on one H100 (400 W) the
-# MViTv2-S step runs 59.0 clips/s with it and 67.3 with the unfused sequence (gemm_batched -> softmax_relpos -> gemm_batched),
-# because the fused kernel is not yet tuned (one warpgroup per CTA, loads not overlapped with the MMAs)
-ATTN_FUSED = os.environ.get("SFB_ATTN_FUSED", "0") != "0"
-# fused first half of the attention backward (dP in shared memory -> dS planes + dRQ); 0 = dP GEMM + softmax_relpos_bwd
-ATTN_FUSED_BWD = os.environ.get("SFB_ATTN_FUSED_BWD", "0") != "0"
 
 
 def _ptr(t):
@@ -585,15 +576,10 @@ class B200MViT(nn.Module):
         Nq, Nk = Lq + 1, Lk + 1
         Nkp = ops.pad8(Nk)
         BH = B * Hn
-        # fused path (csrc/attn_fused.cu): S, the rel-pos bias, the softmax and P.V in ONE kernel with the scores in shared memory,
-        # for the geometry it covers (head_dim 96, 8x7x7 key grid: 12 of MViTv2-S's 16 blocks); else the unfused sequence
-        fused = bool(ATTN_FUSED and lib.sfb_attn_fwd_supported(Nk, hd, *k_thw))
-        S = None
-        if not fused:
-            # S = scale * q k^T
-            S = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
-            self._bgemm(pl["q"], (hd, Nq * hd), False, pl["k"], (hd, Nk * hd), False, Nq, Nk, hd, BH, S, Nkp,
-                        alpha=hd ** -0.5)
+        # S = scale * q k^T
+        S = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
+        self._bgemm(pl["q"], (hd, Nq * hd), False, pl["k"], (hd, Nk * hd), False, Nq, Nk, hd, BH, S, Nkp,
+                    alpha=hd ** -0.5)
         # decomposed relative positions: RQ = q_nocls . [Rh; Rw; Rt]^T
         rq, Ltp, tab = None, 0, None
         has_rel = hasattr(at, "rel_pos_h")
@@ -624,34 +610,18 @@ class B200MViT(nn.Module):
                            (Lq * Ltp, Lq * Ltp, Lq * Ltp, Ltp), nsplit=ctx.nsplit)
         P = self._rows_planes(("b", i, "P"), BH * Nq, Nkp)
         O = ctx.scratch("attn.O", BH * Nq * hd, F32).view(BH, Nq, hd)
-        if fused:
-            fd = L.AttnFwdDesc()
-            fd.q_hi, fd.q_lo = pl["q"].hi_ptr(), pl["q"].lo_ptr()
-            fd.k_hi, fd.k_lo = pl["k"].hi_ptr(), pl["k"].lo_ptr()
-            fd.v_hi, fd.v_lo = pl["v"].hi_ptr(), pl["v"].lo_ptr()
-            fd.rq, fd.rq_pitch = _ptr(rq), Ltp
-            fd.bh, fd.nq, fd.nk, fd.hd = BH, Nq, Nk, hd
-            fd.qt, fd.qh, fd.qw = q_thw
-            fd.kt, fd.kh, fd.kw = k_thw
-            fd.scale = hd ** -0.5
-            fd.out = O.data_ptr()
-            fd.p_hi, fd.p_lo, fd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp   # (the unfused backward reads P)
-            fd.nsplit = ctx.nsplit
-            L.check(lib.sfb_attn_fwd(C.byref(fd), _st()), "sfb_attn_fwd")
-            ops._count()
-        else:
-            # softmax (+ bias) -> P planes
-            sd = L.SoftmaxDesc()
-            sd.s, sd.s_pitch = S.data_ptr(), Nkp
-            sd.rq, sd.rq_pitch = _ptr(rq), Ltp
-            sd.p_hi, sd.p_lo, sd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
-            sd.bh, sd.nq, sd.nk = BH, Nq, Nk
-            sd.qt, sd.qh, sd.qw = q_thw
-            sd.kt, sd.kh, sd.kw = k_thw
-            L.check(lib.sfb_softmax_relpos_fwd(C.byref(sd), _st()), "sfb_softmax_relpos_fwd")
-            ops._count()
-            # O = P v  (v is MN-major: memory [bh][k][hd])
-            self._bgemm(P, (Nkp, Nq * Nkp), False, pl["v"], (hd, Nk * hd), True, Nq, hd, Nk, BH, O, hd)
+        # softmax (+ bias) -> P planes
+        sd = L.SoftmaxDesc()
+        sd.s, sd.s_pitch = S.data_ptr(), Nkp
+        sd.rq, sd.rq_pitch = _ptr(rq), Ltp
+        sd.p_hi, sd.p_lo, sd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
+        sd.bh, sd.nq, sd.nk = BH, Nq, Nk
+        sd.qt, sd.qh, sd.qw = q_thw
+        sd.kt, sd.kh, sd.kw = k_thw
+        L.check(lib.sfb_softmax_relpos_fwd(C.byref(sd), _st()), "sfb_softmax_relpos_fwd")
+        ops._count()
+        # O = P v  (v is MN-major: memory [bh][k][hd])
+        self._bgemm(P, (Nkp, Nq * Nkp), False, pl["v"], (hd, Nk * hd), True, Nq, hd, Nk, BH, O, hd)
         merged = self._rows_planes(("b", i, "merged"), B * Nq, A)
         L.check(lib.sfb_attn_merge(O.data_ptr(), pl["q"].hi_ptr(), pl["q"].lo_ptr(), B, Hn, Nq, hd,
                                    1 if self.residual_pooling else 0, merged.hi_ptr(), merged.lo_ptr(), _st()),
@@ -708,7 +678,7 @@ class B200MViT(nn.Module):
         ops._count()
         sv = dict(x_in=x_in, thw=list(thw), xn=xn, mean1=mean1, rstd1=rstd1, yqkv=yqkv, pooled=pooled, pl=pl,
                   stats=stats, geo=geo, P=P, tab=tab, Ltp=Ltp, merged=merged, x1=x1, x1n=x1n, mean2=mean2, rstd2=rstd2,
-                  yfc1=yfc1, hpl=hpl, amax=amax, pool_skip=pool_skip, q_thw=q_thw, k_thw=k_thw, s1=s1, s2=s2, fused=fused)
+                  yfc1=yfc1, hpl=hpl, amax=amax, pool_skip=pool_skip, q_thw=q_thw, k_thw=k_thw, s1=s1, s2=s2)
         return x2, list(q_thw), sv
 
     # ================================================================================== backward program
@@ -818,33 +788,18 @@ class B200MViT(nn.Module):
         dS = self._rows_planes("attn.dS", BH * Nq, Nkp, scratch=True)
         Ltp = sv["Ltp"]
         drq = ctx.scratch("attn.RQ", BH * Lq * Ltp, F32).view(BH * Lq, Ltp) if Ltp else None
-        if sv["fused"] and ATTN_FUSED_BWD and Nkp == 400:
-            # dP = dO v^T stays in shared memory; dS planes and dRQ come out of one kernel (csrc/attn_fused.cu)
-            bd = L.AttnBwdDesc()
-            bd.do_hi, bd.do_lo = dO.hi_ptr(), dO.lo_ptr()
-            bd.v_hi, bd.v_lo = pl["v"].hi_ptr(), pl["v"].lo_ptr()
-            bd.p_hi, bd.p_lo, bd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
-            bd.ds_hi, bd.ds_lo, bd.ds_pitch = dS.hi_ptr(), dS.lo_ptr(), Nkp
-            bd.drq, bd.rq_pitch = _ptr(drq), Ltp
-            bd.bh, bd.nq, bd.nk, bd.hd = BH, Nq, Nk, hd
-            bd.qt, bd.qh, bd.qw = q_thw
-            bd.kt, bd.kh, bd.kw = k_thw
-            bd.nsplit = ctx.nsplit
-            L.check(lib.sfb_attn_bwd_ds(C.byref(bd), _st()), "sfb_attn_bwd_ds")
-            ops._count()
-        else:
-            dP = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
-            self._bgemm(dO, (hd, Nq * hd), False, pl["v"], (hd, Nk * hd), False, Nq, Nk, hd, BH, dP, Nkp)
-            sd = L.SoftmaxDesc()
-            sd.p_hi, sd.p_lo, sd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
-            sd.bh, sd.nq, sd.nk = BH, Nq, Nk
-            sd.qt, sd.qh, sd.qw = q_thw
-            sd.kt, sd.kh, sd.kw = k_thw
-            sd.dp, sd.dp_pitch = dP.data_ptr(), Nkp
-            sd.ds_hi, sd.ds_lo, sd.ds_pitch = dS.hi_ptr(), dS.lo_ptr(), Nkp
-            sd.drq, sd.rq_pitch = _ptr(drq), Ltp
-            L.check(lib.sfb_softmax_relpos_bwd(C.byref(sd), _st()), "sfb_softmax_relpos_bwd")
-            ops._count()
+        dP = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
+        self._bgemm(dO, (hd, Nq * hd), False, pl["v"], (hd, Nk * hd), False, Nq, Nk, hd, BH, dP, Nkp)
+        sd = L.SoftmaxDesc()
+        sd.p_hi, sd.p_lo, sd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
+        sd.bh, sd.nq, sd.nk = BH, Nq, Nk
+        sd.qt, sd.qh, sd.qw = q_thw
+        sd.kt, sd.kh, sd.kw = k_thw
+        sd.dp, sd.dp_pitch = dP.data_ptr(), Nkp
+        sd.ds_hi, sd.ds_lo, sd.ds_pitch = dS.hi_ptr(), dS.lo_ptr(), Nkp
+        sd.drq, sd.rq_pitch = _ptr(drq), Ltp
+        L.check(lib.sfb_softmax_relpos_bwd(C.byref(sd), _st()), "sfb_softmax_relpos_bwd")
+        ops._count()
         scale = hd ** -0.5
         # dq += scale * dS k ;  dk = scale * dS^T q
         self._bgemm(dS, (Nkp, Nq * Nkp), False, pl["k"], (hd, Nk * hd), True, Nq, hd, Nk, BH, dq, hd, alpha=scale,

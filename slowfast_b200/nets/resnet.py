@@ -643,7 +643,6 @@ class B200SlowFast(_VideoResNetBase):
         ctx = self.ctx
         ctx.device = inputs[0].device
         ctx.training = self.training
-        ctx.begin_phase("fwd")
         if inputs[0].device.type != "cuda":
             raise ops.L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         u = self._engine_units()
@@ -689,7 +688,6 @@ class B200SlowFast(_VideoResNetBase):
         if ctx.training:
             bump_num_batches_tracked(self._train_bns())
         out = self._head_forward([slow, fast])
-        ctx.end_phase()
         return out
 
     def _fuse_forward(self, i: int, fast: Act, out: Act) -> None:
@@ -703,7 +701,6 @@ class B200SlowFast(_VideoResNetBase):
         ctx = self.ctx
         params = [p for p in self.parameters()]
         ctx.begin_backward(params)
-        ctx.begin_phase("bwd")
         u = self._engine_units()
         self._head_backward(dlogits)
         for i in range(5, 1, -1):
@@ -718,5 +715,4 @@ class B200SlowFast(_VideoResNetBase):
         u["fuse1"].bwd(out.grad_view(), out.planes, fast)
         self._stem_backward(0, u["stem0"])
         self._stem_backward(1, u["stem1"])
-        ctx.end_phase()
         return [ctx.grad_of(p) for p in params]

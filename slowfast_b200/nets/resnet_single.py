@@ -77,7 +77,6 @@ class B200ResNet(_VideoResNetBase):
         ctx = self.ctx
         ctx.device = inputs[0].device
         ctx.training = self.training
-        ctx.begin_phase("fwd")
         if inputs[0].device.type != "cuda":
             raise ops.L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         u = self._engine_units()
@@ -108,14 +107,12 @@ class B200ResNet(_VideoResNetBase):
         if ctx.training:
             bump_num_batches_tracked(self._train_bns())
         out = self._head_forward([cur])
-        ctx.end_phase()
         return out
 
     def _engine_backward(self, dlogits: torch.Tensor):
         ctx = self.ctx
         params = [p for p in self.parameters()]
         ctx.begin_backward(params)
-        ctx.begin_phase("bwd")
         u = self._engine_units()
         self._head_backward(dlogits)
         for i in range(5, 1, -1):
@@ -129,5 +126,4 @@ class B200ResNet(_VideoResNetBase):
             for bi in reversed(range(stage.num_blocks[0])):
                 stage.run_block_backward(0, bi)
         self._stem_backward(0, u["stem0"])
-        ctx.end_phase()
         return [ctx.grad_of(p) for p in params]

@@ -346,7 +346,6 @@ class B200X3D(_VideoResNetBase):
         ctx = self.ctx
         ctx.device = inputs[0].device
         ctx.training = self.training
-        ctx.begin_phase("fwd")
         if inputs[0].device.type != "cuda":
             raise L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         u = self._engine_units()
@@ -384,7 +383,6 @@ class B200X3D(_VideoResNetBase):
         if ctx.training:
             bump_num_batches_tracked(self._all_bns())
         out = self._x3d_head_forward(cur)
-        ctx.end_phase()
         return out
 
     def _x3d_head_forward(self, feat: Act) -> torch.Tensor:
@@ -422,7 +420,6 @@ class B200X3D(_VideoResNetBase):
         ctx = self.ctx
         params = [p for p in self.parameters()]
         ctx.begin_backward(params)
-        ctx.begin_phase("bwd")
         u, head = self._engine_units(), self.head
         feat, x5, pooled, l5 = self._head_saved
         n, co = l5.shape
@@ -452,7 +449,6 @@ class B200X3D(_VideoResNetBase):
         ops.dwconv_bwd(g, c1, c1, stem.conv.weight, dy1, ctx.grad_of(stem.conv.weight), None, x_f32=ops.f32view(y0),
                        dx_planes=dy0)
         u["xy"].wgrad(dy0)
-        ctx.end_phase()
         return [ctx.grad_of(p) for p in params]
 
 

@@ -942,73 +942,3 @@ def stem_wgrad_direct(x: torch.Tensor, dy: Planes, k, stride, pad, dw: torch.Ten
                                       _stream()), "sfb_stem_wgrad_direct")
     _count(2)
 
-
-# ------------------------------------------------------------------------------------------------ batched filter packing
-class PackPlan:
-    """All filter packs of one phase (forward / backward) of a model step as ONE kernel launch.
-
-    During the first pass of a phase the engine packs layer by layer (``filter_pack``) and ``record``s each job; from
-    the second pass on ``launch`` replays the whole list with ``sfb_filter_pack_multi``.  A job is (weight, FilterMat,
-    tapmap, transpose); the packed buffers must be persistent (not shared scratch)."""
-
-    ITEMS_PER_BLOCK = 256 * 16  # grid-stride work per block of 256 threads
-
-    def __init__(self):
-        self.jobs = []          # (weight tensor, FilterMat, tapmap tuple | None, transpose)
-        self._table = None      # device uint8 tensor holding the sfb_pack_job array
-        self._sig = None
-        self.total_blocks = 0
-
-    def record(self, w: torch.Tensor, out: "FilterMat", tapmap, transpose: bool) -> bool:
-        ntaps = out.ntaps
-        if ntaps > 32:
-            return False  # (stems) stays an individual launch
-        self.jobs.append((w, out, None if tapmap is None else tuple(int(t) for t in tapmap), bool(transpose)))
-        self._table = None
-        return True
-
-    def signature(self):
-        return tuple((w.data_ptr(), o.hi.data_ptr(), None if o.lo is None else o.lo.data_ptr()) for w, o, _, _ in self.jobs)
-
-    @staticmethod
-    def job_blocks(rows: int, ntaps: int, cols_pad: int) -> int:
-        items = rows * ntaps * cols_pad
-        return max(1, min(64, (items + PackPlan.ITEMS_PER_BLOCK - 1) // PackPlan.ITEMS_PER_BLOCK))
-
-    def build_table(self):
-        """ctypes array of sfb_pack_job (host side); returns (array, total_blocks)."""
-        arr = (L.PackJob * len(self.jobs))()
-        first = 0
-        for k, (w, out, tapmap, transpose) in enumerate(self.jobs):
-            cout, cin = w.shape[0], w.shape[1]
-            taps_total = w[0, 0].numel() if w.dim() > 2 else 1
-            j = arr[k]
-            j.w, j.hi, j.lo = w.data_ptr(), out.hi.data_ptr(), _ptr(out.lo)
-            j.cout, j.cin, j.taps_total, j.ntaps = cout, cin, taps_total, out.ntaps
-            j.transpose, j.cols_pad = 1 if transpose else 0, out.cols_pad
-            tm = tapmap if tapmap is not None else tuple(range(out.ntaps))
-            assert len(tm) == out.ntaps and all(0 <= t < taps_total for t in tm)
-            for i, t in enumerate(tm):
-                j.tapmap[i] = t
-            rows = cin if transpose else cout
-            j.first_block = first
-            j.n_blocks = self.job_blocks(rows, out.ntaps, out.cols_pad)
-            first += j.n_blocks
-        return arr, first
-
-    def finalize(self, device) -> None:
-        arr, total = self.build_table()
-        raw = bytes(arr)
-        self._table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(device)
-        self.total_blocks = total
-        self._sig = self.signature()
-
-    @property
-    def ready(self) -> bool:
-        return self._table is not None and len(self.jobs) > 0
-
-    def launch(self) -> None:
-        assert self.ready
-        L.check(L.load().sfb_filter_pack_multi(self._table.data_ptr(), len(self.jobs), self.total_blocks, _stream()),
-                "sfb_filter_pack_multi")
-        _count()

@@ -343,151 +343,3 @@ def test_device_input_pipeline_matches_reference_host_functions(arch, reverse, c
         assert got[p].shape == ref.shape
         assert torch.allclose(got[p].cpu(), ref, rtol=1e-6, atol=1e-6), (got[p].cpu() - ref).abs().max()
 
-
-@pytest.mark.parametrize("q_thw,bh,rel,nsplit", [((8, 7, 7), 2, True, 3), ((8, 14, 14), 3, True, 3), ((8, 28, 28), 1, True, 3),
-                                                  ((8, 14, 14), 2, False, 3), ((8, 14, 14), 2, True, 1)])
-def test_fused_attention_forward(q_thw, bh, rel, nsplit, cuda_device):
-    """sfb_attn_fwd (csrc/attn_fused.cu): O = softmax(scale q k^T + rel-pos bias) v with the scores kept in shared memory, for the
-    8x7x7 key grid (Nk = 393), against fp64 on the operand values the kernel saw (split planes); also the normalised P planes
-    it leaves for the backward and the log-sum-exp.  Tile tails (Nq = 393, 1569, 6273 are not multiples of 64), cls row /
-    column without bias, and the no-rel-pos variant are covered."""
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
-    k_thw = (8, 7, 7)
-    hd = 96
-    qt, qh, qw = q_thw
-    kt, kh, kw = k_thw
-    Lq, Lk = qt * qh * qw, kt * kh * kw
-    Nq, Nk = Lq + 1, Lk + 1
-    assert lib.sfb_attn_fwd_supported(Nk, hd, kt, kh, kw)
-    Nkp = (Nk + 7) // 8 * 8
-    Lh, Lw, Lt = 2 * max(qh, kh) - 1, 2 * max(qw, kw) - 1, 2 * max(qt, kt) - 1
-    Ltp = (Lh + Lw + Lt + 7) // 8 * 8
-    g = torch.Generator().manual_seed(Lq + bh)
-
-    def planes(x):
-        hi = x.bfloat16()
-        lo = (x - hi.float()).bfloat16()
-        return hi.contiguous(), lo.contiguous()
-
-    q = torch.randn(bh, Nq, hd, generator=g).to(dev)
-    k = torch.randn(bh, Nk, hd, generator=g).to(dev)
-    v = torch.randn(bh, Nk, hd, generator=g).to(dev)
-    qh_, ql_ = planes(q)
-    kh_, kl_ = planes(k)
-    vh_, vl_ = planes(v)
-
-    def val(hi, lo):
-        return hi.double() + (lo.double() if nsplit == 3 else 0)
-
-    rq = None
-    if rel:
-        rq = torch.zeros(bh * Lq, Ltp)
-        rq[:, :Lh + Lw + Lt] = torch.randn(bh * Lq, Lh + Lw + Lt, generator=g)
-        rq = rq.to(dev)
-    out = torch.full((bh, Nq, hd), float("nan"), device=dev)
-    p_hi = torch.full((bh * Nq, Nkp), float("nan"), dtype=torch.bfloat16, device=dev)
-    p_lo = torch.full_like(p_hi, float("nan"))
-    lse = torch.full((bh * Nq,), float("nan"), device=dev)
-    d = L.AttnFwdDesc()
-    d.q_hi, d.q_lo, d.k_hi, d.k_lo, d.v_hi, d.v_lo = (qh_.data_ptr(), ql_.data_ptr(), kh_.data_ptr(), kl_.data_ptr(),
-                                                      vh_.data_ptr(), vl_.data_ptr())
-    d.rq, d.rq_pitch = (rq.data_ptr() if rel else None), Ltp
-    d.bh, d.nq, d.nk, d.hd = bh, Nq, Nk, hd
-    d.qt, d.qh, d.qw = q_thw
-    d.kt, d.kh, d.kw = k_thw
-    d.scale = hd ** -0.5
-    d.out, d.p_hi, d.p_lo, d.p_pitch, d.lse = out.data_ptr(), p_hi.data_ptr(), (p_lo.data_ptr() if nsplit == 3 else None), Nkp, lse.data_ptr()
-    d.nsplit = nsplit
-    L.check(lib.sfb_attn_fwd(C.byref(d), _st()), "sfb_attn_fwd")
-    torch.cuda.synchronize()
-    # fp64 reference on the plane values
-    Q, K, V = val(qh_, ql_).cpu(), val(kh_, kl_).cpu(), val(vh_, vl_).cpu()
-    S = (Q @ K.transpose(1, 2)) * hd ** -0.5
-    if rel:
-        r = rq.double().cpu().view(bh, qt, qh, qw, Ltp)
-        ih, iw, it = _rel_index(qh, kh), _rel_index(qw, kw), _rel_index(qt, kt)
-        rel_h = torch.gather(r, 4, ih[None, None, :, None, :].expand(bh, qt, qh, qw, kh))
-        rel_w = torch.gather(r, 4, iw[None, None, None, :, :].expand(bh, qt, qh, qw, kw) + Lh)
-        rel_t = torch.gather(r, 4, it[None, :, None, None, :].expand(bh, qt, qh, qw, kt) + Lh + Lw)
-        bias = (rel_t[..., :, None, None] + rel_h[..., None, :, None] + rel_w[..., None, None, :]).reshape(bh, Lq, Lk)
-        S = S + F.pad(bias, (1, 0, 1, 0))
-    Pr = torch.softmax(S, dim=-1)
-    Or = Pr @ V
-    tol = 3e-5 if nsplit == 3 else 2e-2
-    got_p = (p_hi.float() + (p_lo.float() if nsplit == 3 else 0)).cpu().view(bh, Nq, Nkp)
-    assert not torch.isnan(out).any() and not torch.isnan(got_p).any()
-    assert relerr(got_p[..., :Nk], Pr) < tol, relerr(got_p[..., :Nk], Pr)
-    assert (got_p[..., Nk:] == 0).all()
-    assert relerr(out.cpu(), Or) < tol, relerr(out.cpu(), Or)
-    assert relerr(lse.cpu().view(bh, Nq), torch.logsumexp(S, dim=-1)) < (1e-5 if nsplit == 3 else 2e-2)
-
-
-@pytest.mark.parametrize("q_thw,bh,rel,nsplit", [((8, 7, 7), 2, True, 3), ((8, 14, 14), 3, True, 3), ((8, 28, 28), 1, True, 3),
-                                                  ((8, 14, 14), 2, False, 3), ((8, 14, 14), 2, True, 1)])
-def test_fused_attention_backward_ds(q_thw, bh, rel, nsplit, cuda_device):
-    """sfb_attn_bwd_ds (csrc/attn_fused.cu): dP = dO v^T in shared memory, dS = P (dP - sum_k P dP) as planes, and the gradient of the
-    decomposed rel-pos bias dRQ, against fp64 on the
-    operand values the kernel saw."""
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
-    k_thw = (8, 7, 7)
-    hd = 96
-    qt, qh, qw = q_thw
-    kt, kh, kw = k_thw
-    Lq, Lk = qt * qh * qw, kt * kh * kw
-    Nq, Nk = Lq + 1, Lk + 1
-    Nkp = (Nk + 7) // 8 * 8
-    assert Nkp == 400
-    Lh, Lw, Lt = 2 * max(qh, kh) - 1, 2 * max(qw, kw) - 1, 2 * max(qt, kt) - 1
-    Ltp = (Lh + Lw + Lt + 7) // 8 * 8
-    g = torch.Generator().manual_seed(Lq + 3 * bh)
-
-    def planes(x):
-        hi = x.bfloat16()
-        lo = (x - hi.float()).bfloat16()
-        return hi.contiguous(), lo.contiguous()
-
-    def val(hi, lo):
-        return hi.double() + (lo.double() if nsplit == 3 else 0)
-
-    dO = torch.randn(bh, Nq, hd, generator=g).to(dev)
-    v = torch.randn(bh, Nk, hd, generator=g).to(dev)
-    P = torch.zeros(bh, Nq, Nkp)
-    P[..., :Nk] = torch.softmax(torch.randn(bh, Nq, Nk, generator=g) * 2.0, dim=-1)
-    P = P.to(dev)
-    doh, dol = planes(dO)
-    vh, vl = planes(v)
-    ph, plo = planes(P.view(bh * Nq, Nkp))
-    ds_hi = torch.full((bh * Nq, Nkp), float("nan"), dtype=torch.bfloat16, device=dev)
-    ds_lo = torch.full_like(ds_hi, float("nan"))
-    drq = torch.full((bh * Lq, Ltp), float("nan"), device=dev) if rel else None
-    d = L.AttnBwdDesc()
-    d.do_hi, d.do_lo, d.v_hi, d.v_lo = doh.data_ptr(), dol.data_ptr(), vh.data_ptr(), vl.data_ptr()
-    d.p_hi, d.p_lo, d.p_pitch = ph.data_ptr(), plo.data_ptr(), Nkp
-    d.ds_hi, d.ds_lo, d.ds_pitch = ds_hi.data_ptr(), (ds_lo.data_ptr() if nsplit == 3 else None), Nkp
-    d.drq, d.rq_pitch = (drq.data_ptr() if rel else None), Ltp
-    d.bh, d.nq, d.nk, d.hd = bh, Nq, Nk, hd
-    d.qt, d.qh, d.qw = q_thw
-    d.kt, d.kh, d.kw = k_thw
-    d.nsplit = nsplit
-    L.check(lib.sfb_attn_bwd_ds(C.byref(d), _st()), "sfb_attn_bwd_ds")
-    torch.cuda.synchronize()
-    DO, V, Pv = val(doh, dol).cpu(), val(vh, vl).cpu(), val(ph, plo).cpu().view(bh, Nq, Nkp)[..., :Nk]
-    dP = DO @ V.transpose(1, 2)
-    dS = Pv * (dP - (Pv * dP).sum(-1, keepdim=True))
-    got = (ds_hi.float() + (ds_lo.float() if nsplit == 3 else 0)).cpu().view(bh, Nq, Nkp)
-    tol = 3e-5 if nsplit == 3 else 2e-2
-    assert not torch.isnan(got).any()
-    assert relerr(got[..., :Nk], dS) < tol, relerr(got[..., :Nk], dS)
-    assert (got[..., Nk:] == 0).all()
-    if rel:
-        # dRQ[q, bin] = sum of dS over the keys whose (kh | kw | kt) coordinate looks that bin up, for non-cls (q, k)
-        gS = dS[:, 1:, 1:].reshape(bh, qt, qh, qw, kt, kh, kw)
-        ih, iw, it = _rel_index(qh, kh), _rel_index(qw, kw), _rel_index(qt, kt)
-        ref = torch.zeros(bh, qt, qh, qw, Ltp, dtype=torch.float64)
-        ref.scatter_add_(4, ih[None, None, :, None, :].expand(bh, qt, qh, qw, kh), gS.sum((4, 6)))
-        ref.scatter_add_(4, iw[None, None, None, :, :].expand(bh, qt, qh, qw, kw) + Lh, gS.sum((4, 5)))
-        ref.scatter_add_(4, it[None, :, None, None, :].expand(bh, qt, qh, qw, kt) + Lh + Lw, gS.sum((5, 6)))
-        assert not torch.isnan(drq).any()
-        assert relerr(drq.cpu().view(bh, qt, qh, qw, Ltp), ref) < (5e-5 if nsplit == 3 else 2e-2)

@@ -63,26 +63,3 @@ def test_no_cpu_fallback_other_models(preset, spec):
     with pytest.raises(NativeLibraryError):
         m([torch.zeros(1, 3, 8, 64, 64)])
 
-
-def test_pack_plan_job_table():
-    """ops.PackPlan (opt-in batched filter packing): the job table matches the C struct and partitions the grid."""
-    import ctypes as C
-
-    from slowfast_b200 import lib as L
-    from slowfast_b200 import ops
-    assert L.load().sfb_pack_job_size() == C.sizeof(L.PackJob)
-    plan = ops.PackPlan()
-    w1 = torch.zeros(64, 24, 1, 1, 1)
-    w2 = torch.zeros(32, 16, 1, 3, 3)
-    f1 = ops.FilterMat(torch.zeros(64, 24, dtype=torch.bfloat16), torch.zeros(64, 24, dtype=torch.bfloat16), 64, 1, 24)
-    f2 = ops.FilterMat(torch.zeros(16, 4 * 32, dtype=torch.bfloat16), None, 16, 4, 32)
-    assert plan.record(w1, f1, None, False)
-    assert plan.record(w2, f2, (0, 2, 6, 8), True)
-    big = ops.FilterMat(torch.zeros(8, 49 * 8, dtype=torch.bfloat16), None, 8, 49, 8)
-    assert not plan.record(torch.zeros(8, 3, 1, 7, 7), big, None, False)  # > 32 taps: stays an individual launch
-    arr, total = plan.build_table()
-    assert [arr[0].first_block, arr[1].first_block] == [0, arr[0].n_blocks] and total == arr[0].n_blocks + arr[1].n_blocks
-    assert (arr[1].cout, arr[1].cin, arr[1].taps_total, arr[1].ntaps, arr[1].transpose, arr[1].cols_pad) == (32, 16, 9, 4, 1, 32)
-    assert list(arr[1].tapmap[:4]) == [0, 2, 6, 8] and arr[0].lo != 0 and not arr[1].lo
-    plan.finalize(torch.device("cpu"))
-    assert plan.ready and plan._table.numel() == 2 * C.sizeof(L.PackJob) and plan.signature() == plan._sig
