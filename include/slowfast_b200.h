@@ -510,6 +510,54 @@ int sfb_hog_targets(const float* x, int32_t b, int32_t ch, int32_t t, int32_t h,
                     int32_t nbins, int32_t cell, int32_t fs, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * MAE pre-training (masked.py MaskMViT with MASK.MAE_ON: _mae_random_masking :283, _mae_forward_encoder :319,
+ * _mae_forward_decoder :394, _get_pixel_label_3d :212).  Token indices are int32; every reduction is a fixed-order sum.
+ * ---------------------------------------------------------------------------------------------- */
+/* Largest token count l of sfb_mae_random_masking (one clip's noise row lives in shared memory). */
+int32_t sfb_mae_max_tokens(void);
+/* Replaces argsort(noise) / argsort(ids_shuffle) / gather(mask) of :283-317, one CTA per clip, ties broken by index
+ * (= torch.argsort(noise, dim=1, stable=True)).  noise [b, l] -> ids_keep [b, keep], ids_restore [b, l], mask [b, l]
+ * (1 = removed) and masked_rows [b * (l - keep)]: the removed tokens of clip 0 in ascending position, then clip 1 ...,
+ * each as the row b*(l+1) + 1 + pos of the [b, l+1] decoder sequence. */
+int sfb_mae_random_masking(const float* noise, int32_t b, int32_t l, int32_t keep, int32_t* ids_keep,
+                           int32_t* ids_restore, float* mask, int32_t* masked_rows, void* stream);
+/* sfb_patchify for the kept patches only (replaces patch_embed + gather(x, ids_keep), :320/:311): rows [b * nkeep], row
+ * (b, j) = patch ids_keep[b, j].  keep == NULL runs sfb_patchify. */
+int sfb_patchify_gather(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt, int32_t kh,
+                        int32_t kw, const int32_t* keep, int32_t nkeep, void* hi, void* lo, void* stream);
+/* Encoder tokens (replaces cat(cls, x_masked) + gather(pos_embed, ids_keep), :340-371): x [b, 1+nkeep, c] with
+ * x[b,0] = cls + pos_class; x[b,1+j] = (y[b,j] + bias) + (pos_spatial[m % hw] + pos_temporal[m / hw]), m = ids_keep[b,j]. */
+int sfb_tokens_assemble_keep(const float* y, const float* bias, const float* cls, const float* pos_spatial,
+                             const float* pos_temporal, const float* pos_class, const int32_t* ids_keep, int32_t b,
+                             int32_t nkeep, int32_t l, int32_t hw, int32_t c, float* x, void* stream);
+/* Its backward onto the dense grid (all "="): dense [b, 1+l, c], dense[b,0] = dx[b,0], dense[b,1+m] = dx[b,1+j] for
+ * m = ids_keep[b,j] (found through ids_restore), 0 at removed tokens; sfb_pos_embed_sep_bwd then reduces it. */
+int sfb_tokens_scatter_keep(const float* dx, const int32_t* ids_restore, int32_t b, int32_t nkeep, int32_t l, int32_t c,
+                            float* dense, void* stream);
+/* Decoder tokens (replaces cat(x, mask_tokens) + gather(ids_restore) + decoder_pos_embed, :403-436): out [b, 1+l, c],
+ * out[b,0] = (z[b,0] + bias) + pos[0]; out[b,1+m] = (r < nkeep ? z[b,1+r] + bias : mask_token) + pos[1+m],
+ * r = ids_restore[b,m]; z = decoder_embed GEMM output [b, 1+nkeep, c] without its bias. */
+int sfb_decoder_assemble(const float* z, const float* bias, const float* mask_token, const float* pos,
+                         const int32_t* ids_restore, int32_t b, int32_t nkeep, int32_t l, int32_t c, float* out,
+                         void* stream);
+/* Its backward (all "="): dz[b,0] = dx[b,0], dz[b,1+j] = dx[b,1+ids_keep[b,j]]; dpos[n] = sum_b dx[b,n];
+ * dmask_token = sum over masked_rows of dx.  partials: [sfb_segment_slabs(1, b*(l-nkeep))][c]. */
+int sfb_decoder_assemble_bwd(const float* dx, const int32_t* ids_keep, const int32_t* masked_rows, int32_t b,
+                             int32_t nkeep, int32_t l, int32_t c, float* dz, float* dpos, float* dmask_token,
+                             float* partials, void* stream);
+/* dst[r, :c] = src[(idx ? idx[r] : r) * src_pitch + :c] (+ bias): the removed tokens' rows for the prediction head
+ * (replaces x[mask] of head_helper.py:668) and the projection bias.  sfb_rows_scatter: dst[idx[r]] = src[r]. */
+int sfb_rows_gather(const float* src, int64_t src_pitch, const int32_t* idx, int64_t rows, int32_t c, const float* bias,
+                    float* dst, void* stream);
+int sfb_rows_scatter(const float* src, const int32_t* idx, int64_t rows, int32_t c, float* dst, void* stream);
+/* Normalised-pixel targets (replaces _get_pixel_label_3d, :212-230) for the decoder rows `rows`: x = [b, ch, t, h, w]
+ * fp32, p x p patches, token (tt, hh, ww) on the (t/t_stride, h/p, w/p) grid, u = 1 (TIME_STRIDE_LOSS: frame
+ * tt*t_stride) or t_stride (frames tt*t_stride + [0, u)); out [nrows, u*p*p*ch] in (u, p, q, c) order; norm:
+ * (v - mean) / sqrt(var + 1e-6) with the unbiased variance. */
+int sfb_pixel_targets(const float* x, int32_t b, int32_t ch, int32_t t, int32_t h, int32_t w, int32_t t_stride,
+                      int32_t u, int32_t p, const int32_t* rows, int32_t nrows, int32_t norm, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Optimizer step + gradient norm / clipping on the flat gradient bucket (SURVEY.md section 8f-1).
  * Replaces: torch.optim.SGD(nesterov) / AdamW as built by slowfast/models/optimizer.py:105-136, get_grad_norm_
  * (optimizer.py:362-379) and clip_grad_norm_ / clip coefficient (tools/train_net.py:154-172).

@@ -84,6 +84,9 @@ _DEFAULTS = {
              "TIME_STRIDE_LOSS": True, "NORM_PRED_PIXEL": True, "SCALE_INIT_BY_DEPTH": False, "DECODER_EMBED_DIM": 512,
              "DECODER_SEP_POS_EMBED": False, "DEC_KV_KERNEL": [], "DEC_KV_STRIDE": [], "PRETRAIN_DEPTH": [15],
              "HEAD_TYPE": "separate", "DECODER_DEPTH": 0, "PRED_HOG": False},
+    # AUG / VIS_MASK keys the MAE model reads (slowfast/config/defaults.py:214-234)
+    "AUG": {"MASK_TUBE": False, "MASK_RATIO": 0.0},
+    "VIS_MASK": {"ENABLE": False},
     # X3D defaults (slowfast/config/defaults.py:333-358)
     "X3D": {"WIDTH_FACTOR": 1.0, "DEPTH_FACTOR": 1.0, "BOTTLENECK_FACTOR": 1.0, "DIM_C5": 2048, "DIM_C1": 12,
             "SCALE_RES2": False, "BN_LIN5": False, "CHANNELWISE_3x3x3": True},
@@ -255,6 +258,28 @@ _PRESETS.update({
         "TRAIN": {"BATCH_SIZE": 16},
         "RNG_SEED": 0,
     },
+})
+# configs/masked_ssl/k400_VIT_{B,L,H}_16x4_MAE_PT.yaml (MAE pre-training: 90 % of the 2x16x16 patches removed, a 4-block
+# 512-wide decoder predicting normalised pixels)
+_VIT_MAE = {
+    "DATA": {"NUM_FRAMES": 16, "TRAIN_CROP_SIZE": 224, "TEST_CROP_SIZE": 224, "INPUT_CHANNEL_NUM": [3]},
+    "MVIT": {"ZERO_DECAY_POS_CLS": False, "SEP_POS_EMBED": True, "PATCH_KERNEL": [2, 16, 16], "PATCH_STRIDE": [2, 16, 16],
+             "PATCH_PADDING": [0, 0, 0], "EMBED_DIM": 768, "NUM_HEADS": 12, "MLP_RATIO": 4.0, "QKV_BIAS": True,
+             "NORM": "layernorm", "DEPTH": 12, "DROPPATH_RATE": 0.0, "MODE": "conv", "CLS_EMBED_ON": True},
+    "MASK": {"ENABLE": True, "MAE_ON": True, "MAE_RND_MASK": True, "PRETRAIN_DEPTH": [11], "HEAD_TYPE": "separate_xformer",
+             "DECODER_DEPTH": 4, "DECODER_EMBED_DIM": 512},
+    "AUG": {"MASK_RATIO": 0.9},
+    "MODEL": {"NUM_CLASSES": 400, "ARCH": "maskmvit", "MODEL_NAME": "MaskMViT", "LOSS_FUNC": "multi_mse",
+              "DROPOUT_RATE": 0.0},
+    "TRAIN": {"BATCH_SIZE": 64},
+    "RNG_SEED": 0,
+}
+_PRESETS.update({
+    "VIT_B_16x4_MAE_PT": _VIT_MAE,
+    "VIT_L_16x4_MAE_PT": dict(copy.deepcopy(_VIT_MAE), MVIT=dict(_VIT_MAE["MVIT"], EMBED_DIM=1024, NUM_HEADS=16, DEPTH=24),
+                              MASK=dict(_VIT_MAE["MASK"], PRETRAIN_DEPTH=[23]), TRAIN={"BATCH_SIZE": 32}),
+    "VIT_H_16x4_MAE_PT": dict(copy.deepcopy(_VIT_MAE), MVIT=dict(_VIT_MAE["MVIT"], EMBED_DIM=1280, NUM_HEADS=16, DEPTH=32),
+                              MASK=dict(_VIT_MAE["MASK"], PRETRAIN_DEPTH=[31]), TRAIN={"BATCH_SIZE": 32}),
 })
 # Non-local recipes (Wang et al., arXiv:1711.07971): the same backbones with Non-local blocks after res3 blocks 1, 3 and
 # res4 blocks 1, 3, 5 (slow pathway only for SlowFast); NONLOCAL.POOL keeps its default [1, 2, 2]

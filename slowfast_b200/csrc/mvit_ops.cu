@@ -379,11 +379,14 @@ __global__ void token_mean_bwd_kernel(const float* __restrict__ dmean, int b, in
 }
 // ------------------------------------------------------------------------------------------- non-overlapping patches
 // stride == kernel, no padding: NCTHW clip -> split rows [b * L, cin*kt*kh*kw], row (b, ot, oh, ow), column
-// (ci, dt, dy, dx) in Conv3d's weight-flatten order, so the patch embedding is one plain [E, K] GEMM
+// (ci, dt, dy, dx) in Conv3d's weight-flatten order, so the patch embedding is one plain [E, K] GEMM.
+// kGather (MAE): only the kept patches, rows [b * nkeep], row (b, j) = patch keep[b * nkeep + j]
+template <bool kGather>
 __global__ void patchify_kernel(const float* __restrict__ x, int b, int cin, int T, int H, int W, int kt, int kh, int kw,
-                                int ot, int oh, int ow, __nv_bfloat16* hi, __nv_bfloat16* lo) {
+                                int ot, int oh, int ow, const int* __restrict__ keep, int nkeep, __nv_bfloat16* hi,
+                                __nv_bfloat16* lo) {
   const int K = cin * kt * kh * kw;
-  const int64_t L = int64_t(ot) * oh * ow;
+  const int64_t L = kGather ? int64_t(nkeep) : int64_t(ot) * oh * ow;
   const int64_t items = int64_t(b) * L * K;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     int k = int(i % K);
@@ -394,7 +397,7 @@ __global__ void patchify_kernel(const float* __restrict__ x, int b, int cin, int
     k /= kh;
     const int dt_ = k % kt;
     const int ci = k / kt;
-    int64_t l = row % L;
+    int64_t l = kGather ? int64_t(keep[row]) : row % L;
     const int64_t bb = row / L;
     const int px = int(l % ow);
     l /= ow;
@@ -1127,9 +1130,26 @@ extern "C" int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, i
   }
   const int ot = t / kt, oh = h / kh, ow = w / kw;
   const int64_t items = int64_t(b) * ot * oh * ow * cin * kt * kh * kw;
-  patchify_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, b, cin, t, h, w, kt, kh, kw, ot, oh, ow,
-                                                                         (bf*)hi, (bf*)lo);
+  patchify_kernel<false><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, b, cin, t, h, w, kt, kh, kw, ot, oh,
+                                                                                ow, nullptr, 0, (bf*)hi, (bf*)lo);
   SFB_MV_CHECK("sfb_patchify");
+  return 0;
+}
+extern "C" int sfb_patchify_gather(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt,
+                                   int32_t kh, int32_t kw, const int32_t* keep, int32_t nkeep, void* hi, void* lo,
+                                   void* stream) {
+  if (!keep) return sfb_patchify(x, b, cin, t, h, w, kt, kh, kw, hi, lo, stream);
+  if (kt < 1 || kh < 1 || kw < 1 || t < kt || h < kh || w < kw || (cin * kt * kh * kw) % 8 != 0 || nkeep < 1 ||
+      int64_t(nkeep) > int64_t(t / kt) * (h / kh) * (w / kw)) {
+    set_error("sfb_patchify_gather: kernel %dx%dx%d over %dx%dx%d with %d channels, %d kept patches", kt, kh, kw, t, h,
+              w, cin, nkeep);
+    return -10;
+  }
+  const int ot = t / kt, oh = h / kh, ow = w / kw;
+  const int64_t items = int64_t(b) * nkeep * cin * kt * kh * kw;
+  patchify_kernel<true><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, b, cin, t, h, w, kt, kh, kw, ot, oh,
+                                                                               ow, keep, nkeep, (bf*)hi, (bf*)lo);
+  SFB_MV_CHECK("sfb_patchify_gather");
   return 0;
 }
 extern "C" int sfb_tokens_split_grad(const float* dx, int32_t b, int32_t l, int32_t c, void* dy_hi, void* dy_lo,

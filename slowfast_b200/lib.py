@@ -347,6 +347,18 @@ _SIGNATURES = [
     ("sfb_flat_adamw", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_int64, C.c_void_p]),
     ("sfb_hog_targets", C.c_int, [C.c_void_p] + [C.c_int32] * 9 + [C.c_void_p, C.c_void_p]),
+    ("sfb_mae_max_tokens", C.c_int32, []),
+    ("sfb_mae_random_masking", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 5),
+    ("sfb_patchify_gather", C.c_int, [C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_int32] + [C.c_void_p] * 3),
+    ("sfb_tokens_assemble_keep", C.c_int, [C.c_void_p] * 7 + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]),
+    ("sfb_tokens_scatter_keep", C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]),
+    ("sfb_decoder_assemble", C.c_int, [C.c_void_p] * 5 + [C.c_int32] * 4 + [C.c_void_p, C.c_void_p]),
+    ("sfb_decoder_assemble_bwd", C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p] * 5),
+    ("sfb_rows_gather", C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
+    ("sfb_rows_scatter", C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
+    ("sfb_pixel_targets", C.c_int, [C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                                                     C.c_void_p]),
     ("sfb_bias_split", C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_int32, C.c_void_p]),
     ("sfb_bn_conv_bias", C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -80,7 +80,14 @@ class MSSeparateHeadModule(Namespace):
 
 
 class B200MaskMViT(B200MViT):
-    """Drop-in for the reference's registered ``MaskMViT`` (MaskFeat with HOG targets)."""
+    """Drop-in for the reference's registered ``MaskMViT`` (MaskFeat with HOG targets).  A config with MASK.MAE_ON
+    builds the MAE pre-training model instead (nets/mae.py), as the reference's one class serves both."""
+
+    def __new__(cls, *args, **kwargs):
+        if cls is B200MaskMViT and args and args[0].MASK.MAE_ON:
+            from .mae import B200MAE
+            return B200MAE(*args, **kwargs)
+        return super().__new__(cls)
 
     def __init__(self, cfg):
         if cfg.MVIT.USE_ABS_POS:
