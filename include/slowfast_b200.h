@@ -321,6 +321,14 @@ int sfb_tokens_assemble(const float* y, const float* bias, const float* cls, con
                         float* x, void* stream);
 int sfb_tokens_split_grad(const float* dx, int32_t b, int32_t l, int32_t c, void* dy_hi, void* dy_lo, float* dy_f32,
                           void* stream);
+/* Joint position table (SEP_POS_EMBED False, video_model_builder.py:1180-1201) and / or no cls token (cls == NULL):
+ * x[b,0,:] = cls + pos[0]; x[b,1+l,:] = (y[b,l,:] + bias) + pos[1+l]   (cls != NULL, x [b, 1+l, c])
+ * x[b,l,:] = (y[b,l,:] + bias) + pos[l]                                 (cls == NULL, x [b, l, c])
+ * pos == NULL adds no position. */
+int sfb_tokens_assemble_joint(const float* y, const float* bias, const float* cls, const float* pos, int32_t b,
+                              int32_t l, int32_t c, float* x, void* stream);
+/* dpos[n] = sum_b dx[b, n] over dx [b, n, c] ("="), a fixed-order sum with no atomics. */
+int sfb_pos_embed_joint_bwd(const float* dx, int32_t b, int32_t n, int32_t c, float* dpos, void* stream);
 /* Slab count of the segmented row sums below: their `partials` scratch is [groups][sfb_segment_slabs(groups, rows)][c]
  * (groups = t for sfb_pos_embed_sep_bwd with rows = hw; groups = b for sfb_token_mean_fwd with rows = n - 1). */
 int32_t sfb_segment_slabs(int32_t groups, int32_t seg_rows);
@@ -333,6 +341,10 @@ int sfb_pos_embed_sep_bwd(const float* dx, int32_t b, int32_t t, int32_t hw, int
  * [b, c]), deterministic; the backward writes dx[b,0] = 0 and dx[b,1+l] = dmean[b] / (n-1). */
 int sfb_token_mean_fwd(const float* x, int32_t b, int32_t n, int32_t c, float* out, float* partials, void* stream);
 int sfb_token_mean_bwd(const float* dmean, int32_t b, int32_t n, int32_t c, float* dx, void* stream);
+/* The same over every row (no cls token; the default readout's mean after the final norm, :1239-1241): out[b] = mean of
+ * x[b, 0..n-1], partials as sfb_token_mean_fwd with rows = n; the backward writes dx[b,r] = dmean[b] / n. */
+int sfb_token_mean_all_fwd(const float* x, int32_t b, int32_t n, int32_t c, float* out, float* partials, void* stream);
+int sfb_token_mean_all_bwd(const float* dmean, int32_t b, int32_t n, int32_t c, float* dx, void* stream);
 /* Non-overlapping patch embedding input (Conv3d with stride == kernel, no padding): NCTHW fp32 clip -> split-bf16 rows
  * [b * (t/kt)(h/kh)(w/kw), cin*kt*kh*kw], columns in Conv3d's weight-flatten order (cin, kt, kh, kw); K % 8 == 0. */
 int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt, int32_t kh,
@@ -348,6 +360,7 @@ typedef struct sfb_dwpool_desc {
   const float* dout; /* bwd: gradient w.r.t. out */
   float* dsrc;       /* bwd: gradient w.r.t. src (+=, same geometry as src) */
   float* wpartials;  /* unused since ABI v1 r1d (the weight gradient is accumulated atomically); kept for layout stability */
+  int32_t no_cls;    /* 1: src / out carry no cls row ([B, L, pitch] -> [B, heads, L', hd]) */
 } sfb_dwpool_desc;
 int sfb_dwpool_fwd(const sfb_dwpool_desc* d, void* stream);
 int32_t sfb_dwpool_wgrad_blocks(const sfb_dwpool_desc* d);
@@ -362,6 +375,8 @@ typedef struct sfb_softmax_desc {
   const float* dp; int64_t dp_pitch;
   void* ds_hi; void* ds_lo; int64_t ds_pitch;
   float* drq;
+  int32_t no_cls;        /* 1: no cls row / column, the bias is on every query and key */
+  int32_t spatial_only;  /* 1: RQ rows are [Rh | Rw] (no Rt table: REL_POS_SPATIAL without REL_POS_TEMPORAL) */
 } sfb_softmax_desc;
 int sfb_softmax_relpos_fwd(const sfb_softmax_desc* d, void* stream);
 int sfb_softmax_relpos_bwd(const sfb_softmax_desc* d, void* stream);
@@ -370,6 +385,11 @@ int sfb_attn_merge(const float* o, const void* q_hi, const void* q_lo, int32_t b
                    int32_t residual, void* m_hi, void* m_lo, void* stream);
 int sfb_attn_split_grad(const float* dm, int32_t b, int32_t h, int32_t n, int32_t hd, int32_t residual, void* do_hi,
                         void* do_lo, float* dq, void* stream);
+/* The same without a cls row: the residual (and its gradient) is on every row n. */
+int sfb_attn_merge_nocls(const float* o, const void* q_hi, const void* q_lo, int32_t b, int32_t h, int32_t n, int32_t hd,
+                         int32_t residual, void* m_hi, void* m_lo, void* stream);
+int sfb_attn_split_grad_nocls(const float* dm, int32_t b, int32_t h, int32_t n, int32_t hd, int32_t residual,
+                              void* do_hi, void* do_lo, float* dq, void* stream);
 /* out = a [+ a_bias] + scale[sample] * (y + y_bias)   (residual adds with Linear biases and stochastic depth) */
 int sfb_residual_add(const float* a, const float* a_bias, const float* y, const float* y_bias, const float* scale,
                      int64_t rows, int32_t c, int64_t rows_per_sample, float* out, void* stream);
@@ -383,6 +403,7 @@ typedef struct sfb_tokpool_desc {
   const float* x; float* out; uint8_t* argmax;
   int32_t b, c, t, h, w, ot, oh, ow, kt, kh, kw, st, sh, sw;
   const float* dout; float* dx; int32_t dx_accumulate;
+  int32_t no_cls;  /* 1: no pass-through row */
 } sfb_tokpool_desc;
 int sfb_token_maxpool_fwd(const sfb_tokpool_desc* d, void* stream);
 int sfb_token_maxpool_bwd(const sfb_tokpool_desc* d, void* stream);

@@ -281,6 +281,44 @@ _PRESETS.update({
     "VIT_H_16x4_MAE_PT": dict(copy.deepcopy(_VIT_MAE), MVIT=dict(_VIT_MAE["MVIT"], EMBED_DIM=1280, NUM_HEADS=16, DEPTH=32),
                               MASK=dict(_VIT_MAE["MASK"], PRETRAIN_DEPTH=[31]), TRAIN={"BATCH_SIZE": 32}),
 })
+# ImageNet recipes (PATCH_2D: one-frame [B, 3, H, W] inputs)
+_IN1K_DATA = {"NUM_FRAMES": 1, "TRAIN_CROP_SIZE": 224, "TEST_CROP_SIZE": 224, "INPUT_CHANNEL_NUM": [3],
+              "MEAN": [0.485, 0.456, 0.406], "STD": [0.229, 0.224, 0.225]}
+_IN1K_MODEL = {"NUM_CLASSES": 1000, "ARCH": "mvit", "MODEL_NAME": "MViT", "LOSS_FUNC": "soft_cross_entropy",
+               "DROPOUT_RATE": 0.0}
+# configs/ImageNet/MVITv2_T.yaml (no cls token, spatial rel-pos, norm-then-mean readout)
+_MVITv2_T = {
+    "DATA": _IN1K_DATA,
+    "MVIT": {"PATCH_2D": True, "ZERO_DECAY_POS_CLS": False, "MODE": "conv", "CLS_EMBED_ON": False,
+             "PATCH_KERNEL": [7, 7], "PATCH_STRIDE": [4, 4], "PATCH_PADDING": [3, 3], "EMBED_DIM": 96, "NUM_HEADS": 1,
+             "MLP_RATIO": 4.0, "QKV_BIAS": True, "DROPPATH_RATE": 0.1, "DEPTH": 10, "NORM": "layernorm",
+             "DIM_MUL": [[1, 2.0], [3, 2.0], [8, 2.0]], "HEAD_MUL": [[1, 2.0], [3, 2.0], [8, 2.0]],
+             "POOL_KVQ_KERNEL": [1, 3, 3],
+             "POOL_KV_STRIDE": [[0, 1, 4, 4], [1, 1, 2, 2], [2, 1, 2, 2]] + [[i, 1, 1, 1] for i in range(3, 10)],
+             "POOL_Q_STRIDE": [[i, 1, 2, 2] if i in (1, 3, 8) else [i, 1, 1, 1] for i in range(10)],
+             "RESIDUAL_POOLING": True, "USE_ABS_POS": False, "REL_POS_SPATIAL": True, "DIM_MUL_IN_ATT": True},
+    "MODEL": _IN1K_MODEL,
+    "RNG_SEED": 0,
+}
+_PRESETS.update({
+    "MVITv2_T": _MVITv2_T,
+    # configs/ImageNet/MVITv2_S.yaml (MViTv2-T at depth 16, the last stage from block 14)
+    "MVITv2_S": dict(copy.deepcopy(_MVITv2_T), MVIT=dict(
+        _MVITv2_T["MVIT"], DEPTH=16, DIM_MUL=[[1, 2.0], [3, 2.0], [14, 2.0]], HEAD_MUL=[[1, 2.0], [3, 2.0], [14, 2.0]],
+        POOL_KV_STRIDE=[[0, 1, 4, 4], [1, 1, 2, 2], [2, 1, 2, 2]] + [[i, 1, 1, 1] for i in range(3, 16)],
+        POOL_Q_STRIDE=[[i, 1, 2, 2] if i in (1, 3, 14) else [i, 1, 1, 1] for i in range(16)])),
+    # configs/masked_ssl/in1k_VIT_B_MaskFeat_FT.yaml (ViT-B/16: 196 patches + cls, a joint pos_embed, mean readout)
+    "VIT_B_IN1K_FT": {
+        "DATA": _IN1K_DATA,
+        "MVIT": {"PATCH_2D": True, "ZERO_DECAY_POS_CLS": False, "MODE": "conv", "CLS_EMBED_ON": True,
+                 "PATCH_KERNEL": [16, 16], "PATCH_STRIDE": [16, 16], "PATCH_PADDING": [0, 0], "EMBED_DIM": 768,
+                 "NUM_HEADS": 12, "MLP_RATIO": 4.0, "QKV_BIAS": True, "DROPPATH_RATE": 0.1,
+                 "LAYER_SCALE_INIT_VALUE": 0.0, "DEPTH": 12, "NORM": "layernorm", "HEAD_INIT_SCALE": 0.001,
+                 "USE_MEAN_POOLING": True},
+        "MODEL": _IN1K_MODEL,
+        "RNG_SEED": 0,
+    },
+})
 # Non-local recipes (Wang et al., arXiv:1711.07971): the same backbones with Non-local blocks after res3 blocks 1, 3 and
 # res4 blocks 1, 3, 5 (slow pathway only for SlowFast); NONLOCAL.POOL keeps its default [1, 2, 2]
 _NLN_R50 = {"LOCATION": [[[]], [[1, 3]], [[1, 3, 5]], [[]]], "GROUP": [[1], [1], [1], [1]]}

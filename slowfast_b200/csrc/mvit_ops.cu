@@ -2,8 +2,8 @@
 // MultiScaleAttention.forward :293, MultiScaleBlock.forward :491; common.py Mlp :26) that are not GEMMs:
 // LayerNorm, depthwise 3-D pooling convolutions on the token grid, the rel-pos-biased softmax, head split/merge with
 // residual pooling, GELU, residual/bias combines, max-pool skip and the bias-gradient column sums.
-// Tokens are [B, N = 1 + T*H*W, C] with the cls token first; the residual stream is fp32, GEMM operands are
-// split-bf16 planes.  All kernels are HBM-bound elementwise / row kernels.
+// Tokens are [B, N = 1 + T*H*W, C] with the cls token first (kCls = 1), or [B, T*H*W, C] without one (kCls = 0: the
+// image recipes with CLS_EMBED_ON False); the residual stream is fp32, GEMM operands are split-bf16 planes.  All kernels are HBM-bound elementwise / row kernels.
 #include <algorithm>
 #include <cstdint>
 #include <cstdlib>
@@ -309,6 +309,33 @@ __global__ void tokens_assemble_kernel(const float* __restrict__ y, const float*
     }
   }
 }
+// joint position table (SEP_POS_EMBED False) and / or no cls row (cls == null):
+//   x[b, 0, :] = cls + pos[0];  x[b, 1 + l, :] = (y[b, l, :] + bias) + pos[1 + l]      (cls != null)
+//   x[b, l, :] = (y[b, l, :] + bias) + pos[l]                                           (cls == null)
+// the reference's order (cat, then +=: video_model_builder.py:1180-1201); pos == null adds no position
+__global__ void tokens_assemble_joint_kernel(const float* __restrict__ y, const float* __restrict__ bias,
+                                             const float* __restrict__ cls, const float* __restrict__ pos, int b, int l,
+                                             int c, float* __restrict__ x) {
+  const int nc = cls ? 1 : 0;
+  const int64_t items = int64_t(b) * (l + nc) * c;
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
+    const int ch = int(i % c);
+    const int64_t t = i / c;
+    const int n = int(t % (l + nc));
+    const int64_t bb = t / (l + nc);
+    const float v = n < nc ? cls[ch] : y[(bb * l + n - nc) * c + ch] + bias[ch];
+    x[i] = pos ? v + pos[int64_t(n) * c + ch] : v;
+  }
+}
+// dpos[n, :] = sum_b dx[b, n, :]: one thread per output element, batch in order (no atomics, replay-exact)
+__global__ void pos_joint_bwd_kernel(const float* __restrict__ dx, int b, int n, int c, float* __restrict__ dpos) {
+  const int64_t items = int64_t(n) * c;
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
+    float acc = 0.f;
+    for (int bb = 0; bb < b; ++bb) acc += dx[int64_t(bb) * items + i];
+    dpos[i] = acc;
+  }
+}
 // ------------------------------------------------------------------------------------------- separable position grads
 // Deterministic: every output element is a fixed-order sum (no atomics), so CUDA-graph replay reproduces eager bitwise.
 // dps[s, :] = sum_b sum_t dx[b, 1 + t*hw + s, :] and dpc[:] = sum_b dx[b, 0, :]: one thread per output element
@@ -366,7 +393,8 @@ __global__ void segment_rowsum_merge_kernel(const float* __restrict__ partials, 
     out[i] = float(s) * scale;
   }
 }
-// mean readout backward: dx[b, 0, :] = 0;  dx[b, 1 + l, :] = dmean[b, :] * scale
+// mean readout backward: dx[b, 0, :] = 0;  dx[b, 1 + l, :] = dmean[b, :] * scale  (kCls = 0: every row gets the share)
+template <int kCls>
 __global__ void token_mean_bwd_kernel(const float* __restrict__ dmean, int b, int n, int c, float scale,
                                       float* __restrict__ dx) {
   const int64_t items = int64_t(b) * n * c;
@@ -374,7 +402,7 @@ __global__ void token_mean_bwd_kernel(const float* __restrict__ dmean, int b, in
     const int ch = int(i % c);
     const int64_t t = i / c;
     const int r = int(t % n);
-    dx[i] = r == 0 ? 0.f : dmean[(t / n) * c + ch] * scale;
+    dx[i] = (kCls && r == 0) ? 0.f : dmean[(t / n) * c + ch] * scale;
   }
 }
 // ------------------------------------------------------------------------------------------- non-overlapping patches
@@ -427,6 +455,7 @@ __global__ void tokens_split_grad_kernel(const float* __restrict__ dx, int b, in
 //   src  : qkv GEMM output [B, 1+L, pitch] fp32, this tensor's channels at src_c0 + h*hd + c, bias added on the fly
 //          (to real tokens only: the zero padding of the conv stays zero)
 //   out  : [B, H, 1+L', hd] fp32 (cls row passes through), to be LayerNorm-ed by ln_fwd_kernel
+// kCls = 0: no cls row in src / out / dout / dsrc ([B, L, pitch] -> [B, H, L', hd]).
 struct DwPoolParams {
   const float* src; int64_t src_pitch; int src_c0; const float* bias;
   const float* w;  // [hd][kt*kh*kw]
@@ -437,28 +466,29 @@ struct DwPoolParams {
   // backward
   const float* dout; float* dsrc; float* wpartials; int has_pool;
 };
+template <int kCls>
 __global__ void dwpool_fwd_kernel(const DwPoolParams p) {
   // one thread = 4 consecutive channels of one (b, head, output token): float4 traffic, taps unrolled
   const int L = p.T * p.Hh * p.W, Lo = p.oT * p.oH * p.oW;
   const int hq = p.hd / 4;
   const int taps = p.kt * p.kh * p.kw;
-  const int64_t items = int64_t(p.B) * p.H * (Lo + 1) * hq;
+  const int64_t items = int64_t(p.B) * p.H * (Lo + kCls) * hq;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int c = int(i % hq) * 4;
     int64_t t = i / hq;
-    const int n = int(t % (Lo + 1));
-    t /= (Lo + 1);
+    const int n = int(t % (Lo + kCls));
+    t /= (Lo + kCls);
     const int h = int(t % p.H);
     const int64_t b = t / p.H;
     const int ch = p.src_c0 + h * p.hd + c;
     const float4 bias = p.bias ? *reinterpret_cast<const float4*>(p.bias + ch) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float* sb = p.src + b * int64_t(L + 1) * p.src_pitch + ch;
+    const float* sb = p.src + b * int64_t(L + kCls) * p.src_pitch + ch;
     float4 acc;
-    if (n == 0 || !p.has_pool) {
+    if ((kCls && n == 0) || !p.has_pool) {
       const float4 v = *reinterpret_cast<const float4*>(sb + int64_t(n) * p.src_pitch);
       acc = make_float4(v.x + bias.x, v.y + bias.y, v.z + bias.z, v.w + bias.w);
     } else {
-      int o = n - 1;
+      int o = n - kCls;
       const int ox = o % p.oW;
       o /= p.oW;
       const int oy = o % p.oH;
@@ -474,7 +504,7 @@ __global__ void dwpool_fwd_kernel(const DwPoolParams p) {
           for (int kx = 0; kx < p.kw; ++kx) {
             const int ix = ox * p.sw - p.pw + kx;
             if (ix < 0 || ix >= p.W) continue;
-            const int64_t pos = 1 + (int64_t(iz) * p.Hh + iy) * p.W + ix;
+            const int64_t pos = kCls + (int64_t(iz) * p.Hh + iy) * p.W + ix;
             const float4 v = *reinterpret_cast<const float4*>(sb + pos * p.src_pitch);
             const int k = (kz * p.kh + ky) * p.kw + kx;
             acc.x = fmaf(v.x + bias.x, w0[k], acc.x);
@@ -485,29 +515,30 @@ __global__ void dwpool_fwd_kernel(const DwPoolParams p) {
         }
       }
     }
-    *reinterpret_cast<float4*>(p.out + ((b * p.H + h) * int64_t(Lo + 1) + n) * p.hd + c) = acc;
+    *reinterpret_cast<float4*>(p.out + ((b * p.H + h) * int64_t(Lo + kCls) + n) * p.hd + c) = acc;
   }
 }
 // data gradient: dsrc[b, n, ch] += sum over outputs/taps of dout * w   (gather form; "+=" because q, k, v and the
 // block's other consumers all write into the same qkv gradient tensor, which the caller zero-fills first)
+template <int kCls>
 __global__ void dwpool_bwd_data_kernel(const DwPoolParams p) {
   const int L = p.T * p.Hh * p.W, Lo = p.oT * p.oH * p.oW;
   const int hq = p.hd / 4;
   const int taps = p.kt * p.kh * p.kw;
-  const int64_t items = int64_t(p.B) * p.H * (L + 1) * hq;
+  const int64_t items = int64_t(p.B) * p.H * (L + kCls) * hq;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int c = int(i % hq) * 4;
     int64_t t = i / hq;
-    const int n = int(t % (L + 1));
-    t /= (L + 1);
+    const int n = int(t % (L + kCls));
+    t /= (L + kCls);
     const int h = int(t % p.H);
     const int64_t b = t / p.H;
-    const float* db = p.dout + ((b * p.H + h) * int64_t(Lo + 1)) * p.hd + c;
+    const float* db = p.dout + ((b * p.H + h) * int64_t(Lo + kCls)) * p.hd + c;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (n == 0 || !p.has_pool) {
+    if ((kCls && n == 0) || !p.has_pool) {
       acc = *reinterpret_cast<const float4*>(db + int64_t(n) * p.hd);
     } else {
-      int q = n - 1;
+      int q = n - kCls;
       const int ix = q % p.W;
       q /= p.W;
       const int iy = q % p.Hh;
@@ -523,7 +554,7 @@ __global__ void dwpool_bwd_data_kernel(const DwPoolParams p) {
           const int ky = iy + p.ph - oy * p.sh;
           for (int ox = x_lo; ox <= x_hi; ++ox) {
             const int kx = ix + p.pw - ox * p.sw;
-            const int64_t opos = 1 + (int64_t(oz) * p.oH + oy) * p.oW + ox;
+            const int64_t opos = kCls + (int64_t(oz) * p.oH + oy) * p.oW + ox;
             const float4 g = *reinterpret_cast<const float4*>(db + opos * p.hd);
             const int k = (kz * p.kh + ky) * p.kw + kx;
             acc.x = fmaf(g.x, w0[k], acc.x);
@@ -534,7 +565,7 @@ __global__ void dwpool_bwd_data_kernel(const DwPoolParams p) {
         }
       }
     }
-    float4* d = reinterpret_cast<float4*>(p.dsrc + (b * int64_t(L + 1) + n) * p.src_pitch + p.src_c0 + h * p.hd + c);
+    float4* d = reinterpret_cast<float4*>(p.dsrc + (b * int64_t(L + kCls) + n) * p.src_pitch + p.src_c0 + h * p.hd + c);
     float4 o = *d;
     o.x += acc.x; o.y += acc.y; o.z += acc.z; o.w += acc.w;
     *d = o;
@@ -543,25 +574,26 @@ __global__ void dwpool_bwd_data_kernel(const DwPoolParams p) {
 // data gradient, scatter form, for strongly strided pooling (the K/V pools: stride 8 / 4 with a 3x3x3 kernel): work
 // is proportional to the (few) OUTPUT positions x 27 taps instead of scanning every input position for taps that
 // almost never exist.  Windows of neighbouring output frames overlap in time, hence atomic adds.
+template <int kCls>
 __global__ void dwpool_bwd_data_scatter_kernel(const DwPoolParams p) {
   const int L = p.T * p.Hh * p.W, Lo = p.oT * p.oH * p.oW;
   const int hq = p.hd / 4;
   const int taps = p.kt * p.kh * p.kw;
-  const int64_t items = int64_t(p.B) * p.H * (Lo + 1) * hq;
+  const int64_t items = int64_t(p.B) * p.H * (Lo + kCls) * hq;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int c = int(i % hq) * 4;
     int64_t t = i / hq;
-    const int n = int(t % (Lo + 1));
-    t /= (Lo + 1);
+    const int n = int(t % (Lo + kCls));
+    t /= (Lo + kCls);
     const int h = int(t % p.H);
     const int64_t b = t / p.H;
-    const float4 g = *reinterpret_cast<const float4*>(p.dout + ((b * p.H + h) * int64_t(Lo + 1) + n) * p.hd + c);
-    float* db = p.dsrc + b * int64_t(L + 1) * p.src_pitch + p.src_c0 + h * p.hd + c;
-    if (n == 0) {  // cls row passes through the pooling
+    const float4 g = *reinterpret_cast<const float4*>(p.dout + ((b * p.H + h) * int64_t(Lo + kCls) + n) * p.hd + c);
+    float* db = p.dsrc + b * int64_t(L + kCls) * p.src_pitch + p.src_c0 + h * p.hd + c;
+    if (kCls && n == 0) {  // cls row passes through the pooling
       atomicAdd(db + 0, g.x); atomicAdd(db + 1, g.y); atomicAdd(db + 2, g.z); atomicAdd(db + 3, g.w);
       continue;
     }
-    int o = n - 1;
+    int o = n - kCls;
     const int ox = o % p.oW;
     o /= p.oW;
     const int oy = o % p.oH;
@@ -577,7 +609,7 @@ __global__ void dwpool_bwd_data_scatter_kernel(const DwPoolParams p) {
           const int ix = ox * p.sw - p.pw + kx;
           if (ix < 0 || ix >= p.W) continue;
           const int k = (kz * p.kh + ky) * p.kw + kx;
-          float* d = db + (1 + (int64_t(iz) * p.Hh + iy) * p.W + ix) * p.src_pitch;
+          float* d = db + (kCls + (int64_t(iz) * p.Hh + iy) * p.W + ix) * p.src_pitch;
           atomicAdd(d + 0, g.x * w0[k]);
           atomicAdd(d + 1, g.y * w0[taps + k]);
           atomicAdd(d + 2, g.z * w0[2 * taps + k]);
@@ -589,6 +621,7 @@ __global__ void dwpool_bwd_data_scatter_kernel(const DwPoolParams p) {
 }
 // weight gradient partials: wpartials[block][c][tap] = sum over the block's (b, h, out position) slab.
 // blockDim = hd * PL threads (channel-fastest => coalesced), PL position lanes per block, smem reduce over the lanes.
+template <int kCls>
 __global__ void __launch_bounds__(512) dwpool_bwd_weight_kernel(const DwPoolParams p) {
   extern __shared__ float wsm[];  // [PL][hd][27]
   const int L = p.T * p.Hh * p.W, Lo = p.oT * p.oH * p.oW;
@@ -609,8 +642,8 @@ __global__ void __launch_bounds__(512) dwpool_bwd_weight_kernel(const DwPoolPara
       const int64_t b = bh / p.H;
       const int ch = p.src_c0 + h * p.hd + c;
       const float bias = p.bias ? p.bias[ch] : 0.f;
-      const float g = p.dout[(bh * int64_t(Lo + 1) + 1 + o) * p.hd + c];
-      const float* sb = p.src + b * int64_t(L + 1) * p.src_pitch + ch;
+      const float g = p.dout[(bh * int64_t(Lo + kCls) + kCls + o) * p.hd + c];
+      const float* sb = p.src + b * int64_t(L + kCls) * p.src_pitch + ch;
       const int ox = o % p.oW;
       o /= p.oW;
       const int oy = o % p.oH;
@@ -627,7 +660,7 @@ __global__ void __launch_bounds__(512) dwpool_bwd_weight_kernel(const DwPoolPara
           for (int kx = 0; kx < 3; ++kx) {
             const int ix = ox * p.sw - p.pw + kx;
             if (kx >= p.kw || ix < 0 || ix >= p.W) continue;
-            const int64_t pos = 1 + (int64_t(iz) * p.Hh + iy) * p.W + ix;
+            const int64_t pos = kCls + (int64_t(iz) * p.Hh + iy) * p.W + ix;
             acc[(kz * 3 + ky) * 3 + kx] = fmaf(g, sb[pos * p.src_pitch] + bias, acc[(kz * 3 + ky) * 3 + kx]);
           }
         }
@@ -650,6 +683,8 @@ __global__ void __launch_bounds__(512) dwpool_bwd_weight_kernel(const DwPoolPara
 // ------------------------------------------------------------------------------------------- rel-pos softmax
 // P[bh, q, k] = softmax_k( S[bh, q, k] + bias(q, k) ),  bias = RQ[q-1, ih(qh,kh)] + RQ[q-1, Lh + iw] + RQ[q-1, Lh+Lw + it]
 // for q > 0 and k > 0 (cls row / column carry no bias); index = floor(i*max(nk/nq,1) - j*max(nq/nk,1) + (nk-1)*max(nq/nk,1)).
+// kCls = 0: no cls row / column, the bias is on every query and key.  kRelT = false: spatial terms only (no Rt table,
+// REL_POS_SPATIAL without REL_POS_TEMPORAL), RQ rows are [Rh | Rw].
 struct SoftmaxParams {
   const float* S; int64_t s_pitch;          // [BH, Nq, s_pitch]
   const float* RQ; int64_t rq_pitch;        // [BH, Lq, rq_pitch]  (may be null: no rel-pos)
@@ -666,6 +701,7 @@ struct SoftmaxParams {
 __device__ __forceinline__ int rel_index(int i, int j, float rq, float rk, int nk) {
   return int(floorf(float(i) * rq - float(j) * rk + float(nk - 1) * rk));
 }
+template <int kCls, bool kRelT>
 __global__ void __launch_bounds__(256) softmax_relpos_fwd_kernel(const SoftmaxParams p) {
   // one warp per (bh, q) row; the biased scores are computed ONCE into a per-warp shared-memory row
   extern __shared__ float srow[];  // [8 warps][Nk]
@@ -679,10 +715,10 @@ __global__ void __launch_bounds__(256) softmax_relpos_fwd_kernel(const SoftmaxPa
     const int q = int(r % p.Nq);
     const int64_t bh = r / p.Nq;
     const float* s = p.S + r * p.s_pitch;
-    const float* rq = (p.RQ && q > 0) ? p.RQ + (bh * (p.Nq - 1) + (q - 1)) * p.rq_pitch : nullptr;
+    const float* rq = (p.RQ && q >= kCls) ? p.RQ + (bh * (p.Nq - kCls) + (q - kCls)) * p.rq_pitch : nullptr;
     int qz = 0, qy = 0, qx = 0;
-    if (q > 0) {
-      int t = q - 1;
+    if (q >= kCls) {
+      int t = q - kCls;
       qx = t % p.qw;
       t /= p.qw;
       qy = t % p.qh;
@@ -694,14 +730,17 @@ __global__ void __launch_bounds__(256) softmax_relpos_fwd_kernel(const SoftmaxPa
     float mx = -INFINITY;
     for (int k = lane; k < p.Nk; k += 32) {
       float v = s[k];
-      if (rq && k > 0) {
-        const int t = k - 1;
+      if (rq && k >= kCls) {
+        const int t = k - kCls;
         const int kz = t / khw;
         const int rem = t - kz * khw;
         const int ky = rem / p.kw;
         const int kx = rem - ky * p.kw;
-        v += rq[int(floorf(bh0 - float(ky) * p.rh_k))] + rq[p.Lh + int(floorf(bw0 - float(kx) * p.rw_k))] +
-             rq[p.Lh + p.Lw + int(floorf(bt0 - float(kz) * p.rt_k))];
+        if (kRelT)
+          v += rq[int(floorf(bh0 - float(ky) * p.rh_k))] + rq[p.Lh + int(floorf(bw0 - float(kx) * p.rw_k))] +
+               rq[p.Lh + p.Lw + int(floorf(bt0 - float(kz) * p.rt_k))];
+        else
+          v += rq[int(floorf(bh0 - float(ky) * p.rh_k))] + rq[p.Lh + int(floorf(bw0 - float(kx) * p.rw_k))];
       }
       buf[k] = v;
       mx = fmaxf(mx, v);
@@ -721,6 +760,7 @@ __global__ void __launch_bounds__(256) softmax_relpos_fwd_kernel(const SoftmaxPa
   }
 }
 // dS = P * (dP - sum_k P*dP) -> planes (pad columns zero);  dRQ[q-1, j] = sum over k with index j of dS[q, k]
+template <int kCls, bool kRelT>
 __global__ void __launch_bounds__(256) softmax_relpos_bwd_kernel(const SoftmaxParams p) {
   // one warp per row.  dS is staged in a per-warp shared row; the relative-position gradient is reduced per key AXIS
   // first (sum over the other two axes, one lane per axis coordinate) and only then scattered into the table bins,
@@ -745,7 +785,7 @@ __global__ void __launch_bounds__(256) softmax_relpos_bwd_kernel(const SoftmaxPa
       dot = fmaf(pv, dp[k], dot);
     }
     dot = warp_sum(dot);
-    const bool rel = p.dRQ != nullptr && q > 0;
+    const bool rel = p.dRQ != nullptr && q >= kCls;
     if (rel)
       for (int j = lane; j < Ltot; j += 32) bins[j] = 0.f;
     for (int k = lane; k < p.ds_pitch; k += 32) {
@@ -758,13 +798,13 @@ __global__ void __launch_bounds__(256) softmax_relpos_bwd_kernel(const SoftmaxPa
     }
     __syncwarp();
     if (rel) {
-      int t = q - 1;
+      int t = q - kCls;
       const int qx = t % p.qw;
       t /= p.qw;
       const int qy = t % p.qh;
       const int qz = t / p.qh;
-      const float* g = buf + 1;  // key grid [kt][kh][kw] behind the cls column
-      for (int a = lane; a < p.kh + p.kw + p.kt; a += 32) {
+      const float* g = buf + kCls;  // key grid [kt][kh][kw] behind the cls column
+      for (int a = lane; a < p.kh + p.kw + (kRelT ? p.kt : 0); a += 32) {
         float sum = 0.f;
         int bin;
         if (a < p.kh) {
@@ -784,7 +824,7 @@ __global__ void __launch_bounds__(256) softmax_relpos_bwd_kernel(const SoftmaxPa
         atomicAdd(&bins[bin], sum);
       }
       __syncwarp();
-      float* o = p.dRQ + (bh * (p.Nq - 1) + (q - 1)) * p.rq_pitch;
+      float* o = p.dRQ + (bh * (p.Nq - kCls) + (q - kCls)) * p.rq_pitch;
       for (int j = lane; j < p.rq_pitch; j += 32) o[j] = j < Ltot ? bins[j] : 0.f;
     }
     __syncwarp();
@@ -793,6 +833,8 @@ __global__ void __launch_bounds__(256) softmax_relpos_bwd_kernel(const SoftmaxPa
 
 // ------------------------------------------------------------------------------------------- head merge / split
 // merged[b, n, h*hd + c] = O[b, h, n, c] + (n > 0 ? q[b, h, n, c] : 0)   -> planes (input of the proj Linear)
+// (kCls = 0: the residual is added on every row)
+template <int kCls>
 __global__ void attn_merge_kernel(const float* __restrict__ O, const __nv_bfloat16* __restrict__ q_hi,
                                   const __nv_bfloat16* __restrict__ q_lo, int B, int H, int N, int hd, int residual,
                                   __nv_bfloat16* __restrict__ m_hi, __nv_bfloat16* __restrict__ m_lo) {
@@ -806,12 +848,13 @@ __global__ void attn_merge_kernel(const float* __restrict__ O, const __nv_bfloat
     const int64_t b = t / N;
     const int64_t src = ((b * H + h) * N + n) * hd + c;
     float v = O[src];
-    if (residual && n > 0) v += get_split(q_hi, q_lo, src);
+    if (residual && n >= kCls) v += get_split(q_hi, q_lo, src);
     put_split(m_hi, m_lo, i, v);
   }
 }
 // backward of the merge: dO[b, h, n, c] = dM[b, n, h*hd + c] -> planes (operand of dP / dV GEMMs) and the
 // residual-pooling gradient dq[b, h, n, c] (= dM for n > 0, 0 for the cls row) as fp32 initialisation of dq
+template <int kCls>
 __global__ void attn_split_grad_kernel(const float* __restrict__ dM, int B, int H, int N, int hd, int residual,
                                        __nv_bfloat16* __restrict__ do_hi, __nv_bfloat16* __restrict__ do_lo,
                                        float* __restrict__ dq) {
@@ -825,7 +868,7 @@ __global__ void attn_split_grad_kernel(const float* __restrict__ dM, int B, int 
     const int64_t b = t / H;
     const float v = dM[(b * N + n) * int64_t(H) * hd + h * hd + c];
     put_split(do_hi, do_lo, i, v);
-    dq[i] = (residual && n > 0) ? v : 0.f;
+    dq[i] = (residual && n >= kCls) ? v : 0.f;
   }
 }
 
@@ -882,26 +925,28 @@ __global__ void scale_split_kernel(const float* __restrict__ src, const float* _
 
 // ------------------------------------------------------------------------------------------- max-pool skip on tokens
 // attention_pool(x, MaxPool3d) of MultiScaleBlock (attention.py:485-489, :496): cls passes through, first max wins
+// (kCls = 0: no pass-through row)
 struct TokPoolParams {
   const float* x; float* out; uint8_t* argmax;
   int B, C, T, Hh, W, oT, oH, oW, kt, kh, kw, st, sh, sw, pt, ph, pw;
   const float* dout; float* dx; int dx_accumulate;
 };
+template <int kCls>
 __global__ void token_maxpool_fwd_kernel(const TokPoolParams p) {
   const int L = p.T * p.Hh * p.W, Lo = p.oT * p.oH * p.oW;
-  const int64_t items = int64_t(p.B) * (Lo + 1) * p.C;
+  const int64_t items = int64_t(p.B) * (Lo + kCls) * p.C;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int c = int(i % p.C);
     int64_t t = i / p.C;
-    const int n = int(t % (Lo + 1));
-    const int64_t b = t / (Lo + 1);
-    const float* xb = p.x + b * int64_t(L + 1) * p.C + c;
-    if (n == 0) {
+    const int n = int(t % (Lo + kCls));
+    const int64_t b = t / (Lo + kCls);
+    const float* xb = p.x + b * int64_t(L + kCls) * p.C + c;
+    if (kCls && n == 0) {
       p.out[i] = xb[0];
       p.argmax[i] = 0;
       continue;
     }
-    int o = n - 1;
+    int o = n - kCls;
     const int ox = o % p.oW;
     o /= p.oW;
     const int oy = o % p.oH;
@@ -917,7 +962,7 @@ __global__ void token_maxpool_fwd_kernel(const TokPoolParams p) {
         for (int kx = 0; kx < p.kw; ++kx) {
           const int ix = ox * p.sw - p.pw + kx;
           if (ix < 0 || ix >= p.W) continue;
-          const float v = xb[(1 + (int64_t(iz) * p.Hh + iy) * p.W + ix) * p.C];
+          const float v = xb[(kCls + (int64_t(iz) * p.Hh + iy) * p.W + ix) * p.C];
           if (v > best) {
             best = v;
             arg = uint8_t((kz * p.kh + ky) * p.kw + kx);
@@ -929,21 +974,22 @@ __global__ void token_maxpool_fwd_kernel(const TokPoolParams p) {
     p.argmax[i] = arg;
   }
 }
+template <int kCls>
 __global__ void token_maxpool_bwd_kernel(const TokPoolParams p) {
   const int L = p.T * p.Hh * p.W, Lo = p.oT * p.oH * p.oW;
-  const int64_t items = int64_t(p.B) * (L + 1) * p.C;
+  const int64_t items = int64_t(p.B) * (L + kCls) * p.C;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int c = int(i % p.C);
     int64_t t = i / p.C;
-    const int n = int(t % (L + 1));
-    const int64_t b = t / (L + 1);
-    const float* db = p.dout + b * int64_t(Lo + 1) * p.C + c;
-    const uint8_t* ab = p.argmax + b * int64_t(Lo + 1) * p.C + c;
+    const int n = int(t % (L + kCls));
+    const int64_t b = t / (L + kCls);
+    const float* db = p.dout + b * int64_t(Lo + kCls) * p.C + c;
+    const uint8_t* ab = p.argmax + b * int64_t(Lo + kCls) * p.C + c;
     float acc = 0.f;
-    if (n == 0) {
+    if (kCls && n == 0) {
       acc = db[0];
     } else {
-      int q = n - 1;
+      int q = n - kCls;
       const int ix = q % p.W;
       q /= p.W;
       const int iy = q % p.Hh;
@@ -958,7 +1004,7 @@ __global__ void token_maxpool_bwd_kernel(const TokPoolParams p) {
           const int ky = iy + p.ph - oy * p.sh;
           for (int ox = x_lo; ox <= x_hi; ++ox) {
             const int kx = ix + p.pw - ox * p.sw;
-            const int64_t opos = (1 + (int64_t(oz) * p.oH + oy) * p.oW + ox) * p.C;
+            const int64_t opos = (kCls + (int64_t(oz) * p.oH + oy) * p.oW + ox) * p.C;
             if (ab[opos] == uint8_t((kz * p.kh + ky) * p.kw + kx)) acc += db[opos];
           }
         }
@@ -1116,9 +1162,47 @@ extern "C" int sfb_token_mean_bwd(const float* dmean, int32_t b, int32_t n, int3
     set_error("sfb_token_mean_bwd: b=%d n=%d c=%d (needs a token besides cls)", b, n, c);
     return -10;
   }
-  token_mean_bwd_kernel<<<mv_grid(int64_t(b) * n * c, 256), 256, 0, (cudaStream_t)stream>>>(dmean, b, n, c,
-                                                                                           1.f / float(n - 1), dx);
+  token_mean_bwd_kernel<1><<<mv_grid(int64_t(b) * n * c, 256), 256, 0, (cudaStream_t)stream>>>(dmean, b, n, c,
+                                                                                              1.f / float(n - 1), dx);
   SFB_MV_CHECK("sfb_token_mean_bwd");
+  return 0;
+}
+extern "C" int sfb_token_mean_all_fwd(const float* x, int32_t b, int32_t n, int32_t c, float* out, float* partials,
+                                      void* stream) {
+  if (b < 1 || n < 1 || c < 1) {
+    set_error("sfb_token_mean_all_fwd: b=%d n=%d c=%d", b, n, c);
+    return -10;
+  }
+  return segment_rowsum(x, c, 1, 0, n, n, b, 1.f / float(n), out, partials, (cudaStream_t)stream);
+}
+extern "C" int sfb_token_mean_all_bwd(const float* dmean, int32_t b, int32_t n, int32_t c, float* dx, void* stream) {
+  if (b < 1 || n < 1 || c < 1) {
+    set_error("sfb_token_mean_all_bwd: b=%d n=%d c=%d", b, n, c);
+    return -10;
+  }
+  token_mean_bwd_kernel<0><<<mv_grid(int64_t(b) * n * c, 256), 256, 0, (cudaStream_t)stream>>>(dmean, b, n, c,
+                                                                                              1.f / float(n), dx);
+  SFB_MV_CHECK("sfb_token_mean_all_bwd");
+  return 0;
+}
+extern "C" int sfb_tokens_assemble_joint(const float* y, const float* bias, const float* cls, const float* pos, int32_t b,
+                                         int32_t l, int32_t c, float* x, void* stream) {
+  if (b < 1 || l < 1 || c < 1) {
+    set_error("sfb_tokens_assemble_joint: b=%d l=%d c=%d", b, l, c);
+    return -10;
+  }
+  const int64_t items = int64_t(b) * (l + (cls ? 1 : 0)) * c;
+  tokens_assemble_joint_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(y, bias, cls, pos, b, l, c, x);
+  SFB_MV_CHECK("sfb_tokens_assemble_joint");
+  return 0;
+}
+extern "C" int sfb_pos_embed_joint_bwd(const float* dx, int32_t b, int32_t n, int32_t c, float* dpos, void* stream) {
+  if (b < 1 || n < 1 || c < 1) {
+    set_error("sfb_pos_embed_joint_bwd: b=%d n=%d c=%d", b, n, c);
+    return -10;
+  }
+  pos_joint_bwd_kernel<<<mv_grid(int64_t(n) * c, 256), 256, 0, (cudaStream_t)stream>>>(dx, b, n, c, dpos);
+  SFB_MV_CHECK("sfb_pos_embed_joint_bwd");
   return 0;
 }
 extern "C" int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt, int32_t kh,
@@ -1169,7 +1253,7 @@ int dw3_run_strided(int mode, const float* x, int64_t x_pitch, int64_t x_so, int
                     int T, int H, int W, int C, cudaStream_t st);
 }
 static bool dwpool_ring_ok(const sfb_dwpool_desc* d) {
-  return d->has_pool && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 1 && d->sw == 1 &&
+  return !d->no_cls && d->has_pool && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 1 && d->sw == 1 &&
          d->t >= 2 && d->h % 7 == 0 && d->w_ % 7 == 0 && d->ot == d->t && d->oh == d->h && d->ow == d->w_ && d->hd % 4 == 0 &&
          d->src_pitch % 4 == 0 && d->src_c0 % 4 == 0;
 }
@@ -1218,8 +1302,11 @@ extern "C" int sfb_dwpool_fwd(const sfb_dwpool_desc* d, void* stream) {
       return 0;
     }
   }
-  const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->ot) * d->oh * d->ow + 1) * (d->hd / 4);
-  dwpool_fwd_kernel<<<mv_grid(items, 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
+  const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->ot) * d->oh * d->ow + (d->no_cls ? 0 : 1)) * (d->hd / 4);
+  if (d->no_cls)
+    dwpool_fwd_kernel<0><<<mv_grid(items, 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
+  else
+    dwpool_fwd_kernel<1><<<mv_grid(items, 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
   SFB_MV_CHECK("sfb_dwpool_fwd");
   return 0;
 }
@@ -1263,12 +1350,19 @@ extern "C" int sfb_dwpool_bwd(const sfb_dwpool_desc* d, float* dw, int32_t dw_ac
       return 0;
     }
   }
+  const int cls = d->no_cls ? 0 : 1;
   if (d->has_pool && d->sh >= d->kh && d->sw >= d->kw) {
-    const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->ot) * d->oh * d->ow + 1) * (d->hd / 4);
-    dwpool_bwd_data_scatter_kernel<<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
+    const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->ot) * d->oh * d->ow + cls) * (d->hd / 4);
+    if (cls)
+      dwpool_bwd_data_scatter_kernel<1><<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
+    else
+      dwpool_bwd_data_scatter_kernel<0><<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
   } else {
-    const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->t) * d->h * d->w_ + 1) * (d->hd / 4);
-    dwpool_bwd_data_kernel<<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
+    const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->t) * d->h * d->w_ + cls) * (d->hd / 4);
+    if (cls)
+      dwpool_bwd_data_kernel<1><<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
+    else
+      dwpool_bwd_data_kernel<0><<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
   }
   SFB_MV_CHECK("sfb_dwpool_bwd(data)");
   if (d->has_pool && dw) {
@@ -1281,7 +1375,10 @@ extern "C" int sfb_dwpool_bwd(const sfb_dwpool_desc* d, float* dw, int32_t dw_ac
     const int n = d->hd * d->kt * d->kh * d->kw;
     if (!dw_accumulate) cudaMemsetAsync(dw, 0, size_t(n) * sizeof(float), stream);
     p.dw = dw;
-    dwpool_bwd_weight_kernel<<<nb, pl * d->hd, size_t(pl) * d->hd * 27 * sizeof(float), stream>>>(p);
+    if (cls)
+      dwpool_bwd_weight_kernel<1><<<nb, pl * d->hd, size_t(pl) * d->hd * 27 * sizeof(float), stream>>>(p);
+    else
+      dwpool_bwd_weight_kernel<0><<<nb, pl * d->hd, size_t(pl) * d->hd * 27 * sizeof(float), stream>>>(p);
     SFB_MV_CHECK("sfb_dwpool_bwd(weight)");
   }
   return 0;
@@ -1295,13 +1392,31 @@ static void fill_sm(SoftmaxParams& p, const sfb_softmax_desc* d) {
   p.qt = d->qt; p.qh = d->qh; p.qw = d->qw; p.kt = d->kt; p.kh = d->kh; p.kw = d->kw;
   p.Lh = 2 * (d->qh > d->kh ? d->qh : d->kh) - 1;
   p.Lw = 2 * (d->qw > d->kw ? d->qw : d->kw) - 1;
-  p.Lt = 2 * (d->qt > d->kt ? d->qt : d->kt) - 1;
+  p.Lt = d->spatial_only ? 0 : 2 * (d->qt > d->kt ? d->qt : d->kt) - 1;
   auto ratio = [](int a, int b) { float r = float(a) / float(b); return r > 1.f ? r : 1.f; };
   p.rh_q = ratio(d->kh, d->qh); p.rh_k = ratio(d->qh, d->kh);
   p.rw_q = ratio(d->kw, d->qw); p.rw_k = ratio(d->qw, d->kw);
   p.rt_q = ratio(d->kt, d->qt); p.rt_k = ratio(d->qt, d->kt);
   p.dP = d->dp; p.dp_pitch = d->dp_pitch;
   p.ds_hi = (bf*)d->ds_hi; p.ds_lo = (bf*)d->ds_lo; p.ds_pitch = d->ds_pitch; p.dRQ = d->drq;
+}
+template <bool kBwd, int kCls, bool kRelT>
+static void softmax_launch(const SoftmaxParams& p, int64_t rows, size_t smem, cudaStream_t stream) {
+  auto kernel = kBwd ? softmax_relpos_bwd_kernel<kCls, kRelT> : softmax_relpos_fwd_kernel<kCls, kRelT>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kSoftmaxSmemMax));
+    attr_set = true;
+  }
+  kernel<<<mv_grid(rows * 32, 256, 16), 256, smem, stream>>>(p);
+}
+template <bool kBwd>
+static void softmax_dispatch(const sfb_softmax_desc* d, const SoftmaxParams& p, int64_t rows, size_t smem,
+                             cudaStream_t stream) {
+  if (!d->no_cls && !d->spatial_only) softmax_launch<kBwd, 1, true>(p, rows, smem, stream);
+  else if (!d->no_cls) softmax_launch<kBwd, 1, false>(p, rows, smem, stream);
+  else if (!d->spatial_only) softmax_launch<kBwd, 0, true>(p, rows, smem, stream);
+  else softmax_launch<kBwd, 0, false>(p, rows, smem, stream);
 }
 extern "C" int sfb_softmax_relpos_fwd(const sfb_softmax_desc* d, void* stream) {
   SoftmaxParams p;
@@ -1312,12 +1427,7 @@ extern "C" int sfb_softmax_relpos_fwd(const sfb_softmax_desc* d, void* stream) {
     set_error("sfb_softmax_relpos_fwd: %d keys exceed the shared-memory row buffer", d->nk);
     return -10;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(softmax_relpos_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kSoftmaxSmemMax));
-    attr_set = true;
-  }
-  softmax_relpos_fwd_kernel<<<mv_grid(rows * 32, 256, 16), 256, smem, (cudaStream_t)stream>>>(p);
+  softmax_dispatch<false>(d, p, rows, smem, (cudaStream_t)stream);
   SFB_MV_CHECK("sfb_softmax_relpos_fwd");
   return 0;
 }
@@ -1330,29 +1440,40 @@ extern "C" int sfb_softmax_relpos_bwd(const sfb_softmax_desc* d, void* stream) {
     set_error("sfb_softmax_relpos_bwd: %d keys exceed the shared-memory row buffer", d->nk);
     return -10;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(softmax_relpos_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kSoftmaxSmemMax));
-    attr_set = true;
-  }
-  softmax_relpos_bwd_kernel<<<mv_grid(rows * 32, 256, 16), 256, smem, (cudaStream_t)stream>>>(p);
+  softmax_dispatch<true>(d, p, rows, smem, (cudaStream_t)stream);
   SFB_MV_CHECK("sfb_softmax_relpos_bwd");
   return 0;
 }
 extern "C" int sfb_attn_merge(const float* o, const void* q_hi, const void* q_lo, int32_t b, int32_t h, int32_t n,
                               int32_t hd, int32_t residual, void* m_hi, void* m_lo, void* stream) {
   const int64_t items = int64_t(b) * n * h * hd;
-  attn_merge_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(o, (const bf*)q_hi, (const bf*)q_lo, b, h, n, hd,
-                                                                          residual, (bf*)m_hi, (bf*)m_lo);
+  attn_merge_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(o, (const bf*)q_hi, (const bf*)q_lo, b, h, n,
+                                                                             hd, residual, (bf*)m_hi, (bf*)m_lo);
   SFB_MV_CHECK("sfb_attn_merge");
+  return 0;
+}
+extern "C" int sfb_attn_merge_nocls(const float* o, const void* q_hi, const void* q_lo, int32_t b, int32_t h, int32_t n,
+                                    int32_t hd, int32_t residual, void* m_hi, void* m_lo, void* stream) {
+  const int64_t items = int64_t(b) * n * h * hd;
+  attn_merge_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(o, (const bf*)q_hi, (const bf*)q_lo, b, h, n,
+                                                                             hd, residual, (bf*)m_hi, (bf*)m_lo);
+  SFB_MV_CHECK("sfb_attn_merge_nocls");
   return 0;
 }
 extern "C" int sfb_attn_split_grad(const float* dm, int32_t b, int32_t h, int32_t n, int32_t hd, int32_t residual,
                                    void* do_hi, void* do_lo, float* dq, void* stream) {
   const int64_t items = int64_t(b) * h * n * hd;
-  attn_split_grad_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dm, b, h, n, hd, residual, (bf*)do_hi,
-                                                                                (bf*)do_lo, dq);
+  attn_split_grad_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dm, b, h, n, hd, residual,
+                                                                                   (bf*)do_hi, (bf*)do_lo, dq);
   SFB_MV_CHECK("sfb_attn_split_grad");
+  return 0;
+}
+extern "C" int sfb_attn_split_grad_nocls(const float* dm, int32_t b, int32_t h, int32_t n, int32_t hd, int32_t residual,
+                                         void* do_hi, void* do_lo, float* dq, void* stream) {
+  const int64_t items = int64_t(b) * h * n * hd;
+  attn_split_grad_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dm, b, h, n, hd, residual,
+                                                                                   (bf*)do_hi, (bf*)do_lo, dq);
+  SFB_MV_CHECK("sfb_attn_split_grad_nocls");
   return 0;
 }
 extern "C" int sfb_residual_add(const float* a, const float* a_bias, const float* y, const float* y_bias,
@@ -1394,16 +1515,22 @@ static void fill_tp(TokPoolParams& p, const sfb_tokpool_desc* d) {
 extern "C" int sfb_token_maxpool_fwd(const sfb_tokpool_desc* d, void* stream) {
   TokPoolParams p;
   fill_tp(p, d);
-  const int64_t items = int64_t(d->b) * (int64_t(d->ot) * d->oh * d->ow + 1) * d->c;
-  token_maxpool_fwd_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
+  const int64_t items = int64_t(d->b) * (int64_t(d->ot) * d->oh * d->ow + (d->no_cls ? 0 : 1)) * d->c;
+  if (d->no_cls)
+    token_maxpool_fwd_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
+  else
+    token_maxpool_fwd_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
   SFB_MV_CHECK("sfb_token_maxpool_fwd");
   return 0;
 }
 extern "C" int sfb_token_maxpool_bwd(const sfb_tokpool_desc* d, void* stream) {
   TokPoolParams p;
   fill_tp(p, d);
-  const int64_t items = int64_t(d->b) * (int64_t(d->t) * d->h * d->w + 1) * d->c;
-  token_maxpool_bwd_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
+  const int64_t items = int64_t(d->b) * (int64_t(d->t) * d->h * d->w + (d->no_cls ? 0 : 1)) * d->c;
+  if (d->no_cls)
+    token_maxpool_bwd_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
+  else
+    token_maxpool_bwd_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
   SFB_MV_CHECK("sfb_token_maxpool_bwd");
   return 0;
 }

@@ -112,7 +112,7 @@ class DwPoolDesc(C.Structure):
         ("w_", C.c_int32), ("ot", C.c_int32), ("oh", C.c_int32), ("ow", C.c_int32),
         ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32), ("st", C.c_int32), ("sh", C.c_int32),
         ("sw", C.c_int32), ("has_pool", C.c_int32),
-        ("dout", C.c_void_p), ("dsrc", C.c_void_p), ("wpartials", C.c_void_p),
+        ("dout", C.c_void_p), ("dsrc", C.c_void_p), ("wpartials", C.c_void_p), ("no_cls", C.c_int32),
     ]
 
 
@@ -125,6 +125,7 @@ class SoftmaxDesc(C.Structure):
         ("kw", C.c_int32),
         ("dp", C.c_void_p), ("dp_pitch", C.c_int64),
         ("ds_hi", C.c_void_p), ("ds_lo", C.c_void_p), ("ds_pitch", C.c_int64), ("drq", C.c_void_p),
+        ("no_cls", C.c_int32), ("spatial_only", C.c_int32),
     ]
 
 
@@ -135,7 +136,7 @@ class TokPoolDesc(C.Structure):
         ("ot", C.c_int32), ("oh", C.c_int32), ("ow", C.c_int32),
         ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32), ("st", C.c_int32), ("sh", C.c_int32),
         ("sw", C.c_int32),
-        ("dout", C.c_void_p), ("dx", C.c_void_p), ("dx_accumulate", C.c_int32),
+        ("dout", C.c_void_p), ("dx", C.c_void_p), ("dx_accumulate", C.c_int32), ("no_cls", C.c_int32),
     ]
 
 
@@ -286,6 +287,10 @@ _SIGNATURES = [
     ("sfb_pos_embed_sep_bwd", C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 5),
     ("sfb_token_mean_fwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
     ("sfb_token_mean_bwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 2),
+    ("sfb_token_mean_all_fwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
+    ("sfb_token_mean_all_bwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 2),
+    ("sfb_tokens_assemble_joint", C.c_int, [C.c_void_p] * 4 + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p]),
+    ("sfb_pos_embed_joint_bwd", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p]),
     ("sfb_patchify", C.c_int, [C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p] * 3),
     ("sfb_dwpool_fwd", C.c_int, [C.POINTER(DwPoolDesc), C.c_void_p]),
     ("sfb_dwpool_wgrad_blocks", C.c_int32, [C.POINTER(DwPoolDesc)]),
@@ -294,6 +299,8 @@ _SIGNATURES = [
     ("sfb_softmax_relpos_bwd", C.c_int, [C.POINTER(SoftmaxDesc), C.c_void_p]),
     ("sfb_attn_merge", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sfb_attn_split_grad", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("sfb_attn_merge_nocls", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("sfb_attn_split_grad_nocls", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sfb_residual_add", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     ("sfb_bias_gelu", C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sfb_bias_gelu_bwd", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -93,6 +93,9 @@ class B200MaskMViT(B200MViT):
         if cfg.MVIT.USE_ABS_POS:
             raise NotImplementedError("MVIT.USE_ABS_POS with MaskMViT (masked tokens before the position tables) is not "
                                       "on the engine path")
+        if cfg.MVIT.PATCH_2D:
+            raise NotImplementedError("MVIT.PATCH_2D with MaskMViT (image MaskFeat pre-training) is not on the engine "
+                                      "path")
         super().__init__(cfg)
         mk = cfg.MASK
         assert mk.PRED_HOG and not mk.MAE_ON and not mk.MAE_RND_MASK, "only the HOG-target MaskFeat path is built"

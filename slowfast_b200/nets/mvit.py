@@ -14,6 +14,10 @@ Scope: the MViTv2 configuration family of the reference's Kinetics configs (cls 
 both DIM_MUL_IN_ATT modes), MViTv1 and ViT with separable absolute position tables (SEP_POS_EMBED) added in the token
 assembly, and the mean-token readout (USE_MEAN_POOLING) of the MaskFeat fine-tuning recipes.  A patch embedding with
 stride == kernel and no padding (ViT's 2x16x16) is packed into rows and runs as one plain GEMM.
+Image recipes (PATCH_2D: configs/ImageNet, in1k fine-tuning): the image [B, 3, H, W] is the memory of a T = 1 clip, so
+the Conv2d embedding runs as a (1, kh, kw) convolution on the same kernels; they add the cls-free token layout
+(CLS_EMBED_ON False, every token-path kernel in its kCls = 0 instantiation), the joint pos_embed table and the default
+readout (norm on every token, then the mean).
 """
 from __future__ import annotations
 
@@ -71,7 +75,7 @@ def block_specs(cfg):
     for e in kv_list:
         stride_kv[e[0]] = list(e[1:])
         pool_kv[e[0]] = list(kvq) if kvq is not None else [s + 1 if s > 1 else s for s in e[1:]]
-    ps = list(mv.PATCH_STRIDE)
+    ps = ([1] if mv.PATCH_2D else []) + list(mv.PATCH_STRIDE)  # video_model_builder.py:832-836
     size = [cfg.DATA.NUM_FRAMES // ps[0], cfg.DATA.TRAIN_CROP_SIZE // ps[1], cfg.DATA.TRAIN_CROP_SIZE // ps[2]]
     embed, heads = mv.EMBED_DIM, mv.NUM_HEADS
     specs = []
@@ -151,9 +155,10 @@ class BlockModule(Namespace):
 
 
 class PatchEmbedModule(Namespace):
-    def __init__(self, cin, cout, kernel, stride, padding):
+    def __init__(self, cin, cout, kernel, stride, padding, conv_2d=False):
         super().__init__()
-        self.proj = nn.Conv3d(cin, cout, kernel_size=tuple(kernel), stride=tuple(stride), padding=tuple(padding))
+        conv = nn.Conv2d if conv_2d else nn.Conv3d
+        self.proj = conv(cin, cout, kernel_size=tuple(kernel), stride=tuple(stride), padding=tuple(padding))
 
 
 class TransformerHeadModule(Namespace):
@@ -189,11 +194,12 @@ class B200MViT(nn.Module):
         assert not mv.SEPARATE_QKV and not mv.NORM_STEM
         assert not cfg.DETECTION.ENABLE and mv.NORM == "layernorm"
         assert float(mv.LAYER_SCALE_INIT_VALUE) == 0.0
+        self._reject_unsupported(cfg)
         self.specs = block_specs(cfg)
-        self._reject_unsupported(cfg, self.specs)
         self.cfg = cfg
         self.ctx = Ctx(nsplit_of(cfg))
-        self.patch_stride = list(mv.PATCH_STRIDE)
+        self.patch_2d = bool(mv.PATCH_2D)
+        self.patch_stride = ([1] if self.patch_2d else []) + list(mv.PATCH_STRIDE)
         self.T = cfg.DATA.NUM_FRAMES // self.patch_stride[0]
         self.H = cfg.DATA.TRAIN_CROP_SIZE // self.patch_stride[1]
         self.W = cfg.DATA.TRAIN_CROP_SIZE // self.patch_stride[2]
@@ -202,17 +208,23 @@ class B200MViT(nn.Module):
         self.dim_mul_in_att = bool(mv.DIM_MUL_IN_ATT)
         self.use_abs_pos = bool(mv.USE_ABS_POS)
         self.use_mean_pooling = bool(mv.USE_MEAN_POOLING)
+        self.sep_pos_embed = bool(mv.SEP_POS_EMBED)
+        self.ncls = 1 if mv.CLS_EMBED_ON else 0  # rows ahead of the token grid in every token tensor
         cin = cfg.DATA.INPUT_CHANNEL_NUM[0]
         # non-overlapping patches (ViT's 2x16x16) are packed into rows and run as one plain GEMM; overlapping ones
         # (MViT's 3x7x7 / stride 2x4x4) take the implicit-GEMM convolution
         self.patchify = (list(mv.PATCH_KERNEL) == list(mv.PATCH_STRIDE) and not any(mv.PATCH_PADDING)
                          and cin * math.prod(mv.PATCH_KERNEL) % 8 == 0)
-        self.patch_embed = PatchEmbedModule(cin, mv.EMBED_DIM, mv.PATCH_KERNEL, mv.PATCH_STRIDE, mv.PATCH_PADDING)
-        self.cls_token = nn.Parameter(torch.zeros(1, 1, mv.EMBED_DIM))
-        if self.use_abs_pos:  # video_model_builder.py:892-901 (zeros: no RNG draw here)
+        self.patch_embed = PatchEmbedModule(cin, mv.EMBED_DIM, mv.PATCH_KERNEL, mv.PATCH_STRIDE, mv.PATCH_PADDING,
+                                            conv_2d=self.patch_2d)
+        if self.ncls:
+            self.cls_token = nn.Parameter(torch.zeros(1, 1, mv.EMBED_DIM))
+        if self.use_abs_pos and self.sep_pos_embed:  # video_model_builder.py:892-910 (zeros: no RNG draw here)
             self.pos_embed_spatial = nn.Parameter(torch.zeros(1, self.H * self.W, mv.EMBED_DIM))
             self.pos_embed_temporal = nn.Parameter(torch.zeros(1, self.T, mv.EMBED_DIM))
             self.pos_embed_class = nn.Parameter(torch.zeros(1, 1, mv.EMBED_DIM))
+        elif self.use_abs_pos:
+            self.pos_embed = nn.Parameter(torch.zeros(1, self.T * self.H * self.W + self.ncls, mv.EMBED_DIM))
         self.blocks = nn.ModuleList()
         for spec in self.specs:
             self.blocks.append(BlockModule(spec, mv.MLP_RATIO, mv.QKV_BIAS, mv.REL_POS_SPATIAL, mv.REL_POS_TEMPORAL,
@@ -220,11 +232,14 @@ class B200MViT(nn.Module):
         embed = self.specs[-1]["dim_out"]
         self.norm = nn.LayerNorm(embed, eps=1e-6)
         self.head = TransformerHeadModule(embed, self.num_classes, cfg.MODEL.DROPOUT_RATE, cfg.MODEL.HEAD_ACT)
-        if self.use_abs_pos:  # drawn after the head and before cls_token, as the reference does (:1057-1077)
-            nn.init.trunc_normal_(self.pos_embed_spatial, std=0.02)
+        if self.use_abs_pos and self.sep_pos_embed:  # drawn after the head and before cls_token, as the reference does
+            nn.init.trunc_normal_(self.pos_embed_spatial, std=0.02)  # (:1057-1077)
             nn.init.trunc_normal_(self.pos_embed_temporal, std=0.02)
             nn.init.trunc_normal_(self.pos_embed_class, std=0.02)
-        nn.init.trunc_normal_(self.cls_token, std=0.02)
+        elif self.use_abs_pos:
+            nn.init.trunc_normal_(self.pos_embed, std=0.02)
+        if self.ncls:
+            nn.init.trunc_normal_(self.cls_token, std=0.02)
         self.apply(self._init_weights)
         self.head.projection.weight.data.mul_(mv.HEAD_INIT_SCALE)
         self.head.projection.bias.data.mul_(mv.HEAD_INIT_SCALE)
@@ -239,19 +254,33 @@ class B200MViT(nn.Module):
         object.__setattr__(self, "_saved", None)
 
     @staticmethod
-    def _reject_unsupported(cfg, specs):
-        """Configurations the reference builds but the engine program does not run fail here, naming the option."""
+    def _reject_unsupported(cfg):
+        """Configurations the reference builds but the engine program does not run fail here, naming the option.  The
+        option checks run before anything reads the patch geometry."""
         mv = cfg.MVIT
+        p2d = bool(mv.PATCH_2D)
+        # the cls-free layout and the joint table are built for image patches; video keeps cls-first separable tables
         bad = [
-            (not mv.CLS_EMBED_ON, "MVIT.CLS_EMBED_ON False (the engine's token layout keeps the cls token first)"),
+            (not mv.CLS_EMBED_ON and not p2d,
+             "MVIT.CLS_EMBED_ON False with 3-D patches (the engine's video token layout keeps the cls token first)"),
             (float(mv.DROPOUT_RATE) != 0.0, "MVIT.DROPOUT_RATE > 0 (position / attention / MLP dropout)"),
-            (bool(mv.PATCH_2D), "MVIT.PATCH_2D (2-D image patch embedding)"),
+            (p2d and any(len(v) != 2 for v in (mv.PATCH_KERNEL, mv.PATCH_STRIDE, mv.PATCH_PADDING)),
+             "MVIT.PATCH_2D with a 3-element PATCH_KERNEL / PATCH_STRIDE / PATCH_PADDING (a 2-D embedding takes [h, w])"),
+            (p2d and cfg.DATA.NUM_FRAMES != 1, "MVIT.PATCH_2D with DATA.NUM_FRAMES != 1 (images are one frame)"),
             (bool(mv.REV.ENABLE), "MVIT.REV.ENABLE (reversible MViT)"),
-            (bool(mv.USE_ABS_POS) and not mv.SEP_POS_EMBED,
-             "MVIT.USE_ABS_POS with SEP_POS_EMBED False (a joint pos_embed table)"),
+            (bool(mv.USE_ABS_POS) and not mv.SEP_POS_EMBED and not p2d,
+             "MVIT.USE_ABS_POS with SEP_POS_EMBED False (a joint pos_embed table) with 3-D patches"),
+            (bool(mv.USE_ABS_POS) and mv.SEP_POS_EMBED and not mv.CLS_EMBED_ON,
+             "MVIT.SEP_POS_EMBED with CLS_EMBED_ON False (separable tables without pos_embed_class)"),
             (bool(mv.USE_FIXED_SINCOS_POS), "MVIT.USE_FIXED_SINCOS_POS (fixed sin-cos position table)"),
+            (bool(mv.REL_POS_TEMPORAL) and not mv.REL_POS_SPATIAL,
+             "MVIT.REL_POS_TEMPORAL without REL_POS_SPATIAL (a temporal-only relative-position bias)"),
         ]
-        for i, s in enumerate(specs):
+        for cond, what in bad:
+            if cond:
+                raise NotImplementedError(f"{what} is not on the engine path")
+        bad = []
+        for i, s in enumerate(block_specs(cfg)):
             for name, k, st in (("q", s["kq"], s["sq"]), ("kv", s["kkv"], s["skv"])):
                 # dwpool_bwd's weight gradient accumulates at most 3 taps per axis (csrc/mvit_ops.cu)
                 bad.append((_is_pool(k, st) and max(k) > 3,
@@ -274,20 +303,26 @@ class B200MViT(nn.Module):
 
     @torch.jit.ignore
     def no_weight_decay(self):
-        names = []
+        names = []  # video_model_builder.py:1095-1116
         if self.cfg.MVIT.ZERO_DECAY_POS_CLS:
-            if self.use_abs_pos:
+            if self.use_abs_pos and self.sep_pos_embed:
                 names.extend(["pos_embed_spatial", "pos_embed_temporal", "pos_embed_class"])
+            elif self.use_abs_pos:
+                names.append("pos_embed")
             if self.cfg.MVIT.REL_POS_SPATIAL:
                 names.extend(["rel_pos_h", "rel_pos_w", "rel_pos_hw"])
             if self.cfg.MVIT.REL_POS_TEMPORAL:
                 names.extend(["rel_pos_t"])
-            names.append("cls_token")
+            if self.ncls:
+                names.append("cls_token")
         return names
 
     def forward(self, x, bboxes=None, return_attn=False):
         assert bboxes is None and not return_attn
         x = [x[0]]
+        if self.patch_2d and x[0].dim() != 4:
+            raise ValueError(f"MVIT.PATCH_2D takes images [B, C, H, W]; got a {x[0].dim()}-D input of shape "
+                             f"{tuple(x[0].shape)}")
         params = [p for p in self.parameters()]
         return ModelFunction.apply(self, 1, *x, *params)
 
@@ -375,6 +410,8 @@ class B200MViT(nn.Module):
     def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
         ctx, lib = self.ctx, L.load()
         x = inputs[0]
+        if self.patch_2d:
+            x = x.unsqueeze(2)  # [B, C, H, W] -> [B, C, 1, H, W]: the same memory as a one-frame clip
         ctx.device = x.device
         ctx.training = self.training
         if x.device.type != "cuda":
@@ -383,7 +420,7 @@ class B200MViT(nn.Module):
         pe = self.patch_embed.proj
         # ---- patch embedding: clip -> [B, L, 96] (+bias, cls) -------------------------------------------------
         n, cin, t, h, w = x.shape
-        k3, s3, p3 = tuple(pe.kernel_size), tuple(pe.stride), tuple(pe.padding)
+        k3, s3, p3 = self._pe_geometry()
         E = pe.out_channels
         if self.patchify:
             # stride == kernel: the clip packs into [B*L, cin*kt*kh*kw] rows and the weight is a plain [E, K] matrix
@@ -412,7 +449,7 @@ class B200MViT(nn.Module):
             Lt = T * H * W
             ype = ctx.buf(("pe.y",), (B, Lt, E))
             ops.conv_igemm(xin_p, fm, geom, ype, (Lt * E, H * W * E, W * E, E), nsplit=ctx.nsplit)
-        x0 = ctx.buf(("x", 0), (B, Lt + 1, E))
+        x0 = ctx.buf(("x", 0), (B, Lt + self.ncls, E))
         self._tokens_assemble(ype, x0, B, Lt, E, inputs)
         # ---- stochastic depth scales ---------------------------------------------------------------------------
         dp = None
@@ -438,10 +475,27 @@ class B200MViT(nn.Module):
         object.__setattr__(self, "_saved", dict(xin=xin_p, geom=geom, blocks=saved, dp=dp, B=B, thw0=(T, H, W)))
         return self._final_forward(cur, thw, B)
 
+    def _pe_geometry(self):
+        """(kernel, stride, padding) of the patch embedding as a 3-D convolution (a Conv2d is its (1, kh, kw) case; its
+        [E, C, kh, kw] weight has the tap order of [E, C, 1, kh, kw])."""
+        pe = self.patch_embed.proj
+        k, s, p = tuple(pe.kernel_size), tuple(pe.stride), tuple(pe.padding)
+        if self.patch_2d:
+            return (1,) + k, (1,) + s, (0,) + p
+        return k, s, p
+
     # ---- hooks the MaskFeat wrapper overrides -------------------------------------------------------------------
     def _tokens_assemble(self, ype, x0, B, Lt, E, inputs) -> None:
         """[cls ; patch embedding + bias] (+ separable positions) (video_model_builder.py:1166-1199)."""
         pe = self.patch_embed.proj
+        if not self.ncls or (self.use_abs_pos and not self.sep_pos_embed):
+            # cls-free layout and / or the joint table: (y + bias) + pos[n], the cls row cls + pos[0]
+            L.check(L.load().sfb_tokens_assemble_joint(ype.data_ptr(), pe.bias.data_ptr(),
+                                                       self.cls_token.data_ptr() if self.ncls else None,
+                                                       self.pos_embed.data_ptr() if self.use_abs_pos else None, B, Lt, E,
+                                                       x0.data_ptr(), _st()), "sfb_tokens_assemble_joint")
+            ops._count()
+            return
         pos = [None] * 3
         if self.use_abs_pos:
             pos = [p.data_ptr() for p in (self.pos_embed_spatial, self.pos_embed_temporal, self.pos_embed_class)]
@@ -453,6 +507,9 @@ class B200MViT(nn.Module):
         """Gradient of the token sequence -> patch-embedding output gradient (planes + fp32)."""
         ctx = self.ctx
         dyp = self._rows_planes("pe.dy", B * Lt, E, scratch=True)
+        if not self.ncls:  # the token gradient is the embedding's output gradient
+            ops.split_planes(dx.view(1, 1, 1, B * Lt, E), dyp)
+            return dyp, dx.view(B * Lt, E)
         dyf = ctx.scratch("pe.dyf", B * Lt * E, F32)
         L.check(L.load().sfb_tokens_split_grad(dx.data_ptr(), B, Lt, E, dyp.hi_ptr(), dyp.lo_ptr(), dyf.data_ptr(),
                                                _st()), "sfb_tokens_split_grad")
@@ -460,22 +517,31 @@ class B200MViT(nn.Module):
         return dyp, dyf
 
     def _final_forward(self, cur: torch.Tensor, thw, B) -> torch.Tensor:
-        """Final LayerNorm on the cls rows, or on the mean of the other tokens (USE_MEAN_POOLING), + TransformerBasicHead
-        (video_model_builder.py:1230-1242)."""
-        ctx = self.ctx
+        """Final LayerNorm on the cls rows, or on the mean of the other tokens (USE_MEAN_POOLING), or (no cls token, the
+        default readout) on every token and then the mean, + TransformerBasicHead (video_model_builder.py:1230-1242)."""
+        ctx, lib = self.ctx, L.load()
         Nf, Cf = cur.shape[1], cur.shape[2]
         if self.use_mean_pooling:
-            lib = L.load()
             ln_in, ln_pitch = ctx.buf(("final.pool",), (B, Cf)), Cf
-            part = ctx.scratch("final.pool.part", B * lib.sfb_segment_slabs(B, Nf - 1) * Cf, F32)
-            L.check(lib.sfb_token_mean_fwd(cur.data_ptr(), B, Nf, Cf, ln_in.data_ptr(), part.data_ptr(), _st()),
-                    "sfb_token_mean_fwd")
+            part = ctx.scratch("final.pool.part", B * lib.sfb_segment_slabs(B, Nf - self.ncls) * Cf, F32)
+            mean_fwd = lib.sfb_token_mean_fwd if self.ncls else lib.sfb_token_mean_all_fwd
+            L.check(mean_fwd(cur.data_ptr(), B, Nf, Cf, ln_in.data_ptr(), part.data_ptr(), _st()), "sfb_token_mean_fwd")
             ops._count(2)
         else:
             ln_in, ln_pitch = cur, Nf * Cf
         cls_n = ctx.buf(("final.cls",), (B, Cf))
-        fmean, frstd = ctx.buf(("final.mean",), (B,)), ctx.buf(("final.rstd",), (B,))
-        self._ln_fwd(ln_in, ln_pitch, B, Cf, self.norm, None, cls_n, fmean, frstd)
+        if not self.use_mean_pooling and not self.ncls:
+            # norm on all B * Nf rows, then the per-image mean (deterministic slab sums)
+            normed = ctx.buf(("final.normed",), (B * Nf, Cf))
+            fmean, frstd = ctx.buf(("final.mean",), (B * Nf,)), ctx.buf(("final.rstd",), (B * Nf,))
+            self._ln_fwd(cur, Cf, B * Nf, Cf, self.norm, None, normed, fmean, frstd)
+            part = ctx.scratch("final.pool.part", B * lib.sfb_segment_slabs(B, Nf) * Cf, F32)
+            L.check(lib.sfb_token_mean_all_fwd(normed.data_ptr(), B, Nf, Cf, cls_n.data_ptr(), part.data_ptr(), _st()),
+                    "sfb_token_mean_all_fwd")
+            ops._count(2)
+        else:
+            fmean, frstd = ctx.buf(("final.mean",), (B,)), ctx.buf(("final.rstd",), (B,))
+            self._ln_fwd(ln_in, ln_pitch, B, Cf, self.norm, None, cls_n, fmean, frstd)
         head = self.head
         feat = cls_n
         mask = None
@@ -508,16 +574,30 @@ class B200MViT(nn.Module):
         if mask is not None:
             ops.dropout_bwd(dfeat, mask, head.dropout_rate)
         dx = ctx.scratch("dx.a", B * Nf * Cf, F32).view(B, Nf, Cf)
+        lib = L.load()
         if self.use_mean_pooling:
             dpool = ctx.scratch("final.dpool", B * Cf, F32).view(B, Cf)
             self._ln_bwd(dfeat, Cf, ln_in, ln_pitch, B, Cf, self.norm, fmean, frstd, dpool, Cf, False)
-            L.check(L.load().sfb_token_mean_bwd(dpool.data_ptr(), B, Nf, Cf, dx.data_ptr(), _st()),
-                    "sfb_token_mean_bwd")
+            mean_bwd = lib.sfb_token_mean_bwd if self.ncls else lib.sfb_token_mean_all_bwd
+            L.check(mean_bwd(dpool.data_ptr(), B, Nf, Cf, dx.data_ptr(), _st()), "sfb_token_mean_bwd")
             ops._count()
+            return dx
+        if not self.ncls:
+            # dmean / Nf on every row, then the norm's backward over all B * Nf rows
+            dn = ctx.scratch("final.dnormed", B * Nf * Cf, F32)
+            L.check(lib.sfb_token_mean_all_bwd(dfeat.data_ptr(), B, Nf, Cf, dn.data_ptr(), _st()),
+                    "sfb_token_mean_all_bwd")
+            ops._count()
+            self._ln_bwd(dn, Cf, cur, Cf, B * Nf, Cf, self.norm, fmean, frstd, dx, Cf, False)
             return dx
         ops.zero_f32(ops.f32view(dx.view(B * Nf, Cf)))
         self._ln_bwd(dfeat, Cf, cur, Nf * Cf, B, Cf, self.norm, fmean, frstd, dx, Nf * Cf, False)
         return dx
+
+    @staticmethod
+    def _rel_tables(at) -> list:
+        """The block's relative-position tables in RQ column order: [Rh, Rw, Rt], [Rh, Rw] (spatial only) or []."""
+        return [getattr(at, n) for n in ("rel_pos_h", "rel_pos_w", "rel_pos_t") if hasattr(at, n)]
 
     def _pool_geom(self, thw, kernel, stride):
         if not _is_pool(kernel, stride):
@@ -532,7 +612,8 @@ class B200MViT(nn.Module):
         hd = A // Hn
         T, Hh, W = thw
         Lin = T * Hh * W
-        N = Lin + 1
+        nc = self.ncls
+        N = Lin + nc
         rows = B * N
         at = blk.attn
         # LN1 -> planes
@@ -549,11 +630,12 @@ class B200MViT(nn.Module):
             d = L.DwPoolDesc()
             d.src, d.src_pitch, d.src_c0 = yqkv.data_ptr(), 3 * A, j * A
             d.bias = _ptr(at.qkv.bias)
-            out = ctx.buf(("b", i, "pool", name), (B, Hn, Lo + 1, hd))
+            out = ctx.buf(("b", i, "pool", name), (B, Hn, Lo + nc, hd))
             d.out = out.data_ptr()
             d.b, d.heads, d.hd, d.t, d.h, d.w_ = B, Hn, hd, T, Hh, W
             d.ot, d.oh, d.ow = othw
             d.has_pool = 1 if has else 0
+            d.no_cls = 1 - nc
             if has:
                 d.w = getattr(at, f"pool_{name}").weight.data_ptr()
                 d.kt, d.kh, d.kw = kern
@@ -562,7 +644,7 @@ class B200MViT(nn.Module):
                 d.kt = d.kh = d.kw = d.st = d.sh = d.sw = 1
             L.check(lib.sfb_dwpool_fwd(C.byref(d), _st()), "sfb_dwpool_fwd")
             ops._count()
-            prow = B * Hn * (Lo + 1)
+            prow = B * Hn * (Lo + nc)
             pp = self._rows_planes(("b", i, "pl", name), prow, hd)
             if has:
                 m_, r_ = ctx.buf(("b", i, "pm", name), (prow,)), ctx.buf(("b", i, "pr", name), (prow,))
@@ -573,21 +655,22 @@ class B200MViT(nn.Module):
             pooled[name], pl[name], geo[name] = out, pp, (othw, has, kern, strd)
         q_thw, k_thw = geo["q"][0], geo["k"][0]
         Lq, Lk = math.prod(q_thw), math.prod(k_thw)
-        Nq, Nk = Lq + 1, Lk + 1
+        Nq, Nk = Lq + nc, Lk + nc
         Nkp = ops.pad8(Nk)
         BH = B * Hn
         # S = scale * q k^T
         S = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
         self._bgemm(pl["q"], (hd, Nq * hd), False, pl["k"], (hd, Nk * hd), False, Nq, Nk, hd, BH, S, Nkp,
                     alpha=hd ** -0.5)
-        # decomposed relative positions: RQ = q_nocls . [Rh; Rw; Rt]^T
+        # decomposed relative positions: RQ = q_nocls . [Rh; Rw; Rt]^T  (Rt absent: spatial terms only)
         rq, Ltp, tab = None, 0, None
-        has_rel = hasattr(at, "rel_pos_h")
-        if has_rel:
-            Lh_, Lw_, Lt_ = at.rel_pos_h.shape[0], at.rel_pos_w.shape[0], at.rel_pos_t.shape[0]
-            assert Lh_ == 2 * max(q_thw[1], k_thw[1]) - 1 and Lt_ == 2 * max(q_thw[0], k_thw[0]) - 1, \
+        tabs = self._rel_tables(at)
+        if tabs:
+            Lh_ = at.rel_pos_h.shape[0]
+            assert Lh_ == 2 * max(q_thw[1], k_thw[1]) - 1, "rel-pos table interpolation is not on the engine path"
+            assert len(tabs) == 2 or tabs[2].shape[0] == 2 * max(q_thw[0], k_thw[0]) - 1, \
                 "rel-pos table interpolation is not on the engine path"
-            Ltot = Lh_ + Lw_ + Lt_
+            Ltot = sum(t_.shape[0] for t_ in tabs)
             Ltp = ops.pad8(Ltot)
             tab_s = ctx.storage(("b", i, "tab"), 1, 1, 1, Ltp, hd)
             tab = Planes(tab_s.hi, tab_s.lo, 1, 1, 1, Ltp, hd, 0)
@@ -595,7 +678,7 @@ class B200MViT(nn.Module):
             if tab_s.lo is not None:
                 tab_s.lo.zero_()
             off = 0
-            for prm in (at.rel_pos_h, at.rel_pos_w, at.rel_pos_t):
+            for prm in tabs:
                 n_ = prm.shape[0]
                 sub = Planes(tab_s.hi[..., off:off + n_, :], None if tab_s.lo is None else tab_s.lo[..., off:off + n_, :],
                              1, 1, 1, n_, hd, 0)
@@ -606,7 +689,7 @@ class B200MViT(nn.Module):
             rq = ctx.scratch("attn.RQ", BH * Lq * Ltp, F32).view(BH * Lq, Ltp)
             qv = Planes(pl["q"].hi, pl["q"].lo, BH, 1, 1, Nq, hd, 0)
             fm = ops.FilterMat(tab.hi.view(Ltp, hd), None if tab.lo is None else tab.lo.view(Ltp, hd), Ltp, 1, hd)
-            ops.conv_igemm(qv, fm, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 1), (1, 1, Lq)), rq,
+            ops.conv_igemm(qv, fm, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, nc), (1, 1, Lq)), rq,
                            (Lq * Ltp, Lq * Ltp, Lq * Ltp, Ltp), nsplit=ctx.nsplit)
         P = self._rows_planes(("b", i, "P"), BH * Nq, Nkp)
         O = ctx.scratch("attn.O", BH * Nq * hd, F32).view(BH, Nq, hd)
@@ -618,14 +701,15 @@ class B200MViT(nn.Module):
         sd.bh, sd.nq, sd.nk = BH, Nq, Nk
         sd.qt, sd.qh, sd.qw = q_thw
         sd.kt, sd.kh, sd.kw = k_thw
+        sd.no_cls, sd.spatial_only = 1 - nc, int(len(tabs) == 2)
         L.check(lib.sfb_softmax_relpos_fwd(C.byref(sd), _st()), "sfb_softmax_relpos_fwd")
         ops._count()
         # O = P v  (v is MN-major: memory [bh][k][hd])
         self._bgemm(P, (Nkp, Nq * Nkp), False, pl["v"], (hd, Nk * hd), True, Nq, hd, Nk, BH, O, hd)
         merged = self._rows_planes(("b", i, "merged"), B * Nq, A)
-        L.check(lib.sfb_attn_merge(O.data_ptr(), pl["q"].hi_ptr(), pl["q"].lo_ptr(), B, Hn, Nq, hd,
-                                   1 if self.residual_pooling else 0, merged.hi_ptr(), merged.lo_ptr(), _st()),
-                "sfb_attn_merge")
+        merge = lib.sfb_attn_merge if nc else lib.sfb_attn_merge_nocls
+        L.check(merge(O.data_ptr(), pl["q"].hi_ptr(), pl["q"].lo_ptr(), B, Hn, Nq, hd, 1 if self.residual_pooling else 0,
+                      merged.hi_ptr(), merged.lo_ptr(), _st()), "sfb_attn_merge")
         ops._count()
         yproj = self._lin_fwd(("b", i, "yproj"), at.proj, merged)
         # skip path
@@ -647,6 +731,7 @@ class B200MViT(nn.Module):
             td.ot, td.oh, td.ow = q_thw
             td.kt, td.kh, td.kw = ks
             td.st, td.sh, td.sw = sq
+            td.no_cls = 1 - nc
             L.check(lib.sfb_token_maxpool_fwd(C.byref(td), _st()), "sfb_token_maxpool_fwd")
             ops._count()
             src = xsp.view(B * Nq, A)
@@ -698,7 +783,11 @@ class B200MViT(nn.Module):
         Lt = T * H * W
         pe = self.patch_embed.proj
         E = pe.out_channels
-        if self.use_abs_pos:
+        if self.use_abs_pos and not self.sep_pos_embed:
+            L.check(lib.sfb_pos_embed_joint_bwd(dx.data_ptr(), B, Lt + self.ncls, E,
+                                                ctx.grad_of(self.pos_embed).data_ptr(), _st()), "sfb_pos_embed_joint_bwd")
+            ops._count()
+        elif self.use_abs_pos:
             part = ctx.scratch("pos.part", T * lib.sfb_segment_slabs(T, H * W) * E, F32)
             L.check(lib.sfb_pos_embed_sep_bwd(dx.data_ptr(), B, T, H * W, E, ctx.grad_of(self.pos_embed_spatial).data_ptr(),
                                               ctx.grad_of(self.pos_embed_temporal).data_ptr(),
@@ -707,7 +796,8 @@ class B200MViT(nn.Module):
             ops._count(3)
         dyp, dyf = self._tokens_split_grad(dx, B, Lt, E)
         self._colsum(dyf, B * Lt, E, ctx.grad_of(pe.bias))
-        self._colsum(dx, B, E, ctx.grad_of(self.cls_token).view(E), pitch=(Lt + 1) * E)
+        if self.ncls:
+            self._colsum(dx, B, E, ctx.grad_of(self.cls_token).view(E), pitch=(Lt + 1) * E)
         if self.patchify:
             xr = sv["xin"]
             gw = ctx.grad_of(pe.weight).view(E, xr.c)
@@ -729,11 +819,12 @@ class B200MViT(nn.Module):
         A = Do if self.dim_mul_in_att else D
         hd = A // Hn
         T, Hh, W = sv["thw"]
-        N = T * Hh * W + 1
+        nc = self.ncls
+        N = T * Hh * W + nc
         rows = B * N
         q_thw, k_thw = sv["q_thw"], sv["k_thw"]
         Lq, Lk = math.prod(q_thw), math.prod(k_thw)
-        Nq, Nk = Lq + 1, Lk + 1
+        Nq, Nk = Lq + nc, Lk + nc
         Nkp = ops.pad8(Nk)
         BH = B * Hn
         rq_rows = B * Nq
@@ -779,8 +870,9 @@ class B200MViT(nn.Module):
         self._lin_bwd(at.proj, gp, gpf, sv["merged"], dmerged)
         dO = self._rows_planes("attn.dO", BH * Nq, hd, scratch=True)
         dq = ctx.scratch("attn.dq", BH * Nq * hd, F32).view(BH, Nq, hd)
-        L.check(lib.sfb_attn_split_grad(dmerged.data_ptr(), B, Hn, Nq, hd, 1 if self.residual_pooling else 0,
-                                        dO.hi_ptr(), dO.lo_ptr(), dq.data_ptr(), _st()), "sfb_attn_split_grad")
+        split_grad = lib.sfb_attn_split_grad if nc else lib.sfb_attn_split_grad_nocls
+        L.check(split_grad(dmerged.data_ptr(), B, Hn, Nq, hd, 1 if self.residual_pooling else 0, dO.hi_ptr(), dO.lo_ptr(),
+                           dq.data_ptr(), _st()), "sfb_attn_split_grad")
         ops._count()
         pl, P = sv["pl"], sv["P"]
         dv = ctx.scratch("attn.dv", BH * Nk * hd, F32).view(BH, Nk, hd)
@@ -798,6 +890,8 @@ class B200MViT(nn.Module):
         sd.dp, sd.dp_pitch = dP.data_ptr(), Nkp
         sd.ds_hi, sd.ds_lo, sd.ds_pitch = dS.hi_ptr(), dS.lo_ptr(), Nkp
         sd.drq, sd.rq_pitch = _ptr(drq), Ltp
+        tabs = self._rel_tables(at)
+        sd.no_cls, sd.spatial_only = 1 - nc, int(len(tabs) == 2)
         L.check(lib.sfb_softmax_relpos_bwd(C.byref(sd), _st()), "sfb_softmax_relpos_bwd")
         ops._count()
         scale = hd ** -0.5
@@ -819,15 +913,15 @@ class B200MViT(nn.Module):
             fm = ops.FilterMat(ft, ftl, hd, 1, Ltp)
             drq_v = Planes(drq_p.hi, drq_p.lo, BH, 1, 1, Lq, Ltp, 0)
             ops.conv_igemm(drq_v, fm, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 0), (1, 1, Lq)), dq,
-                           (Nq * hd, Nq * hd, Nq * hd, hd), out_offset=hd, accumulate=True, nsplit=ctx.nsplit)
+                           (Nq * hd, Nq * hd, Nq * hd, hd), out_offset=nc * hd, accumulate=True, nsplit=ctx.nsplit)
             # d tables = dRQ^T . q_nocls
             dtab = ctx.scratch("attn.dtab", Ltp * hd, F32).view(Ltp, hd)
             ops.zero_f32(ops.f32view(dtab))
             qv = Planes(pl["q"].hi, pl["q"].lo, BH, 1, 1, Nq, hd, 0)
             ops.conv_wgrad(qv, Planes(drq_p.hi, drq_p.lo, BH, 1, 1, Lq, Ltp, 0),
-                           ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 1), (1, 1, Lq)), dtab, nsplit=ctx.nsplit)
+                           ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, nc), (1, 1, Lq)), dtab, nsplit=ctx.nsplit)
             off = 0
-            for prm in (at.rel_pos_h, at.rel_pos_w, at.rel_pos_t):
+            for prm in tabs:
                 n_ = prm.shape[0]
                 g = ctx.grad_of(prm)
                 ops.zero_f32(ops.f32view(g))
@@ -839,7 +933,7 @@ class B200MViT(nn.Module):
         for j, (name, grad) in enumerate((("q", dq), ("k", dk), ("v", dv))):
             othw, has, kern, strd = sv["geo"][name]
             Lo = math.prod(othw)
-            prow = BH * (Lo + 1)
+            prow = BH * (Lo + nc)
             if has:
                 dpool = ctx.scratch("attn.dpool", prow * hd, F32).view(prow, hd)
                 m_, r_ = sv["stats"][name]
@@ -853,6 +947,7 @@ class B200MViT(nn.Module):
             d.b, d.heads, d.hd, d.t, d.h, d.w_ = B, Hn, hd, T, Hh, W
             d.ot, d.oh, d.ow = othw
             d.has_pool = 1 if has else 0
+            d.no_cls = 1 - nc
             d.dout, d.dsrc = dpool.data_ptr(), dyqkv.data_ptr()
             dw = None
             if has:
@@ -887,6 +982,7 @@ class B200MViT(nn.Module):
             td.kt, td.kh, td.kw = ks
             td.st, td.sh, td.sw = sq
             td.dout, td.dx, td.dx_accumulate = dx1.data_ptr(), dsrc.data_ptr(), 0
+            td.no_cls = 1 - nc
             L.check(lib.sfb_token_maxpool_bwd(C.byref(td), _st()), "sfb_token_maxpool_bwd")
             ops._count()
         dx_in = ctx.scratch("dx." + which, rows * D, F32).view(B, N, D)
