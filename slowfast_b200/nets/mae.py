@@ -35,7 +35,7 @@ from .. import ops
 from ..engine import ModelFunction, Namespace
 from ..ops import F32
 from .maskfeat import MSSeparateHeadModule, calc_mvit_feature_geometry
-from .mvit import B200MViT, BlockModule, _is_pool, _st, block_specs
+from .mvit import B200MViT, BlockModule, _is_pool, block_specs
 
 MAE_MAX_TOKENS = 4096  # sfb_mae_max_tokens(): one clip's noise row in the masking kernel's shared memory
 I32 = torch.int32
@@ -153,15 +153,12 @@ class B200MAE(B200MViT):
         B, C, T, H, W = frames.shape
         p = self.pixel_patch
         out = torch.empty((rows.numel(), self.pred_t * p * p * C), dtype=F32, device=frames.device)
-        L.check(L.load().sfb_pixel_targets(frames.contiguous().float().data_ptr(), B, C, T, H, W, self.patch_stride[0],
-                                           self.pred_t, p, rows.data_ptr(), rows.numel(), 1 if self.norm_pix else 0,
-                                           out.data_ptr(), _st()), "sfb_pixel_targets")
-        ops._count()
+        ops.pixel_targets(frames.contiguous().float(), self.patch_stride[0], self.pred_t, p, rows, self.norm_pix, out)
         return out
 
     # ------------------------------------------------------------------------------------------ forward program
     def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         x, noise = inputs
         ctx.device = x.device
         ctx.training = self.training
@@ -176,25 +173,18 @@ class B200MAE(B200MViT):
         ids_restore = ctx.buf(("mae.restore",), (B, Lt), I32)
         mask = ctx.buf(("mae.mask",), (B, Lt))
         rows = ctx.buf(("mae.rows",), (B * M,), I32)
-        L.check(lib.sfb_mae_random_masking(noise.data_ptr(), B, Lt, K, ids_keep.data_ptr(), ids_restore.data_ptr(),
-                                           mask.data_ptr(), rows.data_ptr(), _st()), "sfb_mae_random_masking")
-        ops._count()
+        ops.mae_random_masking(noise, K, ids_keep, ids_restore, mask, rows)
         # ---- patch embedding of the kept patches -> encoder tokens ---------------------------------------------------
         pe = self.patch_embed.proj
         k3, E = tuple(pe.kernel_size), pe.out_channels
         assert (t // k3[0], h // k3[1], w // k3[2]) == (self.T, self.H, self.W)
         Kd = cin * math.prod(k3)
         xin = self._rows_planes(("pe.rows",), B * K, Kd)
-        L.check(lib.sfb_patchify_gather(x.contiguous().float().data_ptr(), B, cin, t, h, w, *k3, ids_keep.data_ptr(), K,
-                                        xin.hi_ptr(), xin.lo_ptr(), _st()), "sfb_patchify_gather")
-        ops._count()
+        ops.patchify_gather(x.contiguous().float(), k3, ids_keep, K, xin)
         ype = self._mat_fwd(("pe.y",), pe.weight.view(E, Kd), xin)
         x0 = ctx.buf(("x", 0), (B, K + 1, E))
-        L.check(lib.sfb_tokens_assemble_keep(ype.data_ptr(), pe.bias.data_ptr(), self.cls_token.data_ptr(),
-                                             self.pos_embed_spatial.data_ptr(), self.pos_embed_temporal.data_ptr(),
-                                             self.pos_embed_class.data_ptr(), ids_keep.data_ptr(), B, K, Lt,
-                                             self.H * self.W, E, x0.data_ptr(), _st()), "sfb_tokens_assemble_keep")
-        ops._count()
+        ops.tokens_assemble_keep(ype, pe.bias, self.cls_token, self.pos_embed_spatial, self.pos_embed_temporal,
+                                 self.pos_embed_class, ids_keep, B, K, Lt, self.H * self.W, E, x0)
         # ---- encoder (the kept tokens as a 1 x 1 x K grid) -----------------------------------------------------------
         saved = []
         cur = x0
@@ -211,10 +201,8 @@ class B200MAE(B200MViT):
         z = self._lin_fwd(("mae.z",), self.decoder_embed, lat)
         D = self.decoder_embed.out_features
         xd = ctx.buf(("mae.xd",), (B, Lt + 1, D))
-        L.check(lib.sfb_decoder_assemble(z.data_ptr(), self.decoder_embed.bias.data_ptr(), self.mask_token.data_ptr(),
-                                         self.decoder_pos_embed.data_ptr(), ids_restore.data_ptr(), B, K, Lt, D,
-                                         xd.data_ptr(), _st()), "sfb_decoder_assemble")
-        ops._count()
+        ops.decoder_assemble(z, self.decoder_embed.bias, self.mask_token, self.decoder_pos_embed, ids_restore, B, K, Lt, D,
+                             xd)
         n_enc = len(self.blocks)
         dec_saved = []
         cur = xd
@@ -224,9 +212,7 @@ class B200MAE(B200MViT):
             dec_saved.append(sv)
         # ---- head on the removed tokens -----------------------------------------------------------------------------
         sel = ctx.buf(("mae.sel",), (B * M, D))
-        L.check(lib.sfb_rows_gather(cur.data_ptr(), D, rows.data_ptr(), B * M, D, None, sel.data_ptr(), _st()),
-                "sfb_rows_gather")
-        ops._count()
+        ops.rows_gather(cur, D, rows, B * M, D, None, sel)
         seln = self._rows_planes(("mae.seln",), B * M, D)
         hm, hr = ctx.buf(("mae.hm",), (B * M,)), ctx.buf(("mae.hr",), (B * M,))
         self._ln_fwd(sel, D, B * M, D, head[len(self.dec_specs)], seln, None, hm, hr)
@@ -234,9 +220,7 @@ class B200MAE(B200MViT):
         y = self._lin_fwd(("mae.y",), proj, seln)
         nc = proj.out_features
         pred = torch.empty((B * M, nc), dtype=F32, device=ctx.device)
-        L.check(lib.sfb_rows_gather(y.data_ptr(), nc, None, B * M, nc, proj.bias.data_ptr(), pred.data_ptr(), _st()),
-                "sfb_rows_gather")
-        ops._count()
+        ops.rows_gather(y, nc, None, B * M, nc, proj.bias, pred)
         object.__setattr__(self, "_saved", dict(B=B, xin=xin, blocks=saved, dec=dec_saved, enc=enc, lat=lat, em=em,
                                                 er=er, sel=sel, seln=seln, hm=hm, hr=hr, ids_keep=ids_keep,
                                                 ids_restore=ids_restore, rows=rows))
@@ -244,7 +228,7 @@ class B200MAE(B200MViT):
 
     # ------------------------------------------------------------------------------------------ backward program
     def _engine_backward(self, dpred: torch.Tensor):
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         params = [p for p in self.parameters()]
         ctx.begin_backward(params)
         sv = self._saved
@@ -264,9 +248,7 @@ class B200MAE(B200MViT):
         self._ln_bwd(dseln, D, sv["sel"], D, B * M, D, head[len(self.dec_specs)], sv["hm"], sv["hr"], dsel, D, False)
         dxd = ctx.scratch("mae.dxd", B * (Lt + 1) * D, F32).view(B, Lt + 1, D)
         ops.zero_f32(ops.f32view(dxd.view(B * (Lt + 1), D)))
-        L.check(lib.sfb_rows_scatter(dsel.data_ptr(), rows.data_ptr(), B * M, D, dxd.data_ptr(), _st()),
-                "sfb_rows_scatter")
-        ops._count()
+        ops.rows_scatter(dsel, rows, B * M, D, dxd)
         # ---- decoder blocks --------------------------------------------------------------------------------------
         n_enc = len(self.blocks)
         which = "a"
@@ -276,12 +258,9 @@ class B200MAE(B200MViT):
             dx = self._block_backward(n_enc + j, head[j], self.dec_specs[j], sv["dec"][j], dx, B, which)
         # ---- decoder assembly: d decoder_embed output, d decoder_pos_embed, d mask_token ---------------------------
         dz = ctx.scratch("mae.dz", B * (K + 1) * D, F32).view(B * (K + 1), D)
-        part = ctx.scratch("mae.part", lib.sfb_segment_slabs(1, B * M) * D, F32)
-        L.check(lib.sfb_decoder_assemble_bwd(dx.data_ptr(), sv["ids_keep"].data_ptr(), rows.data_ptr(), B, K, Lt, D,
-                                             dz.data_ptr(), ctx.grad_of(self.decoder_pos_embed).data_ptr(),
-                                             ctx.grad_of(self.mask_token).data_ptr(), part.data_ptr(), _st()),
-                "sfb_decoder_assemble_bwd")
-        ops._count(4)
+        part = ctx.scratch("mae.part", ops.segment_slabs(1, B * M) * D, F32)
+        ops.decoder_assemble_bwd(dx, sv["ids_keep"], rows, B, K, Lt, D, dz, ctx.grad_of(self.decoder_pos_embed),
+                                 ctx.grad_of(self.mask_token), part)
         rows_e = B * (K + 1)
         dzp = ctx.scratch_planes("mae.dzp", 1, 1, 1, rows_e, D)
         ops.split_planes(dz.view(1, 1, 1, rows_e, D), dzp)
@@ -300,15 +279,10 @@ class B200MAE(B200MViT):
         E = pe.out_channels
         T, HW = self.T, self.H * self.W
         dense = ctx.scratch("mae.dense", B * (Lt + 1) * E, F32)
-        L.check(lib.sfb_tokens_scatter_keep(dx.data_ptr(), sv["ids_restore"].data_ptr(), B, K, Lt, E, dense.data_ptr(),
-                                            _st()), "sfb_tokens_scatter_keep")
-        ops._count()
-        ppart = ctx.scratch("pos.part", T * lib.sfb_segment_slabs(T, HW) * E, F32)
-        L.check(lib.sfb_pos_embed_sep_bwd(dense.data_ptr(), B, T, HW, E, ctx.grad_of(self.pos_embed_spatial).data_ptr(),
-                                          ctx.grad_of(self.pos_embed_temporal).data_ptr(),
-                                          ctx.grad_of(self.pos_embed_class).data_ptr(), ppart.data_ptr(), _st()),
-                "sfb_pos_embed_sep_bwd")
-        ops._count(3)
+        ops.tokens_scatter_keep(dx, sv["ids_restore"], B, K, Lt, E, dense)
+        ppart = ctx.scratch("pos.part", T * ops.segment_slabs(T, HW) * E, F32)
+        ops.pos_embed_sep_bwd(dense, B, T, HW, E, ctx.grad_of(self.pos_embed_spatial), ctx.grad_of(self.pos_embed_temporal),
+                              ctx.grad_of(self.pos_embed_class), ppart)
         dyp, dyf = self._tokens_split_grad(dx, B, K, E)
         self._colsum(dyf, B * K, E, ctx.grad_of(pe.bias))
         self._colsum(dx, B, E, ctx.grad_of(self.cls_token).view(E), pitch=(K + 1) * E)

@@ -26,7 +26,7 @@ from .. import lib as L
 from .. import ops
 from ..engine import ModelFunction, Namespace
 from ..ops import BF16, F32, Planes
-from .mvit import B200MViT, _st
+from .mvit import B200MViT
 
 
 def calc_mvit_feature_geometry(cfg):
@@ -155,41 +155,33 @@ class B200MaskMViT(B200MViT):
         fs = self.feat_size[self.pretrain_depth[-1]][-1]
         u = (H // self.cell_sz) // fs
         out = torch.empty((B, (T // ts) * fs * fs, C * self.nbins * u * u), dtype=F32, device=frames.device)
-        L.check(L.load().sfb_hog_targets(frames.contiguous().float().data_ptr(), B, C, T, H, W, ts, self.nbins,
-                                         self.cell_sz, fs, out.data_ptr(), _st()), "sfb_hog_targets")
-        ops._count()
+        ops.hog_targets(frames.contiguous().float(), ts, self.nbins, self.cell_sz, fs, out)
         return out
 
     # ------------------------------------------------------------------------------------------ engine hooks
     def _tokens_assemble(self, ype, x0, B, Lt, E, inputs) -> None:
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         fmask = inputs[1]
         mb, mt, mh, mw = fmask.shape
         assert mb == B and mt == self.T, "the cube mask must have one slice per token frame"
         tokmask = ctx.buf(("mf.tokmask",), (B, Lt))
-        L.check(lib.sfb_mask_upsample(fmask.data_ptr(), B, mt, mh, mw, self.T, self.H, self.W, tokmask.data_ptr(), _st()),
-                "sfb_mask_upsample")
+        ops.mask_upsample(fmask, (self.T, self.H, self.W), tokmask)
         pe = self.patch_embed.proj
-        L.check(lib.sfb_tokens_assemble_masked(ype.data_ptr(), pe.bias.data_ptr(), self.cls_token.data_ptr(),
-                                               self.mask_token.data_ptr(), tokmask.data_ptr(), B, Lt, E, x0.data_ptr(),
-                                               _st()), "sfb_tokens_assemble_masked")
-        ops._count(2)
+        ops.tokens_assemble_masked(ype, pe.bias, self.cls_token, self.mask_token, tokmask, B, Lt, E, x0)
 
     def _tokens_split_grad(self, dx, B, Lt, E):
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         dyp = self._rows_planes("pe.dy", B * Lt, E, scratch=True)
         dyf = ctx.scratch("pe.dyf", B * Lt * E, F32)
         dxm = ctx.scratch("mf.dxm", B * Lt * E, F32)
         tokmask = ctx.buf(("mf.tokmask",), (B, Lt))
-        L.check(lib.sfb_tokens_split_grad_masked(dx.data_ptr(), tokmask.data_ptr(), B, Lt, E, dyp.hi_ptr(), dyp.lo_ptr(),
-                                                 dyf.data_ptr(), dxm.data_ptr(), _st()), "sfb_tokens_split_grad_masked")
-        ops._count()
+        ops.tokens_split_grad_masked(dx, tokmask, B, Lt, E, dyp, dyf, dxm)
         self._colsum(dxm, B * Lt, E, ctx.grad_of(self.mask_token).view(E))
         return dyp, dyf
 
     def _final_forward(self, cur: torch.Tensor, thw, B) -> torch.Tensor:
         """MSSeparateHead (head_helper.py:656-672) for every token of the last kept block."""
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         Nf, Cf = cur.shape[1], cur.shape[2]
         ln = self.pred_head.transforms[0][0]
         proj = self.pred_head.projections[0]
@@ -200,14 +192,12 @@ class B200MaskMViT(B200MViT):
         self._ln_fwd(cur, Cf, rows, Cf, ln, xn, None, mean, rstd)
         y = self._lin_fwd(("mf.y",), proj, xn)  # [rows, nc] (bias added below)
         pred = torch.empty((B, Nf - 1, nc), dtype=F32, device=ctx.device)
-        L.check(lib.sfb_rows_unpad_bias(y.data_ptr(), nc, proj.bias.data_ptr(), B, Nf - 1, nc, pred.data_ptr(), _st()),
-                "sfb_rows_unpad_bias")
-        ops._count()
+        ops.rows_unpad_bias(y, nc, proj.bias, B, Nf - 1, nc, pred)
         self._saved["final"] = (cur, xn, mean, rstd)
         return pred
 
     def _final_backward(self, dpred: torch.Tensor) -> torch.Tensor:
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         sv = self._saved
         B = sv["B"]
         cur, xn, mean, rstd = sv["final"]
@@ -219,9 +209,7 @@ class B200MaskMViT(B200MViT):
         rows = B * Nf
         # gradient w.r.t. the Linear output for every row (cls rows and the pad columns are zero)
         dyp = ctx.scratch_planes("mf.dy", 1, 1, 1, rows, ncp)
-        L.check(lib.sfb_rows_pad_split(dpred.data_ptr(), B, Nf - 1, nc, ncp, dyp.hi_ptr(), dyp.lo_ptr(), _st()),
-                "sfb_rows_pad_split")
-        ops._count()
+        ops.rows_pad_split(dpred, B, Nf - 1, nc, dyp)
         self._colsum(dpred, B * (Nf - 1), nc, ctx.grad_of(proj.bias))
         # dW [ncp, Cf] (rows >= nc are zero) -> parameter gradient; dxn = dy . W
         dwm = ctx.scratch("mf.dwm", ncp * Cf, F32).view(ncp, Cf)

@@ -21,7 +21,6 @@ readout (norm on every token, then the mean).
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import List, Optional
 
@@ -170,14 +169,6 @@ class TransformerHeadModule(Namespace):
         self.projection = nn.Linear(dim_in, num_classes, bias=True)
         self.dropout_rate = dropout_rate
         self.act_func = act_func
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 class B200MViT(nn.Module):
@@ -382,33 +373,18 @@ class B200MViT(nn.Module):
         ops.colsum(src, rows, c, out, part, pitch=pitch, accumulate=accumulate)
 
     def _ln_fwd(self, x: torch.Tensor, x_pitch, rows, c, ln: nn.LayerNorm, out: Optional[Planes], out_f32, mean, rstd):
-        lib = L.load()
-        L.check(lib.sfb_layernorm_fwd(x.data_ptr(), x_pitch, rows, c, ln.weight.data_ptr(), ln.bias.data_ptr(), ln.eps,
-                                      out.hi_ptr() if out is not None else None,
-                                      out.lo_ptr() if out is not None else None, _ptr(out_f32), c, _ptr(mean),
-                                      _ptr(rstd), _st()), "sfb_layernorm_fwd")
-        ops._count()
+        ops.layernorm_fwd(x, x_pitch, rows, c, ln.weight, ln.bias, ln.eps, mean, rstd, out=out, out_f32=out_f32)
 
     def _ln_bwd(self, dy, dy_pitch, x, x_pitch, rows, c, ln: nn.LayerNorm, mean, rstd, dx, dx_pitch, dx_acc,
                 param_acc=False):
-        lib = L.load()
-        nb = lib.sfb_rowslab_blocks(rows)
-        part = self.ctx.scratch("ln.part", nb * 2 * c, F32)
-        L.check(lib.sfb_layernorm_bwd(dy.data_ptr(), dy_pitch, x.data_ptr(), x_pitch, rows, c, ln.weight.data_ptr(),
-                                      mean.data_ptr(), rstd.data_ptr(), dx.data_ptr(), dx_pitch, 1 if dx_acc else 0,
-                                      self.ctx.grad_of(ln.weight).data_ptr(), self.ctx.grad_of(ln.bias).data_ptr(),
-                                      1 if param_acc else 0, part.data_ptr(), _st()), "sfb_layernorm_bwd")
-        ops._count(2)
-
-    def _bgemm(self, a: Planes, a_shape, a_mn, b: Planes, b_shape, b_mn, m, n, k, batch, out, ldd, alpha=1.0,
-               accumulate=False):
-        """a_shape / b_shape = (pitch, batch_stride) in elements of the storage as laid out in memory."""
-        ops.gemm_batched(a, a_shape, a_mn, b, b_shape, b_mn, m, n, k, batch, out, ldd, alpha=alpha, accumulate=accumulate,
-                         nsplit=self.ctx.nsplit)
+        ctx = self.ctx
+        part = ctx.scratch("ln.part", ops.colsum_blocks(rows) * 2 * c, F32)
+        ops.layernorm_bwd(dy, dy_pitch, x, x_pitch, rows, c, ln.weight, mean, rstd, dx, dx_pitch, ctx.grad_of(ln.weight),
+                          ctx.grad_of(ln.bias), part, dx_accumulate=dx_acc, param_accumulate=param_acc)
 
     # ================================================================================== forward program
     def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         x = inputs[0]
         if self.patch_2d:
             x = x.unsqueeze(2)  # [B, C, H, W] -> [B, C, 1, H, W]: the same memory as a one-frame clip
@@ -429,9 +405,7 @@ class B200MViT(nn.Module):
             Lt = T * H * W
             K = cin * math.prod(k3)
             xin_p = self._rows_planes(("pe.rows",), B * Lt, K)
-            L.check(lib.sfb_patchify(x.contiguous().float().data_ptr(), n, cin, t, h, w, *k3, xin_p.hi_ptr(),
-                                     xin_p.lo_ptr(), _st()), "sfb_patchify")
-            ops._count()
+            ops.patchify(x.contiguous().float(), k3, xin_p)
             geom = None
             ype = self._mat_fwd(("pe.y",), pe.weight.view(E, K), xin_p)
         else:
@@ -463,9 +437,7 @@ class B200MViT(nn.Module):
                 object.__setattr__(self, "_dp_rates_set", rates)
                 object.__setattr__(self, "_dp_counter", torch.zeros(1, dtype=torch.int64, device=ctx.device))
             dp = ctx.buf(("dp.scales",), (2 * nb, B))
-            L.check(lib.sfb_droppath_scales(dp.data_ptr(), rates.data_ptr(), 2 * nb, B, self._seed,
-                                            self._dp_counter.data_ptr(), _st()), "sfb_droppath_scales")
-            ops._count(2)
+            ops.droppath_scales(dp, rates, self._seed, self._dp_counter)
         # ---- blocks --------------------------------------------------------------------------------------------
         saved = []
         cur, thw = x0, [T, H, W]
@@ -490,18 +462,13 @@ class B200MViT(nn.Module):
         pe = self.patch_embed.proj
         if not self.ncls or (self.use_abs_pos and not self.sep_pos_embed):
             # cls-free layout and / or the joint table: (y + bias) + pos[n], the cls row cls + pos[0]
-            L.check(L.load().sfb_tokens_assemble_joint(ype.data_ptr(), pe.bias.data_ptr(),
-                                                       self.cls_token.data_ptr() if self.ncls else None,
-                                                       self.pos_embed.data_ptr() if self.use_abs_pos else None, B, Lt, E,
-                                                       x0.data_ptr(), _st()), "sfb_tokens_assemble_joint")
-            ops._count()
+            ops.tokens_assemble_joint(ype, pe.bias, self.cls_token if self.ncls else None,
+                                      self.pos_embed if self.use_abs_pos else None, B, Lt, E, x0)
             return
         pos = [None] * 3
         if self.use_abs_pos:
-            pos = [p.data_ptr() for p in (self.pos_embed_spatial, self.pos_embed_temporal, self.pos_embed_class)]
-        L.check(L.load().sfb_tokens_assemble(ype.data_ptr(), pe.bias.data_ptr(), self.cls_token.data_ptr(), *pos, B, Lt,
-                                             self.H * self.W, E, x0.data_ptr(), _st()), "sfb_tokens_assemble")
-        ops._count()
+            pos = [self.pos_embed_spatial, self.pos_embed_temporal, self.pos_embed_class]
+        ops.tokens_assemble(ype, pe.bias, self.cls_token, *pos, B, Lt, self.H * self.W, E, x0)
 
     def _tokens_split_grad(self, dx, B, Lt, E):
         """Gradient of the token sequence -> patch-embedding output gradient (planes + fp32)."""
@@ -511,22 +478,18 @@ class B200MViT(nn.Module):
             ops.split_planes(dx.view(1, 1, 1, B * Lt, E), dyp)
             return dyp, dx.view(B * Lt, E)
         dyf = ctx.scratch("pe.dyf", B * Lt * E, F32)
-        L.check(L.load().sfb_tokens_split_grad(dx.data_ptr(), B, Lt, E, dyp.hi_ptr(), dyp.lo_ptr(), dyf.data_ptr(),
-                                               _st()), "sfb_tokens_split_grad")
-        ops._count()
+        ops.tokens_split_grad(dx, B, Lt, E, dyp, dyf)
         return dyp, dyf
 
     def _final_forward(self, cur: torch.Tensor, thw, B) -> torch.Tensor:
         """Final LayerNorm on the cls rows, or on the mean of the other tokens (USE_MEAN_POOLING), or (no cls token, the
         default readout) on every token and then the mean, + TransformerBasicHead (video_model_builder.py:1230-1242)."""
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         Nf, Cf = cur.shape[1], cur.shape[2]
         if self.use_mean_pooling:
             ln_in, ln_pitch = ctx.buf(("final.pool",), (B, Cf)), Cf
-            part = ctx.scratch("final.pool.part", B * lib.sfb_segment_slabs(B, Nf - self.ncls) * Cf, F32)
-            mean_fwd = lib.sfb_token_mean_fwd if self.ncls else lib.sfb_token_mean_all_fwd
-            L.check(mean_fwd(cur.data_ptr(), B, Nf, Cf, ln_in.data_ptr(), part.data_ptr(), _st()), "sfb_token_mean_fwd")
-            ops._count(2)
+            part = ctx.scratch("final.pool.part", B * ops.segment_slabs(B, Nf - self.ncls) * Cf, F32)
+            ops.token_mean_fwd(cur, B, Nf, Cf, ln_in, part, cls=bool(self.ncls))
         else:
             ln_in, ln_pitch = cur, Nf * Cf
         cls_n = ctx.buf(("final.cls",), (B, Cf))
@@ -535,10 +498,8 @@ class B200MViT(nn.Module):
             normed = ctx.buf(("final.normed",), (B * Nf, Cf))
             fmean, frstd = ctx.buf(("final.mean",), (B * Nf,)), ctx.buf(("final.rstd",), (B * Nf,))
             self._ln_fwd(cur, Cf, B * Nf, Cf, self.norm, None, normed, fmean, frstd)
-            part = ctx.scratch("final.pool.part", B * lib.sfb_segment_slabs(B, Nf) * Cf, F32)
-            L.check(lib.sfb_token_mean_all_fwd(normed.data_ptr(), B, Nf, Cf, cls_n.data_ptr(), part.data_ptr(), _st()),
-                    "sfb_token_mean_all_fwd")
-            ops._count(2)
+            part = ctx.scratch("final.pool.part", B * ops.segment_slabs(B, Nf) * Cf, F32)
+            ops.token_mean_fwd(normed, B, Nf, Cf, cls_n, part, cls=False)
         else:
             fmean, frstd = ctx.buf(("final.mean",), (B,)), ctx.buf(("final.rstd",), (B,))
             self._ln_fwd(ln_in, ln_pitch, B, Cf, self.norm, None, cls_n, fmean, frstd)
@@ -574,20 +535,15 @@ class B200MViT(nn.Module):
         if mask is not None:
             ops.dropout_bwd(dfeat, mask, head.dropout_rate)
         dx = ctx.scratch("dx.a", B * Nf * Cf, F32).view(B, Nf, Cf)
-        lib = L.load()
         if self.use_mean_pooling:
             dpool = ctx.scratch("final.dpool", B * Cf, F32).view(B, Cf)
             self._ln_bwd(dfeat, Cf, ln_in, ln_pitch, B, Cf, self.norm, fmean, frstd, dpool, Cf, False)
-            mean_bwd = lib.sfb_token_mean_bwd if self.ncls else lib.sfb_token_mean_all_bwd
-            L.check(mean_bwd(dpool.data_ptr(), B, Nf, Cf, dx.data_ptr(), _st()), "sfb_token_mean_bwd")
-            ops._count()
+            ops.token_mean_bwd(dpool, B, Nf, Cf, dx, cls=bool(self.ncls))
             return dx
         if not self.ncls:
             # dmean / Nf on every row, then the norm's backward over all B * Nf rows
             dn = ctx.scratch("final.dnormed", B * Nf * Cf, F32)
-            L.check(lib.sfb_token_mean_all_bwd(dfeat.data_ptr(), B, Nf, Cf, dn.data_ptr(), _st()),
-                    "sfb_token_mean_all_bwd")
-            ops._count()
+            ops.token_mean_bwd(dfeat, B, Nf, Cf, dn, cls=False)
             self._ln_bwd(dn, Cf, cur, Cf, B * Nf, Cf, self.norm, fmean, frstd, dx, Cf, False)
             return dx
         ops.zero_f32(ops.f32view(dx.view(B * Nf, Cf)))
@@ -605,7 +561,7 @@ class B200MViT(nn.Module):
         return [ops.conv_out_size(i, k, s, k // 2) for i, k, s in zip(thw, kernel, stride)], True
 
     def _block_forward(self, i, blk: BlockModule, spec, x_in: torch.Tensor, thw, B, dp):
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         # D: block input width, A: attention width (= Do with DIM_MUL_IN_ATT, = D without), Do: block output width
         D, Do, Hn = spec["dim"], spec["dim_out"], spec["heads"]
         A = Do if self.dim_mul_in_att else D
@@ -627,23 +583,9 @@ class B200MViT(nn.Module):
                                                 ("v", spec["kkv"], spec["skv"]))):
             othw, has = self._pool_geom(thw, kern, strd)
             Lo = othw[0] * othw[1] * othw[2]
-            d = L.DwPoolDesc()
-            d.src, d.src_pitch, d.src_c0 = yqkv.data_ptr(), 3 * A, j * A
-            d.bias = _ptr(at.qkv.bias)
             out = ctx.buf(("b", i, "pool", name), (B, Hn, Lo + nc, hd))
-            d.out = out.data_ptr()
-            d.b, d.heads, d.hd, d.t, d.h, d.w_ = B, Hn, hd, T, Hh, W
-            d.ot, d.oh, d.ow = othw
-            d.has_pool = 1 if has else 0
-            d.no_cls = 1 - nc
-            if has:
-                d.w = getattr(at, f"pool_{name}").weight.data_ptr()
-                d.kt, d.kh, d.kw = kern
-                d.st, d.sh, d.sw = strd
-            else:
-                d.kt = d.kh = d.kw = d.st = d.sh = d.sw = 1
-            L.check(lib.sfb_dwpool_fwd(C.byref(d), _st()), "sfb_dwpool_fwd")
-            ops._count()
+            ops.dwpool_fwd(yqkv, j * A, at.qkv.bias, getattr(at, f"pool_{name}").weight if has else None, B, Hn, hd, thw,
+                           othw, kern, strd, out, cls=bool(nc))
             prow = B * Hn * (Lo + nc)
             pp = self._rows_planes(("b", i, "pl", name), prow, hd)
             if has:
@@ -660,8 +602,8 @@ class B200MViT(nn.Module):
         BH = B * Hn
         # S = scale * q k^T
         S = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
-        self._bgemm(pl["q"], (hd, Nq * hd), False, pl["k"], (hd, Nk * hd), False, Nq, Nk, hd, BH, S, Nkp,
-                    alpha=hd ** -0.5)
+        ops.gemm_batched(pl["q"], (hd, Nq * hd), False, pl["k"], (hd, Nk * hd), False, Nq, Nk, hd, BH, S, Nkp,
+                         alpha=hd ** -0.5, nsplit=ctx.nsplit)
         # decomposed relative positions: RQ = q_nocls . [Rh; Rw; Rt]^T  (Rt absent: spatial terms only)
         rq, Ltp, tab = None, 0, None
         tabs = self._rel_tables(at)
@@ -682,9 +624,7 @@ class B200MViT(nn.Module):
                 n_ = prm.shape[0]
                 sub = Planes(tab_s.hi[..., off:off + n_, :], None if tab_s.lo is None else tab_s.lo[..., off:off + n_, :],
                              1, 1, 1, n_, hd, 0)
-                L.check(lib.sfb_split_planes(prm.data_ptr(), n_, hd, hd, sub.hi.data_ptr(),
-                                             None if sub.lo is None else sub.lo.data_ptr(), hd, _st()), "split(tab)")
-                ops._count()
+                ops.split_planes(prm, sub)
                 off += n_
             rq = ctx.scratch("attn.RQ", BH * Lq * Ltp, F32).view(BH * Lq, Ltp)
             qv = Planes(pl["q"].hi, pl["q"].lo, BH, 1, 1, Nq, hd, 0)
@@ -694,23 +634,11 @@ class B200MViT(nn.Module):
         P = self._rows_planes(("b", i, "P"), BH * Nq, Nkp)
         O = ctx.scratch("attn.O", BH * Nq * hd, F32).view(BH, Nq, hd)
         # softmax (+ bias) -> P planes
-        sd = L.SoftmaxDesc()
-        sd.s, sd.s_pitch = S.data_ptr(), Nkp
-        sd.rq, sd.rq_pitch = _ptr(rq), Ltp
-        sd.p_hi, sd.p_lo, sd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
-        sd.bh, sd.nq, sd.nk = BH, Nq, Nk
-        sd.qt, sd.qh, sd.qw = q_thw
-        sd.kt, sd.kh, sd.kw = k_thw
-        sd.no_cls, sd.spatial_only = 1 - nc, int(len(tabs) == 2)
-        L.check(lib.sfb_softmax_relpos_fwd(C.byref(sd), _st()), "sfb_softmax_relpos_fwd")
-        ops._count()
+        ops.softmax_relpos_fwd(S, P, BH, Nq, Nk, q_thw, k_thw, rq=rq, cls=bool(nc), spatial_only=len(tabs) == 2)
         # O = P v  (v is MN-major: memory [bh][k][hd])
-        self._bgemm(P, (Nkp, Nq * Nkp), False, pl["v"], (hd, Nk * hd), True, Nq, hd, Nk, BH, O, hd)
+        ops.gemm_batched(P, (Nkp, Nq * Nkp), False, pl["v"], (hd, Nk * hd), True, Nq, hd, Nk, BH, O, hd, nsplit=ctx.nsplit)
         merged = self._rows_planes(("b", i, "merged"), B * Nq, A)
-        merge = lib.sfb_attn_merge if nc else lib.sfb_attn_merge_nocls
-        L.check(merge(O.data_ptr(), pl["q"].hi_ptr(), pl["q"].lo_ptr(), B, Hn, Nq, hd, 1 if self.residual_pooling else 0,
-                      merged.hi_ptr(), merged.lo_ptr(), _st()), "sfb_attn_merge")
-        ops._count()
+        ops.attn_merge(O, pl["q"], B, Hn, Nq, hd, self.residual_pooling, merged, cls=bool(nc))
         yproj = self._lin_fwd(("b", i, "yproj"), at.proj, merged)
         # skip path
         if D != A:
@@ -725,23 +653,13 @@ class B200MViT(nn.Module):
             ks = [s + 1 if s > 1 else s for s in sq]
             xsp = ctx.buf(("b", i, "xsp"), (B, Nq, A))
             amax = ctx.buf(("b", i, "amax"), (B, Nq, A), torch.uint8)
-            td = L.TokPoolDesc()
-            td.x, td.out, td.argmax = src.data_ptr(), xsp.data_ptr(), amax.data_ptr()
-            td.b, td.c, td.t, td.h, td.w = B, A, T, Hh, W
-            td.ot, td.oh, td.ow = q_thw
-            td.kt, td.kh, td.kw = ks
-            td.st, td.sh, td.sw = sq
-            td.no_cls = 1 - nc
-            L.check(lib.sfb_token_maxpool_fwd(C.byref(td), _st()), "sfb_token_maxpool_fwd")
-            ops._count()
+            ops.token_maxpool_fwd(src, B, A, thw, q_thw, ks, sq, xsp, amax, cls=bool(nc))
             src = xsp.view(B * Nq, A)
         rq_rows = B * Nq
         x1 = ctx.buf(("b", i, "x1"), (rq_rows, A))
         s1 = dp[2 * i] if dp is not None else None
         s2 = dp[2 * i + 1] if dp is not None else None
-        L.check(lib.sfb_residual_add(src.data_ptr(), _ptr(src_bias), yproj.data_ptr(), at.proj.bias.data_ptr(), _ptr(s1),
-                                     rq_rows, A, Nq, x1.data_ptr(), _st()), "sfb_residual_add")
-        ops._count()
+        ops.residual_add(src, src_bias, yproj, at.proj.bias, s1, rq_rows, A, Nq, x1)
         # MLP
         x1n = self._rows_planes(("b", i, "x1n"), rq_rows, A)
         mean2, rstd2 = ctx.buf(("b", i, "m2"), (rq_rows,)), ctx.buf(("b", i, "r2"), (rq_rows,))
@@ -749,18 +667,14 @@ class B200MViT(nn.Module):
         yfc1 = self._lin_fwd(("b", i, "yfc1"), blk.mlp.fc1, x1n)
         hidden = blk.mlp.fc1.out_features
         hpl = self._rows_planes(("b", i, "h"), rq_rows, hidden)
-        L.check(lib.sfb_bias_gelu(yfc1.data_ptr(), blk.mlp.fc1.bias.data_ptr(), rq_rows, hidden, hpl.hi_ptr(),
-                                  hpl.lo_ptr(), _st()), "sfb_bias_gelu")
-        ops._count()
+        ops.bias_gelu(yfc1, blk.mlp.fc1.bias, rq_rows, hidden, hpl)
         yfc2 = self._lin_fwd(("b", i, "yfc2"), blk.mlp.fc2, hpl)
         x2 = ctx.buf(("x", i + 1), (B, Nq, Do))
         if A != Do:  # channel expansion in the MLP: the residual is proj(norm2(x1)) (attention.py:507-508)
             base, base_bias = self._lin_fwd(("b", i, "ybase"), blk.proj, x1n), blk.proj.bias
         else:
             base, base_bias = x1, None
-        L.check(lib.sfb_residual_add(base.data_ptr(), _ptr(base_bias), yfc2.data_ptr(), blk.mlp.fc2.bias.data_ptr(),
-                                     _ptr(s2), rq_rows, Do, Nq, x2.data_ptr(), _st()), "sfb_residual_add")
-        ops._count()
+        ops.residual_add(base, base_bias, yfc2, blk.mlp.fc2.bias, s2, rq_rows, Do, Nq, x2)
         sv = dict(x_in=x_in, thw=list(thw), xn=xn, mean1=mean1, rstd1=rstd1, yqkv=yqkv, pooled=pooled, pl=pl,
                   stats=stats, geo=geo, P=P, tab=tab, Ltp=Ltp, merged=merged, x1=x1, x1n=x1n, mean2=mean2, rstd2=rstd2,
                   yfc1=yfc1, hpl=hpl, amax=amax, pool_skip=pool_skip, q_thw=q_thw, k_thw=k_thw, s1=s1, s2=s2)
@@ -768,7 +682,7 @@ class B200MViT(nn.Module):
 
     # ================================================================================== backward program
     def _engine_backward(self, dlogits: torch.Tensor):
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         params = [p for p in self.parameters()]
         ctx.begin_backward(params)
         sv = self._saved
@@ -784,16 +698,11 @@ class B200MViT(nn.Module):
         pe = self.patch_embed.proj
         E = pe.out_channels
         if self.use_abs_pos and not self.sep_pos_embed:
-            L.check(lib.sfb_pos_embed_joint_bwd(dx.data_ptr(), B, Lt + self.ncls, E,
-                                                ctx.grad_of(self.pos_embed).data_ptr(), _st()), "sfb_pos_embed_joint_bwd")
-            ops._count()
+            ops.pos_embed_joint_bwd(dx, B, Lt + self.ncls, E, ctx.grad_of(self.pos_embed))
         elif self.use_abs_pos:
-            part = ctx.scratch("pos.part", T * lib.sfb_segment_slabs(T, H * W) * E, F32)
-            L.check(lib.sfb_pos_embed_sep_bwd(dx.data_ptr(), B, T, H * W, E, ctx.grad_of(self.pos_embed_spatial).data_ptr(),
-                                              ctx.grad_of(self.pos_embed_temporal).data_ptr(),
-                                              ctx.grad_of(self.pos_embed_class).data_ptr(), part.data_ptr(), _st()),
-                    "sfb_pos_embed_sep_bwd")
-            ops._count(3)
+            part = ctx.scratch("pos.part", T * ops.segment_slabs(T, H * W) * E, F32)
+            ops.pos_embed_sep_bwd(dx, B, T, H * W, E, ctx.grad_of(self.pos_embed_spatial),
+                                  ctx.grad_of(self.pos_embed_temporal), ctx.grad_of(self.pos_embed_class), part)
         dyp, dyf = self._tokens_split_grad(dx, B, Lt, E)
         self._colsum(dyf, B * Lt, E, ctx.grad_of(pe.bias))
         if self.ncls:
@@ -814,7 +723,7 @@ class B200MViT(nn.Module):
 
     def _block_backward(self, i, blk: BlockModule, spec, sv, dx2: torch.Tensor, B, which: str) -> torch.Tensor:
         """dx2: gradient w.r.t. the block output [B, Nq, A] (clobbered).  Returns the gradient w.r.t. the block input."""
-        ctx, lib = self.ctx, L.load()
+        ctx = self.ctx
         D, Do, Hn = spec["dim"], spec["dim_out"], spec["heads"]
         A = Do if self.dim_mul_in_att else D
         hd = A // Hn
@@ -834,16 +743,12 @@ class B200MViT(nn.Module):
         # ---------------- MLP branch: x2 = base + s2 * (fc2(gelu(fc1(LN2(x1)) + b1)) + b2),  base = x1 | proj(LN2(x1))
         g2 = self._rows_planes("g.small", rq_rows, Do, scratch=True)
         g2f = ctx.scratch("g.small.f", rq_rows * Do, F32)
-        L.check(lib.sfb_scale_split(dx2.data_ptr(), _ptr(sv["s2"]), rq_rows, Do, Nq, g2.hi_ptr(), g2.lo_ptr(),
-                                    g2f.data_ptr(), _st()), "sfb_scale_split")
-        ops._count()
+        ops.scale_split(dx2, sv["s2"], rq_rows, Do, Nq, g2, g2f)
         dH = ctx.scratch("g.hidden.f", rq_rows * hidden, F32).view(rq_rows, hidden)
         self._lin_bwd(blk.mlp.fc2, g2, g2f, sv["hpl"], dH)
         g1 = self._rows_planes("g.hidden", rq_rows, hidden, scratch=True)
         g1f = ctx.scratch("g.hidden.f2", rq_rows * hidden, F32)
-        L.check(lib.sfb_bias_gelu_bwd(dH.data_ptr(), sv["yfc1"].data_ptr(), blk.mlp.fc1.bias.data_ptr(), rq_rows, hidden,
-                                      g1.hi_ptr(), g1.lo_ptr(), g1f.data_ptr(), _st()), "sfb_bias_gelu_bwd")
-        ops._count()
+        ops.bias_gelu_bwd(dH, sv["yfc1"], blk.mlp.fc1.bias, rq_rows, hidden, g1, g1f)
         dx1n = ctx.scratch("g.small.f2", rq_rows * A, F32).view(rq_rows, A)
         self._lin_bwd(blk.mlp.fc1, g1, g1f, sv["x1n"], dx1n)
         if A != Do:
@@ -863,43 +768,30 @@ class B200MViT(nn.Module):
         # ---------------- attention branch: x1 = skip + s1 * (proj(merged) + bproj)
         gp = self._rows_planes("g.small", rq_rows, A, scratch=True)
         gpf = ctx.scratch("g.small.f", rq_rows * A, F32)
-        L.check(lib.sfb_scale_split(dx1.data_ptr(), _ptr(sv["s1"]), rq_rows, A, Nq, gp.hi_ptr(), gp.lo_ptr(),
-                                    gpf.data_ptr(), _st()), "sfb_scale_split")
-        ops._count()
+        ops.scale_split(dx1, sv["s1"], rq_rows, A, Nq, gp, gpf)
         dmerged = ctx.scratch("g.small.f2", rq_rows * A, F32).view(rq_rows, A)
         self._lin_bwd(at.proj, gp, gpf, sv["merged"], dmerged)
         dO = self._rows_planes("attn.dO", BH * Nq, hd, scratch=True)
         dq = ctx.scratch("attn.dq", BH * Nq * hd, F32).view(BH, Nq, hd)
-        split_grad = lib.sfb_attn_split_grad if nc else lib.sfb_attn_split_grad_nocls
-        L.check(split_grad(dmerged.data_ptr(), B, Hn, Nq, hd, 1 if self.residual_pooling else 0, dO.hi_ptr(), dO.lo_ptr(),
-                           dq.data_ptr(), _st()), "sfb_attn_split_grad")
-        ops._count()
+        ops.attn_split_grad(dmerged, B, Hn, Nq, hd, self.residual_pooling, dO, dq, cls=bool(nc))
         pl, P = sv["pl"], sv["P"]
         dv = ctx.scratch("attn.dv", BH * Nk * hd, F32).view(BH, Nk, hd)
-        self._bgemm(P, (Nkp, Nq * Nkp), True, dO, (hd, Nq * hd), True, Nk, hd, Nq, BH, dv, hd)
+        ops.gemm_batched(P, (Nkp, Nq * Nkp), True, dO, (hd, Nq * hd), True, Nk, hd, Nq, BH, dv, hd, nsplit=ctx.nsplit)
         dS = self._rows_planes("attn.dS", BH * Nq, Nkp, scratch=True)
         Ltp = sv["Ltp"]
         drq = ctx.scratch("attn.RQ", BH * Lq * Ltp, F32).view(BH * Lq, Ltp) if Ltp else None
         dP = ctx.scratch("attn.S", BH * Nq * Nkp, F32).view(BH, Nq, Nkp)
-        self._bgemm(dO, (hd, Nq * hd), False, pl["v"], (hd, Nk * hd), False, Nq, Nk, hd, BH, dP, Nkp)
-        sd = L.SoftmaxDesc()
-        sd.p_hi, sd.p_lo, sd.p_pitch = P.hi_ptr(), P.lo_ptr(), Nkp
-        sd.bh, sd.nq, sd.nk = BH, Nq, Nk
-        sd.qt, sd.qh, sd.qw = q_thw
-        sd.kt, sd.kh, sd.kw = k_thw
-        sd.dp, sd.dp_pitch = dP.data_ptr(), Nkp
-        sd.ds_hi, sd.ds_lo, sd.ds_pitch = dS.hi_ptr(), dS.lo_ptr(), Nkp
-        sd.drq, sd.rq_pitch = _ptr(drq), Ltp
+        ops.gemm_batched(dO, (hd, Nq * hd), False, pl["v"], (hd, Nk * hd), False, Nq, Nk, hd, BH, dP, Nkp,
+                         nsplit=ctx.nsplit)
         tabs = self._rel_tables(at)
-        sd.no_cls, sd.spatial_only = 1 - nc, int(len(tabs) == 2)
-        L.check(lib.sfb_softmax_relpos_bwd(C.byref(sd), _st()), "sfb_softmax_relpos_bwd")
-        ops._count()
+        ops.softmax_relpos_bwd(P, dP, dS, BH, Nq, Nk, q_thw, k_thw, drq=drq, cls=bool(nc), spatial_only=len(tabs) == 2)
         scale = hd ** -0.5
         # dq += scale * dS k ;  dk = scale * dS^T q
-        self._bgemm(dS, (Nkp, Nq * Nkp), False, pl["k"], (hd, Nk * hd), True, Nq, hd, Nk, BH, dq, hd, alpha=scale,
-                    accumulate=True)
+        ops.gemm_batched(dS, (Nkp, Nq * Nkp), False, pl["k"], (hd, Nk * hd), True, Nq, hd, Nk, BH, dq, hd, alpha=scale,
+                         accumulate=True, nsplit=ctx.nsplit)
         dk = ctx.scratch("attn.dk", BH * Nk * hd, F32).view(BH, Nk, hd)
-        self._bgemm(dS, (Nkp, Nq * Nkp), True, pl["q"], (hd, Nq * hd), True, Nk, hd, Nq, BH, dk, hd, alpha=scale)
+        ops.gemm_batched(dS, (Nkp, Nq * Nkp), True, pl["q"], (hd, Nq * hd), True, Nk, hd, Nq, BH, dk, hd, alpha=scale,
+                         nsplit=ctx.nsplit)
         if Ltp:
             tab = sv["tab"]
             drq_p = self._rows_planes("attn.dRQp", BH * Lq, Ltp, scratch=True)
@@ -941,28 +833,13 @@ class B200MViT(nn.Module):
                              r_, dpool, hd, False)
             else:
                 dpool = grad.view(prow, hd)
-            d = L.DwPoolDesc()
-            d.src, d.src_pitch, d.src_c0 = sv["yqkv"].data_ptr(), 3 * A, j * A
-            d.bias = _ptr(at.qkv.bias)
-            d.b, d.heads, d.hd, d.t, d.h, d.w_ = B, Hn, hd, T, Hh, W
-            d.ot, d.oh, d.ow = othw
-            d.has_pool = 1 if has else 0
-            d.no_cls = 1 - nc
-            d.dout, d.dsrc = dpool.data_ptr(), dyqkv.data_ptr()
-            dw = None
+            w = dw = wp = None
             if has:
-                pool = getattr(at, f"pool_{name}")
-                d.w = pool.weight.data_ptr()
-                d.kt, d.kh, d.kw = kern
-                d.st, d.sh, d.sw = strd
-                nb = lib.sfb_dwpool_wgrad_blocks(C.byref(d))
-                wp = ctx.scratch("attn.wpart", nb * hd * math.prod(kern), F32)
-                d.wpartials = wp.data_ptr()
-                dw = ctx.grad_of(pool.weight)
-            else:
-                d.kt = d.kh = d.kw = d.st = d.sh = d.sw = 1
-            L.check(lib.sfb_dwpool_bwd(C.byref(d), _ptr(dw), 0, _st()), "sfb_dwpool_bwd")
-            ops._count(3 if has else 1)
+                w = getattr(at, f"pool_{name}").weight
+                dw = ctx.grad_of(w)
+                wp = ctx.scratch("attn.wpart", ops.dwpool_wgrad_blocks(B, Hn, othw) * hd * math.prod(kern), F32)
+            ops.dwpool_bwd(sv["yqkv"], j * A, at.qkv.bias, w, B, Hn, hd, sv["thw"], othw, kern, strd, dpool, dyqkv, dw=dw,
+                           wpartials=wp, cls=bool(nc))
         if at.qkv.bias is not None:
             self._colsum(dyqkv, rows, 3 * A, ctx.grad_of(at.qkv.bias))
         gq = self._rows_planes("g.qkv", rows, 3 * A, scratch=True)
@@ -975,16 +852,7 @@ class B200MViT(nn.Module):
             sq = spec["sq"]
             ks = [s + 1 if s > 1 else s for s in sq]
             dsrc = ctx.scratch("g.skip.f", rows * A, F32).view(rows, A)
-            td = L.TokPoolDesc()
-            td.argmax = sv["amax"].data_ptr()
-            td.b, td.c, td.t, td.h, td.w = B, A, T, Hh, W
-            td.ot, td.oh, td.ow = q_thw
-            td.kt, td.kh, td.kw = ks
-            td.st, td.sh, td.sw = sq
-            td.dout, td.dx, td.dx_accumulate = dx1.data_ptr(), dsrc.data_ptr(), 0
-            td.no_cls = 1 - nc
-            L.check(lib.sfb_token_maxpool_bwd(C.byref(td), _st()), "sfb_token_maxpool_bwd")
-            ops._count()
+            ops.token_maxpool_bwd(dx1, sv["amax"], B, A, sv["thw"], q_thw, ks, sq, dsrc, cls=bool(nc))
         dx_in = ctx.scratch("dx." + which, rows * D, F32).view(B, N, D)
         if D != A:
             self._colsum(dsrc, rows, A, ctx.grad_of(blk.proj.bias))

@@ -244,7 +244,7 @@ class NonlocalModule(Namespace):
                              alpha=d ** -0.5, nsplit=nsplit)
             ps = ctx.storage((nm, "P"), 1, 1, 1, ng * nq, nkp)
             aux = Planes(ps.hi, ps.lo, 1, 1, 1, ng * nq, nkp, 0)
-            ops.row_softmax_planes(s, nkp, aux, ng, nq, nk)
+            ops.softmax_relpos_fwd(s, aux, ng, nq, nk)
             # O = P g   (g MN-major: memory [n*G][Nk][d])
             ops.gemm_batched(aux, (nkp, nq * nkp), False, gg.planes, (d, nk * d), True, nq, d, nk, ng, o, d, nsplit=nsplit)
         else:
@@ -283,7 +283,7 @@ class NonlocalModule(Namespace):
             dp = ctx.scratch("nl.S", ng * nq * nkp, F32).view(ng * nq, nkp)
             ops.gemm_batched(do, (d, nq * d), False, gg.planes, (d, nk * d), False, nq, nk, d, ng, dp, nkp, nsplit=nsplit)
             ds = ctx.scratch_planes("nl.dS", 1, 1, 1, ng * nq, nkp)
-            ops.row_softmax_planes_bwd(aux, dp, nkp, ds, ng, nq, nk)
+            ops.softmax_relpos_bwd(aux, dp, ds, ng, nq, nk)
             a = d ** -0.5
             # d theta = a dS phi;  d phi = a dS^T theta;  dg = P^T dO
             ops.gemm_batched(ds, (nkp, nq * nkp), False, ph.planes, (d, nk * d), True, nq, d, nk, ng, dth, d, alpha=a,

@@ -1,12 +1,15 @@
 """Torch-tensor front end of the C ABI (``include/slowfast_b200.h``).
 
 PyTorch is used for device memory, streams and dtype bookkeeping only; every function here enqueues one or more
-of the library's own kernels on the current CUDA stream.  There is no CPU path: without the native library or a
+of the library's own kernels on the current CUDA stream.  The model programs (``nets/``) launch the library only through
+these functions, which fill the descriptors, check the return code and count the launches; the optimizer and the uint8
+input pipeline keep their own single calls.  There is no CPU path: without the native library or a
 CUDA device the calls raise ``NativeLibraryError``.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 from typing import Optional, Sequence, Tuple
 
@@ -679,32 +682,6 @@ def gemm_batched(a: Planes, a_shape, a_mn: bool, b: Planes, b_shape, b_mn: bool,
     _count()
 
 
-def row_softmax_planes(s: torch.Tensor, s_pitch: int, p: Planes, batch: int, nq: int, nk: int) -> None:
-    """P = softmax over the nk keys of every row of S [batch * nq, s_pitch] -> planes (pad columns zero): the
-    softmax_relpos kernel without a bias."""
-    lib = L.load()
-    d = L.SoftmaxDesc()
-    d.s, d.s_pitch = s.data_ptr(), s_pitch
-    d.p_hi, d.p_lo, d.p_pitch = p.hi_ptr(), p.lo_ptr(), p.pitch
-    d.bh, d.nq, d.nk = batch, nq, nk
-    d.qt = d.qh = d.qw = d.kt = d.kh = d.kw = 1
-    L.check(lib.sfb_softmax_relpos_fwd(C.byref(d), _stream()), "sfb_softmax_relpos_fwd")
-    _count()
-
-
-def row_softmax_planes_bwd(p: Planes, dp: torch.Tensor, dp_pitch: int, ds: Planes, batch: int, nq: int, nk: int) -> None:
-    """dS = P * (dP - sum_k P dP) -> planes (pad columns zero)."""
-    lib = L.load()
-    d = L.SoftmaxDesc()
-    d.p_hi, d.p_lo, d.p_pitch = p.hi_ptr(), p.lo_ptr(), p.pitch
-    d.dp, d.dp_pitch = dp.data_ptr(), dp_pitch
-    d.ds_hi, d.ds_lo, d.ds_pitch = ds.hi_ptr(), ds.lo_ptr(), ds.pitch
-    d.bh, d.nq, d.nk = batch, nq, nk
-    d.qt = d.qh = d.qw = d.kt = d.kh = d.kw = 1
-    L.check(lib.sfb_softmax_relpos_bwd(C.byref(d), _stream()), "sfb_softmax_relpos_bwd")
-    _count()
-
-
 def bias_split(x: F32View, bias: Optional[torch.Tensor], out: Planes) -> None:
     """planes[rows, out.c] = x[rows, x.c] (+ bias), columns past x.c zero (csrc/nonlocal.cu)."""
     lib = L.load()
@@ -942,3 +919,428 @@ def stem_wgrad_direct(x: torch.Tensor, dy: Planes, k, stride, pad, dw: torch.Ten
                                       _stream()), "sfb_stem_wgrad_direct")
     _count(2)
 
+
+
+# ------------------------------------------------------------------------------------------------ token path (MViT / ViT)
+def layernorm_fwd(x: torch.Tensor, x_pitch: int, rows: int, c: int, weight, bias, eps: float, mean, rstd,
+                  out: Optional[Planes] = None, out_f32: Optional[torch.Tensor] = None) -> None:
+    """LayerNorm of the c channels of every row of x (row pitch ``x_pitch``) -> planes ``out`` and / or the dense fp32
+    [rows, c] ``out_f32``; mean / rstd [rows] are kept for the backward."""
+    assert out is None or (out.rows == rows and out.c == c and out.pitch == c)
+    L.check(L.load().sfb_layernorm_fwd(x.data_ptr(), x_pitch, rows, c, weight.data_ptr(), bias.data_ptr(), eps,
+                                       None if out is None else out.hi_ptr(), None if out is None else out.lo_ptr(),
+                                       _ptr(out_f32), c, mean.data_ptr(), rstd.data_ptr(), _stream()), "sfb_layernorm_fwd")
+    _count()
+
+
+def layernorm_bwd(dy: torch.Tensor, dy_pitch: int, x: torch.Tensor, x_pitch: int, rows: int, c: int, weight, mean, rstd,
+                  dx: torch.Tensor, dx_pitch: int, dweight, dbias, partials: torch.Tensor, dx_accumulate: bool = False,
+                  param_accumulate: bool = False) -> None:
+    """dx (+)= LayerNorm backward of dy; dweight / dbias (+)= the parameter gradients.  ``partials``: fp32 scratch of at
+    least colsum_blocks(rows) * 2 * c elements."""
+    assert partials.numel() >= colsum_blocks(rows) * 2 * c
+    L.check(L.load().sfb_layernorm_bwd(dy.data_ptr(), dy_pitch, x.data_ptr(), x_pitch, rows, c, weight.data_ptr(),
+                                       mean.data_ptr(), rstd.data_ptr(), dx.data_ptr(), dx_pitch, int(dx_accumulate),
+                                       dweight.data_ptr(), dbias.data_ptr(), int(param_accumulate), partials.data_ptr(),
+                                       _stream()), "sfb_layernorm_bwd")
+    _count(2)
+
+
+def tokens_assemble(y: torch.Tensor, bias, cls, pos_spatial, pos_temporal, pos_class, b: int, lt: int, hw: int, e: int,
+                    out: torch.Tensor) -> None:
+    """out[b, 1 + lt, e] = [cls ; y + bias] (+ the separable position tables: spatial [hw, e] in every frame, temporal
+    [lt / hw, e], class [e]; all three or none)."""
+    L.check(L.load().sfb_tokens_assemble(y.data_ptr(), bias.data_ptr(), cls.data_ptr(), _ptr(pos_spatial),
+                                         _ptr(pos_temporal), _ptr(pos_class), b, lt, hw, e, out.data_ptr(), _stream()),
+            "sfb_tokens_assemble")
+    _count()
+
+
+def tokens_assemble_joint(y: torch.Tensor, bias, cls, pos, b: int, lt: int, e: int, out: torch.Tensor) -> None:
+    """out = [cls ;] y + bias (+ pos, the joint [(cls +) lt, e] table): the cls-free layout when ``cls`` is None."""
+    L.check(L.load().sfb_tokens_assemble_joint(y.data_ptr(), bias.data_ptr(), _ptr(cls), _ptr(pos), b, lt, e,
+                                               out.data_ptr(), _stream()), "sfb_tokens_assemble_joint")
+    _count()
+
+
+def tokens_split_grad(dx: torch.Tensor, b: int, lt: int, e: int, dy: Planes, dy_f32: torch.Tensor) -> None:
+    """Gradient of the [b, 1 + lt, e] token sequence -> the patch embedding's output gradient without the cls rows
+    (planes + fp32 [b * lt, e])."""
+    assert dy.rows == b * lt and dy.c == e and dy.pitch == e
+    L.check(L.load().sfb_tokens_split_grad(dx.data_ptr(), b, lt, e, dy.hi_ptr(), dy.lo_ptr(), dy_f32.data_ptr(),
+                                           _stream()), "sfb_tokens_split_grad")
+    _count()
+
+
+def segment_slabs(segments: int, length: int) -> int:
+    """Row slabs per segment of the deterministic segment sums (token means, position gradients)."""
+    return int(L.load().sfb_segment_slabs(segments, length))
+
+
+def pos_embed_sep_bwd(dx: torch.Tensor, b: int, t: int, hw: int, e: int, dspatial, dtemporal, dclass,
+                      partials: torch.Tensor) -> None:
+    """Gradients of the separable position tables from the token gradient [b, 1 + t * hw, e].  ``partials``: fp32
+    scratch of at least t * segment_slabs(t, hw) * e elements."""
+    assert partials.numel() >= t * segment_slabs(t, hw) * e
+    L.check(L.load().sfb_pos_embed_sep_bwd(dx.data_ptr(), b, t, hw, e, dspatial.data_ptr(), dtemporal.data_ptr(),
+                                           dclass.data_ptr(), partials.data_ptr(), _stream()), "sfb_pos_embed_sep_bwd")
+    _count(3)
+
+
+def pos_embed_joint_bwd(dx: torch.Tensor, b: int, n: int, e: int, dpos) -> None:
+    """dpos[n, e] = sum over the batch of the token gradient [b, n, e]."""
+    L.check(L.load().sfb_pos_embed_joint_bwd(dx.data_ptr(), b, n, e, dpos.data_ptr(), _stream()),
+            "sfb_pos_embed_joint_bwd")
+    _count()
+
+
+def token_mean_fwd(x: torch.Tensor, b: int, n: int, c: int, out: torch.Tensor, partials: torch.Tensor,
+                   cls: bool = True) -> None:
+    """out[b, c] = mean over the tokens of x [b, n, c], the cls row (``cls``) excluded.  ``partials``: fp32 scratch of at
+    least b * segment_slabs(b, n - cls) * c elements."""
+    assert partials.numel() >= b * segment_slabs(b, n - int(cls)) * c
+    lib = L.load()
+    fn, name = (lib.sfb_token_mean_fwd, "sfb_token_mean_fwd") if cls else (lib.sfb_token_mean_all_fwd,
+                                                                           "sfb_token_mean_all_fwd")
+    L.check(fn(x.data_ptr(), b, n, c, out.data_ptr(), partials.data_ptr(), _stream()), name)
+    _count(2)
+
+
+def token_mean_bwd(dout: torch.Tensor, b: int, n: int, c: int, dx: torch.Tensor, cls: bool = True) -> None:
+    """dx[b, n, c] = dout / (n - cls) on every averaged token (zero on the cls row)."""
+    lib = L.load()
+    fn, name = (lib.sfb_token_mean_bwd, "sfb_token_mean_bwd") if cls else (lib.sfb_token_mean_all_bwd,
+                                                                           "sfb_token_mean_all_bwd")
+    L.check(fn(dout.data_ptr(), b, n, c, dx.data_ptr(), _stream()), name)
+    _count()
+
+
+def patchify(x: torch.Tensor, k: Sequence[int], out: Planes) -> None:
+    """Non-overlapping patches (stride == kernel k) of the NCTHW fp32 clip -> planes [n * patches, cin * kt * kh * kw]."""
+    n, cin, t, h, w = x.shape
+    assert x.dtype == F32 and x.is_contiguous() and out.pitch == out.c == cin * k[0] * k[1] * k[2]
+    assert out.rows == n * (t // k[0]) * (h // k[1]) * (w // k[2])
+    L.check(L.load().sfb_patchify(x.data_ptr(), n, cin, t, h, w, *k, out.hi_ptr(), out.lo_ptr(), _stream()),
+            "sfb_patchify")
+    _count()
+
+
+def patchify_gather(x: torch.Tensor, k: Sequence[int], ids_keep: Optional[torch.Tensor], keep: int, out: Planes) -> None:
+    """``patchify`` of the ``keep`` patches per clip listed in ids_keep [n, keep] (int32); a null ``ids_keep`` packs every
+    patch."""
+    n, cin, t, h, w = x.shape
+    assert x.dtype == F32 and x.is_contiguous() and out.pitch == out.c == cin * k[0] * k[1] * k[2]
+    L.check(L.load().sfb_patchify_gather(x.data_ptr(), n, cin, t, h, w, *k, _ptr(ids_keep), keep, out.hi_ptr(),
+                                         out.lo_ptr(), _stream()), "sfb_patchify_gather")
+    _count()
+
+
+def _dwpool_desc(src: torch.Tensor, src_c0: int, bias, weight, b, heads, hd, thw, othw, kernel, stride, cls):
+    """Pooling of one third (channels src_c0 ..) of the fused qkv rows src [b, cls + thw, pitch]; ``weight`` None: no
+    pooling, the third is copied (+ bias) into the head-major layout."""
+    d = L.DwPoolDesc()
+    d.src, d.src_pitch, d.src_c0 = src.data_ptr(), src.shape[-1], src_c0
+    d.bias = _ptr(bias)
+    d.b, d.heads, d.hd = b, heads, hd
+    d.t, d.h, d.w_ = thw
+    d.ot, d.oh, d.ow = othw
+    d.has_pool = 1 if weight is not None else 0
+    d.no_cls = 0 if cls else 1
+    if weight is not None:
+        d.w = weight.data_ptr()
+        d.kt, d.kh, d.kw = kernel
+        d.st, d.sh, d.sw = stride
+    else:
+        d.kt = d.kh = d.kw = d.st = d.sh = d.sw = 1
+    return d
+
+
+def dwpool_fwd(src: torch.Tensor, src_c0: int, bias, weight, b: int, heads: int, hd: int, thw, othw, kernel, stride,
+               out: torch.Tensor, cls: bool = True) -> None:
+    """out[b, heads, cls + othw, hd] = depthwise Conv3d (``weight`` [hd, 1, *kernel], padding kernel // 2, shared by the
+    heads) of one third of the fused qkv rows (+ its bias); the cls row passes through."""
+    d = _dwpool_desc(src, src_c0, bias, weight, b, heads, hd, thw, othw, kernel, stride, cls)
+    d.out = out.data_ptr()
+    L.check(L.load().sfb_dwpool_fwd(C.byref(d), _stream()), "sfb_dwpool_fwd")
+    _count()
+
+
+def dwpool_wgrad_blocks(b: int, heads: int, othw) -> int:
+    """Blocks of ``dwpool_bwd``'s weight-gradient partial sums (its ``wpartials`` holds blocks * hd * taps floats)."""
+    d = L.DwPoolDesc()
+    d.b, d.heads = b, heads
+    d.ot, d.oh, d.ow = othw
+    return int(L.load().sfb_dwpool_wgrad_blocks(C.byref(d)))
+
+
+def dwpool_bwd(src: torch.Tensor, src_c0: int, bias, weight, b: int, heads: int, hd: int, thw, othw, kernel, stride,
+               dout: torch.Tensor, dsrc: torch.Tensor, dw: Optional[torch.Tensor] = None,
+               wpartials: Optional[torch.Tensor] = None, cls: bool = True) -> None:
+    """dsrc (same layout as src, only this third is touched) += the data gradient of ``dwpool_fwd``; dw = its weight
+    gradient (pooled thirds, with the ``wpartials`` scratch)."""
+    d = _dwpool_desc(src, src_c0, bias, weight, b, heads, hd, thw, othw, kernel, stride, cls)
+    d.dout, d.dsrc = dout.data_ptr(), dsrc.data_ptr()
+    assert (dw is None) == (weight is None)
+    if weight is not None:
+        assert wpartials.numel() >= dwpool_wgrad_blocks(b, heads, othw) * hd * math.prod(kernel)
+        d.wpartials = wpartials.data_ptr()
+    L.check(L.load().sfb_dwpool_bwd(C.byref(d), _ptr(dw), 0, _stream()), "sfb_dwpool_bwd")
+    _count(3 if weight is not None else 1)
+
+
+def softmax_relpos_fwd(s: torch.Tensor, p: Planes, bh: int, nq: int, nk: int, q_thw=(1, 1, 1), k_thw=(1, 1, 1),
+                       rq: Optional[torch.Tensor] = None, cls: bool = True, spatial_only: bool = False) -> None:
+    """P = softmax over the nk keys of every row of S [bh * nq, pitch] -> planes (pad columns zero), with the decomposed
+    relative-position bias gathered from RQ [bh * (nq - cls), pitch] for the query / key grids q_thw / k_thw (Rt
+    columns absent when ``spatial_only``; the cls row and column get no bias).  Without ``rq``: a plain row softmax."""
+    d = L.SoftmaxDesc()
+    d.s, d.s_pitch = s.data_ptr(), s.shape[-1]
+    if rq is not None:
+        d.rq, d.rq_pitch = rq.data_ptr(), rq.shape[-1]
+    d.p_hi, d.p_lo, d.p_pitch = p.hi_ptr(), p.lo_ptr(), p.pitch
+    d.bh, d.nq, d.nk = bh, nq, nk
+    d.qt, d.qh, d.qw = q_thw
+    d.kt, d.kh, d.kw = k_thw
+    d.no_cls, d.spatial_only = 0 if cls else 1, int(spatial_only)
+    L.check(L.load().sfb_softmax_relpos_fwd(C.byref(d), _stream()), "sfb_softmax_relpos_fwd")
+    _count()
+
+
+def softmax_relpos_bwd(p: Planes, dp: torch.Tensor, ds: Planes, bh: int, nq: int, nk: int, q_thw=(1, 1, 1),
+                       k_thw=(1, 1, 1), drq: Optional[torch.Tensor] = None, cls: bool = True,
+                       spatial_only: bool = False) -> None:
+    """dS = P * (dP - sum_k P dP) -> planes (pad columns zero); ``drq`` receives dS scattered onto the table columns."""
+    d = L.SoftmaxDesc()
+    d.p_hi, d.p_lo, d.p_pitch = p.hi_ptr(), p.lo_ptr(), p.pitch
+    d.dp, d.dp_pitch = dp.data_ptr(), dp.shape[-1]
+    d.ds_hi, d.ds_lo, d.ds_pitch = ds.hi_ptr(), ds.lo_ptr(), ds.pitch
+    if drq is not None:
+        d.drq, d.rq_pitch = drq.data_ptr(), drq.shape[-1]
+    d.bh, d.nq, d.nk = bh, nq, nk
+    d.qt, d.qh, d.qw = q_thw
+    d.kt, d.kh, d.kw = k_thw
+    d.no_cls, d.spatial_only = 0 if cls else 1, int(spatial_only)
+    L.check(L.load().sfb_softmax_relpos_bwd(C.byref(d), _stream()), "sfb_softmax_relpos_bwd")
+    _count()
+
+
+def attn_merge(o: torch.Tensor, q: Planes, b: int, heads: int, nq: int, hd: int, residual: bool, out: Planes,
+               cls: bool = True) -> None:
+    """Head-major attention output O [b * heads, nq, hd] (+ the pooled q: residual pooling) -> token rows [b * nq,
+    heads * hd] (planes)."""
+    lib = L.load()
+    fn, name = (lib.sfb_attn_merge, "sfb_attn_merge") if cls else (lib.sfb_attn_merge_nocls, "sfb_attn_merge_nocls")
+    L.check(fn(o.data_ptr(), q.hi_ptr(), q.lo_ptr(), b, heads, nq, hd, int(residual), out.hi_ptr(), out.lo_ptr(),
+               _stream()), name)
+    _count()
+
+
+def attn_split_grad(dmerged: torch.Tensor, b: int, heads: int, nq: int, hd: int, residual: bool, do: Planes,
+                    dq: torch.Tensor, cls: bool = True) -> None:
+    """The backward of ``attn_merge``: dO planes and (residual pooling) dq [b * heads, nq, hd]."""
+    lib = L.load()
+    fn, name = ((lib.sfb_attn_split_grad, "sfb_attn_split_grad") if cls
+                else (lib.sfb_attn_split_grad_nocls, "sfb_attn_split_grad_nocls"))
+    L.check(fn(dmerged.data_ptr(), b, heads, nq, hd, int(residual), do.hi_ptr(), do.lo_ptr(), dq.data_ptr(), _stream()),
+            name)
+    _count()
+
+
+def _tokpool_desc(b, c, thw, othw, kernel, stride, cls):
+    d = L.TokPoolDesc()
+    d.b, d.c = b, c
+    d.t, d.h, d.w = thw
+    d.ot, d.oh, d.ow = othw
+    d.kt, d.kh, d.kw = kernel
+    d.st, d.sh, d.sw = stride
+    d.no_cls = 0 if cls else 1
+    return d
+
+
+def token_maxpool_fwd(x: torch.Tensor, b: int, c: int, thw, othw, kernel, stride, out: torch.Tensor,
+                      argmax: torch.Tensor, cls: bool = True) -> None:
+    """MaxPool3d(kernel, stride, padding kernel // 2) over the token grid of x [b, cls + thw, c]; the cls row passes
+    through; argmax (uint8 tap) is kept for the backward."""
+    d = _tokpool_desc(b, c, thw, othw, kernel, stride, cls)
+    d.x, d.out, d.argmax = x.data_ptr(), out.data_ptr(), argmax.data_ptr()
+    L.check(L.load().sfb_token_maxpool_fwd(C.byref(d), _stream()), "sfb_token_maxpool_fwd")
+    _count()
+
+
+def token_maxpool_bwd(dout: torch.Tensor, argmax: torch.Tensor, b: int, c: int, thw, othw, kernel, stride,
+                      dx: torch.Tensor, cls: bool = True) -> None:
+    d = _tokpool_desc(b, c, thw, othw, kernel, stride, cls)
+    d.argmax = argmax.data_ptr()
+    d.dout, d.dx, d.dx_accumulate = dout.data_ptr(), dx.data_ptr(), 0
+    L.check(L.load().sfb_token_maxpool_bwd(C.byref(d), _stream()), "sfb_token_maxpool_bwd")
+    _count()
+
+
+def residual_add(src: torch.Tensor, src_bias, y: torch.Tensor, y_bias, scale, rows: int, c: int, tokens: int,
+                 out: torch.Tensor) -> None:
+    """out[rows, c] = (src + src_bias) + scale[row // tokens] * (y + y_bias): a block's residual with stochastic depth
+    (``scale`` None: 1)."""
+    L.check(L.load().sfb_residual_add(src.data_ptr(), _ptr(src_bias), y.data_ptr(), y_bias.data_ptr(), _ptr(scale), rows,
+                                      c, tokens, out.data_ptr(), _stream()), "sfb_residual_add")
+    _count()
+
+
+def bias_gelu(y: torch.Tensor, bias, rows: int, c: int, out: Planes) -> None:
+    """planes[rows, c] = GELU(y + bias) (the exact erf form)."""
+    assert out.rows == rows and out.c == c and out.pitch == c
+    L.check(L.load().sfb_bias_gelu(y.data_ptr(), bias.data_ptr(), rows, c, out.hi_ptr(), out.lo_ptr(), _stream()),
+            "sfb_bias_gelu")
+    _count()
+
+
+def bias_gelu_bwd(dh: torch.Tensor, y: torch.Tensor, bias, rows: int, c: int, dpre: Planes,
+                  dpre_f32: torch.Tensor) -> None:
+    """Gradient w.r.t. y + bias of ``bias_gelu`` -> planes and fp32 [rows, c]."""
+    assert dpre.rows == rows and dpre.c == c and dpre.pitch == c
+    L.check(L.load().sfb_bias_gelu_bwd(dh.data_ptr(), y.data_ptr(), bias.data_ptr(), rows, c, dpre.hi_ptr(),
+                                       dpre.lo_ptr(), dpre_f32.data_ptr(), _stream()), "sfb_bias_gelu_bwd")
+    _count()
+
+
+def scale_split(dx: torch.Tensor, scale, rows: int, c: int, tokens: int, out: Planes, out_f32: torch.Tensor) -> None:
+    """out = scale[row // tokens] * dx -> planes and fp32 [rows, c] (``scale`` None: 1)."""
+    assert out.rows == rows and out.c == c and out.pitch == c
+    L.check(L.load().sfb_scale_split(dx.data_ptr(), _ptr(scale), rows, c, tokens, out.hi_ptr(), out.lo_ptr(),
+                                     out_f32.data_ptr(), _stream()), "sfb_scale_split")
+    _count()
+
+
+def droppath_scales(out: torch.Tensor, rates: torch.Tensor, seed: int, step: torch.Tensor) -> None:
+    """out[i, j] = per-sample stochastic-depth scale (0 or 1 / keep) of row i's rate for sample j; ``step``: the int64
+    device counter mixed into the seed and incremented after use (graph-replay safe)."""
+    n, b = out.shape
+    assert rates.numel() == n
+    L.check(L.load().sfb_droppath_scales(out.data_ptr(), rates.data_ptr(), n, b, seed, step.data_ptr(), _stream()),
+            "sfb_droppath_scales")
+    _count(2)
+
+
+# ------------------------------------------------------------------------------------------------ MAE / MaskFeat
+def mae_random_masking(noise: torch.Tensor, keep: int, ids_keep: torch.Tensor, ids_restore: torch.Tensor,
+                       mask: torch.Tensor, rows: torch.Tensor) -> None:
+    """Stable-argsort ranks of noise [b, l] -> ids_keep [b, keep] / ids_restore [b, l] (int32), mask [b, l] and the rows of
+    the removed tokens in the [b, 1 + l] decoder sequence (int32)."""
+    b, l = noise.shape
+    L.check(L.load().sfb_mae_random_masking(noise.data_ptr(), b, l, keep, ids_keep.data_ptr(), ids_restore.data_ptr(),
+                                            mask.data_ptr(), rows.data_ptr(), _stream()), "sfb_mae_random_masking")
+    _count()
+
+
+def tokens_assemble_keep(y: torch.Tensor, bias, cls, pos_spatial, pos_temporal, pos_class, ids_keep: torch.Tensor,
+                         b: int, keep: int, lt: int, hw: int, e: int, out: torch.Tensor) -> None:
+    """``tokens_assemble`` of the kept patches: the separable positions are gathered by ids_keep."""
+    L.check(L.load().sfb_tokens_assemble_keep(y.data_ptr(), bias.data_ptr(), cls.data_ptr(), pos_spatial.data_ptr(),
+                                              pos_temporal.data_ptr(), pos_class.data_ptr(), ids_keep.data_ptr(), b,
+                                              keep, lt, hw, e, out.data_ptr(), _stream()), "sfb_tokens_assemble_keep")
+    _count()
+
+
+def tokens_scatter_keep(dx: torch.Tensor, ids_restore: torch.Tensor, b: int, keep: int, lt: int, e: int,
+                        dense: torch.Tensor) -> None:
+    """The kept-token gradient [b, 1 + keep, e] scattered onto the dense grid [b, 1 + lt, e] (zero elsewhere)."""
+    L.check(L.load().sfb_tokens_scatter_keep(dx.data_ptr(), ids_restore.data_ptr(), b, keep, lt, e, dense.data_ptr(),
+                                             _stream()), "sfb_tokens_scatter_keep")
+    _count()
+
+
+def decoder_assemble(z: torch.Tensor, bias, mask_token, pos, ids_restore: torch.Tensor, b: int, keep: int, lt: int,
+                     c: int, out: torch.Tensor) -> None:
+    """out[b, 1 + lt, c] = the encoder tokens z + bias un-shuffled by ids_restore, mask_token in the removed places, + the
+    joint table pos."""
+    L.check(L.load().sfb_decoder_assemble(z.data_ptr(), bias.data_ptr(), mask_token.data_ptr(), pos.data_ptr(),
+                                          ids_restore.data_ptr(), b, keep, lt, c, out.data_ptr(), _stream()),
+            "sfb_decoder_assemble")
+    _count()
+
+
+def decoder_assemble_bwd(dx: torch.Tensor, ids_keep: torch.Tensor, rows: torch.Tensor, b: int, keep: int, lt: int,
+                         c: int, dz: torch.Tensor, dpos, dmask, partials: torch.Tensor) -> None:
+    """Gradients of ``decoder_assemble``: dz [b, 1 + keep, c], dpos [1 + lt, c], dmask [c].  ``partials``: fp32 scratch of
+    at least segment_slabs(1, b * (lt - keep)) * c elements."""
+    assert partials.numel() >= segment_slabs(1, b * (lt - keep)) * c
+    L.check(L.load().sfb_decoder_assemble_bwd(dx.data_ptr(), ids_keep.data_ptr(), rows.data_ptr(), b, keep, lt, c,
+                                              dz.data_ptr(), dpos.data_ptr(), dmask.data_ptr(), partials.data_ptr(),
+                                              _stream()), "sfb_decoder_assemble_bwd")
+    _count(4)
+
+
+def rows_gather(src: torch.Tensor, src_pitch: int, rows: Optional[torch.Tensor], n: int, c: int, bias,
+                out: torch.Tensor) -> None:
+    """out[n, c] = src[rows[i], :c] (+ bias); a null ``rows`` takes rows 0 .. n - 1."""
+    L.check(L.load().sfb_rows_gather(src.data_ptr(), src_pitch, _ptr(rows), n, c, _ptr(bias), out.data_ptr(),
+                                     _stream()), "sfb_rows_gather")
+    _count()
+
+
+def rows_scatter(src: torch.Tensor, rows: torch.Tensor, n: int, c: int, out: torch.Tensor) -> None:
+    """out[rows[i], :c] = src[i] (the other rows untouched)."""
+    L.check(L.load().sfb_rows_scatter(src.data_ptr(), rows.data_ptr(), n, c, out.data_ptr(), _stream()),
+            "sfb_rows_scatter")
+    _count()
+
+
+def pixel_targets(frames: torch.Tensor, t_stride: int, pred_t: int, patch: int, rows: torch.Tensor, norm: bool,
+                  out: torch.Tensor) -> None:
+    """The (normalised) pixel labels of the decoder rows ``rows`` of the NCTHW fp32 clip: [len(rows), pred_t * p * p * C]."""
+    b, c, t, h, w = frames.shape
+    assert frames.dtype == F32 and frames.is_contiguous()
+    L.check(L.load().sfb_pixel_targets(frames.data_ptr(), b, c, t, h, w, t_stride, pred_t, patch, rows.data_ptr(),
+                                       rows.numel(), int(norm), out.data_ptr(), _stream()), "sfb_pixel_targets")
+    _count()
+
+
+def hog_targets(frames: torch.Tensor, t_stride: int, nbins: int, cell: int, fs: int, out: torch.Tensor) -> None:
+    """HOG regression targets of every output token of the NCTHW fp32 clip: [b, (t / t_stride) * fs * fs, ...]."""
+    b, c, t, h, w = frames.shape
+    assert frames.dtype == F32 and frames.is_contiguous()
+    L.check(L.load().sfb_hog_targets(frames.data_ptr(), b, c, t, h, w, t_stride, nbins, cell, fs, out.data_ptr(),
+                                     _stream()), "sfb_hog_targets")
+    _count()
+
+
+def mask_upsample(fmask: torch.Tensor, thw, out: torch.Tensor) -> None:
+    """The cube mask [b, mt, mh, mw] at the token grid thw: out [b, t * h * w]."""
+    b, mt, mh, mw = fmask.shape
+    L.check(L.load().sfb_mask_upsample(fmask.data_ptr(), b, mt, mh, mw, *thw, out.data_ptr(), _stream()),
+            "sfb_mask_upsample")
+    _count()
+
+
+def tokens_assemble_masked(y: torch.Tensor, bias, cls, mask_token, tokmask: torch.Tensor, b: int, lt: int, e: int,
+                           out: torch.Tensor) -> None:
+    """out = [cls ; y + bias] with mask_token in place of the masked tokens (tokmask [b, lt])."""
+    L.check(L.load().sfb_tokens_assemble_masked(y.data_ptr(), bias.data_ptr(), cls.data_ptr(), mask_token.data_ptr(),
+                                                tokmask.data_ptr(), b, lt, e, out.data_ptr(), _stream()),
+            "sfb_tokens_assemble_masked")
+    _count()
+
+
+def tokens_split_grad_masked(dx: torch.Tensor, tokmask: torch.Tensor, b: int, lt: int, e: int, dy: Planes,
+                             dy_f32: torch.Tensor, dmasked: torch.Tensor) -> None:
+    """``tokens_split_grad`` of ``tokens_assemble_masked``: the masked tokens' gradient goes to dmasked [b * lt, e]."""
+    assert dy.rows == b * lt and dy.c == e and dy.pitch == e
+    L.check(L.load().sfb_tokens_split_grad_masked(dx.data_ptr(), tokmask.data_ptr(), b, lt, e, dy.hi_ptr(), dy.lo_ptr(),
+                                                  dy_f32.data_ptr(), dmasked.data_ptr(), _stream()),
+            "sfb_tokens_split_grad_masked")
+    _count()
+
+
+def rows_unpad_bias(y: torch.Tensor, y_pitch: int, bias, b: int, n: int, c: int, out: torch.Tensor) -> None:
+    """out[b, n, c] = y[b, 1 + i, :c] + bias: the prediction rows without the cls row."""
+    L.check(L.load().sfb_rows_unpad_bias(y.data_ptr(), y_pitch, bias.data_ptr(), b, n, c, out.data_ptr(), _stream()),
+            "sfb_rows_unpad_bias")
+    _count()
+
+
+def rows_pad_split(src: torch.Tensor, b: int, n: int, c: int, out: Planes) -> None:
+    """The backward of ``rows_unpad_bias``: src [b, n, c] -> planes [b * (1 + n), out.c] (cls rows and pad columns
+    zero)."""
+    assert out.rows == b * (n + 1) and out.pitch == out.c >= c
+    L.check(L.load().sfb_rows_pad_split(src.data_ptr(), b, n, c, out.c, out.hi_ptr(), out.lo_ptr(), _stream()),
+            "sfb_rows_pad_split")
+    _count()

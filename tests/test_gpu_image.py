@@ -7,7 +7,6 @@ positions, the joint position table and the norm-then-mean readout.
   * CUDA-graph replay against eager over AdamW steps (within the eager-vs-eager noise), and the unmodified train / test
     drivers on a synthetic image set.
 """
-import ctypes as C
 import math
 
 import pytest
@@ -15,15 +14,6 @@ import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
-
-
-def _lib():
-    from slowfast_b200 import lib as L
-    return L, L.load()
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _rel(a, b):
@@ -40,7 +30,7 @@ def _planes_value(hi, lo):
 def test_dwpool_without_cls_matches_fp64(name, kern, stride, out, cuda_device):
     """Depthwise pooling of MViTv2-T's first stage (56^2 tokens, one head of 96) with no cls row: forward, data gradient
     (both the gather and the scatter form) and weight gradient against fp64 conv3d."""
-    L, lib = _lib()
+    from slowfast_b200 import ops
     B, Hn, hd, side = 2, 1, 96, 56
     Ltok, A = side * side, Hn * hd
     g = torch.Generator().manual_seed(out)
@@ -51,26 +41,17 @@ def test_dwpool_without_cls_matches_fp64(name, kern, stride, out, cuda_device):
     s_d, b_d, w_d, do_d = (v.to(cuda_device) for v in (src, bias, w, dout))
     o = torch.full((B, Hn, out * out, hd), float("nan"), device=cuda_device)
     dsrc = torch.zeros(B, Ltok, 3 * A, device=cuda_device)
-    d = L.DwPoolDesc()
-    d.src, d.src_pitch, d.src_c0, d.bias = s_d.data_ptr(), 3 * A, A, b_d.data_ptr()
-    d.w, d.out = w_d.data_ptr(), o.data_ptr()
-    d.b, d.heads, d.hd, d.t, d.h, d.w_ = B, Hn, hd, 1, side, side
-    d.ot, d.oh, d.ow = 1, out, out
-    d.kt, d.kh, d.kw = kern
-    d.st, d.sh, d.sw = stride
-    d.has_pool, d.no_cls = 1, 1
-    L.check(lib.sfb_dwpool_fwd(C.byref(d), _st()), "dwpool fwd")
+    geom = (B, Hn, hd, (1, side, side), (1, out, out), kern, stride)
+    ops.dwpool_fwd(s_d, A, b_d, w_d, *geom, o, cls=False)
     x = (src[:, :, A:2 * A] + bias[A:2 * A]).double().view(B, side, side, Hn, hd).permute(0, 3, 4, 1, 2)
     x = x.reshape(B * Hn, hd, 1, side, side).requires_grad_(True)
     w64 = w.double().requires_grad_(True)
     y = F.conv3d(x, w64, stride=stride, padding=[k // 2 for k in kern], groups=hd)
     want = y.reshape(B, Hn, hd, out * out).permute(0, 1, 3, 2)
     assert _rel(o.cpu().double(), want) < 1e-6
-    d.dout, d.dsrc = do_d.data_ptr(), dsrc.data_ptr()
     dw = torch.full_like(w_d, float("nan"))
-    wp = torch.empty(lib.sfb_dwpool_wgrad_blocks(C.byref(d)) * hd * math.prod(kern), device=cuda_device)
-    d.wpartials = wp.data_ptr()
-    L.check(lib.sfb_dwpool_bwd(C.byref(d), dw.data_ptr(), 0, _st()), "dwpool bwd")
+    wp = torch.empty(ops.dwpool_wgrad_blocks(B, Hn, (1, out, out)) * hd * math.prod(kern), device=cuda_device)
+    ops.dwpool_bwd(s_d, A, b_d, w_d, *geom, do_d, dsrc, dw=dw, wpartials=wp, cls=False)
     want.backward(dout.double())
     gx = x.grad.view(B, Hn, hd, side * side).permute(0, 3, 1, 2).reshape(B, Ltok, A)
     got = dsrc.cpu().double()
@@ -101,7 +82,7 @@ def test_softmax_spatial_relpos_matches_fp64(cls, cuda_device):
     spatial-only layout) the cls row / column carry no bias.  The fp64 formulation is checked against the reference's
     cal_rel_pos_spatial first."""
     from oracle import refshim
-    L, lib = _lib()
+    from slowfast_b200 import ops
     BH, side, kside, hd = 2, 56, 14, 96
     Lq, Lk = side * side, kside * kside
     Nq, Nk = Lq + cls, Lk + cls
@@ -131,13 +112,9 @@ def test_softmax_spatial_relpos_matches_fp64(cls, cuda_device):
     rqd = torch.zeros(BH * Lq, Ltp, device=cuda_device)
     rqd[:, :Lh + Lw] = RQ.float().view(BH * Lq, -1).to(cuda_device)
     ph, plo = (torch.empty(BH, Nq, Nkp, dtype=torch.bfloat16, device=cuda_device) for _ in range(2))
-    sd = L.SoftmaxDesc()
-    sd.s, sd.s_pitch, sd.rq, sd.rq_pitch = Sd.data_ptr(), Nkp, rqd.data_ptr(), Ltp
-    sd.p_hi, sd.p_lo, sd.p_pitch = ph.data_ptr(), plo.data_ptr(), Nkp
-    sd.bh, sd.nq, sd.nk = BH, Nq, Nk
-    sd.qt, sd.qh, sd.qw, sd.kt, sd.kh, sd.kw = 1, side, side, 1, kside, kside
-    sd.no_cls, sd.spatial_only = 1 - cls, 1
-    L.check(lib.sfb_softmax_relpos_fwd(C.byref(sd), _st()), "softmax fwd")
+    grids = dict(q_thw=(1, side, side), k_thw=(1, kside, kside), cls=bool(cls), spatial_only=True)
+    P_planes = ops.Planes(ph, plo, 1, 1, 1, BH * Nq, Nkp)
+    ops.softmax_relpos_fwd(Sd, P_planes, BH, Nq, Nk, rq=rqd, **grids)
     P = _planes_value(ph, plo).cpu()
     assert _rel(P[..., :Nk], P64.detach()) < 3e-5   # split-bf16 planes carry ~16 mantissa bits
     assert P[..., Nk:].abs().max() == 0
@@ -145,9 +122,7 @@ def test_softmax_spatial_relpos_matches_fp64(cls, cuda_device):
     dPd[..., :Nk] = dP.float().to(cuda_device)
     dsh, dsl = (torch.empty(BH, Nq, Nkp, dtype=torch.bfloat16, device=cuda_device) for _ in range(2))
     drq = torch.full((BH * Lq, Ltp), float("nan"), device=cuda_device)
-    sd.dp, sd.dp_pitch = dPd.data_ptr(), Nkp
-    sd.ds_hi, sd.ds_lo, sd.ds_pitch, sd.drq = dsh.data_ptr(), dsl.data_ptr(), Nkp, drq.data_ptr()
-    L.check(lib.sfb_softmax_relpos_bwd(C.byref(sd), _st()), "softmax bwd")
+    ops.softmax_relpos_bwd(P_planes, dPd, ops.Planes(dsh, dsl, 1, 1, 1, BH * Nq, Nkp), BH, Nq, Nk, drq=drq, **grids)
     dS = _planes_value(dsh, dsl).cpu()
     assert _rel(dS[..., :Nk], S_leaf.grad) < 5e-5
     got = drq.cpu().double()
@@ -158,14 +133,13 @@ def test_softmax_spatial_relpos_matches_fp64(cls, cuda_device):
 @pytest.mark.parametrize("cls,pos", [(True, True), (False, True), (False, False)])
 @pytest.mark.parametrize("b,l,e", [(2, 3136, 96), (3, 196, 768), (1, 5, 8)])
 def test_tokens_assemble_joint_is_bitwise_the_reference_arithmetic(b, l, e, cls, pos, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     g = torch.Generator().manual_seed(l + e)
     y, bias, c = torch.randn(b, l, e, generator=g), torch.randn(e, generator=g), torch.randn(e, generator=g)
     p = torch.randn(1, l + int(cls), e, generator=g)
     yd, bd, cd, pd = (v.to(cuda_device) for v in (y, bias, c, p))
     out = torch.full((b, l + int(cls), e), float("nan"), device=cuda_device)
-    L.check(lib.sfb_tokens_assemble_joint(yd.data_ptr(), bd.data_ptr(), cd.data_ptr() if cls else None,
-                                          pd.data_ptr() if pos else None, b, l, e, out.data_ptr(), _st()), "assemble")
+    ops.tokens_assemble_joint(yd, bd, cd if cls else None, pd if pos else None, b, l, e, out)
     want = y + bias                                                        # the patch embedding's conv + bias
     if cls:
         want = torch.cat([c.view(1, 1, e).expand(b, 1, e), want], 1)      # cat(cls_tokens, x)
@@ -176,13 +150,13 @@ def test_tokens_assemble_joint_is_bitwise_the_reference_arithmetic(b, l, e, cls,
 
 @pytest.mark.parametrize("b,n,e", [(64, 3137, 96), (64, 197, 768), (3, 7, 8)])
 def test_pos_embed_joint_bwd_matches_fp64_and_is_deterministic(b, n, e, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     dx = torch.randn(b, n, e, generator=torch.Generator().manual_seed(n))
     d = dx.to(cuda_device)
     outs = []
     for _ in range(2):
         dp = torch.full((n, e), float("nan"), device=cuda_device)
-        L.check(lib.sfb_pos_embed_joint_bwd(d.data_ptr(), b, n, e, dp.data_ptr(), _st()), "joint pos bwd")
+        ops.pos_embed_joint_bwd(d, b, n, e, dp)
         outs.append(dp.cpu())
     assert _rel(outs[0].double(), dx.double().sum(0)) < 1e-6
     assert torch.equal(outs[0], outs[1])
@@ -192,7 +166,7 @@ def test_pos_embed_joint_bwd_matches_fp64_and_is_deterministic(b, n, e, cuda_dev
 def test_norm_then_mean_readout_forward_backward(b, n, c, cuda_device):
     """The default readout without cls (video_model_builder.py:1239-1241): LayerNorm on all b*n rows, per-image mean, and
     its backward (dmean / n to every row, then LayerNorm backward) against fp64 autograd; the mean is deterministic."""
-    L, lib = _lib()
+    from slowfast_b200 import ops
     g = torch.Generator().manual_seed(n * c)
     x, dm = torch.randn(b, n, c, generator=g) * 2 + 0.3, torch.randn(b, c, generator=g)
     gamma, beta = torch.rand(c, generator=g) + 0.5, torch.randn(c, generator=g) * 0.1
@@ -200,22 +174,19 @@ def test_norm_then_mean_readout_forward_backward(b, n, c, cuda_device):
     rows = b * n
     y = torch.empty(rows, c, device=cuda_device)
     mean, rstd = torch.empty(rows, device=cuda_device), torch.empty(rows, device=cuda_device)
-    L.check(lib.sfb_layernorm_fwd(xd.data_ptr(), c, rows, c, gd.data_ptr(), bd.data_ptr(), 1e-6, None, None, y.data_ptr(),
-                                  c, mean.data_ptr(), rstd.data_ptr(), _st()), "ln fwd")
-    part = torch.empty(b * lib.sfb_segment_slabs(b, n) * c, device=cuda_device)
+    ops.layernorm_fwd(xd, c, rows, c, gd, bd, 1e-6, mean, rstd, out_f32=y)
+    part = torch.empty(b * ops.segment_slabs(b, n) * c, device=cuda_device)
     outs = []
     for _ in range(2):
         o = torch.full((b, c), float("nan"), device=cuda_device)
-        L.check(lib.sfb_token_mean_all_fwd(y.data_ptr(), b, n, c, o.data_ptr(), part.data_ptr(), _st()), "mean fwd")
+        ops.token_mean_fwd(y, b, n, c, o, part, cls=False)
         outs.append(o.cpu())
     assert torch.equal(outs[0], outs[1])
     dn = torch.full((rows, c), float("nan"), device=cuda_device)
-    L.check(lib.sfb_token_mean_all_bwd(dmd.data_ptr(), b, n, c, dn.data_ptr(), _st()), "mean bwd")
+    ops.token_mean_bwd(dmd, b, n, c, dn, cls=False)
     dx, dg, db = (torch.empty(s, device=cuda_device) for s in ((rows, c), (c,), (c,)))
-    lp = torch.empty(lib.sfb_rowslab_blocks(rows) * 2 * c, device=cuda_device)
-    L.check(lib.sfb_layernorm_bwd(dn.data_ptr(), c, xd.data_ptr(), c, rows, c, gd.data_ptr(), mean.data_ptr(),
-                                  rstd.data_ptr(), dx.data_ptr(), c, 0, dg.data_ptr(), db.data_ptr(), 0, lp.data_ptr(),
-                                  _st()), "ln bwd")
+    lp = torch.empty(ops.colsum_blocks(rows) * 2 * c, device=cuda_device)
+    ops.layernorm_bwd(dn, c, xd, c, rows, c, gd, mean, rstd, dx, c, dg, db, lp)
     xr = x.double().requires_grad_(True)
     gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
     out = F.layer_norm(xr, (c,), gr, br, 1e-6).mean(1)
@@ -227,7 +198,7 @@ def test_norm_then_mean_readout_forward_backward(b, n, c, cuda_device):
 
 def test_token_maxpool_without_cls_matches_max_pool(cuda_device):
     """The skip path of a Q-pooled block (kernel 3x3, stride 2 over 56^2 tokens) with no pass-through row."""
-    L, lib = _lib()
+    from slowfast_b200 import ops
     B, C_, side, o = 2, 96, 56, 28
     x = torch.randn(B, side * side, C_, generator=torch.Generator().manual_seed(5))
     dout = torch.randn(B, o * o, C_, generator=torch.Generator().manual_seed(6))
@@ -235,15 +206,9 @@ def test_token_maxpool_without_cls_matches_max_pool(cuda_device):
     out = torch.empty(B, o * o, C_, device=cuda_device)
     am = torch.empty(B, o * o, C_, dtype=torch.uint8, device=cuda_device)
     dx = torch.full((B, side * side, C_), float("nan"), device=cuda_device)
-    td = L.TokPoolDesc()
-    td.x, td.out, td.argmax = xd.data_ptr(), out.data_ptr(), am.data_ptr()
-    td.b, td.c, td.t, td.h, td.w = B, C_, 1, side, side
-    td.ot, td.oh, td.ow = 1, o, o
-    td.kt, td.kh, td.kw, td.st, td.sh, td.sw = 1, 3, 3, 1, 2, 2
-    td.no_cls = 1
-    L.check(lib.sfb_token_maxpool_fwd(C.byref(td), _st()), "maxpool fwd")
-    td.dout, td.dx, td.dx_accumulate = dd.data_ptr(), dx.data_ptr(), 0
-    L.check(lib.sfb_token_maxpool_bwd(C.byref(td), _st()), "maxpool bwd")
+    geom = (B, C_, (1, side, side), (1, o, o), (1, 3, 3), (1, 2, 2))
+    ops.token_maxpool_fwd(xd, *geom, out, am, cls=False)
+    ops.token_maxpool_bwd(dd, am, *geom, dx, cls=False)
     xr = x.double().view(B, side, side, C_).permute(0, 3, 1, 2).requires_grad_(True)
     y = F.max_pool2d(xr, 3, 2, 1)
     assert torch.equal(out.cpu().double(), y.detach().permute(0, 2, 3, 1).reshape(B, o * o, C_))

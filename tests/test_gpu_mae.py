@@ -44,15 +44,14 @@ def _restate_masking(noise, keep):
 
 
 def _run_masking(noise, keep):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     B, Lt = noise.shape
     dev = noise.device
     ids_keep = torch.full((B, keep), -1, dtype=torch.int32, device=dev)
     ids_restore = torch.full((B, Lt), -1, dtype=torch.int32, device=dev)
     mask = torch.full((B, Lt), float("nan"), device=dev)
     rows = torch.full((B * (Lt - keep),), -1, dtype=torch.int32, device=dev)
-    L.check(lib.sfb_mae_random_masking(noise.data_ptr(), B, Lt, keep, ids_keep.data_ptr(), ids_restore.data_ptr(),
-                                       mask.data_ptr(), rows.data_ptr(), _st()), "masking")
+    ops.mae_random_masking(noise, keep, ids_keep, ids_restore, mask, rows)
     return ids_keep, ids_restore, mask, rows
 
 
@@ -106,7 +105,6 @@ def test_patchify_gather_gemm_and_wgrad_match_conv3d(nsplit, cuda_device):
     from slowfast_b200 import ops
     from slowfast_b200.engine import Ctx
     from slowfast_b200.ops import Planes
-    L, lib = _lib()
     g = torch.Generator().manual_seed(5)
     B, cin, k = 3, 3, (2, 16, 16)
     shape = (B, cin, 4, 64, 48)
@@ -122,8 +120,7 @@ def test_patchify_gather_gemm_and_wgrad_match_conv3d(nsplit, cuda_device):
     s = ctx.storage(("rows",), 1, 1, 1, rows, K)
     xr = Planes(s.hi, s.lo, 1, 1, 1, rows, K, 0)
     xd, kd = x.to(cuda_device), keep.to(cuda_device)
-    L.check(lib.sfb_patchify_gather(xd.data_ptr(), B, cin, *shape[2:], *k, kd.data_ptr(), nkeep, xr.hi_ptr(),
-                                    xr.lo_ptr(), _st()), "patchify_gather")
+    ops.patchify_gather(xd, k, kd, nkeep, xr)
     fm = ops.alloc_filter(E, 1, K, nsplit, cuda_device)
     ops.filter_pack(w.to(cuda_device).view(E, K), fm)
     y = torch.empty(rows, E, device=cuda_device)
@@ -145,10 +142,8 @@ def test_patchify_gather_gemm_and_wgrad_match_conv3d(nsplit, cuda_device):
     # a null table is sfb_patchify, bitwise
     s2 = ctx.storage(("rows2",), 1, 1, 1, B * Lt, K)
     s3 = ctx.storage(("rows3",), 1, 1, 1, B * Lt, K)
-    L.check(lib.sfb_patchify_gather(xd.data_ptr(), B, cin, *shape[2:], *k, None, 0, s2.hi.data_ptr(),
-                                    None if s2.lo is None else s2.lo.data_ptr(), _st()), "patchify_gather(null)")
-    L.check(lib.sfb_patchify(xd.data_ptr(), B, cin, *shape[2:], *k, s3.hi.data_ptr(),
-                             None if s3.lo is None else s3.lo.data_ptr(), _st()), "patchify")
+    ops.patchify_gather(xd, k, None, 0, Planes(s2.hi, s2.lo, 1, 1, 1, B * Lt, K, 0))
+    ops.patchify(xd, k, Planes(s3.hi, s3.lo, 1, 1, 1, B * Lt, K, 0))
     assert torch.equal(s2.hi, s3.hi) and (s2.lo is None or torch.equal(s2.lo, s3.lo))
 
 
@@ -159,7 +154,7 @@ def _mask_setup(b, lt, keep, dev, seed):
 
 @pytest.mark.parametrize("b,t,hw,e,keep", [(4, 8, 196, 768, 156), (3, 2, 16, 40, 3)])
 def test_encoder_assembly_forward_bitwise_and_backward(b, t, hw, e, keep, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     lt = t * hw
     ids_keep, ids_restore, _, _ = _mask_setup(b, lt, keep, cuda_device, 11)
     g = torch.Generator().manual_seed(hw)
@@ -167,8 +162,7 @@ def test_encoder_assembly_forward_bitwise_and_backward(b, t, hw, e, keep, cuda_d
     ps, pt, pc = torch.randn(hw, e, generator=g), torch.randn(t, e, generator=g), torch.randn(e, generator=g)
     d = [v.to(cuda_device) for v in (y, bias, cls, ps, pt, pc)]
     out = torch.empty(b, keep + 1, e, device=cuda_device)
-    L.check(lib.sfb_tokens_assemble_keep(*(v.data_ptr() for v in d), ids_keep.data_ptr(), b, keep, lt, hw, e,
-                                         out.data_ptr(), _st()), "assemble_keep")
+    ops.tokens_assemble_keep(*d, ids_keep, b, keep, lt, hw, e, out)
     # masked.py:340-371 in fp32: cat(cls, x_masked) + cat(pc, gather(ps.repeat(t) + pt.repeat_interleave(hw), ids_keep))
     pos = (d[3].repeat(t, 1) + d[4].repeat_interleave(hw, dim=0)).unsqueeze(0).expand(b, lt, e)
     pos = torch.gather(pos, 1, ids_keep.long().unsqueeze(-1).expand(b, keep, e))
@@ -180,8 +174,7 @@ def test_encoder_assembly_forward_bitwise_and_backward(b, t, hw, e, keep, cuda_d
     outs = []
     for _ in range(2):
         dense = torch.full((b, lt + 1, e), float("nan"), device=cuda_device)
-        L.check(lib.sfb_tokens_scatter_keep(dx.data_ptr(), ids_restore.data_ptr(), b, keep, lt, e, dense.data_ptr(),
-                                            _st()), "scatter_keep")
+        ops.tokens_scatter_keep(dx, ids_restore, b, keep, lt, e, dense)
         outs.append(dense)
     want = torch.zeros(b, lt + 1, e, device=cuda_device)
     want[:, 0] = dx[:, 0]
@@ -191,15 +184,14 @@ def test_encoder_assembly_forward_bitwise_and_backward(b, t, hw, e, keep, cuda_d
 
 @pytest.mark.parametrize("b,lt,c,keep", [(4, 1568, 512, 156), (3, 32, 40, 3)])
 def test_decoder_assembly_forward_bitwise_backward_fp64_deterministic(b, lt, c, keep, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     ids_keep, ids_restore, mask, rows = _mask_setup(b, lt, keep, cuda_device, 13)
     g = torch.Generator().manual_seed(lt)
     z, bias = torch.randn(b, keep + 1, c, generator=g), torch.randn(c, generator=g)
     mtok, pos = torch.randn(c, generator=g), torch.randn(lt + 1, c, generator=g)
     zd, bd, md, pd = (v.to(cuda_device) for v in (z, bias, mtok, pos))
     out = torch.empty(b, lt + 1, c, device=cuda_device)
-    L.check(lib.sfb_decoder_assemble(zd.data_ptr(), bd.data_ptr(), md.data_ptr(), pd.data_ptr(), ids_restore.data_ptr(),
-                                     b, keep, lt, c, out.data_ptr(), _st()), "decoder_assemble")
+    ops.decoder_assemble(zd, bd, md, pd, ids_restore, b, keep, lt, c, out)
     # masked.py:396-436 in fp32
     x = zd + bd
     x_ = torch.cat([x[:, 1:], md.view(1, 1, c).expand(b, lt - keep, c)], 1)
@@ -208,15 +200,13 @@ def test_decoder_assembly_forward_bitwise_backward_fp64_deterministic(b, lt, c, 
     assert torch.equal(out, want)
     dx = torch.randn(b, lt + 1, c, generator=g)
     dxd = dx.to(cuda_device)
-    part = torch.empty(lib.sfb_segment_slabs(1, b * (lt - keep)) * c, device=cuda_device)
+    part = torch.empty(ops.segment_slabs(1, b * (lt - keep)) * c, device=cuda_device)
     res = []
     for _ in range(2):
         dz = torch.full((b, keep + 1, c), float("nan"), device=cuda_device)
         dpos = torch.full((lt + 1, c), float("nan"), device=cuda_device)
         dm = torch.full((c,), float("nan"), device=cuda_device)
-        L.check(lib.sfb_decoder_assemble_bwd(dxd.data_ptr(), ids_keep.data_ptr(), rows.data_ptr(), b, keep, lt, c,
-                                             dz.data_ptr(), dpos.data_ptr(), dm.data_ptr(), part.data_ptr(), _st()),
-                "decoder_assemble_bwd")
+        ops.decoder_assemble_bwd(dxd, ids_keep, rows, b, keep, lt, c, dz, dpos, dm, part)
         res.append((dz.cpu(), dpos.cpu(), dm.cpu()))
     zr, mr, pr = z.double().requires_grad_(True), mtok.double().requires_grad_(True), pos.double().requires_grad_(True)
     ir = ids_restore.long().cpu()
@@ -232,7 +222,7 @@ def test_decoder_assembly_forward_bitwise_backward_fp64_deterministic(b, lt, c, 
 @pytest.mark.parametrize("norm", [True, False])
 @pytest.mark.parametrize("time_stride_loss", [True, False])
 def test_pixel_targets_match_fp64(norm, time_stride_loss, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     B, C, T, H, W, ts, p = 3, 3, 8, 64, 48, 2, 16
     x = torch.randn(B, C, T, H, W, generator=torch.Generator().manual_seed(3))
     x[1, :, 4:6, 16:32, 32:48] = 0.25      # a constant patch (zero variance) in both target layouts
@@ -244,8 +234,7 @@ def test_pixel_targets_match_fp64(norm, time_stride_loss, cuda_device):
     rows = (b * (lt + 1) + 1 + l).int()
     u = 1 if time_stride_loss else ts
     out = torch.empty(rows.numel(), u * p * p * C, device=cuda_device)
-    L.check(lib.sfb_pixel_targets(x.to(cuda_device).data_ptr(), B, C, T, H, W, ts, u, p, rows.data_ptr(), rows.numel(),
-                                  1 if norm else 0, out.data_ptr(), _st()), "pixel targets")
+    ops.pixel_targets(x.to(cuda_device), ts, u, p, rows, norm, out)
     # _get_pixel_label_3d (masked.py:212-230) in fp64
     xf = x.double()[:, :, ::ts] if time_stride_loss else x.double()
     t = xf.shape[2] // u

@@ -48,16 +48,12 @@ def test_dropout_kernel_statistics_and_mask_identity(cuda_device):
 
 
 def test_droppath_scales_kernel(cuda_device):
-    import ctypes as C
-
-    from slowfast_b200 import lib as L
-    lib = L.load()
+    from slowfast_b200 import ops
     b = 8192
     rates = torch.tensor([0.0, 0.1, 0.2, 0.5], device=cuda_device)
     out = torch.empty(4, b, device=cuda_device)
     step = torch.zeros(1, dtype=torch.int64, device=cuda_device)
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    L.check(lib.sfb_droppath_scales(out.data_ptr(), rates.data_ptr(), 4, b, 99, step.data_ptr(), st))
+    ops.droppath_scales(out, rates, 99, step)
     first = out.clone()
     assert torch.all(first[0] == 1.0)  # rate 0: exact identity
     for i, r in enumerate(rates.tolist()[1:], start=1):
@@ -67,11 +63,11 @@ def test_droppath_scales_kernel(cuda_device):
         assert torch.allclose(vals[kept], torch.full_like(vals[kept], 1.0 / keep))  # x / keep * floor(keep + U)
         frac = kept.float().mean().item()
         assert abs(frac - keep) < 5 * math.sqrt(keep * r / b), (r, frac)
-    L.check(lib.sfb_droppath_scales(out.data_ptr(), rates.data_ptr(), 4, b, 99, step.data_ptr(), st))
+    ops.droppath_scales(out, rates, 99, step)
     assert int(step.item()) == 2
     assert (out[3] != first[3]).float().mean().item() > 0.3  # a different draw per step
     step.zero_()
-    L.check(lib.sfb_droppath_scales(out.data_ptr(), rates.data_ptr(), 4, b, 99, step.data_ptr(), st))
+    ops.droppath_scales(out, rates, 99, step)
     assert torch.equal(out, first)
 
 

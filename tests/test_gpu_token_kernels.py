@@ -1,5 +1,5 @@
 """GPU: the MViT token-path kernels (csrc/mvit_ops.cu) and the MaskFeat HOG kernel (csrc/maskfeat.cu), each on its own
-through the C ABI against a PyTorch fp64 restatement of the reference operator it replaces:
+through its ``slowfast_b200.ops`` function against a PyTorch fp64 restatement of the reference operator it replaces:
 
   sfb_layernorm_fwd/bwd        nn.LayerNorm(eps=1e-6)                        attention.py:40-44, :500, :509
   sfb_dwpool_fwd/bwd           attention_pool's depthwise Conv3d on tokens   attention.py:13-45 (all four MViTv2-S
@@ -10,7 +10,6 @@ through the C ABI against a PyTorch fp64 restatement of the reference operator i
   sfb_hog_targets              HOGLayerC + per-token regrouping              operators.py:79-122, masked.py:254-281
 Whole-model tests only run these at B <= 3 with one geometry each; here shapes are ragged on purpose.
 """
-import ctypes as C
 import math
 
 import pytest
@@ -18,10 +17,6 @@ import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def relerr(a, b):
@@ -34,8 +29,8 @@ def planes_to_float(hi, lo):
 
 @pytest.mark.parametrize("rows,c", [(1000, 96), (777, 192), (130, 768), (515, 384)])
 def test_layernorm_forward_backward(rows, c, cuda_device):
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
+    from slowfast_b200 import ops
+    dev = cuda_device
     g = torch.Generator().manual_seed(rows + c)
     x = torch.randn(rows, c, generator=g).to(dev) * 2 + 0.5
     gamma = (torch.rand(c, generator=g) + 0.5).to(dev)
@@ -44,8 +39,7 @@ def test_layernorm_forward_backward(rows, c, cuda_device):
     lo = torch.empty_like(hi)
     of = torch.empty(rows, c, device=dev)
     mean, rstd = torch.empty(rows, device=dev), torch.empty(rows, device=dev)
-    L.check(lib.sfb_layernorm_fwd(x.data_ptr(), c, rows, c, gamma.data_ptr(), beta.data_ptr(), 1e-6, hi.data_ptr(),
-                                  lo.data_ptr(), of.data_ptr(), c, mean.data_ptr(), rstd.data_ptr(), _st()))
+    ops.layernorm_fwd(x, c, rows, c, gamma, beta, 1e-6, mean, rstd, out=ops.Planes(hi, lo, 1, 1, 1, rows, c), out_f32=of)
     xd = x.double().requires_grad_(True)
     gd, bd = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
     ref = F.layer_norm(xd, (c,), gd, bd, 1e-6)
@@ -53,19 +47,16 @@ def test_layernorm_forward_backward(rows, c, cuda_device):
     assert relerr(planes_to_float(hi, lo), ref) < 2e-5          # split planes carry ~16 mantissa bits
     dy = torch.randn(rows, c, generator=g).to(dev)
     ref.backward(dy.double())
-    nb = lib.sfb_rowslab_blocks(rows)
+    nb = ops.colsum_blocks(rows)
     part = torch.empty(nb * 2 * c, device=dev)
     dx = torch.full((rows, c), float("nan"), device=dev)
     dg, db = torch.empty(c, device=dev), torch.empty(c, device=dev)
-    L.check(lib.sfb_layernorm_bwd(dy.data_ptr(), c, x.data_ptr(), c, rows, c, gamma.data_ptr(), mean.data_ptr(),
-                                  rstd.data_ptr(), dx.data_ptr(), c, 0, dg.data_ptr(), db.data_ptr(), 0, part.data_ptr(),
-                                  _st()))
+    ops.layernorm_bwd(dy, c, x, c, rows, c, gamma, mean, rstd, dx, c, dg, db, part)
     assert relerr(dx, xd.grad) < 1e-5 and relerr(dg, gd.grad) < 1e-5 and relerr(db, bd.grad) < 1e-5
     base = torch.randn(rows, c, generator=g).to(dev)   # accumulate forms (dx +=, parameter gradients +=)
     acc = base.clone()
-    L.check(lib.sfb_layernorm_bwd(dy.data_ptr(), c, x.data_ptr(), c, rows, c, gamma.data_ptr(), mean.data_ptr(),
-                                  rstd.data_ptr(), acc.data_ptr(), c, 1, dg.data_ptr(), db.data_ptr(), 1, part.data_ptr(),
-                                  _st()))
+    ops.layernorm_bwd(dy, c, x, c, rows, c, gamma, mean, rstd, acc, c, dg, db, part, dx_accumulate=True,
+                      param_accumulate=True)
     assert relerr(acc - base, xd.grad) < 1e-4 and relerr(dg, 2 * gd.grad) < 1e-5
 
 
@@ -86,8 +77,8 @@ DWPOOL_CASES = [
 def test_dwpool_forward_backward(case, cuda_device):
     """attention_pool (attention.py:13-45): tokens [B, 1+THW, 3A] (fused qkv output, + qkv bias) -> per head NCTHW ->
     depthwise Conv3d(kernel, stride, pad k//2, weight shared by the heads) -> tokens, cls passes through."""
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
+    from slowfast_b200 import ops
+    dev = cuda_device
     B, Hn, hd, T, Hh, W, kern, strd = case
     A = Hn * hd
     Lin = T * Hh * W
@@ -103,19 +94,7 @@ def test_dwpool_forward_backward(case, cuda_device):
         w, othw = None, [T, Hh, W]
     Lo = math.prod(othw)
     out = torch.full((B, Hn, Lo + 1, hd), float("nan"), device=dev)
-    d = L.DwPoolDesc()
-    d.src, d.src_pitch, d.src_c0, d.bias = src.data_ptr(), 3 * A, j * A, bias.data_ptr()
-    d.out = out.data_ptr()
-    d.b, d.heads, d.hd, d.t, d.h, d.w_ = B, Hn, hd, T, Hh, W
-    d.ot, d.oh, d.ow = othw
-    d.has_pool = 1 if has else 0
-    if has:
-        d.w = w.data_ptr()
-        d.kt, d.kh, d.kw = kern
-        d.st, d.sh, d.sw = strd
-    else:
-        d.kt = d.kh = d.kw = d.st = d.sh = d.sw = 1
-    L.check(lib.sfb_dwpool_fwd(C.byref(d), _st()))
+    ops.dwpool_fwd(src, j * A, bias, w, B, Hn, hd, (T, Hh, W), othw, kern, strd, out)
     # reference in fp64
     sd = src.double().requires_grad_(True)
     wd = w.double().requires_grad_(True) if has else None
@@ -130,14 +109,12 @@ def test_dwpool_forward_backward(case, cuda_device):
     dout = torch.randn(B, Hn, Lo + 1, hd, generator=g).to(dev)
     ref.backward(dout.double())
     dsrc = torch.zeros(B, Lin + 1, 3 * A, device=dev)
-    d.dout, d.dsrc = dout.data_ptr(), dsrc.data_ptr()
-    dw = None
+    dw = wp = None
     if has:
-        nb = lib.sfb_dwpool_wgrad_blocks(C.byref(d))
+        nb = ops.dwpool_wgrad_blocks(B, Hn, othw)
         wp = torch.empty(max(nb, 1) * hd * math.prod(kern), device=dev)
-        d.wpartials = wp.data_ptr()
         dw = torch.full_like(w, float("nan"))
-    L.check(lib.sfb_dwpool_bwd(C.byref(d), dw.data_ptr() if has else None, 0, _st()))
+    ops.dwpool_bwd(src, j * A, bias, w, B, Hn, hd, (T, Hh, W), othw, kern, strd, dout, dsrc, dw=dw, wpartials=wp)
     assert relerr(dsrc, sd.grad) < 1e-5
     assert (dsrc[:, :, :j * A] == 0).all() and (dsrc[:, :, (j + 1) * A:] == 0).all()   # only this third is touched
     if has:
@@ -157,8 +134,8 @@ def test_softmax_relpos_forward_backward(q_thw, k_thw, bh, cuda_device):
     """P = softmax(S + bias), bias[q,k] = RQ[q, ih(q,k)] + RQ[q, Lh + iw] + RQ[q, Lh+Lw + it] for non-cls (q, k)
     (cal_rel_pos_spatial / cal_rel_pos_temporal, attention.py:64-147; the cls row and column get no bias); backward
     dS = P * (dP - sum(dP*P)) and dRQ = the scatter of dS onto the table columns."""
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
+    from slowfast_b200 import ops
+    dev = cuda_device
     qt, qh, qw = q_thw
     kt, kh, kw = k_thw
     Lq, Lk = qt * qh * qw, kt * kh * kw
@@ -174,13 +151,8 @@ def test_softmax_relpos_forward_backward(q_thw, k_thw, bh, cuda_device):
     S, rq = S.to(dev), rq.to(dev)
     p_hi = torch.full((bh, Nq, Nkp), float("nan"), dtype=torch.bfloat16, device=dev)
     p_lo = torch.full_like(p_hi, float("nan"))
-    sd = L.SoftmaxDesc()
-    sd.s, sd.s_pitch, sd.rq, sd.rq_pitch = S.data_ptr(), Nkp, rq.data_ptr(), Ltp
-    sd.p_hi, sd.p_lo, sd.p_pitch = p_hi.data_ptr(), p_lo.data_ptr(), Nkp
-    sd.bh, sd.nq, sd.nk = bh, Nq, Nk
-    sd.qt, sd.qh, sd.qw = q_thw
-    sd.kt, sd.kh, sd.kw = k_thw
-    L.check(lib.sfb_softmax_relpos_fwd(C.byref(sd), _st()))
+    P_planes = ops.Planes(p_hi, p_lo, 1, 1, 1, bh * Nq, Nkp)
+    ops.softmax_relpos_fwd(S, P_planes, bh, Nq, Nk, q_thw, k_thw, rq=rq)
     # fp64 reference with explicit index tables
     Sd = S[..., :Nk].double().cpu().requires_grad_(True)
     rqd = rq.double().cpu().requires_grad_(True)
@@ -206,10 +178,8 @@ def test_softmax_relpos_forward_backward(q_thw, k_thw, bh, cuda_device):
     ds_hi = torch.full((bh, Nq, Nkp), float("nan"), dtype=torch.bfloat16, device=dev)
     ds_lo = torch.full_like(ds_hi, float("nan"))
     drq = torch.full((bh * Lq, Ltp), float("nan"), device=dev)
-    sd.dp, sd.dp_pitch = dPd.data_ptr(), Nkp
-    sd.ds_hi, sd.ds_lo, sd.ds_pitch = ds_hi.data_ptr(), ds_lo.data_ptr(), Nkp
-    sd.drq = drq.data_ptr()
-    L.check(lib.sfb_softmax_relpos_bwd(C.byref(sd), _st()))
+    ops.softmax_relpos_bwd(P_planes, dPd, ops.Planes(ds_hi, ds_lo, 1, 1, 1, bh * Nq, Nkp), bh, Nq, Nk, q_thw, k_thw,
+                           drq=drq)
     dS = planes_to_float(ds_hi, ds_lo).cpu()
     assert relerr(dS[..., :Nk], Sd.grad) < 5e-5
     assert relerr(drq.cpu()[:, :Lh + Lw + Lt], rqd.grad[:, :Lh + Lw + Lt]) < 1e-4
@@ -217,14 +187,14 @@ def test_softmax_relpos_forward_backward(q_thw, k_thw, bh, cuda_device):
 
 @pytest.mark.parametrize("rows,c", [(1000, 384), (333, 1536), (64, 3072)])
 def test_bias_gelu_forward_backward(rows, c, cuda_device):
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
+    from slowfast_b200 import ops
+    dev = cuda_device
     g = torch.Generator().manual_seed(c)
     y = (torch.randn(rows, c, generator=g) * 2).to(dev)
     b = torch.randn(c, generator=g).to(dev)
     hi = torch.empty(rows, c, dtype=torch.bfloat16, device=dev)
     lo = torch.empty_like(hi)
-    L.check(lib.sfb_bias_gelu(y.data_ptr(), b.data_ptr(), rows, c, hi.data_ptr(), lo.data_ptr(), _st()))
+    ops.bias_gelu(y, b, rows, c, ops.Planes(hi, lo, 1, 1, 1, rows, c))
     pre = (y.double() + b.double()).requires_grad_(True)
     ref = F.gelu(pre)  # exact erf form (nn.GELU default, common.py:33)
     assert relerr(planes_to_float(hi, lo), ref) < 2e-5
@@ -233,8 +203,7 @@ def test_bias_gelu_forward_backward(rows, c, cuda_device):
     ghi = torch.empty_like(hi)
     glo = torch.empty_like(hi)
     dpre = torch.empty(rows, c, device=dev)
-    L.check(lib.sfb_bias_gelu_bwd(dh.data_ptr(), y.data_ptr(), b.data_ptr(), rows, c, ghi.data_ptr(), glo.data_ptr(),
-                                  dpre.data_ptr(), _st()))
+    ops.bias_gelu_bwd(dh, y, b, rows, c, ops.Planes(ghi, glo, 1, 1, 1, rows, c), dpre)
     assert relerr(dpre, pre.grad) < 1e-5
     assert relerr(planes_to_float(ghi, glo), pre.grad) < 2e-5
 
@@ -243,8 +212,8 @@ def test_bias_gelu_forward_backward(rows, c, cuda_device):
                                             (1, 384, (3, 7, 7), (1, 2, 2))])
 def test_token_maxpool_forward_backward(B, c, thw, stride, cuda_device):
     """MaxPool3d(kernel s+1, stride s, padding k//2) on tokens, cls passes through (attention.py:485-489, :13-45)."""
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
+    from slowfast_b200 import ops
+    dev = cuda_device
     T, Hh, W = thw
     ks = [s + 1 if s > 1 else s for s in stride]
     pad = [k // 2 for k in ks]
@@ -254,13 +223,7 @@ def test_token_maxpool_forward_backward(B, c, thw, stride, cuda_device):
     x = torch.randn(B, Lin + 1, c, generator=g).to(dev)
     out = torch.full((B, Lo + 1, c), float("nan"), device=dev)
     amax = torch.empty(B, Lo + 1, c, dtype=torch.uint8, device=dev)
-    td = L.TokPoolDesc()
-    td.x, td.out, td.argmax = x.data_ptr(), out.data_ptr(), amax.data_ptr()
-    td.b, td.c, td.t, td.h, td.w = B, c, T, Hh, W
-    td.ot, td.oh, td.ow = othw
-    td.kt, td.kh, td.kw = ks
-    td.st, td.sh, td.sw = stride
-    L.check(lib.sfb_token_maxpool_fwd(C.byref(td), _st()))
+    ops.token_maxpool_fwd(x, B, c, thw, othw, ks, stride, out, amax)
     xd = x.double().requires_grad_(True)
     tok = xd[:, 1:].reshape(B, T, Hh, W, c).permute(0, 4, 1, 2, 3)
     pooled = F.max_pool3d(tok, ks, stride, pad).reshape(B, c, Lo).transpose(1, 2)
@@ -269,8 +232,7 @@ def test_token_maxpool_forward_backward(B, c, thw, stride, cuda_device):
     dout = torch.randn(B, Lo + 1, c, generator=g).to(dev)
     ref.backward(dout.double())
     dx = torch.full((B, Lin + 1, c), float("nan"), device=dev)
-    td.dout, td.dx, td.dx_accumulate = dout.data_ptr(), dx.data_ptr(), 0
-    L.check(lib.sfb_token_maxpool_bwd(C.byref(td), _st()))
+    ops.token_maxpool_bwd(dout, amax, B, c, thw, othw, ks, stride, dx)
     assert relerr(dx, xd.grad) < 1e-6
 
 
@@ -280,15 +242,15 @@ def test_hog_targets_kernel(B, T, H, fs, cuda_device):
     _get_hog_label_3d (bit-identical to the reference on the CPU, tests/test_oracle.py).  Orientation bins are decided by
     atan2 in fp32: a pixel within an ulp of a bin edge may land in the neighbouring bin on the GPU."""
     from oracle import torch_oracle as TO
-    from slowfast_b200 import lib as L
-    lib, dev = L.load(), cuda_device
+    from slowfast_b200 import ops
+    dev = cuda_device
     g = torch.Generator().manual_seed(H)
     frames = torch.randn(B, 3, T, H, H, generator=g)
     ts, nbins, cell = 2, 9, 8
     u = (H // cell) // fs
     out = torch.full((B, (T // ts) * fs * fs, 3 * nbins * u * u), float("nan"), device=dev)
     fd = frames.to(dev)
-    L.check(lib.sfb_hog_targets(fd.data_ptr(), B, 3, T, H, H, ts, nbins, cell, fs, out.data_ptr(), _st()))
+    ops.hog_targets(fd, ts, nbins, cell, fs, out)
     torch.cuda.synchronize()
     x = frames[:, :, ::ts].transpose(1, 2)
     hog = TO.hog_layer(x.flatten(0, 1)).flatten(1, 2)

@@ -37,21 +37,20 @@ POS_SHAPES = [  # (B, T, HW, E): ViT-B 16x224, MViTv1-B 16x224, odd extents
 
 @pytest.mark.parametrize("b,t,hw,e", POS_SHAPES)
 def test_tokens_assemble_with_positions(b, t, hw, e, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     g = torch.Generator().manual_seed(b * 1000 + hw)
     Lt = t * hw
     y, bias, cls = torch.randn(b, Lt, e, generator=g), torch.randn(e, generator=g), torch.randn(e, generator=g)
     ps, pt, pc = torch.randn(hw, e, generator=g), torch.randn(t, e, generator=g), torch.randn(e, generator=g)
     d = [v.to(cuda_device) for v in (y, bias, cls, ps, pt, pc)]
     out = torch.empty(b, Lt + 1, e, device=cuda_device)
-    L.check(lib.sfb_tokens_assemble(*(v.data_ptr() for v in d), b, Lt, hw, e, out.data_ptr(), _st()), "assemble")
+    ops.tokens_assemble(*d, b, Lt, hw, e, out)
     # the reference's arithmetic in fp32: x = cat(cls, y + bias) + cat(pc, ps.repeat(t) + pt.repeat_interleave(hw))
     pos = torch.cat([pc.view(1, e), ps.repeat(t, 1) + pt.repeat_interleave(hw, dim=0)])
     want = torch.cat([cls.view(1, 1, e).expand(b, 1, e), y + bias], 1) + pos
     assert torch.equal(out.cpu(), want)
     # null tables: the plain assembly, bitwise
-    L.check(lib.sfb_tokens_assemble(d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(), None, None, None, b, Lt, hw, e,
-                                    out.data_ptr(), _st()), "assemble")
+    ops.tokens_assemble(d[0], d[1], d[2], None, None, None, b, Lt, hw, e, out)
     assert torch.equal(out.cpu(), torch.cat([cls.view(1, 1, e).expand(b, 1, e), y + bias], 1))
 
 
@@ -65,15 +64,14 @@ def test_tokens_assemble_rejects_partial_tables(cuda_device):
 
 @pytest.mark.parametrize("b,t,hw,e", POS_SHAPES)
 def test_pos_embed_sep_bwd_matches_fp64_and_is_deterministic(b, t, hw, e, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     dx = torch.randn(b, 1 + t * hw, e, generator=torch.Generator().manual_seed(7))
     d = dx.to(cuda_device)
-    part = torch.empty(t * lib.sfb_segment_slabs(t, hw) * e, device=cuda_device)
+    part = torch.empty(t * ops.segment_slabs(t, hw) * e, device=cuda_device)
     outs = []
     for _ in range(2):
         dps, dpt, dpc = (torch.full(s, float("nan"), device=cuda_device) for s in ((hw, e), (t, e), (e,)))
-        L.check(lib.sfb_pos_embed_sep_bwd(d.data_ptr(), b, t, hw, e, dps.data_ptr(), dpt.data_ptr(), dpc.data_ptr(),
-                                          part.data_ptr(), _st()), "pos bwd")
+        ops.pos_embed_sep_bwd(d, b, t, hw, e, dps, dpt, dpc, part)
         outs.append((dps.cpu(), dpt.cpu(), dpc.cpu()))
     x = dx.double()[:, 1:].view(b, t, hw, e)
     want = (x.sum((0, 1)), x.sum((0, 2)), dx.double()[:, 0].sum(0))
@@ -84,19 +82,19 @@ def test_pos_embed_sep_bwd_matches_fp64_and_is_deterministic(b, t, hw, e, cuda_d
 
 @pytest.mark.parametrize("b,n,c", [(8, 1569, 768), (2, 393, 768), (3, 50, 40), (1, 2, 8)])
 def test_token_mean_fwd_bwd(b, n, c, cuda_device):
-    L, lib = _lib()
+    from slowfast_b200 import ops
     g = torch.Generator().manual_seed(n)
     x, dm = torch.randn(b, n, c, generator=g), torch.randn(b, c, generator=g)
     xd, dmd = x.to(cuda_device), dm.to(cuda_device)
     out = torch.empty(b, c, device=cuda_device)
-    part = torch.empty(b * lib.sfb_segment_slabs(b, n - 1) * c, device=cuda_device)
-    L.check(lib.sfb_token_mean_fwd(xd.data_ptr(), b, n, c, out.data_ptr(), part.data_ptr(), _st()), "mean fwd")
+    part = torch.empty(b * ops.segment_slabs(b, n - 1) * c, device=cuda_device)
+    ops.token_mean_fwd(xd, b, n, c, out, part)
     assert _rel(out.cpu().double(), x.double()[:, 1:].mean(1)) < 1e-6
     out2 = torch.empty_like(out)
-    L.check(lib.sfb_token_mean_fwd(xd.data_ptr(), b, n, c, out2.data_ptr(), part.data_ptr(), _st()), "mean fwd")
+    ops.token_mean_fwd(xd, b, n, c, out2, part)
     assert torch.equal(out, out2)
     dx = torch.full((b, n, c), float("nan"), device=cuda_device)
-    L.check(lib.sfb_token_mean_bwd(dmd.data_ptr(), b, n, c, dx.data_ptr(), _st()), "mean bwd")
+    ops.token_mean_bwd(dmd, b, n, c, dx)
     want = torch.cat([torch.zeros(b, 1, c), (dm / (n - 1)).view(b, 1, c).expand(b, n - 1, c)], 1)
     torch.testing.assert_close(dx.cpu(), want, rtol=1e-6, atol=0)
 
@@ -108,7 +106,6 @@ def test_patchify_gemm_and_wgrad_match_conv3d(shape, k, nsplit, cuda_device):
     from slowfast_b200 import ops
     from slowfast_b200.engine import Ctx
     from slowfast_b200.ops import Planes
-    L, lib = _lib()
     g = torch.Generator().manual_seed(3)
     x = torch.randn(*shape, generator=g)
     B, cin = shape[:2]
@@ -120,8 +117,7 @@ def test_patchify_gemm_and_wgrad_match_conv3d(shape, k, nsplit, cuda_device):
     rows = B * ot * oh * ow
     s = ctx.storage(("rows",), 1, 1, 1, rows, K)
     xr = Planes(s.hi, s.lo, 1, 1, 1, rows, K, 0)
-    L.check(lib.sfb_patchify(x.to(cuda_device).data_ptr(), B, cin, *shape[2:], *k, xr.hi_ptr(), xr.lo_ptr(), _st()),
-            "patchify")
+    ops.patchify(x.to(cuda_device), k, xr)
     wd = w.to(cuda_device).view(E, K)
     fm = ops.alloc_filter(E, 1, K, nsplit, cuda_device)
     ops.filter_pack(wd, fm)
@@ -147,7 +143,7 @@ def test_patchify_gemm_and_wgrad_match_conv3d(shape, k, nsplit, cuda_device):
 def test_layernorm_wide_rows_match_fp64(c, cuda_device):
     """LayerNorm at ViT-L (1024), MViTv2-L's last stage (1152) and ViT-H (1280) widths, an odd width, and 768 (the widest
     row of the register-resident kernel), forward and backward (dx accumulated, dgamma / dbeta) against fp64."""
-    L, lib = _lib()
+    from slowfast_b200 import ops
     rows = 3 * 1569
     g = torch.Generator().manual_seed(c)
     x, dy = torch.randn(rows, c, generator=g) * 2 + 0.5, torch.randn(rows, c, generator=g)
@@ -156,13 +152,10 @@ def test_layernorm_wide_rows_match_fp64(c, cuda_device):
     xd, dyd, gd, bd = (v.to(cuda_device) for v in (x, dy, gamma, beta))
     y = torch.empty(rows, c, device=cuda_device)
     mean, rstd = torch.empty(rows, device=cuda_device), torch.empty(rows, device=cuda_device)
-    L.check(lib.sfb_layernorm_fwd(xd.data_ptr(), c, rows, c, gd.data_ptr(), bd.data_ptr(), 1e-6, None, None, y.data_ptr(),
-                                  c, mean.data_ptr(), rstd.data_ptr(), _st()), "ln fwd")
+    ops.layernorm_fwd(xd, c, rows, c, gd, bd, 1e-6, mean, rstd, out_f32=y)
     dx, dg, db = dx0.to(cuda_device), torch.empty(c, device=cuda_device), torch.empty(c, device=cuda_device)
-    part = torch.empty(lib.sfb_rowslab_blocks(rows) * 2 * c, device=cuda_device)
-    L.check(lib.sfb_layernorm_bwd(dyd.data_ptr(), c, xd.data_ptr(), c, rows, c, gd.data_ptr(), mean.data_ptr(),
-                                  rstd.data_ptr(), dx.data_ptr(), c, 1, dg.data_ptr(), db.data_ptr(), 0, part.data_ptr(),
-                                  _st()), "ln bwd")
+    part = torch.empty(ops.colsum_blocks(rows) * 2 * c, device=cuda_device)
+    ops.layernorm_bwd(dyd, c, xd, c, rows, c, gd, mean, rstd, dx, c, dg, db, part, dx_accumulate=True)
     xr = x.double().requires_grad_(True)
     gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
     yr = F.layer_norm(xr, (c,), gr, br, 1e-6)
