@@ -57,14 +57,19 @@ typedef struct sfb_conv_desc {
   float* out;
   int64_t os_n, os_t, os_h, os_w;
   int32_t accumulate; /* 0: out = result, 1: out += result (read-modify-write), 2: out += result with red.global.add (each
-                         element gets one add per call: same sums, no dependent load) */
-  /* optional per-tile BatchNorm partials: [2][cout][m_tiles] = (sum, sum of squares) over each tile's rows */
+                         element gets one add per call: same sums, no dependent load).  A split-K launch (a grid that
+                         fills too little of its last wave, see conv_ksplit) adds one partial sum per k-slice with
+                         red.global.add in every mode, after zero-filling the view for mode 0. */
+  /* optional BatchNorm partials: [2][cout][sfb_conv_m_tiles(d)] = (sum, sum of squares) over blocks of rows */
   float* stats;
   int32_t nsplit; /* 1 (bf16 operands) or 3 (split-bf16, fp32-class operands) */
 } sfb_conv_desc;
 
-/* Number of 128-row output tiles (last extent of `stats`). */
+/* Columns of the BatchNorm partials a launch with this descriptor writes (last extent of `stats`): its 128-row output
+ * tiles, or the row blocks of sfb_bn_split_stats when the launch is split over K. */
 int64_t sfb_conv_m_tiles(const sfb_conv_desc* d);
+/* CTAs that share each output tile of the launch, each over a slice of K (1 = no split-K). */
+int32_t sfb_conv_ksplit(const sfb_conv_desc* d);
 int sfb_conv_igemm(const sfb_conv_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------------------------------

@@ -7,6 +7,10 @@
 // * B (filter matrix, K-major) arrives through a tiled TMA load (128B swizzle).
 // * wgmma (64 x BN x 16 per warpgroup, bf16 -> fp32) accumulates in registers; in parity mode every product is the
 //   3-term split  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi.
+// * The tile width BN is a template parameter and a k-block is always KSTEPS k16 steps, so the wgmmas of a k-block are
+//   issued back to back (a runtime width switch makes ptxas serialise them).
+// * Split-K (conv_ksplit): a grid that fills too little of its last wave gives each tile to s CTAs, each over a slice
+//   of the k-blocks; the partial tiles meet in the output with red.global.add.
 // * Persistent CTAs, warp-specialised: warps 0..7 = two MMA warpgroups (rows 0..63 / 64..127 of the tile),
 //   warp 8 = TMA producer, warps 9..16 = epilogue.  The MMA warpgroups hand a finished tile to the epilogue through a
 //   shared-memory accumulator tile and go on with the main loop of the next one.
@@ -24,7 +28,6 @@
 namespace sfb {
 
 constexpr int BLOCK_M = 128;
-constexpr int A_PLANE_BYTES = BLOCK_M * 128;  // 128 pixels x 64 bf16
 constexpr int MAX_STAGES = 8;
 constexpr int EPI_WARPS = 8;                     // two per 32-row quarter of the tile: the pair splits the tile's 16-column chunks
 constexpr int EPI_STAGE_FLOATS = 64;             // per epilogue warp: 32 row offsets (int64)
@@ -33,6 +36,8 @@ constexpr int PRODUCER_WARP = MMA_WARPS;
 constexpr int EPI_WARP0 = MMA_WARPS + 1;
 constexpr int CONV_THREADS = 32 * (MMA_WARPS + 1 + EPI_WARPS);
 constexpr int BN_MAX = 128;                      // accumulator columns per tile: 64 registers per MMA thread
+constexpr int BLOCK_K = 64;                      // K columns per k-block (pipeline stage)
+constexpr int KSTEPS = BLOCK_K / 16;             // wgmma k16 steps per k-block
 
 struct ConvParams {
   CUtensorMap tmA[2];
@@ -42,12 +47,14 @@ struct ConvParams {
   int lw, lh, ld;
   int kw, kh, kd;
   int dw, dh, dd;
-  int CK, cpt, n_chunks, n_chunks_padded, cps, k_blocks;
+  int CK, cpt, n_chunks, cps, k_blocks;
   int Ntot, BN, n_tiles, m_tiles;
+  int ksplit;  // CTAs sharing one output tile, each over a contiguous slice of the k-blocks (1 = no split-K)
   int stages;
   int a_tiled;  // tap-free stride-1 conv: A is the plain [M][C] matrix, loaded with tiled (not im2col) TMA
   uint32_t stage_bytes, chunk_bytes, b_bytes, a_total_bytes, a_plane_bytes;
   uint32_t a_layout, a_sbo, a_lbo;
+  uint32_t a_kstep[KSTEPS];  // start of k-step ks's A columns in the stage, in 16-byte units
   uint32_t acc_pitch;  // floats per row of the shared-memory accumulator tile
   uint32_t off_acc, off_staging, off_red, off_bars;
   float* out;
@@ -57,11 +64,17 @@ struct ConvParams {
   float* stats;
 };
 
+// First k-block of slice `kpart` of p.ksplit (balanced; every slice is non-empty because ksplit <= k_blocks).
+__device__ __forceinline__ int k_block_begin(const ConvParams& p, int kpart) {
+  return kpart * p.k_blocks / p.ksplit;
+}
+
 // csrc/conv_direct.cu: fp32 SIMT body for narrow layers (C_in <= 8); returns 1 when it handled the call
 int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out);
 
-template <int NSPLIT>
+template <int NSPLIT, int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
+  static_assert(BN % 16 == 0 && BN <= BN_MAX, "tile width: a multiple of 16 up to BN_MAX");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
@@ -86,7 +99,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
   }
   __syncthreads();
 
-  const int total_tiles = p.m_tiles * p.n_tiles;
+  // A work unit is one output tile and one of its p.ksplit slices of k-blocks; a tile's slices are consecutive units.
+  const int total_units = p.m_tiles * p.n_tiles * p.ksplit;
 
   if (warp == PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
@@ -100,8 +114,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
     }
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
+      const int tile = unit / p.ksplit, kpart = unit - tile * p.ksplit;
       const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+      const int kb0 = k_block_begin(p, kpart), kb1 = k_block_begin(p, kpart + 1);
       int t = mt * BLOCK_M;
       const int q0 = t % p.oq;
       t /= p.oq;
@@ -110,15 +126,14 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
       const int z0 = t % p.oz;
       const int n0 = t / p.oz;
       const int cw = p.lw + q0 * p.sw, ch = p.lh + p0 * p.sh, cd = p.ld + z0 * p.sd;
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
+      for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&empty[stage], phase ^ 1);
         if (elect_one()) {
           const int chunk0 = kb * p.cps;
-          const int nch = min(p.cps, p.n_chunks_padded - chunk0);
-          const uint32_t bytes = (uint32_t(nch) * p.chunk_bytes + p.b_bytes) * (NSPLIT == 3 ? 2u : 1u);
+          const uint32_t bytes = (uint32_t(p.cps) * p.chunk_bytes + p.b_bytes) * (NSPLIT == 3 ? 2u : 1u);
           mbar_expect_tx(&full[stage], bytes);
           uint8_t* st = smem + size_t(stage) * p.stage_bytes;
-          for (int j = 0; j < nch; ++j) {
+          for (int j = 0; j < p.cps; ++j) {
             const int idx = chunk0 + j;
             int nn = p.nb, c0 = 0;  // out-of-range batch index => the unit writes a zero chunk
             uint16_t ow = 0, oh = 0, od = 0;
@@ -149,9 +164,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
               tma_load_im2col_5d(st + p.a_plane_bytes + j * p.chunk_bytes, &p.tmA[1], &full[stage], c0, cw, ch, cd,
                                  nn, ow, oh, od);
           }
-          tma_load_2d(st + p.a_total_bytes, &p.tmB[0], &full[stage], kb * 64, nt * p.BN);
+          tma_load_2d(st + p.a_total_bytes, &p.tmB[0], &full[stage], kb * 64, nt * BN);
           if (NSPLIT == 3)
-            tma_load_2d(st + p.a_total_bytes + p.b_bytes, &p.tmB[1], &full[stage], kb * 64, nt * p.BN);
+            tma_load_2d(st + p.a_total_bytes + p.b_bytes, &p.tmB[1], &full[stage], kb * 64, nt * BN);
         }
         __syncwarp();
         if (++stage == p.stages) {
@@ -162,44 +177,39 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
     }
   } else if (warp < MMA_WARPS) {
     // ------------------------------------------------------------------ MMA warpgroups
+    // Every k-block is KSTEPS k16 steps (the producer pads the last one with zero chunks) and the tile width is the
+    // template's BN, so the k-block's 3 x KSTEPS wgmmas are straight-line code issued back to back.
     const int g = warp >> 2;  // tile rows 64g .. 64g+63: 8 core-matrix row groups (SBO apart) further into the A tile
     const uint32_t a_row_off = uint32_t(g) * 8u * p.a_sbo;
-    float d[BN_MAX / 2];
+    float d[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+    for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++it) {
+      const int kpart = unit % p.ksplit;
+      const int kb0 = k_block_begin(p, kpart), kb1 = k_block_begin(p, kpart + 1);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       int held = -1;  // stage whose MMAs may still be reading shared memory
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
+      for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
         wgmma_fence();
-        const int chunk0 = kb * p.cps;
-        const int nch = min(p.cps, p.n_chunks_padded - chunk0);
-        const int ksteps = (nch * p.CK) >> 4;
-        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-        const uint32_t b_base = a_base + p.a_total_bytes;
-        for (int ks = 0; ks < ksteps; ++ks) {
-          uint32_t a_addr;
-          if (p.CK >= 16) {
-            const int k0 = ks * 16;
-            const int chunk = k0 / p.CK;
-            a_addr = a_base + uint32_t(chunk) * p.chunk_bytes + uint32_t(k0 - chunk * p.CK) * 2u;
-          } else {
-            a_addr = a_base + uint32_t(ks * 2) * p.chunk_bytes;
-          }
-          a_addr += a_row_off;
-          const uint64_t a_hi = make_smem_desc(a_addr, p.a_lbo, p.a_sbo, p.a_layout);
-          const uint64_t b_hi = make_smem_desc(b_base + uint32_t(ks) * 32u, 16, 1024, 2);
-          const uint32_t acc_flag = (kb | ks) != 0 ? 1u : 0u;
+        // descriptors of k-step 0; a later k-step adds its offset to the start-address field (16-byte units)
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + a_row_off;
+        const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + p.a_total_bytes;
+        const uint64_t a_hi0 = make_smem_desc(a_base, p.a_lbo, p.a_sbo, p.a_layout);
+        const uint64_t b_hi0 = make_smem_desc(b_base, 16, 1024, 2);
+#pragma unroll
+        for (int ks = 0; ks < KSTEPS; ++ks) {
+          const uint64_t a_hi = a_hi0 + p.a_kstep[ks];
+          const uint64_t b_hi = b_hi0 + uint64_t(ks * 2);  // 32 bytes = 16 bf16 of the 128-byte swizzled rows
           if (NSPLIT == 3) {
-            const uint64_t a_lo = make_smem_desc(a_addr + p.a_plane_bytes, p.a_lbo, p.a_sbo, p.a_layout);
-            const uint64_t b_lo = make_smem_desc(b_base + p.b_bytes + uint32_t(ks) * 32u, 16, 1024, 2);
-            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_lo, b_hi, acc_flag);
-            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_hi, b_lo, 1u);
-            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, 1u);
-          } else {
-            wgmma_bf16<BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, acc_flag);
+            const uint64_t a_lo = a_hi + (p.a_plane_bytes >> 4);
+            const uint64_t b_lo = b_hi + (p.b_bytes >> 4);
+            wgmma_m64n<BN>(d, a_lo, b_hi);
+            wgmma_m64n<BN>(d, a_hi, b_lo);
           }
+          wgmma_m64n<BN>(d, a_hi, b_hi);
         }
         wgmma_commit();
         wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage can be refilled
@@ -213,7 +223,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
       wgmma_wait<0>();
       mbar_arrive(&empty[held]);
       mbar_wait(tempty, (it & 1) ^ 1);  // the epilogue has read the previous tile
-      acc_store<BN_MAX>(d, p.BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
+      acc_store<BN>(d, BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
       mbar_arrive(tfull);
     }
   } else {
@@ -227,13 +237,14 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
     long long* roff_s = reinterpret_cast<long long*>(reinterpret_cast<float*>(smem + p.off_staging) + ew * EPI_STAGE_FLOATS);
     float* red = reinterpret_cast<float*>(smem + p.off_red);  // [2][4][BN][2]
     const int sub = lane >> 2, cq = lane & 3;   // row within a group of 8, 16-byte piece of the chunk's 64-byte row
-    const int nchunks = p.BN >> 4;
+    constexpr int nchunks = BN >> 4;
     const float* qtile = acc_tile + size_t(q) * 32 * p.acc_pitch;
     int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+    for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++it) {
+      const int tile = unit / p.ksplit;
       const int acc = it & 1;
       const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
-      const int ncol0 = nt * p.BN;
+      const int ncol0 = nt * BN;
       const int row = mt * BLOCK_M + q * 32 + lane;
       const bool rvalid = row < p.M;
       long long roff = 0;
@@ -248,7 +259,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
         roff = on_ * p.os_n + oz_ * p.os_z + op_ * p.os_p + oq_ * p.os_q;
       }
       const uint32_t rmask = __ballot_sync(0xffffffffu, rvalid);
-      float* red_w = red + ((size_t(acc) * 4 + q) * p.BN) * 2;
+      float* red_w = red + ((size_t(acc) * 4 + q) * BN) * 2;
       roff_s[lane] = roff;
       __syncwarp();
       long long ro[4];
@@ -258,7 +269,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
       mbar_wait(tfull, it & 1);
       for (int ch = half; ch < nchunks; ch += 2) {
         const int c0 = ch * 16;
-        const int limit = min(p.BN, p.Ntot - ncol0) - c0;      // valid columns of this chunk (a multiple of 4)
+        const int limit = min(BN, p.Ntot - ncol0) - c0;      // valid columns of this chunk (a multiple of 4)
         const bool cvalid = cq * 4 < limit;
         float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -305,15 +316,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
       if (p.stats != nullptr) {
         named_bar_sync(1, 32 * EPI_WARPS);
         // the four quarter partials of this tile are in red[acc]; spread the column reduction over the epilogue warps
-        const float* rb = red + size_t(acc) * 4 * p.BN * 2;
-        for (int cl = ew * 32 + lane; cl < p.BN; cl += 32 * EPI_WARPS) {
+        const float* rb = red + size_t(acc) * 4 * BN * 2;
+        for (int cl = ew * 32 + lane; cl < BN; cl += 32 * EPI_WARPS) {
           const int col = ncol0 + cl;
           if (col < p.Ntot) {
             float s = 0.f, s2 = 0.f;
 #pragma unroll
             for (int w = 0; w < 4; ++w) {
-              s += rb[(size_t(w) * p.BN + cl) * 2 + 0];
-              s2 += rb[(size_t(w) * p.BN + cl) * 2 + 1];
+              s += rb[(size_t(w) * BN + cl) * 2 + 0];
+              s2 += rb[(size_t(w) * BN + cl) * 2 + 1];
             }
             // [2][cout][m_tiles]: tile axis contiguous for the finalize kernel's per-channel reduction
             p.stats[size_t(col) * p.m_tiles + mt] = s;
@@ -348,13 +359,65 @@ static int pick_ck(int c) {
   return 8;
 }
 
+// Tile grid of a launch: 128 x BN output tiles, K in 64-column k-blocks (the last one padded with zero chunks).
+struct ConvGrid {
+  int64_t M;
+  int CK, cps, n_chunks, k_blocks, BN, m_tiles, n_tiles;
+};
+static ConvGrid conv_grid(const sfb_conv_desc* d) {
+  ConvGrid g;
+  g.M = int64_t(d->n) * d->out_t * d->out_h * d->out_w;
+  g.CK = pick_ck(d->c);
+  g.cps = BLOCK_K / g.CK;
+  g.n_chunks = d->kt * d->kh * d->kw * (d->c / g.CK);
+  g.k_blocks = (g.n_chunks + g.cps - 1) / g.cps;
+  g.BN = std::min((d->cout + 15) / 16 * 16, BN_MAX);
+  g.m_tiles = int((g.M + BLOCK_M - 1) / BLOCK_M);
+  g.n_tiles = (d->cout + g.BN - 1) / g.BN;
+  return g;
+}
+
+// The output view is a plain row matrix (rows n*t*h*w apart by os_w): it can be zero-filled with one 2-D memset and
+// its BatchNorm statistics taken by sfb_bn_split_stats.
+static bool rows_regular(const sfb_conv_desc* d) {
+  return d->os_h == int64_t(d->out_w) * d->os_w && d->os_t == int64_t(d->out_h) * d->os_h &&
+         d->os_n == int64_t(d->out_t) * d->os_t;
+}
+
+// Split-K for grids that leave much of their last wave idle: each tile's k-blocks are split over s CTAs whose partial
+// tiles meet in the output with red.global.add.  s minimises the waves per tile, ceil(tiles * s / SMs) / s, with a 2 %
+// charge per extra slice (zero fill, s partial-tile epilogues), and is taken only when that beats s = 1 by 10 %.
+// Each slice keeps at least 4 k-blocks so that its pipeline fill is amortised.  Not split: grids under half a wave
+// (short launches, where the zero fill and the statistics pass are fixed costs), narrow inputs (C_in <= 8 may take
+// the SIMT body), overwrites of views that are not a row matrix, and statistics of accumulating launches or over
+// channels that are not a multiple of 8 (sfb_bn_split_stats).
+static int conv_ksplit(const sfb_conv_desc* d, const ConvGrid& g, bool with_stats) {
+  const int tiles = g.m_tiles * g.n_tiles;
+  const int P = g_num_sms;
+  if (P <= 0 || d->c <= 8 || 2 * tiles < P) return 1;
+  if ((d->accumulate == 0 || with_stats) && !rows_regular(d)) return 1;
+  if (with_stats && (d->accumulate != 0 || d->cout % 8 != 0 || d->os_w % 4 != 0)) return 1;
+  auto cost = [&](int s) { return double((int64_t(tiles) * s + P - 1) / P) / s * (1.0 + 0.02 * (s - 1)); };
+  int best = 1;
+  for (int s = 2; s <= 8 && 4 * s <= g.k_blocks; ++s)
+    if (cost(s) < cost(best)) best = s;
+  return cost(best) < 0.9 * cost(1) ? best : 1;
+}
+
 }  // namespace sfb
 
 using namespace sfb;
 
 extern "C" int64_t sfb_conv_m_tiles(const sfb_conv_desc* d) {
-  const int64_t m = int64_t(d->n) * d->out_t * d->out_h * d->out_w;
-  return (m + BLOCK_M - 1) / BLOCK_M;
+  const ConvGrid g = conv_grid(d);
+  if (device_props() == 0 && conv_ksplit(d, g, true) > 1)
+    return sfb_bn_split_stats_tiles(g.M, g.M, 1, d->cout);  // statistics from y after the split GEMM
+  return g.m_tiles;
+}
+
+extern "C" int32_t sfb_conv_ksplit(const sfb_conv_desc* d) {
+  if (device_props()) return 1;
+  return conv_ksplit(d, conv_grid(d), d->stats != nullptr);
 }
 
 extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
@@ -402,25 +465,22 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   p.dw = d->dil_w;
   p.dh = d->dil_h;
   p.dd = d->dil_t;
-  p.CK = pick_ck(d->c);
-  p.cpt = d->c / p.CK;
+  const ConvGrid g = conv_grid(d);
   const int taps = d->kt * d->kh * d->kw;
-  p.n_chunks = taps * p.cpt;
-  const int pad_to = p.CK >= 16 ? 1 : 16 / p.CK;
-  p.n_chunks_padded = (p.n_chunks + pad_to - 1) / pad_to * pad_to;
-  p.cps = 64 / p.CK;
-  p.k_blocks = (p.n_chunks_padded + p.cps - 1) / p.cps;
+  p.CK = g.CK;
+  p.cpt = d->c / p.CK;
+  p.n_chunks = g.n_chunks;
+  p.cps = g.cps;
+  p.k_blocks = g.k_blocks;
   p.Ntot = d->cout;
-  const int n16 = (d->cout + 15) / 16 * 16;
-  p.BN = std::min(n16, BN_MAX);
-  p.n_tiles = (d->cout + p.BN - 1) / p.BN;
-  p.m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  p.BN = g.BN;
+  p.n_tiles = g.n_tiles;
+  p.m_tiles = g.m_tiles;
+  p.ksplit = conv_ksplit(d, g, d->stats != nullptr);
   p.chunk_bytes = BLOCK_M * p.CK * 2;
   p.b_bytes = p.BN * 128;
-  // one A plane holds the chunks of ONE k-block: 64 K-columns at most, fewer for small-K layers (C x taps < 64: the
-  // fast pathway's first stages) - sizing the stage by what is actually loaded leaves room for more stages / CTAs
-  const int chunks_per_kb = std::min(p.cps, p.n_chunks_padded);
-  p.a_plane_bytes = (uint32_t(chunks_per_kb) * p.chunk_bytes + 1023u) / 1024u * 1024u;
+  // one A plane holds the chunks of ONE k-block, 64 K-columns (zero chunks past the last filter tap)
+  p.a_plane_bytes = (uint32_t(p.cps) * p.chunk_bytes + 1023u) / 1024u * 1024u;
   p.a_total_bytes = p.a_plane_bytes * (d->nsplit == 3 ? 2 : 1);
   p.stage_bytes = p.a_total_bytes + p.b_bytes * (d->nsplit == 3 ? 2 : 1);
   p.stage_bytes = (p.stage_bytes + 1023) / 1024 * 1024;
@@ -429,6 +489,12 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
     case 32: p.a_layout = 4; p.a_sbo = 512; p.a_lbo = 16; break;
     case 16: p.a_layout = 6; p.a_sbo = 256; p.a_lbo = 16; break;
     default: p.a_layout = 0; p.a_sbo = 128; p.a_lbo = p.chunk_bytes; break;
+  }
+  for (int ks = 0; ks < KSTEPS; ++ks) {
+    const int k0 = ks * 16;
+    const uint32_t off = p.CK >= 16 ? uint32_t(k0 / p.CK) * p.chunk_bytes + uint32_t(k0 % p.CK) * 2u
+                                    : uint32_t(ks * 2) * p.chunk_bytes;  // CK = 8: two chunks, LBO apart
+    p.a_kstep[ks] = off >> 4;
   }
   p.acc_pitch = uint32_t(p.BN) + 4;  // 16-byte rows; the 4-float skew spreads the fragment stores over the banks
   const uint32_t acc_bytes = BLOCK_M * p.acc_pitch * 4;
@@ -451,9 +517,10 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   p.os_z = d->os_t;
   p.os_p = d->os_h;
   p.os_q = d->os_w;
-  p.accumulate = d->accumulate;
+  // split-K: the slices add into the output (zero-filled first by an overwrite) and the statistics come from y afterwards
+  p.accumulate = p.ksplit > 1 ? 2 : d->accumulate;
   p.epi_coalesced = 1;
-  p.stats = d->stats;
+  p.stats = p.ksplit > 1 ? nullptr : d->stats;
 
   // ---- tensor maps
   const int lower[3] = {d->low_w, d->low_h, d->low_t};
@@ -485,25 +552,38 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
     if (rc) return rc;
   }
 
-  const int total_tiles = p.m_tiles * p.n_tiles;
-  const int grid = std::min(total_tiles, g_num_sms * ctas_per_sm);
-  cudaError_t e;
+  if (p.ksplit > 1 && d->accumulate == 0) {
+    // the epilogue writes whole float4 groups: columns [cout, cout rounded up to 4) take zeros too
+    const size_t width = size_t((d->cout + 3) & ~3) * sizeof(float);
+    if (cudaMemset2DAsync(d->out, size_t(d->os_w) * sizeof(float), 0, width, size_t(p.M), stream) != cudaSuccess) {
+      set_error("sfb_conv_igemm: zero fill of the split-K output failed: %s", cudaGetErrorString(cudaGetLastError()));
+      return -20;
+    }
+  }
+  const int units = p.m_tiles * p.n_tiles * p.ksplit;
+  const int grid = std::min(units, g_num_sms * ctas_per_sm);
   {
     typedef void (*KernelFn)(const ConvParams);
-    static const KernelFn fns[2] = {conv_igemm_kernel<1>, conv_igemm_kernel<3>};
-    static bool attr[2] = {false, false};
-    const int a = d->nsplit == 3 ? 1 : 0;
-    if (!attr[a]) {
-      cudaFuncSetAttribute(fns[a], cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
-      attr[a] = true;
+#define SFB_CONV_FNS(S) {conv_igemm_kernel<S, 16>, conv_igemm_kernel<S, 32>, conv_igemm_kernel<S, 48>, \
+                         conv_igemm_kernel<S, 64>, conv_igemm_kernel<S, 80>, conv_igemm_kernel<S, 96>, \
+                         conv_igemm_kernel<S, 112>, conv_igemm_kernel<S, 128>}
+    static const KernelFn fns[2][BN_MAX / 16] = {SFB_CONV_FNS(1), SFB_CONV_FNS(3)};
+#undef SFB_CONV_FNS
+    static bool attr[2][BN_MAX / 16] = {};
+    const int a = d->nsplit == 3 ? 1 : 0, b = p.BN / 16 - 1;
+    if (!attr[a][b]) {
+      cudaFuncSetAttribute(fns[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
+      attr[a][b] = true;
     }
-    fns[a]<<<grid, CONV_THREADS, smem_bytes, stream>>>(p);
+    fns[a][b]<<<grid, CONV_THREADS, smem_bytes, stream>>>(p);
   }
-  e = cudaGetLastError();
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
-    set_error("sfb_conv_igemm launch failed: %s (grid=%d smem=%u stages=%d BN=%d CK=%d)", cudaGetErrorString(e), grid,
-              smem_bytes, p.stages, p.BN, p.CK);
+    set_error("sfb_conv_igemm launch failed: %s (grid=%d smem=%u stages=%d BN=%d CK=%d ksplit=%d)",
+              cudaGetErrorString(e), grid, smem_bytes, p.stages, p.BN, p.CK, p.ksplit);
     return -20;
   }
+  if (p.ksplit > 1 && d->stats != nullptr)  // [2][cout][sfb_conv_m_tiles(d)] partials of the finished output
+    return sfb_bn_split_stats(d->out, d->os_w, p.M, d->cout, 1, p.M, d->stats, stream);
   return 0;
 }

@@ -79,7 +79,23 @@ __device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t a, uint64_t b, 
       : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
-// Runtime N (a multiple of 16 up to MAXN) -> the matching instruction; d holds MAXN/2 registers.
+// Compile-time N -> the matching instruction; d holds N/2 registers.
+template <int N, int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma_m64n(float* d, uint64_t a, uint64_t b, uint32_t accumulate = 1u) {
+  static_assert(N % 16 == 0 && N >= 16 && N <= 128, "wgmma_m64n: N is a multiple of 16 up to 128");
+  if constexpr (N == 16) wgmma_m64n16<TA, TB>(d, a, b, accumulate);
+  else if constexpr (N == 32) wgmma_m64n32<TA, TB>(d, a, b, accumulate);
+  else if constexpr (N == 48) wgmma_m64n48<TA, TB>(d, a, b, accumulate);
+  else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, a, b, accumulate);
+  else if constexpr (N == 80) wgmma_m64n80<TA, TB>(d, a, b, accumulate);
+  else if constexpr (N == 96) wgmma_m64n96<TA, TB>(d, a, b, accumulate);
+  else if constexpr (N == 112) wgmma_m64n112<TA, TB>(d, a, b, accumulate);
+  else wgmma_m64n128<TA, TB>(d, a, b, accumulate);
+}
+
+// Runtime N (a multiple of 16 up to MAXN) -> the matching instruction; d holds MAXN/2 registers.  A call site with a
+// runtime N is a branch over eight wgmmas: ptxas serialises the wgmmas of the function around it (warning C7520), so
+// only kernels whose MMA issue is not their limit use it (conv_wgrad, gemm_batched, the W-shift stem's wgrad).
 template <int MAXN, int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16(float* d, int n, uint64_t a, uint64_t b, uint32_t accumulate) {
   switch (n) {

@@ -295,7 +295,8 @@ class ConvBN:
         ops.filter_pack(self.conv.weight, fm)
         c, cp = self.cout, self.cout_pad
         y = ctx.buf((self.name, "y"), (x.n, ot, oh, ow, cp))
-        m_tiles = ops.conv_m_tiles(x.n, geom)
+        strides = (ot * oh * ow * cp, oh * ow * cp, ow * cp, cp)
+        m_tiles = ops.conv_stats_tiles(x, fm, geom, y, strides, nsplit=ctx.nsplit)
         self.splits = self.bn.num_splits if (self.sub and ctx.training) else 1
         self.rows_per_clip = ot * oh * ow
         # (sub-batch BN: the epilogue's 128-row tiles cross clips, so the statistics are a separate pass)
@@ -303,7 +304,7 @@ class ConvBN:
             if (ctx.training and self.bn is not None and self.splits == 1) else None
         # (the epilogue stores whole float4 groups: columns [c, cp) receive the zero accumulators of filter rows
         # the TMA box reads out of bounds)
-        ops.conv_igemm(x, fm, geom, y, (ot * oh * ow * cp, oh * ow * cp, ow * cp, cp), stats=stats, nsplit=ctx.nsplit)
+        ops.conv_igemm(x, fm, geom, y, strides, stats=stats, nsplit=ctx.nsplit)
         self.x, self.geom, self.y = x, geom, y
         if self.bn is None:
             return y

@@ -235,6 +235,7 @@ _SIGNATURES = [
     ("sfb_abi_version", C.c_int, []),
     ("sfb_build_arch", C.c_char_p, []),
     ("sfb_conv_m_tiles", C.c_int64, [C.POINTER(ConvDesc)]),
+    ("sfb_conv_ksplit", C.c_int32, [C.POINTER(ConvDesc)]),
     ("sfb_conv_igemm", C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
     ("sfb_conv_wgrad", C.c_int, [C.POINTER(WgradDesc), C.c_void_p]),
     ("sfb_zero_f32_2d", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),

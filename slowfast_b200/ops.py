@@ -221,16 +221,14 @@ def fprop_geom(x: Planes, k, stride, pad, dil=(1, 1, 1)) -> ConvGeom:
 
 
 def conv_m_tiles(n: int, geom: ConvGeom) -> int:
+    """128-row output tiles of a convolution (the tile rows of an unsplit launch).  The BatchNorm partials of a launch
+    have ``conv_stats_tiles`` columns."""
     m = n * geom.out[0] * geom.out[1] * geom.out[2]
     return (m + 127) // 128
 
 
-def conv_igemm(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor, out_strides: Tuple[int, int, int, int],
-               out_offset: int = 0, accumulate: bool = False, stats: Optional[torch.Tensor] = None,
-               nsplit: int = 3) -> None:
-    """out view[n, z, p, q, :f.rows] (+)= conv(x, f).  ``out_strides`` are element strides for (n, t, h, w);
-    ``out_offset`` an element offset into ``out`` (channel slice / strided scatter)."""
-    lib = L.load()
+def _conv_desc(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor, out_strides: Tuple[int, int, int, int],
+               out_offset: int, accumulate, stats: Optional[torch.Tensor], nsplit: int):
     assert f.cols_pad == x.c, (f.cols_pad, x.c)
     d = L.ConvDesc()
     d.a_hi, d.a_lo = x.hi_ptr(), x.lo_ptr()
@@ -247,6 +245,32 @@ def conv_igemm(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor, out_s
     d.accumulate = int(accumulate)     # 0 overwrite, 1 read-modify-write, 2 fire-and-forget float atomics (same sums)
     d.stats = _ptr(stats)
     d.nsplit = nsplit
+    return d
+
+
+def conv_stats_tiles(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor,
+                     out_strides: Tuple[int, int, int, int], out_offset: int = 0, nsplit: int = 3) -> int:
+    """Columns of the BatchNorm partials ``[2][f.rows][columns]`` that ``conv_igemm`` writes for these arguments
+    with ``stats`` (a split-K launch takes them from its output afterwards, in its own row blocks)."""
+    d = _conv_desc(x, f, geom, out, out_strides, out_offset, 0, None, nsplit)
+    return int(L.load().sfb_conv_m_tiles(C.byref(d)))
+
+
+def conv_ksplit(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor, out_strides: Tuple[int, int, int, int],
+                out_offset: int = 0, accumulate=0, stats: Optional[torch.Tensor] = None, nsplit: int = 3) -> int:
+    """CTAs per output tile (split-K slices) that ``conv_igemm`` would use for these arguments; 1 = no split."""
+    d = _conv_desc(x, f, geom, out, out_strides, out_offset, accumulate, stats, nsplit)
+    return int(L.load().sfb_conv_ksplit(C.byref(d)))
+
+
+def conv_igemm(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor, out_strides: Tuple[int, int, int, int],
+               out_offset: int = 0, accumulate: bool = False, stats: Optional[torch.Tensor] = None,
+               nsplit: int = 3) -> None:
+    """out view[n, z, p, q, :f.rows] (+)= conv(x, f).  ``out_strides`` are element strides for (n, t, h, w);
+    ``out_offset`` an element offset into ``out`` (channel slice / strided scatter).  ``stats``: BatchNorm partials
+    ``[2][f.rows][conv_stats_tiles(...)]``."""
+    lib = L.load()
+    d = _conv_desc(x, f, geom, out, out_strides, out_offset, accumulate, stats, nsplit)
     L.check(lib.sfb_conv_igemm(C.byref(d), _stream()), "sfb_conv_igemm")
     _count()
 
