@@ -438,6 +438,12 @@ int sfb_small_linear_fwd(const float* x, const float* w, const float* b, float* 
                          void* stream);
 int sfb_small_linear_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx, int32_t m,
                          int32_t k, int32_t j, int32_t accumulate, void* stream);
+/* MLPHead layers (head_helper.py:147-196): _relu_fwd writes relu(x w^T + b); _relu_bwd is sfb_small_linear_bwd with the
+ * data gradient zeroed where x <= 0 (x = the output of the ReLU feeding this layer). */
+int sfb_small_linear_relu_fwd(const float* x, const float* w, const float* b, float* y, int32_t m, int32_t k, int32_t j,
+                              void* stream);
+int sfb_small_linear_relu_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx,
+                              int32_t m, int32_t k, int32_t j, int32_t accumulate, void* stream);
 int sfb_row_softmax(float* x, int32_t rows, int32_t cols, void* stream);
 /* Stochastic depth (common.py:46-59): out[i*b + s] = floor(keep_i + U)/keep_i for n_rates drop rates and b samples. */
 int sfb_droppath_scales(float* out, const float* rates, int32_t n_rates, int32_t b, uint64_t seed, uint64_t* step,
@@ -607,6 +613,17 @@ int sfb_flat_sgd(const void* chunks, int32_t n_chunks, const float* grad, float*
 int sfb_flat_adamw(const void* chunks, int32_t n_chunks, const float* grad, float* exp_avg, float* exp_avg_sq,
                    const float* group_lr, const float* group_wd, const float* gscale, float beta1, float beta2, float eps,
                    int64_t step, void* stream);
+
+/* MoCo key-encoder update (contrastive.py:152-166 _update_history), in place over paired parameter lists:
+ * key = fl(fl(query * c1) + fl(key * c2)) with c1 = float(1 - m), c2 = float(m), no FMA contraction - bitwise the
+ * reference's `q * (1 - m) + k * m` in fp32.  One chunk = up to sfb_momentum_chunk elements of one tensor pair. */
+typedef struct sfb_momentum_chunk {
+  float* key;          /* first element of this chunk inside the key-encoder parameter (updated in place) */
+  const float* query;  /* the same element of the query-encoder parameter */
+  int64_t count;       /* elements in the chunk */
+} sfb_momentum_chunk;
+int32_t sfb_momentum_chunk_size(void);
+int sfb_momentum_update(const void* chunks, int32_t n_chunks, float c1, float c2, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Device-side input pipeline head (SURVEY.md section 8f-3): uint8 clip [b, t, h, w, 3] (decoder layout) ->

@@ -63,7 +63,7 @@ _DEFAULTS = {
              "MEAN": [0.45, 0.45, 0.45], "STD": [0.225, 0.225, 0.225], "REVERSE_INPUT_CHANNEL": False},
     "DETECTION": {"ENABLE": False},
     "MULTIGRID": {"SHORT_CYCLE": False},
-    "CONTRASTIVE": {"NUM_MLP_LAYERS": 1, "PREDICTOR_DEPTHS": []},
+    "CONTRASTIVE": {"NUM_MLP_LAYERS": 1, "MLP_DIM": 2048, "BN_MLP": False, "BN_SYNC_MLP": False, "PREDICTOR_DEPTHS": []},
     "TRAIN": {"MIXED_PRECISION": False, "BATCH_SIZE": 64},
     "NUM_GPUS": 1,
     "RNG_SEED": 1,

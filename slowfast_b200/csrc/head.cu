@@ -129,6 +129,8 @@ __global__ void dropout_bwd_kernel(float* __restrict__ dx, const uint8_t* __rest
 }
 
 // y[m, k] = sum_j x[m, j] * w[k, j] + b[k]     one warp per output, fp32 (fma order: lane-strided then butterfly)
+// RELU: y = relu(...) (the hidden layers of MLPHead, head_helper.py:147-196)
+template <bool RELU>
 __global__ void small_linear_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                         const float* __restrict__ b, float* __restrict__ y, int m, int k, int j) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -141,7 +143,10 @@ __global__ void small_linear_fwd_kernel(const float* __restrict__ x, const float
   for (int t = lane; t < j; t += 32) acc = fmaf(xr[t], wr[t], acc);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (lane == 0) y[warp] = acc + (b ? b[ki] : 0.f);
+  if (lane == 0) {
+    const float v = acc + (b ? b[ki] : 0.f);
+    y[warp] = RELU ? (v < 0.f ? 0.f : v) : v;
+  }
 }
 // dw[k, j] (+)= sum_m dy[m, k] x[m, j];  db[k] (+)= sum_m dy[m, k]
 __global__ void small_linear_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x,
@@ -162,15 +167,18 @@ __global__ void small_linear_wgrad_kernel(const float* __restrict__ dy, const fl
   }
 }
 // dx[m, j] = sum_k dy[m, k] w[k, j]
+// RELU_MASK: dx[m, j] = 0 where x[m, j] <= 0 - x is the output of the ReLU in front of this layer, so this is
+// torch's threshold_backward(dx, x, 0) fused into the data gradient
+template <bool RELU_MASK>
 __global__ void small_linear_dgrad_kernel(const float* __restrict__ dy, const float* __restrict__ w,
-                                          float* __restrict__ dx, int m, int k, int j) {
+                                          float* __restrict__ dx, int m, int k, int j, const float* __restrict__ x) {
   const int64_t items = int64_t(m) * j;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
     const int ji = int(i % j);
     const int mi = int(i / j);
     float acc = 0.f;
     for (int ki = 0; ki < k; ++ki) acc = fmaf(dy[int64_t(mi) * k + ki], w[int64_t(ki) * j + ji], acc);
-    dx[i] = acc;
+    dx[i] = RELU_MASK ? (x[i] > 0.f ? acc : 0.f) : acc;
   }
 }
 // row softmax in place (eval-mode head activation), one warp per row
@@ -260,25 +268,44 @@ extern "C" int sfb_dropout_bwd(float* dx, const uint8_t* mask, int64_t nelem, fl
   SFB_HEAD_CHECK("sfb_dropout_bwd");
   return 0;
 }
-extern "C" int sfb_small_linear_fwd(const float* x, const float* w, const float* b, float* y, int32_t m, int32_t k,
-                                    int32_t j, void* stream) {
+template <bool RELU>
+static int small_linear_fwd(const float* x, const float* w, const float* b, float* y, int32_t m, int32_t k, int32_t j,
+                            void* stream, const char* name) {
   const int64_t threads = int64_t(m) * k * 32;
-  small_linear_fwd_kernel<<<int((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, w, b, y, m, k, j);
-  SFB_HEAD_CHECK("sfb_small_linear_fwd");
+  small_linear_fwd_kernel<RELU><<<int((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, w, b, y, m, k, j);
+  SFB_HEAD_CHECK(name);
   return 0;
 }
-extern "C" int sfb_small_linear_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx,
-                                    int32_t m, int32_t k, int32_t j, int32_t accumulate, void* stream) {
+template <bool RELU_MASK>
+static int small_linear_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx, int32_t m,
+                            int32_t k, int32_t j, int32_t accumulate, void* stream) {
   if (dw) {
     small_linear_wgrad_kernel<<<hd_grid(int64_t(k) * j, 256), 256, 0, (cudaStream_t)stream>>>(dy, x, dw, db, m, k, j,
                                                                                              accumulate);
     SFB_HEAD_CHECK("sfb_small_linear_bwd(wgrad)");
   }
   if (dx) {
-    small_linear_dgrad_kernel<<<hd_grid(int64_t(m) * j, 256), 256, 0, (cudaStream_t)stream>>>(dy, w, dx, m, k, j);
+    small_linear_dgrad_kernel<RELU_MASK><<<hd_grid(int64_t(m) * j, 256), 256, 0, (cudaStream_t)stream>>>(dy, w, dx, m,
+                                                                                                        k, j, x);
     SFB_HEAD_CHECK("sfb_small_linear_bwd(dgrad)");
   }
   return 0;
+}
+extern "C" int sfb_small_linear_fwd(const float* x, const float* w, const float* b, float* y, int32_t m, int32_t k,
+                                    int32_t j, void* stream) {
+  return small_linear_fwd<false>(x, w, b, y, m, k, j, stream, "sfb_small_linear_fwd");
+}
+extern "C" int sfb_small_linear_relu_fwd(const float* x, const float* w, const float* b, float* y, int32_t m, int32_t k,
+                                         int32_t j, void* stream) {
+  return small_linear_fwd<true>(x, w, b, y, m, k, j, stream, "sfb_small_linear_relu_fwd");
+}
+extern "C" int sfb_small_linear_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx,
+                                    int32_t m, int32_t k, int32_t j, int32_t accumulate, void* stream) {
+  return small_linear_bwd<false>(dy, x, w, dw, db, dx, m, k, j, accumulate, stream);
+}
+extern "C" int sfb_small_linear_relu_bwd(const float* dy, const float* x, const float* w, float* dw, float* db,
+                                         float* dx, int32_t m, int32_t k, int32_t j, int32_t accumulate, void* stream) {
+  return small_linear_bwd<true>(dy, x, w, dw, db, dx, m, k, j, accumulate, stream);
 }
 extern "C" int sfb_row_softmax(float* x, int32_t rows, int32_t cols, void* stream) {
   row_softmax_kernel<<<(rows * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(x, rows, cols);

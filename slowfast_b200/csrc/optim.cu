@@ -118,6 +118,21 @@ __global__ void __launch_bounds__(OPT_THREADS) flat_update_kernel(const OptChunk
   }
 }
 
+struct MomentumChunk {  // mirrors sfb_momentum_chunk
+  float* key;
+  const float* query;
+  int64_t count;
+};
+
+// key = fl(fl(q * c1) + fl(key * c2)): the explicit _rn intrinsics keep the compiler from contracting this into an FMA,
+// which would round once instead of three times and differ from the reference's three ATen kernels in the last bit
+__global__ void __launch_bounds__(OPT_THREADS) momentum_update_kernel(const MomentumChunk* __restrict__ chunks, float c1,
+                                                                      float c2) {
+  const MomentumChunk c = chunks[blockIdx.x];
+  for (int64_t i = threadIdx.x; i < c.count; i += OPT_THREADS)
+    c.key[i] = __fadd_rn(__fmul_rn(c.query[i], c1), __fmul_rn(c.key[i], c2));
+}
+
 #define SFB_OPT_CHECK(name)                                              \
   do {                                                                   \
     cudaError_t e_ = cudaGetLastError();                                 \
@@ -168,5 +183,15 @@ extern "C" int sfb_flat_adamw(const void* chunks, int32_t n_chunks, const float*
       (const sfb::OptChunk*)chunks, grad, exp_avg, exp_avg_sq, group_lr, group_wd, gscale, 0.f, 0.f, 0, 0, beta1, beta2,
       eps, float(bc1), float(sqrt(bc2)));
   SFB_OPT_CHECK("flat_adamw");
+  return 0;
+}
+
+extern "C" int32_t sfb_momentum_chunk_size(void) { return int32_t(sizeof(sfb::MomentumChunk)); }
+
+extern "C" int sfb_momentum_update(const void* chunks, int32_t n_chunks, float c1, float c2, void* stream) {
+  if (n_chunks <= 0) return 0;
+  sfb::momentum_update_kernel<<<n_chunks, sfb::OPT_THREADS, 0, (cudaStream_t)stream>>>(
+      (const sfb::MomentumChunk*)chunks, c1, c2);
+  SFB_OPT_CHECK("momentum_update");
   return 0;
 }

@@ -23,6 +23,7 @@ ENGINE_CLASSES: Dict[str, str] = {
     "MViT": "slowfast_b200.nets.mvit:B200MViT",
     "X3D": "slowfast_b200.nets.x3d:B200X3D",
     "MaskMViT": "slowfast_b200.nets.maskfeat:B200MaskMViT",
+    "ContrastiveModel": "slowfast_b200.nets.contrastive:B200ContrastiveModel",
 }
 
 

@@ -90,6 +90,12 @@ class OptChunk(C.Structure):
     _fields_ = [("param", C.c_void_p), ("offset", C.c_int64), ("count", C.c_int32), ("group", C.c_int32)]
 
 
+class MomentumChunk(C.Structure):
+    """Mirror of ``sfb_momentum_chunk``."""
+
+    _fields_ = [("key", C.c_void_p), ("query", C.c_void_p), ("count", C.c_int64)]
+
+
 class PoolDesc(C.Structure):
     _fields_ = [
         ("y", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p),
@@ -321,6 +327,10 @@ _SIGNATURES = [
                                        C.c_int32, C.c_void_p]),
     ("sfb_small_linear_bwd", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    ("sfb_small_linear_relu_fwd", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                            C.c_int32, C.c_void_p]),
+    ("sfb_small_linear_relu_bwd", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_row_softmax", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_droppath_scales", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
     ("sfb_stem_wgrad_direct", C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p] + [C.c_int32] * 10 +
@@ -354,6 +364,8 @@ _SIGNATURES = [
                                C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_flat_adamw", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_int64, C.c_void_p]),
+    ("sfb_momentum_chunk_size", C.c_int32, []),
+    ("sfb_momentum_update", C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_void_p]),
     ("sfb_hog_targets", C.c_int, [C.c_void_p] + [C.c_int32] * 9 + [C.c_void_p, C.c_void_p]),
     ("sfb_mae_max_tokens", C.c_int32, []),
     ("sfb_mae_random_masking", C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 5),

@@ -10,7 +10,8 @@ but executes with the library's kernels:
             planes of the next conv; the block tail is relu(x + c_bn) or relu(branch1_bn + c_bn) in ONE kernel
   lateral : FuseFastToSlow's conv+BN+ReLU writes straight into the channel slice of the slow pathway's next input
             (torch.cat never happens)
-  head    : global average pools -> dropout -> Linear
+  head    : global average pools -> dropout -> Linear, or the MLPHead of CONTRASTIVE.NUM_MLP_LAYERS > 1
+            (Linear -> ReLU -> ... -> Linear; bias + ReLU fused into each hidden layer's kernel)
 """
 from __future__ import annotations
 
@@ -370,23 +371,64 @@ class StageModule(Namespace):
         self.blocks(p)[i].run_backward()
 
 
-class BasicHeadModule(Namespace):
-    """ResNetBasicHead container: projection (+ inert pools / dropout / act)."""
+class MLPHeadModule(Namespace):
+    """MLPHead container (head_helper.py:147-196) without BN: projection = Sequential(Linear, ReLU, ..., Linear), every
+    Linear with a bias and ``xavier_init`` (c2_xavier_fill in init_resnet_weights)."""
 
-    def __init__(self, dim_in, num_classes, dropout_rate, act_func, pool_size=None):
+    def __init__(self, dim_in, dim_out, mlp_dim, num_layers):
         super().__init__()
+        layers = [nn.Linear(dim_in, mlp_dim, bias=True)]
+        for i in range(1, num_layers):
+            layers.append(nn.ReLU(inplace=True))
+            layers.append(nn.Linear(mlp_dim, dim_out if i == num_layers - 1 else mlp_dim, bias=True))
+        for m in layers:
+            if isinstance(m, nn.Linear):
+                m.xavier_init = True
+        self.projection = nn.Sequential(*layers)
+
+
+def _check_contrastive_head(contrastive) -> int:
+    """NUM_MLP_LAYERS of the head; the BN variants of MLPHead and the predictor heads are rejected by name."""
+    if contrastive is None:
+        return 1
+    if list(contrastive.get("PREDICTOR_DEPTHS", [])):
+        raise NotImplementedError("CONTRASTIVE.PREDICTOR_DEPTHS (predictor MLP heads) is not on the engine path")
+    layers = int(contrastive.get("NUM_MLP_LAYERS", 1))
+    if layers > 1:
+        for opt in ("BN_MLP", "BN_SYNC_MLP"):
+            if contrastive.get(opt, False):
+                raise NotImplementedError(f"CONTRASTIVE.{opt} (BatchNorm inside the MLP head) is not on the engine path")
+    return layers
+
+
+class BasicHeadModule(Namespace):
+    """ResNetBasicHead container: projection (+ inert pools / dropout / act).  ``contrastive`` (cfg.CONTRASTIVE)
+    selects the MLPHead projection when NUM_MLP_LAYERS > 1."""
+
+    def __init__(self, dim_in, num_classes, dropout_rate, act_func, pool_size=None, contrastive=None):
+        super().__init__()
+        mlp_layers = _check_contrastive_head(contrastive)
         # AvgPool3d(pool_size, stride=1) per pathway (None = adaptive 1x1x1, video_model_builder.py:398-416)
         self.pool_size = [None] * len(dim_in) if pool_size is None else [None if p is None else tuple(p) for p in pool_size]
         for p in range(len(dim_in)):
             self.add_module(f"pathway{p}_avgpool", nn.Identity())
         if dropout_rate > 0.0:
             self.dropout = nn.Dropout(dropout_rate)
-        self.projection = nn.Linear(sum(dim_in), num_classes, bias=True)
+        if mlp_layers == 1:
+            self.projection = nn.Linear(sum(dim_in), num_classes, bias=True)
+        else:
+            self.projection = MLPHeadModule(sum(dim_in), num_classes, int(contrastive.MLP_DIM), mlp_layers)
         if act_func not in ("softmax", "none"):
             raise NotImplementedError(f"head activation {act_func!r} is not on the engine path")
         self.act_func = act_func
         self.dropout_rate = dropout_rate
         self.dim_in = list(dim_in)
+
+    def linears(self) -> List[nn.Linear]:
+        """The projection's Linear layers in order; a ReLU sits between consecutive ones."""
+        if isinstance(self.projection, nn.Linear):
+            return [self.projection]
+        return [m for m in self.projection.projection if isinstance(m, nn.Linear)]
 
 
 def init_resnet_weights(model: nn.Module, fc_init_std, zero_init_final_bn, zero_init_final_conv) -> None:
@@ -407,7 +449,10 @@ def init_resnet_weights(model: nn.Module, fc_init_std, zero_init_final_bn, zero_
             if m.bias is not None:
                 m.bias.data.zero_()
         if isinstance(m, nn.Linear):
-            m.weight.data.normal_(mean=0.0, std=fc_init_std)
+            if getattr(m, "xavier_init", False):
+                nn.init.kaiming_uniform_(m.weight, a=1)  # c2_xavier_fill (MLPHead layers)
+            else:
+                m.weight.data.normal_(mean=0.0, std=fc_init_std)
             if m.bias is not None:
                 m.bias.data.zero_()
 
@@ -516,11 +561,10 @@ class _VideoResNetBase(nn.Module):
             for f, ps in zip(feats, head.pool_size):
                 ops.window_avgpool_fwd(f.planes, ps, pooled, col)
                 col += f.c
-            proj = ctx.buf(("head.proj.win",), (n * g, head.projection.out_features))
-            ops.small_linear_fwd(pooled, head.projection.weight, head.projection.bias, proj)
+            proj = self._head_mlp_forward(pooled, ("head.proj.win",))[-1]
             if head.act_func == "softmax":
                 ops.row_softmax(proj)
-            logits = torch.empty((n, head.projection.out_features), dtype=torch.float32, device=ctx.device)
+            logits = torch.empty((n, proj.shape[1]), dtype=torch.float32, device=ctx.device)
             ops.rows_group_mean(proj, logits, g)
             self._head_saved = None
             return logits
@@ -536,20 +580,41 @@ class _VideoResNetBase(nn.Module):
             if getattr(self, "_drop_counter", None) is None or self._drop_counter.device != ctx.device:
                 self._drop_counter = torch.zeros(1, dtype=torch.int64, device=ctx.device)
             ops.dropout_fwd(pooled, self._drop_mask, p, self._drop_seed, self._drop_counter)
-        logits = torch.empty((n, head.projection.out_features), dtype=torch.float32, device=ctx.device)
-        ops.small_linear_fwd(pooled, head.projection.weight, head.projection.bias, logits)
+        acts = self._head_mlp_forward(pooled, None)
+        logits = acts[-1]
         if not ctx.training and head.act_func == "softmax":
             ops.row_softmax(logits)
-        self._head_saved = (feats, pooled)
+        self._head_saved = (feats, acts[:-1])
         return logits
+
+    def _head_mlp_forward(self, x: torch.Tensor, key) -> List[torch.Tensor]:
+        """[x, hidden activations..., output] of the projection; the output is a fresh tensor when ``key`` is None
+        (the logits handed to autograd), else a buffer named by ``key``."""
+        ctx, lins = self.ctx, self.head.linears()
+        acts = [x]
+        for i, lin in enumerate(lins):
+            last = i == len(lins) - 1
+            shape = (x.shape[0], lin.out_features)
+            if not last:
+                y = ctx.buf(("head.mlp", i, key is not None), shape)
+            elif key is None:
+                y = torch.empty(shape, dtype=torch.float32, device=ctx.device)
+            else:
+                y = ctx.buf(key, shape)
+            ops.small_linear_fwd(acts[-1], lin.weight, lin.bias, y, relu=not last)
+            acts.append(y)
+        return acts
 
     def _head_backward(self, dlogits: torch.Tensor) -> None:
         ctx, head = self.ctx, self.head
-        feats, pooled = self._head_saved
-        n, dim = pooled.shape
-        dpooled = ctx.buf(("head.dpooled",), (n, dim))
-        proj = head.projection
-        ops.small_linear_bwd(dlogits, pooled, proj.weight, ctx.grad_of(proj.weight), ctx.grad_of(proj.bias), dpooled)
+        feats, acts = self._head_saved
+        dy = dlogits
+        for i in reversed(range(len(acts))):
+            lin, x = head.linears()[i], acts[i]
+            dx = ctx.buf(("head.dpooled",) if i == 0 else ("head.dmlp", i), x.shape)
+            ops.small_linear_bwd(dy, x, lin.weight, ctx.grad_of(lin.weight), ctx.grad_of(lin.bias), dx, relu_mask=i > 0)
+            dy = dx
+        dpooled = dy
         if self._drop_mask is not None:
             ops.dropout_bwd(dpooled, self._drop_mask, head.dropout_rate)
         col = 0
@@ -608,10 +673,10 @@ class B200SlowFast(_VideoResNetBase):
                     self.add_module(f"pathway{p}_pool", nn.Identity())
             prev = wd
         crop32 = cfg.DATA.TRAIN_CROP_SIZE // 32
-        pools = None if cfg.MULTIGRID.SHORT_CYCLE else [[cfg.DATA.NUM_FRAMES // alpha, crop32, crop32],
+        pools = None if cfg.MULTIGRID.SHORT_CYCLE or cfg.MODEL.MODEL_NAME == "ContrastiveModel" else [[cfg.DATA.NUM_FRAMES // alpha, crop32, crop32],
                                                          [cfg.DATA.NUM_FRAMES, crop32, crop32]]
         self.head = BasicHeadModule([wpg * 32, wpg * 32 // beta_inv], cfg.MODEL.NUM_CLASSES, cfg.MODEL.DROPOUT_RATE,
-                                    cfg.MODEL.HEAD_ACT, pool_size=pools)
+                                    cfg.MODEL.HEAD_ACT, pool_size=pools, contrastive=cfg.get("CONTRASTIVE"))
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN,
                             cfg.RESNET.ZERO_INIT_FINAL_CONV)
         self._ratio = ratio

@@ -52,9 +52,9 @@ class B200ResNet(_VideoResNetBase):
             prev = wd
         crop32 = cfg.DATA.TRAIN_CROP_SIZE // 32
         p1 = self._pool1
-        pools = None if cfg.MULTIGRID.SHORT_CYCLE else [[cfg.DATA.NUM_FRAMES // p1[0], crop32 // p1[1], crop32 // p1[2]]]
+        pools = None if cfg.MULTIGRID.SHORT_CYCLE or cfg.MODEL.MODEL_NAME == "ContrastiveModel" else [[cfg.DATA.NUM_FRAMES // p1[0], crop32 // p1[1], crop32 // p1[2]]]
         self.head = BasicHeadModule([wpg * 32], cfg.MODEL.NUM_CLASSES, cfg.MODEL.DROPOUT_RATE, cfg.MODEL.HEAD_ACT,
-                                    pool_size=pools)
+                                    pool_size=pools, contrastive=cfg.get("CONTRASTIVE"))
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN,
                             cfg.RESNET.ZERO_INIT_FINAL_CONV)
         self._init_graph_state()

@@ -468,22 +468,54 @@ def dropout_bwd(dx: torch.Tensor, mask: torch.Tensor, p: float) -> None:
     _count()
 
 
-def small_linear_fwd(x, w, b, y) -> None:
+def small_linear_fwd(x, w, b, y, relu: bool = False) -> None:
+    """y = x w^T + b; ``relu``: y = relu(x w^T + b) in the same pass."""
     lib = L.load()
     m, j = x.shape
     k = w.shape[0]
-    L.check(lib.sfb_small_linear_fwd(x.data_ptr(), w.data_ptr(), _ptr(b), y.data_ptr(), m, k, j, _stream()),
-            "sfb_small_linear_fwd")
+    name = "sfb_small_linear_relu_fwd" if relu else "sfb_small_linear_fwd"
+    L.check(getattr(lib, name)(x.data_ptr(), w.data_ptr(), _ptr(b), y.data_ptr(), m, k, j, _stream()), name)
     _count()
 
 
-def small_linear_bwd(dy, x, w, dw, db, dx, accumulate: bool = False) -> None:
+def small_linear_bwd(dy, x, w, dw, db, dx, accumulate: bool = False, relu_mask: bool = False) -> None:
+    """``relu_mask``: x is the output of a ReLU, and dx is the gradient at that ReLU's input (zero where x <= 0)."""
     lib = L.load()
     m, j = x.shape
     k = w.shape[0]
-    L.check(lib.sfb_small_linear_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), _ptr(dw), _ptr(db), _ptr(dx), m, k, j,
-                                     1 if accumulate else 0, _stream()), "sfb_small_linear_bwd")
+    name = "sfb_small_linear_relu_bwd" if relu_mask else "sfb_small_linear_bwd"
+    L.check(getattr(lib, name)(dy.data_ptr(), x.data_ptr(), w.data_ptr(), _ptr(dw), _ptr(db), _ptr(dx), m, k, j,
+                               1 if accumulate else 0, _stream()), name)
     _count((1 if dw is not None else 0) + (1 if dx is not None else 0))
+
+
+MOMENTUM_CHUNK = 8192  # elements per thread block of sfb_momentum_update
+
+
+def momentum_table(pairs: Sequence[Tuple[torch.Tensor, torch.Tensor]]) -> torch.Tensor:
+    """Device chunk table of sfb_momentum_update for (query, key) parameter pairs; it holds their current pointers."""
+    lib = L.load()
+    assert lib.sfb_momentum_chunk_size() == C.sizeof(L.MomentumChunk)
+    chunks = []
+    for q, k in pairs:
+        assert q.shape == k.shape and q.dtype == k.dtype == F32 and q.is_contiguous() and k.is_contiguous()
+        assert q.device == k.device and k.is_cuda
+        n = k.numel()
+        for c0 in range(0, n, MOMENTUM_CHUNK):
+            chunks.append((k.data_ptr() + 4 * c0, q.data_ptr() + 4 * c0, min(MOMENTUM_CHUNK, n - c0)))
+    arr = (L.MomentumChunk * len(chunks))()
+    for i, (kp, qp, cnt) in enumerate(chunks):
+        arr[i].key, arr[i].query, arr[i].count = kp, qp, cnt
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(pairs[0][1].device)
+
+
+def momentum_update(table: torch.Tensor, m: float) -> None:
+    """key = query * (1 - m) + key * m in place over every chunk of ``table`` (``momentum_table``).  The coefficients
+    are rounded to fp32 the way ATen rounds a Python scalar: 1 - m in double first."""
+    lib = L.load()
+    n = table.numel() // C.sizeof(L.MomentumChunk)
+    L.check(lib.sfb_momentum_update(table.data_ptr(), n, 1.0 - float(m), float(m), _stream()), "sfb_momentum_update")
+    _count()
 
 
 def row_softmax(x: torch.Tensor) -> None:
