@@ -97,6 +97,22 @@ typedef struct sfb_wgrad_desc {
 } sfb_wgrad_desc;
 
 int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream);
+
+/* How sfb_conv_wgrad runs a descriptor on a device with num_sms multiprocessors (no device needed to ask; the operand
+ * pointers are not read).  The reduction over output positions runs in k-blocks of 64 positions. */
+typedef struct sfb_wgrad_plan {
+  int32_t direct;       /* 1: the fp32 SIMT body takes the launch and the fields below are 0 */
+  int32_t transposed;   /* 0: tile rows are output channels, columns (tap, ci); 1: rows (tap, ci), columns output channels */
+  int32_t tile_rows;    /* 64 or 128 */
+  int32_t bn;           /* tile columns */
+  int32_t ck;           /* input channels per (tap, channel chunk) */
+  int32_t tiles;        /* dW tiles */
+  int32_t k_blocks;
+  int32_t slices;       /* CTAs per tile, each over a contiguous slice of the k-blocks (split-K, combined with red.add) */
+  int32_t ctas;         /* tiles * slices */
+} sfb_wgrad_plan;
+int sfb_conv_wgrad_plan(const sfb_wgrad_desc* d, int32_t num_sms, sfb_wgrad_plan* out);
+
 /* Layers with c*cout <= 512 and >= 32768 output positions (the fast pathway's narrow stages) take an fp32 SIMT body inside
  * sfb_conv_wgrad (csrc/conv_wgrad_direct.cu); enabled = 0 keeps every layer on the tensor-core kernel (the tests' reference for the SIMT body). */
 int sfb_set_wgrad_direct(int32_t enabled);

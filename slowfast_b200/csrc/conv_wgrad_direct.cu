@@ -152,16 +152,22 @@ static int g_wgd_sms = 0;
 
 void wgrad_direct_configure(int enabled) { g_wgd_enabled = enabled; }
 
-// Returns 1 and sets *rc_out when the direct kernel took the job.
-int wgrad_direct_try(const sfb_wgrad_desc* d, cudaStream_t stream, int* rc_out) {
-  if (!g_wgd_enabled) return 0;
+// Whether the direct kernel takes the job: narrow layers with many positions only (at most 8 channels on one side, at
+// most 14 (tap, 8 x 8 channel block) jobs); wider layers fill the tensor-core kernel's tiles.
+bool wgrad_direct_takes(const sfb_wgrad_desc* d) {
+  if (!g_wgd_enabled) return false;
   const int taps = d->kt * d->kh * d->kw;
   const int64_t M = int64_t(d->n) * d->out_t * d->out_h * d->out_w;
   const int jobs = taps * (d->c / 8) * (d->cout / 8);
-  // narrow layers with many positions only (at most 8 channels on one side, at most 14 (tap, 8 x 8 channel block) jobs):
-  // wider layers fill the tensor-core kernel's tiles
-  if (d->c * d->cout > 256 || std::min(d->c, d->cout) > 8 || jobs > 14 || M < 32768) return 0;
-  if (int64_t(d->n) * d->d * d->h * d->w * d->c_pitch >= (int64_t(1) << 31) || M * d->dy_pitch >= (int64_t(1) << 31)) return 0;
+  if (d->c * d->cout > 256 || std::min(d->c, d->cout) > 8 || jobs > 14 || M < 32768) return false;
+  return int64_t(d->n) * d->d * d->h * d->w * d->c_pitch < (int64_t(1) << 31) && M * d->dy_pitch < (int64_t(1) << 31);
+}
+
+// Returns 1 and sets *rc_out when the direct kernel took the job.
+int wgrad_direct_try(const sfb_wgrad_desc* d, cudaStream_t stream, int* rc_out) {
+  if (!wgrad_direct_takes(d)) return 0;
+  const int taps = d->kt * d->kh * d->kw;
+  const int jobs = taps * (d->c / 8) * (d->cout / 8);
   if (!g_wgd_sms) {
     int dev = 0;
     cudaGetDevice(&dev);

@@ -56,6 +56,13 @@ class WgradDesc(C.Structure):
     ]
 
 
+class WgradPlan(C.Structure):
+    """Mirror of ``sfb_wgrad_plan``."""
+
+    _fields_ = [(name, C.c_int32) for name in ("direct", "transposed", "tile_rows", "bn", "ck", "tiles", "k_blocks",
+                                               "slices", "ctas")]
+
+
 class BnApplyDesc(C.Structure):
     _fields_ = [
         ("y", C.c_void_p), ("y_pitch", C.c_int64), ("scale", C.c_void_p), ("shift", C.c_void_p),
@@ -244,6 +251,7 @@ _SIGNATURES = [
     ("sfb_conv_ksplit", C.c_int32, [C.POINTER(ConvDesc)]),
     ("sfb_conv_igemm", C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
     ("sfb_conv_wgrad", C.c_int, [C.POINTER(WgradDesc), C.c_void_p]),
+    ("sfb_conv_wgrad_plan", C.c_int, [C.POINTER(WgradDesc), C.c_int32, C.POINTER(WgradPlan)]),
     ("sfb_zero_f32_2d", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]),
     ("sfb_add_f32_2d", C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]),
     ("sfb_split_planes", C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,

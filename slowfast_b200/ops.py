@@ -275,9 +275,7 @@ def conv_igemm(x: Planes, f: FilterMat, geom: ConvGeom, out: torch.Tensor, out_s
     _count()
 
 
-def conv_wgrad(x: Planes, dy: Planes, geom: ConvGeom, dwm: torch.Tensor, nsplit: int = 3) -> None:
-    """dwm[cout, taps*x.c] += dY^T * im2col(x).  dy must be dense rows [M, cout] (its pitch may exceed cout)."""
-    lib = L.load()
+def _wgrad_desc(x: Planes, dy: Planes, geom: ConvGeom, dwm: Optional[torch.Tensor], nsplit: int):
     d = L.WgradDesc()
     d.x_hi, d.x_lo = x.hi_ptr(), x.lo_ptr()
     d.n, d.d, d.h, d.w, d.c, d.c_pitch = x.n, x.t, x.h, x.w, x.c, x.pitch
@@ -289,8 +287,26 @@ def conv_wgrad(x: Planes, dy: Planes, geom: ConvGeom, dwm: torch.Tensor, nsplit:
     d.low_t, d.low_h, d.low_w = geom.low
     d.out_t, d.out_h, d.out_w = geom.out
     assert dy.rows == x.n * geom.out[0] * geom.out[1] * geom.out[2]
-    d.dw = dwm.data_ptr()
+    d.dw = _ptr(dwm)
     d.nsplit = nsplit
+    return d
+
+
+def conv_wgrad_plan(x: Planes, dy: Planes, geom: ConvGeom, nsplit: int = 3, num_sms: Optional[int] = None):
+    """The tiling ``conv_wgrad`` uses for these operands on a device with ``num_sms`` multiprocessors (default: the
+    current device's).  Needs no device when ``num_sms`` is given."""
+    if num_sms is None:
+        num_sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    plan = L.WgradPlan()
+    L.check(L.load().sfb_conv_wgrad_plan(C.byref(_wgrad_desc(x, dy, geom, None, nsplit)), num_sms, C.byref(plan)),
+            "sfb_conv_wgrad_plan")
+    return plan
+
+
+def conv_wgrad(x: Planes, dy: Planes, geom: ConvGeom, dwm: torch.Tensor, nsplit: int = 3) -> None:
+    """dwm[cout, taps*x.c] += dY^T * im2col(x).  dy must be dense rows [M, cout] (its pitch may exceed cout)."""
+    lib = L.load()
+    d = _wgrad_desc(x, dy, geom, dwm, nsplit)
     L.check(lib.sfb_conv_wgrad(C.byref(d), _stream()), "sfb_conv_wgrad")
     _count()
 
