@@ -30,10 +30,11 @@ constexpr int ST_SEG_STRIDE = 2304;   // 136 granules (128 pixels + halo) rounde
 constexpr int ST_SEG_PIX = 136;
 constexpr int ST_WSEG_STRIDE = 1152;  // wgrad: 72 granules (64 pixels + halo)
 constexpr int ST_WSEG_PIX = 72;
-constexpr int ST_MMA_WARPS = 8;   // fprop: two warpgroups of 64 pixels; wgrad: the first warpgroup only (64 co rows)
+constexpr int ST_MMA_WARPS = 8;   // fprop: two warpgroups of 64 pixels; wgrad: two warpgroups, half the positions each
 constexpr int ST_FPROP_THREADS = 32 * (ST_MMA_WARPS + 1 + 4);
-constexpr int ST_WGRAD_THREADS = 32 * (4 + 1);
-constexpr int ST_BN_MAX = 128;
+constexpr int ST_WGRAD_THREADS = 32 * (ST_MMA_WARPS + 1);
+constexpr int ST_BN_MAX = 64;     // the widest stem of the supported models (StemConvBN.supported)
+constexpr int ST_KSTEPS = 4;      // k16 steps per k-block: 64 K elements = pps pairs x KW taps x 8 slots
 constexpr int ST_NPG_MAX = 4;     // wgrad: pairs per CTA, each a <= 32-column accumulator
 
 __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* tm, uint64_t* bar, int32_t c0, int32_t c1,
@@ -59,6 +60,7 @@ struct StemParams {
   int st, sh, pt, ph, pw;
   int KT, KH, KW;       // KW = folded taps (2 or 4)
   int pairs, pps, k_blocks;
+  uint32_t a_kstep[ST_KSTEPS];  // fprop: start of k-step ks's A columns in the stage (pair segment + tap), 16-byte units
   int cout, BN, w_tiles, m_tiles;
   int stages;
   uint32_t stage_bytes, a_plane_bytes, b_bytes;
@@ -71,7 +73,10 @@ struct StemParams {
 };
 
 // ------------------------------------------------------------------------------------------------ fprop
-template <int NSPLIT>
+// Every k-block is ST_KSTEPS k16 steps over pps pairs (the producer zero-fills the pairs past the last one, whose filter
+// columns the weight map's bounds also zero) and the tile width is the template's BN, so a k-block's wgmmas are
+// straight-line code behind one warpgroup arrive.
+template <int NSPLIT, int BN>
 __global__ void __launch_bounds__(ST_FPROP_THREADS, 1) stem_fprop_kernel(const __grid_constant__ StemParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -94,7 +99,6 @@ __global__ void __launch_bounds__(ST_FPROP_THREADS, 1) stem_fprop_kernel(const _
   __syncthreads();
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
   const int total_tiles = p.m_tiles;
-  const int ksteps_per_pair = p.KW / 2;
 
   if (warp == ST_MMA_WARPS) {
     int stage = 0;
@@ -111,13 +115,13 @@ __global__ void __launch_bounds__(ST_FPROP_THREADS, 1) stem_fprop_kernel(const _
         mbar_wait(&empty[stage], phase ^ 1);
         if (elect_one()) {
           const int pair0 = kb * p.pps;
-          const int nq = min(p.pps, p.pairs - pair0);
-          mbar_expect_tx(&full[stage], (uint32_t(nq) * ST_SEG_PIX * 16u + p.b_bytes) * NP);
+          mbar_expect_tx(&full[stage], (uint32_t(p.pps) * ST_SEG_PIX * 16u + p.b_bytes) * NP);
           uint8_t* st = smem + size_t(stage) * p.stage_bytes;
-          for (int qq = 0; qq < nq; ++qq) {
+          for (int qq = 0; qq < p.pps; ++qq) {
             const int pair = pair0 + qq;
             const int kt = pair / p.KH, kh = pair - kt * p.KH;
-            const int h = oh * p.sh - p.ph + kh, t = ot * p.st - p.pt + kt;
+            // a pair past the last one reads row -1: entirely out of bounds, so the unit fills it with zeros
+            const int h = pair < p.pairs ? oh * p.sh - p.ph + kh : -1, t = ot * p.st - p.pt + kt;
             for (uint32_t pl = 0; pl < NP; ++pl)
               tma_load_5d(st + pl * p.a_plane_bytes + qq * ST_SEG_STRIDE, &p.tmX[pl], &full[stage], 0, w0, h, t, n);
           }
@@ -134,36 +138,33 @@ __global__ void __launch_bounds__(ST_FPROP_THREADS, 1) stem_fprop_kernel(const _
   } else if (warp < ST_MMA_WARPS) {
     // MMA warpgroup g: pixels 64g .. 64g+63 of the tile = 8 more 128-byte row groups into each segment
     const int g = warp >> 2;
-    float d[ST_BN_MAX / 2];
+    float d[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       int held = -1;
       for (int kb = 0; kb < p.k_blocks; ++kb) {
         mbar_wait(&full[stage], phase);
         wgmma_fence();
-        const int nq = min(p.pps, p.pairs - kb * p.pps);
         const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 1024u;
         const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + NP * p.a_plane_bytes;
-        int kstep = 0;
-        for (int qq = 0; qq < nq; ++qq) {
-          for (int j = 0; j < ksteps_per_pair; ++j, ++kstep) {
-            // A: rows = pixels 16 B apart (8-row groups 128 B), the two K chunks are taps 2j and 2j+1 = +16 B
-            const uint32_t aa = a_base + qq * ST_SEG_STRIDE + uint32_t(2 * j) * 16u;
-            const uint64_t a_hi = make_smem_desc(aa, 16, 128, 0);
-            const uint64_t b_hi = make_smem_desc(b_base + uint32_t(kstep) * 32u, 16, 1024, 2);
-            const uint32_t acc_flag = (kb | kstep) != 0 ? 1u : 0u;
-            if (NSPLIT == 3) {
-              const uint64_t a_lo = make_smem_desc(aa + p.a_plane_bytes, 16, 128, 0);
-              const uint64_t b_lo = make_smem_desc(b_base + p.b_bytes + uint32_t(kstep) * 32u, 16, 1024, 2);
-              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_lo, b_hi, acc_flag);
-              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_hi, b_lo, 1u);
-              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, 1u);
-            } else {
-              wgmma_bf16<ST_BN_MAX, 0, 0>(d, p.BN, a_hi, b_hi, acc_flag);
-            }
+        // A: rows = pixels 16 B apart (8-row groups 128 B); a k-step's two K chunks are two taps of one pair, 16 B apart
+        const uint64_t a_hi0 = make_smem_desc(a_base, 16, 128, 0);
+        const uint64_t b_hi0 = make_smem_desc(b_base, 16, 1024, 2);
+#pragma unroll
+        for (int ks = 0; ks < ST_KSTEPS; ++ks) {
+          const uint64_t a_hi = a_hi0 + p.a_kstep[ks];
+          const uint64_t b_hi = b_hi0 + uint64_t(ks * 2);  // 32 bytes = 16 bf16 of the 128-byte swizzled rows
+          if (NSPLIT == 3) {
+            const uint64_t a_lo = a_hi + (p.a_plane_bytes >> 4);
+            const uint64_t b_lo = b_hi + (p.b_bytes >> 4);
+            wgmma_m64n<BN>(d, a_lo, b_hi);
+            wgmma_m64n<BN>(d, a_hi, b_lo);
           }
+          wgmma_m64n<BN>(d, a_hi, b_hi);
         }
         wgmma_commit();
         wgmma_wait<1>();
@@ -177,7 +178,7 @@ __global__ void __launch_bounds__(ST_FPROP_THREADS, 1) stem_fprop_kernel(const _
       wgmma_wait<0>();
       mbar_arrive(&empty[held]);
       mbar_wait(tempty, (it & 1) ^ 1);
-      acc_store<ST_BN_MAX>(d, p.BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
+      acc_store<BN>(d, BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
       mbar_arrive(tfull);
     }
   } else {
@@ -287,7 +288,11 @@ __device__ __forceinline__ void st_red_add_v4(float* addr, float a, float b, flo
                : "memory");
 }
 
-template <int NSPLIT>
+// CTA = (group of NPG pairs, split of the (row, 64-pixel chunk) k-blocks).  Both MMA warpgroups hold the whole
+// [64 co, NPG x KW*8] tile: warpgroup g takes k-steps 2g, 2g+1 (positions 32g .. 32g+31) of every stage, and the
+// epilogue adds warpgroup 1's tile to warpgroup 0's through shared memory.  NPG and the pair width KW*8 are
+// compile-time, so a stage's wgmmas are straight-line code; pairs past the last one are zero-filled and not stored.
+template <int NSPLIT, int KWF, int NPG>
 __global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const __grid_constant__ StemParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -295,19 +300,20 @@ __global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const _
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + ST_MAX_STAGES;
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
+  constexpr int NC = KWF * 8;             // accumulator columns per pair
+  constexpr int NACC = NPG * NC / 2;      // accumulator registers per thread
 
   const int split = blockIdx.x % p.splits;
-  const int grp = blockIdx.x / p.splits;  // pair group (co_tiles == 1: cout <= 128)
+  const int grp = blockIdx.x / p.splits;  // pair group (co_tiles == 1: cout <= 64)
   const int kb0 = split * p.kb_per_split;
   const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-  const int pair_base = grp * p.npg;
-  const int npairs = min(p.npg, p.pairs - pair_base);
-  const int ncols_pair = p.KW * 8;
+  const int pair_base = grp * NPG;
+  const int npairs = min(NPG, p.pairs - pair_base);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 128);
+      mbar_init(&empty[s], 32 * ST_MMA_WARPS);
     }
     fence_mbar_init();
     fence_proxy_async_smem();
@@ -315,8 +321,8 @@ __global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const _
   __syncthreads();
   const uint32_t dy_plane = 8192;  // one [64 pos][64 co] box = the 64 rows of the MMA
 
-  if (kb1 > kb0 && npairs > 0) {
-    if (warp == 4) {
+  if (kb1 > kb0) {
+    if (warp == ST_MMA_WARPS) {
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
@@ -330,16 +336,17 @@ __global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const _
           const int ot = r % p.OT;
           const int n = r / p.OT;
           const int ow0 = wc * 64;
-          mbar_expect_tx(&full[stage], (dy_plane + uint32_t(npairs) * ST_WSEG_PIX * 16u) * NP);
+          mbar_expect_tx(&full[stage], (dy_plane + uint32_t(NPG) * ST_WSEG_PIX * 16u) * NP);
           uint8_t* st = smem + size_t(stage) * p.stage_bytes;
           for (uint32_t pl = 0; pl < NP; ++pl) {
             tma_load_3d_(st + pl * dy_plane, &p.tmB[pl], &full[stage], 0, ow0, rowi);
             uint8_t* xb = st + NP * dy_plane + pl * p.a_plane_bytes;
-            for (int j = 0; j < npairs; ++j) {
+            for (int j = 0; j < NPG; ++j) {
               const int pair = pair_base + j;
               const int kt = pair / p.KH, kh = pair - kt * p.KH;
-              tma_load_5d(xb + j * ST_WSEG_STRIDE, &p.tmX[pl], &full[stage], 0, ow0 - p.pw, oh * p.sh - p.ph + kh,
-                          ot * p.st - p.pt + kt, n);
+              // a pair past the last one reads row -1: entirely out of bounds, so the unit fills it with zeros
+              const int h = j < npairs ? oh * p.sh - p.ph + kh : -1;
+              tma_load_5d(xb + j * ST_WSEG_STRIDE, &p.tmX[pl], &full[stage], 0, ow0 - p.pw, h, ot * p.st - p.pt + kt, n);
             }
           }
         }
@@ -350,37 +357,34 @@ __global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const _
         }
       }
     } else {
-      // one MMA warpgroup: accumulator of pair j = registers d[16 j ..] (ncols_pair <= 32 columns)
-      float d[ST_NPG_MAX * 16];
+      // accumulator of pair j = registers d[j NC/2 ..]
+      const int g = warp >> 2;
+      float d[NACC];
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) d[i] = 0.f;
       int stage = 0;
       uint32_t phase = 0;
       int held = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full[stage], phase);
         wgmma_fence();
-        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-        const uint32_t x_base = a_base + NP * dy_plane;
+        // A' = dY (MN-major, 128B swizzle), 16 positions = 2048 B per k-step; B' = segment: tap atoms 16 B apart,
+        // positions 16 B apart, 8-position groups 128 B apart (no swizzle)
+        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 2u * 2048u;
+        const uint32_t x_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + NP * dy_plane + uint32_t(g) * 2u * 256u;
 #pragma unroll
-        for (int j = 0; j < ST_NPG_MAX; ++j) {
-          if (j < npairs) {
+        for (int j = 0; j < NPG; ++j) {
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              // A' = dY (MN-major, 128B swizzle); B' = segment: tap atoms 16 B apart, positions 16 B apart,
-              // 8-position groups 128 B apart (no swizzle)
-              const uint64_t a_hi = make_smem_desc(a_base + ks * 2048, 0, 1024, 2);
-              const uint64_t b_hi = make_smem_desc(x_base + j * ST_WSEG_STRIDE + ks * 256, 128, 16, 0);
-              const uint32_t acc_flag = (kb != kb0 || ks != 0) ? 1u : 0u;
-              if (NSPLIT == 3) {
-                const uint64_t a_lo = make_smem_desc(a_base + dy_plane + ks * 2048, 0, 1024, 2);
-                const uint64_t b_lo =
-                    make_smem_desc(x_base + p.a_plane_bytes + j * ST_WSEG_STRIDE + ks * 256, 128, 16, 0);
-                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_lo, b_hi, acc_flag);
-                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_hi, b_lo, 1u);
-                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_hi, b_hi, 1u);
-              } else {
-                wgmma_bf16<32, 1, 1>(d + 16 * j, ncols_pair, a_hi, b_hi, acc_flag);
-              }
+          for (int ks = 0; ks < 2; ++ks) {
+            const uint64_t a_hi = make_smem_desc(a_base + ks * 2048, 0, 1024, 2);
+            const uint64_t b_hi = make_smem_desc(x_base + j * ST_WSEG_STRIDE + ks * 256, 128, 16, 0);
+            if (NSPLIT == 3) {
+              const uint64_t a_lo = a_hi + (dy_plane >> 4);
+              const uint64_t b_lo = b_hi + (p.a_plane_bytes >> 4);
+              wgmma_m64n<NC, 1, 1>(d + j * (NC / 2), a_lo, b_hi);
+              wgmma_m64n<NC, 1, 1>(d + j * (NC / 2), a_hi, b_lo);
             }
+            wgmma_m64n<NC, 1, 1>(d + j * (NC / 2), a_hi, b_hi);
           }
         }
         wgmma_commit();
@@ -393,22 +397,34 @@ __global__ void __launch_bounds__(ST_WGRAD_THREADS, 1) stem_wgrad_kernel(const _
         }
       }
       wgmma_wait<0>();
-      // epilogue straight from the fragments: rows co = 16 w + lane/4 (+8), columns 8 c + 2 (lane % 4) (+1)
-      const int co0 = warp * 16 + (lane >> 2);
-      const int col_base = pair_base * ncols_pair;
+      // warpgroup 1 hands its tile to warpgroup 0 through the stages (every load has landed and both warpgroups' MMAs
+      // are done once both pass the first barrier); the same thread of the other warpgroup holds the same elements
+      float* red = reinterpret_cast<float*>(smem);
+      const int t = threadIdx.x & 127;
+      named_bar_sync(1, 32 * ST_MMA_WARPS);
+      if (g == 1) {
 #pragma unroll
-      for (int j = 0; j < ST_NPG_MAX; ++j) {
-        if (j < npairs) {
+        for (int i = 0; i < NACC; ++i) red[i * 128 + t] = d[i];
+      }
+      named_bar_sync(1, 32 * ST_MMA_WARPS);
+      if (g == 0) {
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            if (8 * c < ncols_pair) {
+        for (int i = 0; i < NACC; ++i) d[i] += red[i * 128 + t];
+        // epilogue straight from the fragments: rows co = 16 w + lane/4 (+8), columns 8 c + 2 (lane % 4) (+1)
+        const int co0 = warp * 16 + (lane >> 2);
+        const int col_base = pair_base * NC;
+#pragma unroll
+        for (int j = 0; j < NPG; ++j) {
+          if (j < npairs) {
+#pragma unroll
+            for (int c = 0; c < NC / 8; ++c) {
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const int co = co0 + 8 * h;
                 if (co < p.cout) {
-                  float* dst = p.dw + size_t(co) * p.ktot + col_base + j * ncols_pair + 8 * c + 2 * (lane & 3);
-                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[16 * j + 4 * c + 2 * h]),
-                               "f"(d[16 * j + 4 * c + 2 * h + 1]) : "memory");
+                  float* dst = p.dw + size_t(co) * p.ktot + col_base + j * NC + 8 * c + 2 * (lane & 3);
+                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(d[j * (NC / 2) + 4 * c + 2 * h]),
+                               "f"(d[j * (NC / 2) + 4 * c + 2 * h + 1]) : "memory");
                 }
               }
             }
@@ -621,6 +637,11 @@ extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
   const int np = d->nsplit == 3 ? 2 : 1;
   p.pps = 64 / (d->kwf * 8);
   p.k_blocks = (p.pairs + p.pps - 1) / p.pps;
+  for (int ks = 0; ks < ST_KSTEPS; ++ks) {
+    const int per_pair = d->kwf / 2;  // k-steps per pair: taps 2j and 2j+1 of pair qq
+    const int qq = ks / per_pair, j = ks % per_pair;
+    p.a_kstep[ks] = uint32_t(qq * ST_SEG_STRIDE + 2 * j * 16) >> 4;
+  }
   p.BN = (d->cout + 15) / 16 * 16;
   if (p.BN > ST_BN_MAX) {
     set_error("sfb_stem_fprop: cout=%d > %d not supported", d->cout, ST_BN_MAX);
@@ -653,14 +674,19 @@ extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
     if (rc) return rc;
   }
   const int grid = std::min(p.m_tiles, st_sms);
-  if (d->nsplit == 3) {
-    static bool a = false;
-    if (!a) { cudaFuncSetAttribute(stem_fprop_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_fprop_kernel<3><<<grid, ST_FPROP_THREADS, smem_bytes, stream>>>(p);
-  } else {
-    static bool a = false;
-    if (!a) { cudaFuncSetAttribute(stem_fprop_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_fprop_kernel<1><<<grid, ST_FPROP_THREADS, smem_bytes, stream>>>(p);
+  {
+    typedef void (*KernelFn)(const StemParams);
+#define SFB_STEM_FNS(S) {stem_fprop_kernel<S, 16>, stem_fprop_kernel<S, 32>, stem_fprop_kernel<S, 48>, \
+                         stem_fprop_kernel<S, 64>}
+    static const KernelFn fns[2][ST_BN_MAX / 16] = {SFB_STEM_FNS(1), SFB_STEM_FNS(3)};
+#undef SFB_STEM_FNS
+    static bool attr[2][ST_BN_MAX / 16] = {};
+    const int a = d->nsplit == 3 ? 1 : 0, b = p.BN / 16 - 1;
+    if (!attr[a][b]) {
+      cudaFuncSetAttribute(fns[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem);
+      attr[a][b] = true;
+    }
+    fns[a][b]<<<grid, ST_FPROP_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -687,7 +713,8 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
     set_error("sfb_stem_wgrad: %d folded W taps > 4 not supported", d->kwf);
     return -10;
   }
-  p.npg = std::min(p.pairs, ST_NPG_MAX);
+  // 3 or 4 pairs per CTA, whichever issues fewer padded pairs (4 on a tie: fewer groups re-read dY)
+  p.npg = ((p.pairs + 2) / 3) * 3 < ((p.pairs + 3) / 4) * 4 ? 3 : ST_NPG_MAX;
   p.n_groups = (p.pairs + p.npg - 1) / p.npg;
   p.w_chunks = (d->out_w + 63) / 64;
   p.kb_total = d->n * d->out_t * d->out_h * p.w_chunks;
@@ -700,7 +727,8 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
   // keep the X planes contiguous after the dY planes: offsets used by the kernel are NP*8192 + pl*a_plane_bytes
   p.stages = std::min<int>(ST_MAX_STAGES, (uint32_t(st_smem) - 1024 - 256) / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.kb_per_split));
-  p.off_bars = p.stages * p.stage_bytes;
+  // the epilogue passes one warpgroup's [64 co][npg x kwf*8] fp32 tile through the drained stages
+  p.off_bars = std::max(p.stages * p.stage_bytes, uint32_t(64 * p.npg * ncols_pair * 4));
   const uint32_t smem_bytes = p.off_bars + 256 + 1024;
   p.dw = d->dwm;
   const int64_t rows = int64_t(d->n) * d->out_t * d->out_h;
@@ -711,14 +739,19 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
     if (rc) return rc;
   }
   const int grid = p.n_groups * p.splits;
-  if (d->nsplit == 3) {
-    static bool a = false;
-    if (!a) { cudaFuncSetAttribute(stem_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_wgrad_kernel<3><<<grid, ST_WGRAD_THREADS, smem_bytes, stream>>>(p);
-  } else {
-    static bool a = false;
-    if (!a) { cudaFuncSetAttribute(stem_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem); a = true; }
-    stem_wgrad_kernel<1><<<grid, ST_WGRAD_THREADS, smem_bytes, stream>>>(p);
+  {
+    typedef void (*KernelFn)(const StemParams);
+#define SFB_STEM_FNS(S) {stem_wgrad_kernel<S, 2, 3>, stem_wgrad_kernel<S, 2, 4>, stem_wgrad_kernel<S, 4, 3>, \
+                         stem_wgrad_kernel<S, 4, 4>}
+    static const KernelFn fns[2][4] = {SFB_STEM_FNS(1), SFB_STEM_FNS(3)};
+#undef SFB_STEM_FNS
+    static bool attr[2][4] = {};
+    const int a = d->nsplit == 3 ? 1 : 0, b = (d->kwf / 2 - 1) * 2 + (p.npg - 3);
+    if (!attr[a][b]) {
+      cudaFuncSetAttribute(fns[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, st_smem);
+      attr[a][b] = true;
+    }
+    fns[a][b]<<<grid, ST_WGRAD_THREADS, smem_bytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

@@ -22,8 +22,8 @@
 // into two resident groups of 11 input rows: one stage = (8 output rows, input frame t) is loaded once per kt and
 // feeds 7 x 6 MMAs (x3 split products).
 //
-// wgrad runs the same operands with the reduction over the row index: dZ[(kt sel, j, co), g*8+s] for the 4 (or 3) H taps
-// of one parity class in registers (2 x 64 rows: two T taps share one pass over the clip), then
+// wgrad runs the same operands with the reduction over the row index: dZ[(j, co), g*8+s] of one T tap for the 4 (or 3) H
+// taps of one parity class in registers (one warpgroup per H tap), then
 // dWf[co][kt][kh][kw'][s] = sum_j dZ[(j,co), (j + kw')*8 + s] is folded into the W-shift gradient matrix by atomics.
 #include <algorithm>
 #include <cstdint>
@@ -39,8 +39,9 @@ namespace sfb {
 constexpr int T8_ROWS = 8;     // output rows per tile
 constexpr int T8_SLOTS = 11;   // resident input rows per parity class: 8 + 3
 constexpr int T8_KSTEPS = 6;   // 12 granules of 8 slots = 96 K elements per (kt, kh)
+constexpr int T8_MAX_STAGES = 4;
 constexpr int T8_FPROP_THREADS = 32 * (8 + 1);    // two MMA warpgroups (rows 0..63 / 64..127) + producer warp
-constexpr int T8_WGRAD_THREADS = 32 * (16 + 1);   // four MMA warpgroups (row half x tap pair) + producer warp
+constexpr int T8_WGRAD_THREADS = 32 * (16 + 1);   // four MMA warpgroups (one H tap each) + producer warp
 
 __device__ __forceinline__ void t8_tma_5d(void* smem, const CUtensorMap* tm, uint64_t* bar, int32_t c0, int32_t c1,
                                           int32_t c2, int32_t c3, int32_t c4) {
@@ -56,6 +57,7 @@ struct Stem8Params {
   CUtensorMap tmB[2];   // fprop: Z planes [kt*G rows, 64 el];  wgrad: dY [64 el, OW/8, OH, OT, N]
   int N, T, OT, OH, OW, MR;   // MR = OW/8 + 1 granule rows per input row and array
   int KT, pt, bands, tiles;
+  int stages;
   uint32_t ab;            // bytes of one R_j array in shared memory (11 slots, 128-byte multiple)
   uint32_t a_plane, a_bytes, b_plane, stage_bytes, off_red, off_bars;
   uint32_t zg;            // granules per kt in Z (7*12 + 8)
@@ -64,7 +66,7 @@ struct Stem8Params {
   int m_tiles;
   // wgrad
   int splits0, splits1;   // CTAs per (kt group) for class 0 (kh odd: 3 taps) and class 1 (kh even: 4 taps)
-  int kt_groups, steps;
+  int steps;
   float* dwm;
   int kfold;
 };
@@ -76,10 +78,10 @@ __global__ void __launch_bounds__(T8_FPROP_THREADS, 1) stem8_fprop_kernel(const 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
-  uint64_t* empty = full + 2;
+  uint64_t* empty = full + T8_MAX_STAGES;
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 256);
     }
@@ -115,7 +117,7 @@ __global__ void __launch_bounds__(T8_FPROP_THREADS, 1) stem8_fprop_kernel(const 
           }
         }
         __syncwarp();
-        if (++stage == 2) {
+        if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
@@ -135,12 +137,16 @@ __global__ void __launch_bounds__(T8_FPROP_THREADS, 1) stem8_fprop_kernel(const 
       const int rowg = tile / p.bands;            // (n, ot) flattened
       const int ot = rowg % p.OT;
       const int kt_lo = max(0, p.pt - ot), kt_hi = min(p.KT, p.T + p.pt - ot);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) d[i] = 0.f;
       int held = -1;
       for (int kt = kt_lo; kt < kt_hi; ++kt) {
         mbar_wait(&full[stage], phase);
         wgmma_fence();
         const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + uint32_t(g) * 1024u;
         const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + p.a_bytes;
+        // the 7 x 6 k-steps of a stage are straight-line code: every operand offset but the array stride is constant
+#pragma unroll
         for (int kh = 0; kh < 7; ++kh) {
           const int cls = (kh & 1) ^ 1;             // kh even -> odd input rows (class 1)
           const int so = cls ? (kh >> 1) : ((kh - 1) >> 1);   // slot of output row 0's tap
@@ -152,23 +158,20 @@ __global__ void __launch_bounds__(T8_FPROP_THREADS, 1) stem8_fprop_kernel(const 
             const uint32_t bb = b_base + uint32_t(kh * 12 + 1 + 2 * i) * 128u;
             const uint64_t a_hi = make_smem_desc(aa, p.ab, 128, 0);
             const uint64_t b_hi = make_smem_desc(bb, 128, 128, 0);
-            const uint32_t acc_flag = (kt != kt_lo || kh != 0 || i != 0) ? 1u : 0u;
             if (NSPLIT == 3) {
-              const uint64_t a_lo = make_smem_desc(aa + p.a_plane, p.ab, 128, 0);
-              const uint64_t b_lo = make_smem_desc(bb + p.b_plane, 128, 128, 0);
-              wgmma_m64n64<0, 0>(d, a_lo, b_hi, acc_flag);
+              const uint64_t a_lo = a_hi + (p.a_plane >> 4);
+              const uint64_t b_lo = b_hi + (p.b_plane >> 4);
+              wgmma_m64n64<0, 0>(d, a_lo, b_hi, 1u);
               wgmma_m64n64<0, 0>(d, a_hi, b_lo, 1u);
-              wgmma_m64n64<0, 0>(d, a_hi, b_hi, 1u);
-            } else {
-              wgmma_m64n64<0, 0>(d, a_hi, b_hi, acc_flag);
             }
+            wgmma_m64n64<0, 0>(d, a_hi, b_hi, 1u);
           }
         }
         wgmma_commit();
         wgmma_wait<1>();
         if (held >= 0) mbar_arrive(&empty[held]);
         held = stage;
-        if (++stage == 2) {
+        if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
@@ -228,49 +231,51 @@ __device__ __forceinline__ void t8_red_add_v4(float* addr, float a, float b, flo
                : "memory");
 }
 
-// CTA = (parity class, group of two T taps, split of the (n, input frame, band) steps).  Stage = the class's 8 arrays of
-// the input band + the dY row groups of the two output frames the taps pair this input frame with.
+constexpr uint32_t T8_DY_TILE = 16384;   // 128 rows x 128 bytes (120 written by the TMA, the rest stay zero)
+
+// CTA = (parity class, T tap kt, split of the (n, input frame, band) steps).  Stage = the class's 8 arrays of the input
+// band + the dY row group of the output frame tap kt pairs this input frame with.  MMA warpgroup tq takes H tap tq of the
+// class (class 1: kh = 2 tq, class 0: kh = 2 tq + 1, slot offset tq; the 3-tap class leaves warpgroup 3 idle): a
+// 64-column accumulator (granules 0..7, B0) and a 32-column one (granules 8..11, B1), 48 registers, so a stage's wgmmas
+// are straight-line code and the accumulators stay in registers.
 template <int NSPLIT>
 __global__ void __launch_bounds__(T8_WGRAD_THREADS, 1) stem8_wgrad_kernel(const __grid_constant__ Stem8Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
-  uint64_t* empty = full + 2;
+  uint64_t* empty = full + T8_MAX_STAGES;
   constexpr uint32_t NP = NSPLIT == 3 ? 2u : 1u;
-  constexpr uint32_t DY_TILE = 16384;   // 128 rows x 128 bytes (120 written by the TMA, the rest stay zero)
 
   // decode the CTA's job
-  const int per0 = p.kt_groups * p.splits0;
-  int cls, ktg, split, nsplits;
+  const int per0 = p.KT * p.splits0;
+  int cls, kt, split, nsplits;
   if (int(blockIdx.x) < per0) {
     cls = 0;
-    ktg = blockIdx.x / p.splits0;
-    split = blockIdx.x - ktg * p.splits0;
+    kt = blockIdx.x / p.splits0;
+    split = blockIdx.x - kt * p.splits0;
     nsplits = p.splits0;
   } else {
     const int b = blockIdx.x - per0;
     cls = 1;
-    ktg = b / p.splits1;
-    split = b - ktg * p.splits1;
+    kt = b / p.splits1;
+    split = b - kt * p.splits1;
     nsplits = p.splits1;
   }
   const int ntaps = cls ? 4 : 3;
-  const int kta = 2 * ktg, ktb = 2 * ktg + 1;
-  const bool has_b = ktb < p.KT;
   const int per = (p.steps + nsplits - 1) / nsplits;
   const int s0 = split * per, s1 = min(p.steps, s0 + per);
 
   // zero the whole operand area once: rows the TMA never writes (dY rows 120..127, array tails) must be finite
   {
     uint4* z = reinterpret_cast<uint4*>(smem);
-    const uint32_t n16 = (2u * p.stage_bytes) / 16u;
+    const uint32_t n16 = (uint32_t(p.stages) * p.stage_bytes) / 16u;
     for (uint32_t i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 512);
+      mbar_init(&empty[s], 128 * ntaps);
     }
     fence_mbar_init();
   }
@@ -291,28 +296,28 @@ __global__ void __launch_bounds__(T8_WGRAD_THREADS, 1) stem8_wgrad_kernel(const 
         mbar_wait(&empty[stage], phase ^ 1);
         if (elect_one()) {
           const uint32_t dyb = uint32_t(T8_ROWS * p.MR) * 128u;
-          mbar_expect_tx(&full[stage], NP * (8u * uint32_t(T8_SLOTS * p.MR * 16) + (has_b ? 2u : 1u) * dyb));
+          mbar_expect_tx(&full[stage], NP * (8u * uint32_t(T8_SLOTS * p.MR * 16) + dyb));
           uint8_t* st = smem + size_t(stage) * p.stage_bytes;
           const int h2 = oh0 - 1 - cls;
           for (uint32_t pl = 0; pl < NP; ++pl) {
             for (int j = 0; j < 8; ++j)
               t8_tma_5d(st + (pl * 8 + j) * p.ab, &p.tmX[pl], &full[stage], 0, j, h2, 2 * tin + cls, n);
-            uint8_t* dyd = st + x_bytes + pl * 2 * DY_TILE;
-            t8_tma_5d(dyd, &p.tmB[pl], &full[stage], 0, 0, oh0, tin - kta + p.pt, n);
-            if (has_b) t8_tma_5d(dyd + DY_TILE, &p.tmB[pl], &full[stage], 0, 0, oh0, tin - ktb + p.pt, n);
+            t8_tma_5d(st + x_bytes + pl * T8_DY_TILE, &p.tmB[pl], &full[stage], 0, 0, oh0, tin - kt + p.pt, n);
           }
         }
         __syncwarp();
-        if (++stage == 2) {
+        if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
-    } else {
-      // MMA warpgroup (g, th): 64-row half g (T tap kta / ktb) and H taps tq = 2 th, 2 th + 1; per tap a 64-column
-      // accumulator (granules 0..7, B0) and a 32-column one (granules 8..11, B1)
-      const int wg = warp >> 2, g = wg & 1, th = wg >> 1;
-      float d0[2][32], d1[2][16];
+    } else if ((warp >> 2) < ntaps) {
+      const int tq = warp >> 2;
+      float d0[32], d1[16];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) d0[i] = 0.f;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) d1[i] = 0.f;
       int stage = 0;
       uint32_t phase = 0;
       int held = -1;
@@ -320,70 +325,50 @@ __global__ void __launch_bounds__(T8_WGRAD_THREADS, 1) stem8_wgrad_kernel(const 
         mbar_wait(&full[stage], phase);
         wgmma_fence();
         const uint32_t x_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
-        const uint32_t lbo_a = has_b ? DY_TILE : 0u;       // second 64-row atom = the other T tap's dY (or an alias)
-        const uint32_t dy_base = x_base + x_bytes + uint32_t(g) * lbo_a;
+        const uint32_t dy_base = x_base + x_bytes;
 #pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int tq = 2 * th + u;   // class 1: kh = 2 tq, slot offset tq; class 0: kh = 2 tq + 1, slot offset tq
-          if (tq < ntaps) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {
-              const uint32_t xa = x_base + uint32_t(tq * p.MR) * 16u + uint32_t(ks) * 256u;
-              const uint64_t a_hi = make_smem_desc(dy_base + ks * 2048, lbo_a, 1024, 2);
-              const uint64_t b0_hi = make_smem_desc(xa, 128, p.ab, 0);
-              const uint64_t b1_hi = make_smem_desc(xa + 16u, 128, p.ab, 0);
-              const uint32_t acc_flag = (step != s0 || ks != 0) ? 1u : 0u;
-              if (NSPLIT == 3) {
-                const uint64_t a_lo = make_smem_desc(dy_base + 2 * DY_TILE + ks * 2048, lbo_a, 1024, 2);
-                const uint64_t b0_lo = make_smem_desc(xa + 8u * p.ab, 128, p.ab, 0);
-                const uint64_t b1_lo = make_smem_desc(xa + 8u * p.ab + 16u, 128, p.ab, 0);
-                wgmma_m64n64<1, 1>(d0[u], a_lo, b0_hi, acc_flag);
-                wgmma_m64n64<1, 1>(d0[u], a_hi, b0_lo, 1u);
-                wgmma_m64n64<1, 1>(d0[u], a_hi, b0_hi, 1u);
-                wgmma_m64n32<1, 1>(d1[u], a_lo, b1_hi, acc_flag);
-                wgmma_m64n32<1, 1>(d1[u], a_hi, b1_lo, 1u);
-                wgmma_m64n32<1, 1>(d1[u], a_hi, b1_hi, 1u);
-              } else {
-                wgmma_m64n64<1, 1>(d0[u], a_hi, b0_hi, acc_flag);
-                wgmma_m64n32<1, 1>(d1[u], a_hi, b1_hi, acc_flag);
-              }
-            }
+        for (int ks = 0; ks < 8; ++ks) {
+          const uint32_t xa = x_base + uint32_t(tq * p.MR) * 16u + uint32_t(ks) * 256u;
+          const uint64_t a_hi = make_smem_desc(dy_base + ks * 2048, 0, 1024, 2);
+          const uint64_t b0_hi = make_smem_desc(xa, 128, p.ab, 0);
+          const uint64_t b1_hi = b0_hi + 1;   // one granule (16 bytes) further
+          if (NSPLIT == 3) {
+            const uint64_t a_lo = a_hi + (T8_DY_TILE >> 4);
+            const uint64_t b0_lo = b0_hi + ((8u * p.ab) >> 4);
+            const uint64_t b1_lo = b0_lo + 1;
+            wgmma_m64n64<1, 1>(d0, a_lo, b0_hi, 1u);
+            wgmma_m64n64<1, 1>(d0, a_hi, b0_lo, 1u);
+            wgmma_m64n32<1, 1>(d1, a_lo, b1_hi, 1u);
+            wgmma_m64n32<1, 1>(d1, a_hi, b1_lo, 1u);
           }
+          wgmma_m64n64<1, 1>(d0, a_hi, b0_hi, 1u);
+          wgmma_m64n32<1, 1>(d1, a_hi, b1_hi, 1u);
         }
         wgmma_commit();
         wgmma_wait<1>();
         if (held >= 0) mbar_arrive(&empty[held]);
         held = stage;
-        if (++stage == 2) {
+        if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
       wgmma_wait<0>();
       // fragments -> dWf: row mu = (j, co), column granule gi = kw' + j, slots 2 (lane % 4) (+1)
-      const int kt = g ? ktb : kta;
-      if (kt < p.KT) {
-        const int sl = 2 * (lane & 3);
+      const int kh = cls ? 2 * tq : 2 * tq + 1;
+      const int sl = 2 * (lane & 3);
 #pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int tq = 2 * th + u;
-          if (tq < ntaps) {
-            const int kh = cls ? 2 * tq : 2 * tq + 1;
+      for (int h = 0; h < 2; ++h) {
+        const int mu = (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        const int j = mu >> 3, co = mu & 7;
+        float* dst = p.dwm + size_t(co) * p.kfold + size_t((kt * 7 + kh) * 4) * 8 + sl;
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int mu = (warp & 3) * 16 + (lane >> 2) + 8 * h;
-              const int j = mu >> 3, co = mu & 7;
-              float* dst = p.dwm + size_t(co) * p.kfold + size_t((kt * 7 + kh) * 4) * 8 + sl;
-#pragma unroll
-              for (int gi = 0; gi < 12; ++gi) {
-                const int kwp = gi - j;   // folded W tap this granule is for pixel j of the group
-                if (kwp >= 0 && kwp < 4) {
-                  const float y0 = gi < 8 ? d0[u][4 * gi + 2 * h] : d1[u][4 * (gi - 8) + 2 * h];
-                  const float y1 = gi < 8 ? d0[u][4 * gi + 2 * h + 1] : d1[u][4 * (gi - 8) + 2 * h + 1];
-                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + kwp * 8), "f"(y0), "f"(y1) : "memory");
-                }
-              }
-            }
+        for (int gi = 0; gi < 12; ++gi) {
+          const int kwp = gi - j;   // folded W tap this granule is for pixel j of the group
+          if (kwp >= 0 && kwp < 4) {
+            const float y0 = gi < 8 ? d0[4 * gi + 2 * h] : d1[4 * (gi - 8) + 2 * h];
+            const float y1 = gi < 8 ? d0[4 * gi + 2 * h + 1] : d1[4 * (gi - 8) + 2 * h + 1];
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + kwp * 8), "f"(y0), "f"(y1) : "memory");
           }
         }
       }
@@ -585,7 +570,9 @@ extern "C" int sfb_stem8_fprop(const sfb_stem_desc* d, void* stream_) {
   p.a_bytes = np * p.a_plane;
   p.b_plane = p.zg * 128u;
   p.stage_bytes = (p.a_bytes + np * p.b_plane + 1023u) / 1024u * 1024u;
-  p.off_red = 2 * p.stage_bytes;
+  const uint32_t tail = 2 * 8 * 16 * 4 + 128 + 1024;
+  p.stages = std::max(2, std::min<int>(T8_MAX_STAGES, (uint32_t(t8_smem) - tail) / p.stage_bytes));
+  p.off_red = p.stages * p.stage_bytes;
   p.off_bars = p.off_red + 2 * 8 * 16 * 4;
   const uint32_t smem_bytes = p.off_bars + 128 + 1024;
   if (smem_bytes > uint32_t(t8_smem)) {
@@ -626,21 +613,21 @@ extern "C" int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream_) {
   int rc = t8_fill(p, d);
   if (rc) return rc;
   const int np = d->nsplit == 3 ? 2 : 1;
-  p.stage_bytes = (np * 8u * p.ab + np * 2u * 16384u + 1023u) / 1024u * 1024u;
+  p.stage_bytes = (np * 8u * p.ab + np * T8_DY_TILE + 1023u) / 1024u * 1024u;
   if ((np * 8u * p.ab) % 1024u) {
     set_error("sfb_stem8_wgrad: operand arrays (%u bytes) do not keep the dY tiles 1024-byte aligned", np * 8u * p.ab);
     return -11;
   }
-  p.off_bars = 2 * p.stage_bytes;
+  p.stages = std::max(2, std::min<int>(T8_MAX_STAGES, (uint32_t(t8_smem) - 128 - 1024) / p.stage_bytes));
+  p.off_bars = p.stages * p.stage_bytes;
   const uint32_t smem_bytes = p.off_bars + 128 + 1024;
   if (smem_bytes > uint32_t(t8_smem)) {
     set_error("sfb_stem8_wgrad: %u bytes of shared memory needed, %d available", smem_bytes, t8_smem);
     return -11;
   }
-  p.kt_groups = (d->kt + 1) / 2;
   p.steps = d->n * d->t * p.bands;
   // CTAs: class 1 carries 4 H taps per step, class 0 three -> split the machine 4 : 3
-  const int per_group = std::max(2, t8_sms / p.kt_groups);
+  const int per_group = std::max(2, t8_sms / p.KT);
   p.splits1 = std::max(1, std::min(p.steps, (per_group * 4 + 3) / 7));
   p.splits0 = std::max(1, std::min(p.steps, per_group - p.splits1));
   p.dwm = d->dwm;
@@ -658,7 +645,7 @@ extern "C" int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream_) {
       if (rc) return rc;
     }
   }
-  const int grid = p.kt_groups * (p.splits0 + p.splits1);
+  const int grid = p.KT * (p.splits0 + p.splits1);
   if (d->nsplit == 3) {
     static bool a = false;
     if (!a) { cudaFuncSetAttribute(stem8_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }

@@ -95,7 +95,7 @@ __device__ __forceinline__ void wgmma_m64n(float* d, uint64_t a, uint64_t b, uin
 
 // Runtime N (a multiple of 16 up to MAXN) -> the matching instruction; d holds MAXN/2 registers.  A call site with a
 // runtime N is a branch over eight wgmmas: ptxas serialises the wgmmas of the function around it (warning C7520), so
-// only kernels whose MMA issue is not their limit use it (gemm_batched, the W-shift stem's wgrad).
+// only kernels whose MMA issue is not their limit use it (gemm_batched).
 template <int MAXN, int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16(float* d, int n, uint64_t a, uint64_t b, uint32_t accumulate) {
   switch (n) {

@@ -617,8 +617,8 @@ def stem_m_tiles(x: Planes, g: StemGeom) -> int:
 
 def stem_fprop(x: Planes, f: FilterMat, g: StemGeom, out: torch.Tensor, stats: Optional[torch.Tensor],
                nsplit: int = 3) -> None:
-    """W-shift stem forward (csrc/conv_stem.cu): up to 128 output channels (one accumulator tile of 128 columns); the
-    stems of the supported models have 8, 24 or 64."""
+    """W-shift stem forward (csrc/conv_stem.cu): up to 64 output channels (one accumulator tile of 16, 32, 48 or 64
+    columns); the stems of the supported models have 8, 24 or 64."""
     lib = L.load()
     d = _stem_desc(x, g, nsplit)
     d.f_hi, d.f_lo = f.hi.data_ptr(), _ptr(f.lo)
