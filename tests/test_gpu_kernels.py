@@ -431,18 +431,27 @@ def test_stem_wshift_fprop_wgrad(case, nsplit, cuda_device):
 
 
 def test_gemm_batched_all_layouts(cuda_device):
-    """Batched wgmma GEMM in the four operand-major combinations the attention products need."""
+    """Batched wgmma GEMM in the four operand-major combinations the attention products need, at the attention's own
+    layouts: output rows at a padded pitch whose pad columns stay untouched, and accumulation onto a prefilled output."""
     ops = _ops()
     from slowfast_b200 import lib as L
     import ctypes as C
     dev = cuda_device
     lib = L.load()
     g = torch.Generator(device="cpu").manual_seed(2)
+    plain = [(3, 200, 96, 96, 0, 0), (2, 300, 96, 393, 0, 1), (2, 393, 96, 300, 1, 1), (3, 130, 200, 96, 0, 0),
+             (2, 96, 40, 520, 1, 1),
+             # long reductions over few tiles: the split-K path (float atomics into the zeroed output)
+             (2, 393, 96, 4100, 1, 1), (1, 100, 96, 2500, 0, 0), (2, 200, 96, 3000, 0, 1)]
+    attention = []
+    for hd in (32, 64, 72, 80):
+        # S = q k^T and dP = dO v^T (K = head dim) stored at pitch pad8(Nk) = 400 > Nk; O = P v (N = head dim)
+        attention += [(2, 393, 393, hd, 0, 0, 400, 0), (2, 393, hd, 393, 0, 1, hd, 0)]
+    # dq += alpha dS k onto the residual-pooling seed: the plain path, and (few tiles, K = 3136) the split-K path
+    attention += [(2, 393, 72, 393, 0, 1, 72, 1), (3, 50, 80, 393, 0, 1, 80, 1), (1, 200, 72, 3136, 0, 1, 72, 1),
+                  (2, 100, 96, 4100, 0, 1, 96, 1)]
     for nsplit in (1, 3):
-        for (bt, m, n, k, a_mn, b_mn) in [(3, 200, 96, 96, 0, 0), (2, 300, 96, 393, 0, 1), (2, 393, 96, 300, 1, 1),
-                                          (3, 130, 200, 96, 0, 0), (2, 96, 40, 520, 1, 1),
-                                          # long reductions over few tiles: the split-K path (float atomics into the zeroed output)
-                                          (2, 393, 96, 4100, 1, 1), (1, 100, 96, 2500, 0, 0), (2, 200, 96, 3000, 0, 1)]:
+        for (bt, m, n, k, a_mn, b_mn, ldd, acc) in [c + (c[2], 0) for c in plain] + attention:
             kp, mp, np_ = (k + 7) // 8 * 8, (m + 7) // 8 * 8, (n + 7) // 8 * 8
             A = torch.randn(bt, m, k, generator=g).to(dev)
             Bm = torch.randn(bt, n, k, generator=g).to(dev)
@@ -462,13 +471,17 @@ def test_gemm_batched_all_layouts(cuda_device):
                 return hi, (v - hi.float()).bfloat16()
             a_hi, a_lo = split(a_st)
             b_hi, b_lo = split(b_st)
-            out = torch.full((bt, m, n), float("nan"), device=dev)
+            # NaN where the kernel must write (plain store) or must not touch (pad columns); a prefill to accumulate onto
+            out = torch.full((bt, m, ldd), float("nan"), device=dev)
+            pre = torch.randn(bt, m, n, generator=g).to(dev) if acc else torch.zeros(bt, m, n, device=dev)
+            if acc:
+                out[:, :, :n] = pre
             d = L.BgemmDesc()
             d.a_hi, d.a_lo, d.lda, d.batch_stride_a, d.a_mn_major = a_hi.data_ptr(), a_lo.data_ptr(), a_st.shape[2], a_st[0].numel(), a_mn
             d.b_hi, d.b_lo, d.ldb, d.batch_stride_b, d.b_mn_major = b_hi.data_ptr(), b_lo.data_ptr(), b_st.shape[2], b_st[0].numel(), b_mn
             d.m, d.n, d.k, d.batch = m, n, k, bt
-            d.out, d.ldd, d.batch_stride_d = out.data_ptr(), n, m * n
-            d.alpha, d.accumulate, d.nsplit = 0.5, 0, nsplit
+            d.out, d.ldd, d.batch_stride_d = out.data_ptr(), ldd, m * ldd
+            d.alpha, d.accumulate, d.nsplit = 0.5, acc, nsplit
             L.check(lib.sfb_gemm_batched(C.byref(d), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "bgemm")
             def val(hi, lo):
                 return hi.double() + (lo.double() if nsplit == 3 else 0)
@@ -477,8 +490,11 @@ def test_gemm_batched_all_layouts(cuda_device):
             Ar = Ar[:, :, :m].transpose(1, 2) if a_mn else Ar[:, :, :k]
             Br = Br[:, :, :n].transpose(1, 2) if b_mn else Br[:, :, :k]
             ref = 0.5 * Ar @ Br.transpose(1, 2)
-            assert not torch.isnan(out).any(), (nsplit, bt, m, n, k, a_mn, b_mn)
-            assert relerr(out, ref) < TOL[nsplit], (nsplit, bt, m, n, k, a_mn, b_mn, relerr(out, ref))
+            case = (nsplit, bt, m, n, k, a_mn, b_mn, ldd, acc)
+            assert torch.isnan(out[:, :, n:]).all(), case
+            got = out[:, :, :n].double() - pre.double()
+            assert not torch.isnan(got).any(), case
+            assert relerr(got, ref) < TOL[nsplit], case + (relerr(got, ref),)
 
 
 @pytest.mark.parametrize("k,s,p", [((2, 1, 1), (2, 1, 1), (0, 0, 0)), ((1, 3, 3), (1, 2, 2), (0, 1, 1)),

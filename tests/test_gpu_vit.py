@@ -303,8 +303,11 @@ def test_model_step_and_eval_match_reference(yaml, frames, crop, extra, fast, cu
     assert rel_max < 1e-3 and torch.equal(lm.argmax(1), lr.argmax(1))
     # test_gpu_models.py's sampled-gradient bounds.  Measured on an H100: median 2.0e-5 (ViT-B 64^2), 1.2e-5 (ViT-B 224^2),
     # 1.2e-5 / 1.4e-5 (ViT-L / ViT-H, two blocks at 224^2), 5.7e-4 / 5.2e-5 (MViTv1-B 64^2 / 224^2), 4.0e-3 (MViTv2-S FT;
-    # worst rel_pos_w 1.3e-2), 2.5e-3 (MViTv2-L FT) - the pooled-attention blocks carry the split-bf16 operand error of
-    # the existing MViTv2 path, the new position / mean-readout / patchify / wide-LayerNorm code adds none measurable
+    # worst rel_pos_w 1.3e-2), 2.5e-3 (MViTv2-L FT).  The MViT excess comes from the skip max-pool, not the block math: where
+    # a window's top two values are closer than the forward error, the engine and fp64 pick different inputs, and the
+    # gradient upstream of that block moves by far more than rounding.  One such window in 98 304 takes a 3-block
+    # MViTv2-S FT stack from 4.6e-5 to 6.9e-4 worst; with the routing pinned, every MViT block kind is within 5e-5 of fp64
+    # (test_gpu_mvit_blocks.py holds them to 1e-3).  Hence the wide per-parameter bound here
     assert ratio[wk] < 1.0, (wk, err[wk], env[wk])
     assert em_ < max(8 * en_, 0.15), (em_, en_)
     for k in zero:
