@@ -290,12 +290,6 @@ int sfb_stem8_input_fold(const float* x, int32_t n, int32_t cin, int32_t t, int3
 int sfb_stem8_filter_fold(const float* w, int32_t cin, int32_t kt, void* hi, void* lo, void* stream);
 int sfb_stem8_fprop(const sfb_stem_desc* d, void* stream);
 int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream);
-/* Direct (fp32 SIMT) weight gradient of the narrow stem (3 -> 8 channels, stride (1,2,2): the fast pathway's
- * conv, stem_helper.py:182): reads the fp32 NCTHW clip and the dY planes, writes dw in the parameter's own layout
- * [8][3][kt][kh][kw].  8 output channels would fill 8 of 128 UMMA rows; the fp32 pipes do this layer faster. */
-int sfb_stem_wgrad_direct(const float* x, int32_t n, int32_t cin, int32_t t, int32_t h, int32_t w, const void* dy_hi,
-                          const void* dy_lo, int32_t cout, int32_t kt, int32_t kh, int32_t kw, int32_t st, int32_t sh,
-                          int32_t sw, int32_t pt, int32_t ph, int32_t pw, float* dw, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Batched GEMM for the attention products of MultiScaleAttention (attention.py:355 `(q*scale) @ k^T`, :379
@@ -470,11 +464,13 @@ int sfb_droppath_scales(float* out, const float* rates, int32_t n_rates, int32_t
  * operators.py:55 SE, head_helper.py:461 X3DHead).  Channel counts are padded to multiples of 8 (`c`), `c_valid`
  * is the module's real width; pad channels hold exact zeros.
  * ---------------------------------------------------------------------------------------------- */
-/* Channelwise Conv3d (groups == channels; nn.Conv3d weight [c_valid, 1, kt, kh, kw], no bias), <= 27 taps.
- * Input = split planes (x_hi/x_lo) or fp32 (x_f32); output y fp32 + BatchNorm partials stats[2][c_valid][m_tiles]
+/* Channelwise Conv3d (groups == channels; nn.Conv3d weight [c_valid, 1, kt, kh, kw], no bias): c a multiple of 8 up
+ * to 512, temporal stride 1, a 3x3x3 filter at spatial stride 1 or 2 or a 5x1x1 filter at stride 1; fwd / bwd return
+ * nonzero for any other geometry and sfb_dwconv_tiles_per_sample returns 0.  Input x_f32 fp32 (x_pitch a multiple of
+ * 4); output y fp32 + BatchNorm partials stats[2][c_valid][m_tiles]
  * (tiles never straddle samples: sample s owns tiles [s*tps, (s+1)*tps), which is what sfb_se_fwd pools over). */
 typedef struct sfb_dwconv_desc {
-  const void* x_hi; const void* x_lo; const float* x_f32; int64_t x_pitch;
+  const float* x_f32; int64_t x_pitch;
   const float* w;
   float* y; int64_t y_pitch; float* stats;
   int32_t n, t, h, w_, c, c_valid, ot, oh, ow, kt, kh, kw, st, sh, sw, pt, ph, pw;
@@ -482,15 +478,13 @@ typedef struct sfb_dwconv_desc {
   float* dx;                           /* bwd: fp32 data gradient (stored, or += when dx_accumulate) ...     */
   void* dx_hi; void* dx_lo;            /* ... or, when dx == NULL, split planes (operand of the next wgrad)  */
   int64_t dx_pitch; int32_t dx_accumulate;
-  float* wpartials;                    /* bwd scratch [sfb_dwconv_wgrad_blocks()][c][taps] */
-  /* optional producer transform fused into every input read (fp32 input only): x := relu?(x*in_scale + in_shift),
+  /* optional producer transform fused into every input read: x := relu?(x*in_scale + in_shift),
    * i.e. the BatchNorm (+ReLU) of the layer that produced x; padding stays zero AFTER the transform */
   const float* in_scale; const float* in_shift; int32_t in_relu;
 } sfb_dwconv_desc;
 int32_t sfb_dwconv_m_tiles(const sfb_dwconv_desc* d);
 int32_t sfb_dwconv_tiles_per_sample(const sfb_dwconv_desc* d);
 int sfb_dwconv_fwd(const sfb_dwconv_desc* d, void* stream);
-int32_t sfb_dwconv_wgrad_blocks(const sfb_dwconv_desc* d);
 /* dw == NULL skips the weight gradient; dx == dx_hi == NULL skips the data gradient */
 int sfb_dwconv_bwd(const sfb_dwconv_desc* d, float* dw, void* stream);
 /* out = act( (y*scale + shift) * gate[sample] ),  act: 0 identity, 1 ReLU, 2 Swish (x*sigmoid(x)); planes out.

@@ -760,153 +760,3 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
   }
   return 0;
 }
-
-// ------------------------------------------------------------------------------------------------ direct (SIMT) wgrad
-// The fast pathway's stem (3 -> 8 channels, 5x7x7, stride (1,2,2)) has only 8 output channels: as a tensor-core GEMM
-// dW[8, 735] it fills 8 of the 128 UMMA rows and was MMA-issue-bound (4.5 ms per step).  Its 19 GMAC are cheap on the
-// fp32 pipes, exact, and the operands are read once: one thread owns 3 of the 735 (ci,kt,kh,kw) taps for all 8 output
-// channels (24 register accumulators), a block stages the 5x7 input rows one output row touches (straight from the
-// fp32 NCTHW clip) and that row's dY in shared memory, and walks the 112 output pixels: per pixel and thread 2
-// broadcast LDS.128 (dY) + 3 LDS (taps) feed 24 FMAs.  Persistent blocks, one atomic add per (tap, channel) and block.
-namespace sfb {
-constexpr int SD_COUT = 8, SD_CIN = 3, SD_THREADS = 256, SD_TPT = 3;
-struct StemDirectParams {
-  const float* x;  // [n][3][T][H][W]
-  const __nv_bfloat16* dy_hi; const __nv_bfloat16* dy_lo;  // [n][OT][OH][OW][8]
-  float* dw;       // [8][3][KT][KH][KW]
-  int n, T, H, W, OT, OH, OW, KT, KH, KW, pt, ph, pw;
-  int xw;          // padded row length in shared memory
-  int rows_total, rows_per_block;
-};
-__global__ void __launch_bounds__(SD_THREADS) stem_wgrad_direct_kernel(const StemDirectParams p) {
-  extern __shared__ float sm[];
-  float* xs = sm;                                           // [KT][KH][3][xw]
-  float* dys = sm + size_t(p.KT) * p.KH * SD_CIN * p.xw;    // [OW][8]
-  const int taps = SD_CIN * p.KT * p.KH * p.KW;
-  int toff[SD_TPT], tkw[SD_TPT];
-  bool tok[SD_TPT];
-#pragma unroll
-  for (int j = 0; j < SD_TPT; ++j) {
-    const int tap = threadIdx.x + j * SD_THREADS;
-    tok[j] = tap < taps;
-    const int tt = tok[j] ? tap : 0;
-    const int kw = tt % p.KW;
-    int r = tt / p.KW;
-    const int kh = r % p.KH;
-    r /= p.KH;
-    const int kt = r % p.KT;
-    const int ci = r / p.KT;
-    toff[j] = ((kt * p.KH + kh) * SD_CIN + ci) * p.xw + kw;
-    tkw[j] = kw;
-  }
-  float acc[SD_TPT][SD_COUT];
-#pragma unroll
-  for (int j = 0; j < SD_TPT; ++j)
-#pragma unroll
-    for (int c = 0; c < SD_COUT; ++c) acc[j][c] = 0.f;
-  const int r0 = blockIdx.x * p.rows_per_block;
-  const int r1 = min(p.rows_total, r0 + p.rows_per_block);
-  const int xrows = p.KT * p.KH * SD_CIN;
-  const int w4 = p.W / 4;
-  for (int row = r0; row < r1; ++row) {
-    const int oh = row % p.OH;
-    int r = row / p.OH;
-    const int ot = r % p.OT;
-    const int n = r / p.OT;
-    __syncthreads();  // previous row fully consumed
-    // ---- stage the KT x KH x 3 input rows (zero rows / columns where the padding is)
-    for (int i = threadIdx.x; i < xrows * (p.xw / 4); i += SD_THREADS) {
-      const int q = i % (p.xw / 4);
-      int rr = i / (p.xw / 4);
-      const int ci = rr % SD_CIN;
-      rr /= SD_CIN;
-      const int kh = rr % p.KH;
-      const int kt = rr / p.KH;
-      const int it = ot - p.pt + kt, ih = oh * 2 - p.ph + kh;
-      // smem column s holds input column s - pw'; pw' = 4 (>= pw) keeps the float4 copies aligned
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      const int wq = q - 1;  // float4 index into the input row
-      if (it >= 0 && it < p.T && ih >= 0 && ih < p.H && wq >= 0 && wq < w4)
-        v = *reinterpret_cast<const float4*>(p.x + (((int64_t(n) * SD_CIN + ci) * p.T + it) * p.H + ih) * p.W + wq * 4);
-      *reinterpret_cast<float4*>(xs + ((kt * p.KH + kh) * SD_CIN + ci) * p.xw + q * 4) = v;
-    }
-    for (int i = threadIdx.x; i < p.OW * 2; i += SD_THREADS) {
-      const int64_t off = (int64_t(row) * p.OW) * SD_COUT + i * 4;
-      const uint2 h = *reinterpret_cast<const uint2*>(p.dy_hi + off);
-      float4 v = make_float4(__uint_as_float(h.x << 16), __uint_as_float(h.x & 0xffff0000u), __uint_as_float(h.y << 16),
-                             __uint_as_float(h.y & 0xffff0000u));
-      if (p.dy_lo) {
-        const uint2 l = *reinterpret_cast<const uint2*>(p.dy_lo + off);
-        v.x += __uint_as_float(l.x << 16); v.y += __uint_as_float(l.x & 0xffff0000u);
-        v.z += __uint_as_float(l.y << 16); v.w += __uint_as_float(l.y & 0xffff0000u);
-      }
-      *reinterpret_cast<float4*>(dys + i * 4) = v;
-    }
-    __syncthreads();
-    // ---- accumulate: input column of tap kw for output pixel ow = 2*ow - pw + kw  -> smem column + 4
-    const int cbase = 4 - p.pw;
-#pragma unroll 4
-    for (int ow = 0; ow < p.OW; ++ow) {
-      const float4 d0 = *reinterpret_cast<const float4*>(dys + ow * 8);
-      const float4 d1 = *reinterpret_cast<const float4*>(dys + ow * 8 + 4);
-#pragma unroll
-      for (int j = 0; j < SD_TPT; ++j) {
-        const float xv = xs[toff[j] + cbase + 2 * ow];
-        acc[j][0] = fmaf(d0.x, xv, acc[j][0]); acc[j][1] = fmaf(d0.y, xv, acc[j][1]);
-        acc[j][2] = fmaf(d0.z, xv, acc[j][2]); acc[j][3] = fmaf(d0.w, xv, acc[j][3]);
-        acc[j][4] = fmaf(d1.x, xv, acc[j][4]); acc[j][5] = fmaf(d1.y, xv, acc[j][5]);
-        acc[j][6] = fmaf(d1.z, xv, acc[j][6]); acc[j][7] = fmaf(d1.w, xv, acc[j][7]);
-      }
-    }
-  }
-  (void)tkw;
-#pragma unroll
-  for (int j = 0; j < SD_TPT; ++j) {
-    if (!tok[j]) continue;
-    const int tap = threadIdx.x + j * SD_THREADS;  // = ((ci*KT + kt)*KH + kh)*KW + kw: the parameter's own tap order
-#pragma unroll
-    for (int c = 0; c < SD_COUT; ++c) atomicAdd(p.dw + size_t(c) * taps + tap, acc[j][c]);
-  }
-}
-}  // namespace sfb
-
-extern "C" int sfb_stem_wgrad_direct(const float* x, int32_t n, int32_t cin, int32_t t, int32_t h, int32_t w,
-                                     const void* dy_hi, const void* dy_lo, int32_t cout, int32_t kt, int32_t kh,
-                                     int32_t kw, int32_t st, int32_t sh, int32_t sw, int32_t pt, int32_t ph, int32_t pw,
-                                     float* dw, void* stream) {
-  using namespace sfb;
-  if (cin != SD_CIN || cout != SD_COUT || st != 1 || sh != 2 || sw != 2 || pw > 4 || w % 4 ||
-      cin * kt * kh * kw > SD_THREADS * SD_TPT) {
-    set_error("sfb_stem_wgrad_direct: only the 3 -> 8 channel, stride (1,2,2) stem with <= %d taps is supported",
-              SD_THREADS * SD_TPT);
-    return -10;
-  }
-  StemDirectParams p;
-  p.x = x; p.dy_hi = (const __nv_bfloat16*)dy_hi; p.dy_lo = (const __nv_bfloat16*)dy_lo; p.dw = dw;
-  p.n = n; p.T = t; p.H = h; p.W = w;
-  p.OT = (t + 2 * pt - kt) / st + 1; p.OH = (h + 2 * ph - kh) / sh + 1; p.OW = (w + 2 * pw - kw) / sw + 1;
-  p.KT = kt; p.KH = kh; p.KW = kw; p.pt = pt; p.ph = ph; p.pw = pw;
-  // smem row: 4 zero columns, the W input columns, then zeros up to the last column any tap reads, rounded to 4
-  const int need = 4 - pw + 2 * (p.OW - 1) + kw;
-  p.xw = (std::max(need, w + 4) + 3) / 4 * 4 + 4;
-  p.rows_total = n * p.OT * p.OH;
-  int blocks = 148 * 2;
-  if (blocks > p.rows_total) blocks = p.rows_total;
-  p.rows_per_block = (p.rows_total + blocks - 1) / blocks;
-  blocks = (p.rows_total + p.rows_per_block - 1) / p.rows_per_block;
-  const size_t smem = (size_t(kt) * kh * SD_CIN * p.xw + size_t(p.OW) * SD_COUT) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(stem_wgrad_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    attr = true;
-  }
-  cudaStream_t s = (cudaStream_t)stream;
-  cudaMemsetAsync(dw, 0, size_t(cout) * cin * kt * kh * kw * sizeof(float), s);
-  stem_wgrad_direct_kernel<<<blocks, SD_THREADS, smem, s>>>(p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem_wgrad_direct launch failed: %s (smem=%zu)", cudaGetErrorString(e), smem);
-    return -20;
-  }
-  return 0;
-}

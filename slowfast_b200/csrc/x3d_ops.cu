@@ -2,7 +2,7 @@
 //   * channelwise (depthwise) Conv3d  kt x kh x kw, stride (st,sh,sw)           - resnet_helper.py:217-229 (X3DTransform.b),
 //                                                                               stem_helper.py:268-276 (X3DStem.conv)
 //     fwd (+ per-tile BatchNorm partial sums, tiles aligned to samples so that the SE average pool falls out of
-//     the same partials), data gradient (gather form), weight gradient (per-block partials + merge);
+//     the same partials), data gradient, weight gradient; fp32 input, 3x3x3 or 5x1x1 filters at temporal stride 1;
 //   * BN -> [SE gate] -> ReLU | Swish, forward and backward, with the BN backward sums derived from per-sample sums
 //     so that the SE branch costs no extra pass over the activation                 - operators.py:55-59 (SE.forward);
 //   * the SE bottleneck itself (AvgPool -> 1x1x1 -> ReLU -> 1x1x1 -> Sigmoid), one block per sample.
@@ -36,18 +36,6 @@ static int x3_grid(int64_t items, int block, int waves = 8) {
   return int(want < 1 ? 1 : (want > cap ? cap : want));
 }
 
-__device__ __forceinline__ float4 bf4_to_f4(uint2 v) {
-  return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u), __uint_as_float(v.y << 16),
-                     __uint_as_float(v.y & 0xffff0000u));
-}
-__device__ __forceinline__ float4 load_planes4(const bf* hi, const bf* lo, int64_t off) {
-  float4 a = bf4_to_f4(*reinterpret_cast<const uint2*>(hi + off));
-  if (lo) {
-    const float4 b = bf4_to_f4(*reinterpret_cast<const uint2*>(lo + off));
-    a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-  }
-  return a;
-}
 __device__ __forceinline__ uint32_t pack_bf2(float a, float b) {
   const __nv_bfloat162 t = __halves2bfloat162(__float2bfloat16_rn(a), __float2bfloat16_rn(b));
   return *reinterpret_cast<const uint32_t*>(&t);
@@ -70,237 +58,11 @@ __device__ __forceinline__ void store_planes4(bf* hi, bf* lo, int64_t off, float
   }
 }
 
-// ============================================================================================ depthwise Conv3d
-struct DwParams {
-  const bf* x_hi; const bf* x_lo; const float* x_f32; int64_t x_pitch;
-  const float* w;
-  float* y; int64_t y_pitch; float* stats;
-  int n, T, H, W, C, Cv, oT, oH, oW, kt, kh, kw, st, sh, sw, pt, ph, pw;
-  int tiles_per_sample, tile_pos, m_tiles;
-  const float* dy; int64_t dy_pitch;
-  float* dx; bf* dx_hi; bf* dx_lo; int64_t dx_pitch; int dx_accumulate;
-  float* wpartials; int wblocks;
-};
-
-__device__ __forceinline__ float4 dw_load_x(const DwParams& p, int64_t row, int c) {
-  const int64_t off = row * p.x_pitch + c;
-  if (p.x_f32) return *reinterpret_cast<const float4*>(p.x_f32 + off);
-  return load_planes4(p.x_hi, p.x_lo, off);
-}
-// stage the filter transposed ([tap][C], pad channels zero) so that one LDS.128 fetches a tap for 4 channels
-__device__ __forceinline__ void dw_stage_filter(const DwParams& p, float* wsm, int taps) {
-  for (int i = threadIdx.x; i < taps * p.C; i += blockDim.x) {
-    const int k = i / p.C, c = i - k * p.C;
-    wsm[i] = c < p.Cv ? p.w[c * taps + k] : 0.f;
-  }
-}
-
-__global__ void __launch_bounds__(256) dwconv_fwd_kernel(const DwParams p) {
-  extern __shared__ float sm[];
-  const int taps = p.kt * p.kh * p.kw;
-  float* wsm = sm;                 // [taps][C]
-  float* red = sm + taps * p.C;    // [PL][2][C]
-  dw_stage_filter(p, wsm, taps);
-  __syncthreads();
-  const int cq = p.C >> 2;
-  const int PL = blockDim.x / cq;
-  const int tile = blockIdx.x;
-  const int n = tile / p.tiles_per_sample;
-  const int tl = tile - n * p.tiles_per_sample;
-  const int P = p.oT * p.oH * p.oW;
-  const int pos0 = tl * p.tile_pos;
-  const int pos1 = min(P, pos0 + p.tile_pos);
-  const int pl = threadIdx.x / cq;
-  const int c = (threadIdx.x - pl * cq) * 4;
-  if (pl < PL) {
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s;
-    for (int pos = pos0 + pl; pos < pos1; pos += PL) {
-      const int ox = pos % p.oW;
-      const int t2 = pos / p.oW;
-      const int oy = t2 % p.oH;
-      const int oz = t2 / p.oH;
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int kz = 0; kz < p.kt; ++kz) {
-        const int iz = oz * p.st - p.pt + kz;
-        if (iz < 0 || iz >= p.T) continue;
-        for (int ky = 0; ky < p.kh; ++ky) {
-          const int iy = oy * p.sh - p.ph + ky;
-          if (iy < 0 || iy >= p.H) continue;
-          const int64_t rbase = ((int64_t(n) * p.T + iz) * p.H + iy) * p.W;
-          for (int kx = 0; kx < p.kw; ++kx) {
-            const int ix = ox * p.sw - p.pw + kx;
-            if (ix < 0 || ix >= p.W) continue;
-            const float4 v = dw_load_x(p, rbase + ix, c);
-            const float4 wv = *reinterpret_cast<const float4*>(wsm + ((kz * p.kh + ky) * p.kw + kx) * p.C + c);
-            acc.x = fmaf(v.x, wv.x, acc.x);
-            acc.y = fmaf(v.y, wv.y, acc.y);
-            acc.z = fmaf(v.z, wv.z, acc.z);
-            acc.w = fmaf(v.w, wv.w, acc.w);
-          }
-        }
-      }
-      *reinterpret_cast<float4*>(p.y + (int64_t(n) * P + pos) * p.y_pitch + c) = acc;
-      s.x += acc.x; s.y += acc.y; s.z += acc.z; s.w += acc.w;
-      s2.x = fmaf(acc.x, acc.x, s2.x); s2.y = fmaf(acc.y, acc.y, s2.y);
-      s2.z = fmaf(acc.z, acc.z, s2.z); s2.w = fmaf(acc.w, acc.w, s2.w);
-    }
-    if (p.stats) {
-      *reinterpret_cast<float4*>(red + (pl * 2 + 0) * p.C + c) = s;
-      *reinterpret_cast<float4*>(red + (pl * 2 + 1) * p.C + c) = s2;
-    }
-  }
-  if (!p.stats) return;
-  __syncthreads();
-  for (int ch = threadIdx.x; ch < p.Cv; ch += blockDim.x) {
-    float a = 0.f, b = 0.f;
-    for (int j = 0; j < PL; ++j) {
-      a += red[(j * 2 + 0) * p.C + ch];
-      b += red[(j * 2 + 1) * p.C + ch];
-    }
-    p.stats[size_t(ch) * p.m_tiles + tile] = a;
-    p.stats[(size_t(p.Cv) + ch) * p.m_tiles + tile] = b;
-  }
-}
-
-// dx[n, ipos, c] (=|+=) sum over taps of dy[n, opos(tap), c] * w[c][tap]     (gather form: no atomics)
-__global__ void __launch_bounds__(256) dwconv_bwd_data_kernel(const DwParams p) {
-  extern __shared__ float sm[];
-  const int taps = p.kt * p.kh * p.kw;
-  dw_stage_filter(p, sm, taps);
-  __syncthreads();
-  const int cq = p.C >> 2;
-  const int P = p.oT * p.oH * p.oW;
-  const int64_t items = int64_t(p.n) * p.T * p.H * p.W * cq;
-  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < items; i += int64_t(gridDim.x) * blockDim.x) {
-    const int64_t row = i / cq;
-    const int c = int(i - row * cq) * 4;
-    int64_t t = row;
-    const int ix = int(t % p.W);
-    t /= p.W;
-    const int iy = int(t % p.H);
-    t /= p.H;
-    const int iz = int(t % p.T);
-    const int64_t n = t / p.T;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int kz = 0; kz < p.kt; ++kz) {
-      const int zz = iz + p.pt - kz;
-      if (zz < 0 || zz % p.st) continue;
-      const int oz = zz / p.st;
-      if (oz >= p.oT) continue;
-      for (int ky = 0; ky < p.kh; ++ky) {
-        const int yy = iy + p.ph - ky;
-        if (yy < 0 || yy % p.sh) continue;
-        const int oy = yy / p.sh;
-        if (oy >= p.oH) continue;
-        for (int kx = 0; kx < p.kw; ++kx) {
-          const int xx = ix + p.pw - kx;
-          if (xx < 0 || xx % p.sw) continue;
-          const int ox = xx / p.sw;
-          if (ox >= p.oW) continue;
-          const int64_t orow = n * P + (int64_t(oz) * p.oH + oy) * p.oW + ox;
-          const float4 g = *reinterpret_cast<const float4*>(p.dy + orow * p.dy_pitch + c);
-          const float4 wv = *reinterpret_cast<const float4*>(sm + ((kz * p.kh + ky) * p.kw + kx) * p.C + c);
-          acc.x = fmaf(g.x, wv.x, acc.x);
-          acc.y = fmaf(g.y, wv.y, acc.y);
-          acc.z = fmaf(g.z, wv.z, acc.z);
-          acc.w = fmaf(g.w, wv.w, acc.w);
-        }
-      }
-    }
-    if (p.dx) {
-      float4* d = reinterpret_cast<float4*>(p.dx + row * p.dx_pitch + c);
-      if (p.dx_accumulate) {
-        const float4 o = *d;
-        acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
-      }
-      *d = acc;
-    } else {
-      store_planes4(p.dx_hi, p.dx_lo, row * p.dx_pitch + c, acc);
-    }
-  }
-}
-
-// weight-gradient partials: wpartials[block][c][tap] = sum over the block's output positions of dy * x(tap)
-// block = C x PL threads (channel fastest: coalesced), one register accumulator per tap (the tap loops are fully
-// unrolled over the template's maximum extents so every accumulator index is static), smem tree over PL
-constexpr int DW_MAX_TAPS = 27;
-template <int KT, int KH, int KW>
-__global__ void __launch_bounds__(512) dwconv_bwd_weight_kernel(const DwParams p) {
-  extern __shared__ float sm[];  // [PL][C][taps]
-  const int taps = p.kt * p.kh * p.kw;
-  const int PL = blockDim.x / p.C;
-  const int pl = threadIdx.x / p.C;
-  const int c = threadIdx.x - pl * p.C;
-  const int P = p.oT * p.oH * p.oW;
-  const int64_t total = int64_t(p.n) * P;
-  const int64_t per = (total + gridDim.x - 1) / gridDim.x;
-  const int64_t r0 = blockIdx.x * per, r1 = min(total, r0 + per);
-  float acc[KT * KH * KW];
-#pragma unroll
-  for (int k = 0; k < KT * KH * KW; ++k) acc[k] = 0.f;
-  for (int64_t r = r0 + pl; r < r1; r += PL) {
-    const float g = p.dy[r * p.dy_pitch + c];
-    int64_t t = r;
-    const int ox = int(t % p.oW);
-    t /= p.oW;
-    const int oy = int(t % p.oH);
-    t /= p.oH;
-    const int oz = int(t % p.oT);
-    const int64_t n = t / p.oT;
-#pragma unroll
-    for (int kz = 0; kz < KT; ++kz) {
-      const int iz = oz * p.st - p.pt + kz;
-      if (kz >= p.kt || iz < 0 || iz >= p.T) continue;
-#pragma unroll
-      for (int ky = 0; ky < KH; ++ky) {
-        const int iy = oy * p.sh - p.ph + ky;
-        if (ky >= p.kh || iy < 0 || iy >= p.H) continue;
-#pragma unroll
-        for (int kx = 0; kx < KW; ++kx) {
-          const int ix = ox * p.sw - p.pw + kx;
-          if (kx >= p.kw || ix < 0 || ix >= p.W) continue;
-          const int64_t off = (((n * p.T + iz) * p.H + iy) * p.W + ix) * p.x_pitch + c;
-          float xv;
-          if (p.x_f32) {
-            xv = p.x_f32[off];
-          } else {
-            xv = __bfloat162float(p.x_hi[off]);
-            if (p.x_lo) xv += __bfloat162float(p.x_lo[off]);
-          }
-          acc[(kz * KH + ky) * KW + kx] = fmaf(g, xv, acc[(kz * KH + ky) * KW + kx]);
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int kz = 0; kz < KT; ++kz)
-#pragma unroll
-    for (int ky = 0; ky < KH; ++ky)
-#pragma unroll
-      for (int kx = 0; kx < KW; ++kx)
-        if (kz < p.kt && ky < p.kh && kx < p.kw)
-          sm[(size_t(pl) * p.C + c) * taps + (kz * p.kh + ky) * p.kw + kx] = acc[(kz * KH + ky) * KW + kx];
-  __syncthreads();
-  for (int i = threadIdx.x; i < p.C * taps; i += blockDim.x) {
-    float v = 0.f;
-    for (int j = 0; j < PL; ++j) v += sm[size_t(j) * p.C * taps + i];
-    p.wpartials[size_t(blockIdx.x) * p.C * taps + i] = v;
-  }
-}
-__global__ void dwconv_wmerge_kernel(const float* __restrict__ partials, int nblocks, int C, int Cv, int taps,
-                                     float* __restrict__ dw) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;  // over Cv*taps
-  if (i >= Cv * taps) return;
-  double v = 0.0;
-  for (int b = 0; b < nblocks; ++b) v += double(partials[size_t(b) * C * taps + i]);
-  dw[i] = float(v);
-}
-
 // ============================================================================================ channelwise conv, v2
 // Register-tiled kernels for fp32 inputs: one thread owns ONE channel (consecutive lanes = consecutive channels, so
 // every load / store instruction of a warp is a contiguous 128-byte line) and a micro-tile of OTT x OHT x OWT
 // outputs; the filter lives in registers, every loaded input value feeds up to KH*KW FMAs of several outputs
-// (3.0 FMA per load for 3x3x3 stride 1 against 1.0 for the per-output gather above).  The producer's BatchNorm + ReLU
+// (3.0 FMA per load for 3x3x3 stride 1 against 1.0 for a per-output gather).  The producer's BatchNorm + ReLU
 // can be applied on the fly (x = relu(x*in_scale + in_shift)), so the activation between X3DTransform.a and .b is
 // never materialised.  The same kernel computes stride-1 data gradients (correlation with the mirrored filter).
 struct Dw2Params {
@@ -1258,44 +1020,6 @@ static int dw_tiles_per_sample(int n, int64_t P) {
   if (want > maxt) want = maxt;
   return int(want < 1 ? 1 : want);
 }
-static int dw_fill(DwParams& p, const sfb_dwconv_desc* d, const char* who) {
-  memset(&p, 0, sizeof(p));
-  if (d->c % 8 || d->c <= 0 || d->c > 1024 || d->c_valid > d->c || d->c_valid <= 0) {
-    set_error("%s: c=%d must be a positive multiple of 8 (<= 1024) with c_valid=%d <= c", who, d->c, d->c_valid);
-    return -10;
-  }
-  if (d->kt * d->kh * d->kw > DW_MAX_TAPS || d->kh > 3 || d->kw > 3 || d->kt > 5 ||
-      (d->kt > 3 && (d->kh > 1 || d->kw > 1))) {
-    set_error("%s: filter %dx%dx%d is outside the supported range (<= 27 taps, kh,kw <= 3, kt <= 5)", who, d->kt,
-              d->kh, d->kw);
-    return -10;
-  }
-  if (d->x_pitch % 4 || (d->x_f32 == nullptr && d->x_hi == nullptr)) {
-    set_error("%s: bad input operand", who);
-    return -10;
-  }
-  p.x_hi = (const bf*)d->x_hi; p.x_lo = (const bf*)d->x_lo; p.x_f32 = d->x_f32; p.x_pitch = d->x_pitch;
-  p.w = d->w; p.y = d->y; p.y_pitch = d->y_pitch; p.stats = d->stats;
-  p.n = d->n; p.T = d->t; p.H = d->h; p.W = d->w_; p.C = d->c; p.Cv = d->c_valid;
-  p.oT = d->ot; p.oH = d->oh; p.oW = d->ow;
-  p.kt = d->kt; p.kh = d->kh; p.kw = d->kw; p.st = d->st; p.sh = d->sh; p.sw = d->sw;
-  p.pt = d->pt; p.ph = d->ph; p.pw = d->pw;
-  const int64_t P = int64_t(d->ot) * d->oh * d->ow;
-  p.tiles_per_sample = dw_tiles_per_sample(d->n, P);
-  p.tile_pos = int((P + p.tiles_per_sample - 1) / p.tiles_per_sample);
-  p.m_tiles = d->n * p.tiles_per_sample;
-  p.dy = d->dy; p.dy_pitch = d->dy_pitch;
-  p.dx = d->dx; p.dx_hi = (bf*)d->dx_hi; p.dx_lo = (bf*)d->dx_lo; p.dx_pitch = d->dx_pitch;
-  p.dx_accumulate = d->dx_accumulate;
-  p.wpartials = d->wpartials;
-  return 0;
-}
-static int dw_wblocks(const sfb_dwconv_desc* d) {
-  const int64_t total = int64_t(d->n) * d->ot * d->oh * d->ow;
-  int64_t nb = (total + 63) / 64;
-  if (nb > 148 * 4) nb = 148 * 4;
-  return int(nb < 1 ? 1 : nb);
-}
 static void bnact_fill(BnActParams& p, const sfb_bnact_desc* d) {
   memset(&p, 0, sizeof(p));
   p.y = d->y; p.y_pitch = d->y_pitch; p.scale = d->scale; p.shift = d->shift; p.mean = d->mean; p.invstd = d->invstd;
@@ -1331,12 +1055,29 @@ static void se_fill(SeParams& p, const sfb_se_desc* d) {
 
 
 // ------------------------------------------------------------------------------------------------ v2 dispatch
-// cfg: 0 = 3x3x3 stride (1,1,1), 1 = 3x3x3 stride (1,2,2), 2 = 5x1x1 stride 1;  -1 = use the generic kernels
+// The geometries the channelwise kernels take: c a multiple of 8 up to 512 (one block of <= 512 threads spans the
+// channels), temporal stride 1, and a 3x3x3 filter at spatial stride 1 or 2 or a 5x1x1 filter at stride 1.
+// cfg: 0 = 3x3x3 stride (1,1,1), 1 = 3x3x3 stride (1,2,2), 2 = 5x1x1 stride 1;  -1 = no kernel takes the geometry
 static int dw2_cfg(const sfb_dwconv_desc* d) {
-  if (d->x_f32 == nullptr || d->st != 1 || d->c > 512) return -1;
+  if (d->c % 8 || d->c <= 0 || d->c > 512 || d->st != 1) return -1;
   if (d->kt == 3 && d->kh == 3 && d->kw == 3 && d->sh == d->sw && (d->sh == 1 || d->sh == 2)) return d->sh == 1 ? 0 : 1;
   if (d->kt == 5 && d->kh == 1 && d->kw == 1 && d->sh == 1 && d->sw == 1) return 2;
   return -1;
+}
+// dw2_cfg of a convolution call, or -1 with the error set when no kernel takes its geometry or operands
+static int dw2_cfg_checked(const sfb_dwconv_desc* d, const char* who) {
+  const int cfg = dw2_cfg(d);
+  if (cfg < 0) {
+    set_error("%s: c=%d, filter %dx%dx%d, stride (%d,%d,%d): the channelwise kernels take c a multiple of 8 <= 512, "
+              "temporal stride 1 and a 3x3x3 filter at spatial stride 1 or 2 or a 5x1x1 filter at stride 1",
+              who, d->c, d->kt, d->kh, d->kw, d->st, d->sh, d->sw);
+    return -1;
+  }
+  if (d->x_f32 == nullptr || d->x_pitch % 4 || d->c_valid <= 0 || d->c_valid > d->c) {
+    set_error("%s: needs an fp32 input with a pitch multiple of 4 and 0 < c_valid=%d <= c=%d", who, d->c_valid, d->c);
+    return -1;
+  }
+  return cfg;
 }
 static const int kDw2Tile[3][3] = {{1, 2, 4}, {1, 1, 4}, {4, 1, 1}};
 // spatial lanes of a block: 512 threads over the channels
@@ -1373,12 +1114,12 @@ static void dw2_block_split(Dw2Params& p, int c, int* blocks) {
   p.mts_per_block = (p.total_mts + nb - 1) / nb;
   *blocks = int((p.total_mts + p.mts_per_block - 1) / p.mts_per_block);
 }
-// v3 (shared-memory ring) eligibility: 3x3x3, stride 1, padding 1, fp32 input, H and W multiples of 7.  tile = 14x14 or 7x7
+// v3 (shared-memory ring) eligibility: 3x3x3, stride 1, padding 1, H and W multiples of 7.  tile = 14x14 or 7x7
 // `samples` x `c` decide between 14x14 tiles (31 % halo) and 7x7 tiles (65 % halo, 4x the blocks): the big tile only when it
 // still yields two blocks per SM (ncu r2h: 48-block launches at 255 GB/s on the 14x14 stages of MViT)
 static int dw3_tile(int t, int h, int w, int ot, int oh, int ow, int kt, int kh, int kw, int st, int sh, int sw, int pt,
-                    int ph, int pw, bool f32, int samples, int c, bool wgrad = false) {
-  if (!f32 || kt != 3 || kh != 3 || kw != 3 || st != 1 || sh != 1 || sw != 1 || pt != 1 || ph != 1 ||
+                    int ph, int pw, int samples, int c, bool wgrad = false) {
+  if (kt != 3 || kh != 3 || kw != 3 || st != 1 || sh != 1 || sw != 1 || pt != 1 || ph != 1 ||
       pw != 1 || ot != t || oh != h || ow != w || t < 2)
     return 0;
   if (h % 14 == 0 && w % 14 == 0) {
@@ -1392,7 +1133,7 @@ static int dw3_tile(int t, int h, int w, int ot, int oh, int ow, int kt, int kh,
 }
 static int dw3_tile_of(const sfb_dwconv_desc* d, bool wgrad = false) {
   return dw3_tile(d->t, d->h, d->w_, d->ot, d->oh, d->ow, d->kt, d->kh, d->kw, d->st, d->sh, d->sw, d->pt, d->ph, d->pw,
-                  d->x_f32 != nullptr, d->n, d->c, wgrad);
+                  d->n, d->c, wgrad);
 }
 template <int TILE, int S>
 static size_t dw3_smem(bool wgrad) {
@@ -1437,9 +1178,9 @@ static int dw3_launch(int tile, bool wgrad, Dw2Params& p, cudaStream_t st, int s
   return 0;
 }
 
-// stride (1,2,2) eligibility: 3x3x3, padding 1, fp32 input, even input extents, output extents multiples of 7
+// stride (1,2,2) eligibility: 3x3x3, padding 1, even input extents, output extents multiples of 7
 static bool dw3_s2_ok(const sfb_dwconv_desc* d) {
-  return d->x_f32 != nullptr && d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 2 &&
+  return d->kt == 3 && d->kh == 3 && d->kw == 3 && d->st == 1 && d->sh == 2 &&
          d->sw == 2 && d->pt == 1 && d->ph == 1 && d->pw == 1 && d->ot == d->t && d->h == 2 * d->oh && d->w_ == 2 * d->ow &&
          d->oh % 7 == 0 && d->ow % 7 == 0 && d->t >= 2;
 }
@@ -1450,7 +1191,7 @@ int dw3_run_strided(int mode, const float* x, int64_t x_pitch, int64_t x_so, int
                     const float* w, int flip, float* y, int64_t y_pitch, int64_t y_so, int64_t y_si, int y_accumulate,
                     const float* dy, int64_t dy_pitch, int64_t dy_so, int64_t dy_si, float* dw, int n_outer, int n_inner,
                     int T, int H, int W, int C, cudaStream_t st) {
-  const int tile = dw3_tile(T, H, W, T, H, W, 3, 3, 3, 1, 1, 1, 1, 1, 1, true, n_outer * n_inner, C, mode == 1);
+  const int tile = dw3_tile(T, H, W, T, H, W, 3, 3, 3, 1, 1, 1, 1, 1, 1, n_outer * n_inner, C, mode == 1);
   if (!tile || C % 4) return -100;
   Dw2Params p;
   memset(&p, 0, sizeof(p));
@@ -1503,24 +1244,20 @@ using namespace sfb;
 
 extern "C" int32_t sfb_dwconv_tiles_per_sample(const sfb_dwconv_desc* d) {
   const int cfg = dw2_cfg(d);
+  if (cfg < 0) return 0;
   if (cfg == 0) {
-    // (the tiling query carries only the null-ness of x_f32; dims decide)
     const int t3 = dw3_tile_of(d);
     if (t3) return (d->h / t3) * (d->w_ / t3);
   }
   if (cfg == 1 && dw3_s2_ok(d)) return (d->oh / 7) * (d->ow / 7);
-  if (cfg >= 0) {
-    Dw2Params p;
-    dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg, p);
-    return p.tiles_per_sample;
-  }
-  return dw_tiles_per_sample(d->n, int64_t(d->ot) * d->oh * d->ow);
+  Dw2Params p;
+  dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg, p);
+  return p.tiles_per_sample;
 }
 extern "C" int32_t sfb_dwconv_m_tiles(const sfb_dwconv_desc* d) { return d->n * sfb_dwconv_tiles_per_sample(d); }
 extern "C" int sfb_dwconv_fwd(const sfb_dwconv_desc* d, void* stream) {
-  DwParams p;
-  if (int rc = dw_fill(p, d, "sfb_dwconv_fwd")) return rc;
-  const int cfg2 = dw2_cfg(d);
+  const int cfg2 = dw2_cfg_checked(d, "sfb_dwconv_fwd");
+  if (cfg2 < 0) return -10;
   if (cfg2 == 0) {
     if (const int t3 = dw3_tile_of(d)) {
       Dw2Params q;
@@ -1535,135 +1272,76 @@ extern "C" int sfb_dwconv_fwd(const sfb_dwconv_desc* d, void* stream) {
     q.y = d->y; q.y_pitch = d->y_pitch; q.stats = d->stats;
     return dw3_launch(7, false, q, (cudaStream_t)stream, 2);
   }
-  if (cfg2 >= 0) {
+  Dw2Params q;
+  dw2_common(q, d);
+  dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg2, q);
+  q.y = d->y; q.y_pitch = d->y_pitch; q.stats = d->stats;
+  const int sp = dw2_sp(d->c);
+  return dw2_launch_conv(cfg2, q, sp * d->c, size_t(sp) * 2 * d->c * sizeof(float), (cudaStream_t)stream);
+}
+extern "C" int sfb_dwconv_bwd(const sfb_dwconv_desc* d, float* dw, void* stream) {
+  const int cfg2 = dw2_cfg_checked(d, "sfb_dwconv_bwd");
+  if (cfg2 < 0) return -10;
+  const int taps = d->kt * d->kh * d->kw;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int sp = dw2_sp(d->c);
+  const int threads = sp * d->c;
+  const int t3 = cfg2 == 0 ? dw3_tile_of(d) : 0;
+  if (dw != nullptr && cfg2 == 1 && dw3_s2_ok(d)) {
+    Dw2Params q;
+    dw2_common(q, d);
+    q.dy = d->dy; q.dy_pitch = d->dy_pitch; q.dw = dw;
+    cudaMemsetAsync(dw, 0, size_t(d->c_valid) * taps * sizeof(float), st);
+    if (int rc = dw3_launch(7, true, q, st, 2)) return rc;
+  } else if (dw != nullptr && t3) {
+    Dw2Params q;
+    dw2_common(q, d);
+    q.dy = d->dy; q.dy_pitch = d->dy_pitch; q.dw = dw;
+    cudaMemsetAsync(dw, 0, size_t(d->c_valid) * taps * sizeof(float), st);
+    if (int rc = dw3_launch(dw3_tile_of(d, true), true, q, st)) return rc;
+  } else if (dw != nullptr) {
     Dw2Params q;
     dw2_common(q, d);
     dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg2, q);
-    q.y = d->y; q.y_pitch = d->y_pitch; q.stats = d->stats;
-    const int sp = dw2_sp(d->c);
-    return dw2_launch_conv(cfg2, q, sp * d->c, size_t(sp) * 2 * d->c * sizeof(float), (cudaStream_t)stream);
-  }
-  if (d->in_scale != nullptr) {
-    set_error("sfb_dwconv_fwd: the fused input transform needs an fp32 input and a 3x3x3 / 5x1x1 filter");
-    return -10;
-  }
-  const int taps = d->kt * d->kh * d->kw;
-  const int cq = d->c / 4;
-  const int PL = 256 / cq;
-  const size_t smem = (size_t(taps) * d->c + size_t(PL) * 2 * d->c) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(dwconv_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr = true;
-  }
-  dwconv_fwd_kernel<<<p.m_tiles, 256, smem, (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_dwconv_fwd");
-  return 0;
-}
-extern "C" int32_t sfb_dwconv_wgrad_blocks(const sfb_dwconv_desc* d) { return dw_wblocks(d); }
-extern "C" int sfb_dwconv_bwd(const sfb_dwconv_desc* d, float* dw, void* stream) {
-  DwParams p;
-  if (int rc = dw_fill(p, d, "sfb_dwconv_bwd")) return rc;
-  const int taps = d->kt * d->kh * d->kw;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int cfg2 = dw2_cfg(d);
-  if (cfg2 >= 0) {
-    const int sp = dw2_sp(d->c);
-    const int threads = sp * d->c;
-    const int t3 = cfg2 == 0 ? dw3_tile_of(d) : 0;
-    if (dw != nullptr && cfg2 == 1 && dw3_s2_ok(d)) {
-      Dw2Params q;
-      dw2_common(q, d);
-      q.dy = d->dy; q.dy_pitch = d->dy_pitch; q.dw = dw;
-      cudaMemsetAsync(dw, 0, size_t(d->c_valid) * taps * sizeof(float), st);
-      if (int rc = dw3_launch(7, true, q, st, 2)) return rc;
-    } else if (dw != nullptr && t3) {
-      Dw2Params q;
-      dw2_common(q, d);
-      q.dy = d->dy; q.dy_pitch = d->dy_pitch; q.dw = dw;
-      cudaMemsetAsync(dw, 0, size_t(d->c_valid) * taps * sizeof(float), st);
-      if (int rc = dw3_launch(dw3_tile_of(d, true), true, q, st)) return rc;
-    } else if (dw != nullptr) {
-      Dw2Params q;
-      dw2_common(q, d);
-      dw2_fwd_tiling(d->n, d->ot, d->oh, d->ow, d->c, cfg2, q);
-      q.dy = d->dy; q.dy_pitch = d->dy_pitch; q.dw = dw;
-      int blocks = 1;
-      dw2_block_split(q, d->c, &blocks);
-      cudaMemsetAsync(dw, 0, size_t(d->c_valid) * taps * sizeof(float), st);
-      if (int rc = dw2_launch_wgrad(cfg2, q, blocks, threads, size_t(sp) * d->c * taps * sizeof(float), st)) return rc;
-    }
-    if (d->dx != nullptr || d->dx_hi != nullptr) {
-      Dw2Params q;
-      dw2_common(q, d);
-      q.in_scale = nullptr; q.in_shift = nullptr; q.in_relu = 0;
-      q.x = d->dy; q.x_pitch = d->dy_pitch;
-      q.y = d->dx; q.y_hi = (bf*)d->dx_hi; q.y_lo = (bf*)d->dx_lo; q.y_pitch = d->dx_pitch;
-      q.y_accumulate = d->dx_accumulate;
-      if (cfg2 == 1) {
-        if (d->pt != 1 || d->ph != 1 || d->pw != 1 || d->dx == nullptr) {
-          set_error("sfb_dwconv_bwd: the stride-2 data gradient expects padding (1,1,1) and an fp32 output");
-          return -10;
-        }
-        // micro-tiles over the INPUT extent: one frame x 4 x 4 positions
-        q.mt_t = d->t; q.mt_h = (d->h + 3) / 4; q.mt_w = (d->w_ + 3) / 4;
-        q.MT = q.mt_t * q.mt_h * q.mt_w;
-        int blocks = 1;
-        dw2_block_split(q, d->c, &blocks);
-        dw2_dgrad_s2_kernel<<<blocks, threads, 0, st>>>(q);
-        SFB_X3_CHECK("sfb_dwconv_bwd (v2 stride-2 data)");
-      } else {
-        // stride 1: dx = correlation of dy with the mirrored filter, padding K-1-p; "input" = dy, "output" = dx
-        q.flip = 1;
-        q.T = d->ot; q.H = d->oh; q.W = d->ow;
-        q.oT = d->t; q.oH = d->h; q.oW = d->w_;
-        q.pt = d->kt - 1 - d->pt; q.ph = d->kh - 1 - d->ph; q.pw = d->kw - 1 - d->pw;
-        if (t3) {  // same extents in and out, padding 1: the ring kernel with the mirrored filter
-          q.stats = nullptr;
-          if (int rc = dw3_launch(t3, false, q, st)) return rc;
-          return 0;
-        }
-        dw2_fwd_tiling(d->n, d->t, d->h, d->w_, d->c, cfg2, q);
-        if (int rc = dw2_launch_conv(cfg2, q, threads, size_t(sp) * 2 * d->c * sizeof(float), st)) return rc;
-      }
-    }
-    return 0;
-  }
-  if (d->in_scale != nullptr) {
-    set_error("sfb_dwconv_bwd: the fused input transform needs an fp32 input and a 3x3x3 / 5x1x1 filter");
-    return -10;
-  }
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(dwconv_bwd_data_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(dwconv_bwd_weight_kernel<3, 3, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(dwconv_bwd_weight_kernel<5, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr = true;
-  }
-  if (dw != nullptr) {
-    if (d->wpartials == nullptr) {
-      set_error("sfb_dwconv_bwd: wpartials scratch missing");
-      return -10;
-    }
-    const int nb = dw_wblocks(d);
-    int threads = 512;
-    if (d->c > threads) threads = d->c;  // c <= 1024
-    const int PL = threads / d->c;
-    threads = PL * d->c;
-    const size_t smem = size_t(PL) * d->c * taps * sizeof(float);
-    if (d->kh == 1 && d->kw == 1)
-      dwconv_bwd_weight_kernel<5, 1, 1><<<nb, threads, smem, st>>>(p);
-    else
-      dwconv_bwd_weight_kernel<3, 3, 3><<<nb, threads, smem, st>>>(p);
-    SFB_X3_CHECK("sfb_dwconv_bwd(weight)");
-    const int items = d->c_valid * taps;
-    dwconv_wmerge_kernel<<<(items + 127) / 128, 128, 0, st>>>(d->wpartials, nb, d->c, d->c_valid, taps, dw);
-    SFB_X3_CHECK("sfb_dwconv_bwd(merge)");
+    q.dy = d->dy; q.dy_pitch = d->dy_pitch; q.dw = dw;
+    int blocks = 1;
+    dw2_block_split(q, d->c, &blocks);
+    cudaMemsetAsync(dw, 0, size_t(d->c_valid) * taps * sizeof(float), st);
+    if (int rc = dw2_launch_wgrad(cfg2, q, blocks, threads, size_t(sp) * d->c * taps * sizeof(float), st)) return rc;
   }
   if (d->dx != nullptr || d->dx_hi != nullptr) {
-    const int64_t items = int64_t(d->n) * d->t * d->h * d->w_ * (d->c / 4);
-    dwconv_bwd_data_kernel<<<x3_grid(items, 256, 16), 256, size_t(taps) * d->c * sizeof(float), st>>>(p);
-    SFB_X3_CHECK("sfb_dwconv_bwd(data)");
+    Dw2Params q;
+    dw2_common(q, d);
+    q.in_scale = nullptr; q.in_shift = nullptr; q.in_relu = 0;
+    q.x = d->dy; q.x_pitch = d->dy_pitch;
+    q.y = d->dx; q.y_hi = (bf*)d->dx_hi; q.y_lo = (bf*)d->dx_lo; q.y_pitch = d->dx_pitch;
+    q.y_accumulate = d->dx_accumulate;
+    if (cfg2 == 1) {
+      if (d->pt != 1 || d->ph != 1 || d->pw != 1 || d->dx == nullptr) {
+        set_error("sfb_dwconv_bwd: the stride-2 data gradient expects padding (1,1,1) and an fp32 output");
+        return -10;
+      }
+      // micro-tiles over the INPUT extent: one frame x 4 x 4 positions
+      q.mt_t = d->t; q.mt_h = (d->h + 3) / 4; q.mt_w = (d->w_ + 3) / 4;
+      q.MT = q.mt_t * q.mt_h * q.mt_w;
+      int blocks = 1;
+      dw2_block_split(q, d->c, &blocks);
+      dw2_dgrad_s2_kernel<<<blocks, threads, 0, st>>>(q);
+      SFB_X3_CHECK("sfb_dwconv_bwd (v2 stride-2 data)");
+    } else {
+      // stride 1: dx = correlation of dy with the mirrored filter, padding K-1-p; "input" = dy, "output" = dx
+      q.flip = 1;
+      q.T = d->ot; q.H = d->oh; q.W = d->ow;
+      q.oT = d->t; q.oH = d->h; q.oW = d->w_;
+      q.pt = d->kt - 1 - d->pt; q.ph = d->kh - 1 - d->ph; q.pw = d->kw - 1 - d->pw;
+      if (t3) {  // same extents in and out, padding 1: the ring kernel with the mirrored filter
+        q.stats = nullptr;
+        if (int rc = dw3_launch(t3, false, q, st)) return rc;
+        return 0;
+      }
+      dw2_fwd_tiling(d->n, d->t, d->h, d->w_, d->c, cfg2, q);
+      if (int rc = dw2_launch_conv(cfg2, q, threads, size_t(sp) * 2 * d->c * sizeof(float), st)) return rc;
+    }
   }
   return 0;
 }

@@ -395,16 +395,16 @@ class StemConvBN(ConvBN):
 
     def pack_input(self, x: torch.Tensor, key) -> "Act":
         n, c, t, h, w = x.shape
-        self.x_f32 = x.contiguous().float()  # kept for the direct weight-gradient kernel (narrow stems)
+        x_f32 = x.contiguous().float()
         # 8 output channels: one GEMM row = 8 output pixels (Toeplitz operands, csrc/conv_stem8.cu) when the extent allows
         self.t8 = bool(self.cout == 8 and
                        ops.stem8_supported(self.cin, self.cout, self.k, self.stride, self.pad, t, h, w))
         if self.t8:
             xin = Act(self.ctx.storage((key, "t8"), *ops.stem8_plane_dims(n, t, h, w)))
-            ops.stem8_input_fold(self.x_f32, xin.planes)
+            ops.stem8_input_fold(x_f32, xin.planes)
             return xin
         xin = Act(self.ctx.storage(key, n, t, h, w // 2, 8))
-        ops.stem_input_fold(self.x_f32, xin.planes)
+        ops.stem_input_fold(x_f32, xin.planes)
         return xin
 
     def fprop(self, x: Planes) -> torch.Tensor:
@@ -440,21 +440,12 @@ class StemConvBN(ConvBN):
 
     def wgrad(self, dy: Planes) -> None:
         ctx, g = self.ctx, self.g
-        if self.t8 and dy.pitch == 8:
-            dwm = ctx.scratch("dwm", self.cout * g.kfold, F32).view(self.cout, g.kfold)
-            ops.zero_f32(ops.f32view(dwm))
-            ops.stem8_wgrad(self.x, dy, g, dwm, nsplit=ctx.nsplit)
-            ops.stem_filter_unfold_grad(dwm, ctx.grad_of(self.conv.weight), g)
-            return
-        if (self.cout == 8 and self.cin == 3 and self.stride == (1, 2, 2) and self.pad[2] <= 4
-                and self.cin * self.taps <= 768 and dy.pitch == 8):
-            # 8 output channels fill 8 of the 128 UMMA rows: the fp32 SIMT kernel is ~3x faster and exact
-            ops.stem_wgrad_direct(self.x_f32, dy, self.k, self.stride, self.pad, ctx.grad_of(self.conv.weight))
-            return
-        assert not self.t8, "the W-shift weight gradient needs the W-shift clip layout"
         dwm = ctx.scratch("dwm", self.cout * g.kfold, F32).view(self.cout, g.kfold)
         ops.zero_f32(ops.f32view(dwm))
-        ops.stem_wgrad(self.x, dy, g, dwm, nsplit=ctx.nsplit)
+        if self.t8:
+            ops.stem8_wgrad(self.x, dy, g, dwm, nsplit=ctx.nsplit)
+        else:
+            ops.stem_wgrad(self.x, dy, g, dwm, nsplit=ctx.nsplit)
         ops.stem_filter_unfold_grad(dwm, ctx.grad_of(self.conv.weight), g)
 
     def dgrad(self, dy, x_act):  # pragma: no cover - the clip needs no gradient

@@ -198,7 +198,7 @@ _LIB = None
 # every symbol include/slowfast_b200.h declares: (name, restype, argtypes)
 class DwConvDesc(C.Structure):
     _fields_ = [
-        ("x_hi", C.c_void_p), ("x_lo", C.c_void_p), ("x_f32", C.c_void_p), ("x_pitch", C.c_int64),
+        ("x_f32", C.c_void_p), ("x_pitch", C.c_int64),
         ("w", C.c_void_p),
         ("y", C.c_void_p), ("y_pitch", C.c_int64), ("stats", C.c_void_p),
         ("n", C.c_int32), ("t", C.c_int32), ("h", C.c_int32), ("w_", C.c_int32), ("c", C.c_int32),
@@ -208,7 +208,6 @@ class DwConvDesc(C.Structure):
         ("dy", C.c_void_p), ("dy_pitch", C.c_int64),
         ("dx", C.c_void_p), ("dx_hi", C.c_void_p), ("dx_lo", C.c_void_p), ("dx_pitch", C.c_int64),
         ("dx_accumulate", C.c_int32),
-        ("wpartials", C.c_void_p),
         ("in_scale", C.c_void_p), ("in_shift", C.c_void_p), ("in_relu", C.c_int32),
     ]
 
@@ -341,12 +340,9 @@ _SIGNATURES = [
                                             C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_row_softmax", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_droppath_scales", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
-    ("sfb_stem_wgrad_direct", C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p] + [C.c_int32] * 10 +
-     [C.c_void_p, C.c_void_p]),
     ("sfb_dwconv_m_tiles", C.c_int32, [C.POINTER(DwConvDesc)]),
     ("sfb_dwconv_tiles_per_sample", C.c_int32, [C.POINTER(DwConvDesc)]),
     ("sfb_dwconv_fwd", C.c_int, [C.POINTER(DwConvDesc), C.c_void_p]),
-    ("sfb_dwconv_wgrad_blocks", C.c_int32, [C.POINTER(DwConvDesc)]),
     ("sfb_dwconv_bwd", C.c_int, [C.POINTER(DwConvDesc), C.c_void_p, C.c_void_p]),
     ("sfb_bnact_fwd", C.c_int, [C.POINTER(BnActDesc), C.c_void_p]),
     ("sfb_bnact_tiles_per_sample", C.c_int32, [C.c_int64, C.c_int64]),

@@ -143,7 +143,7 @@ class X3DBlockModule(Namespace):
         ot, oh, ow = g.out
         rps = ot * oh * ow
         yb = ctx.buf((nm, "yb"), (n, ot, oh, ow, cp))
-        m_tiles, tps = ops.dwconv_tiles(g, cp, True)
+        m_tiles, tps = ops.dwconv_tiles(g, cp)
         stats = ctx.buf((nm, "b.stats"), (2, c, m_tiles))
         ops.dwconv_fwd(g, cp, c, b2.b.weight, ops.f32view(yb), stats, x_f32=ops.f32view(ya), in_affine=a_affine)
         bb = {k: ctx.buf((nm, "b." + k), (cp,), zero=True) for k in ("scale", "shift", "mean", "invstd")}
@@ -196,7 +196,7 @@ class X3DBlockModule(Namespace):
             x.s.grad_written = True
         dyb = bn_gate_act_backward(ctx, ops.f32view(yb), bb, gate, sed, act, g.n, self._dim_inner, xb.grad_view(),
                                    b2.b_bn, getattr(b2, "se", None))
-        ops.dwconv_bwd(g, yb.shape[-1], self._dim_inner, b2.b.weight, dyb, ctx.grad_of(b2.b.weight), None,
+        ops.dwconv_bwd(g, yb.shape[-1], self._dim_inner, b2.b.weight, dyb, ctx.grad_of(b2.b.weight),
                        x_f32=ops.f32view(ya), in_affine=a_affine, dx=xa.grad_view(), dx_accumulate=False)
         xa.s.grad_written = True
         u["a"].bwd(xa.grad_view(), None, x, mask_from_y=True)
@@ -312,6 +312,7 @@ class B200X3D(_VideoResNetBase):
                                                           (1, 2, 2), (2, 1, 1)))
         dim_in = dim_res1
         dim_out = dim_inner = None
+        channelwise = [dim_res1]
         for stage, (reps, width, stride) in enumerate(block_basis):
             dim_out = round_width(width, w_mul)
             dim_inner = int(cfg.X3D.BOTTLENECK_FACTOR * dim_out)
@@ -319,6 +320,9 @@ class B200X3D(_VideoResNetBase):
             self.add_module(f"s{stage + 2}", X3DStageModule(f"s{stage + 2}", dim_in, dim_out, dim_inner, 3, stride,
                                                             n_rep, cfg.RESNET.STRIDE_1X1, ctx))
             dim_in = dim_out
+            channelwise.append(dim_inner)
+        assert max(channelwise) <= 512, \
+            f"channelwise width {max(channelwise)}: the engine's channelwise convolutions take at most 512 channels"
         self.head = X3DHeadModule(dim_out, dim_inner, cfg.X3D.DIM_C5, cfg.MODEL.NUM_CLASSES, cfg.MODEL.DROPOUT_RATE,
                                   cfg.MODEL.HEAD_ACT, cfg.X3D.BN_LIN5)
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN, False)
@@ -362,7 +366,7 @@ class B200X3D(_VideoResNetBase):
                        tuple(stem.conv.padding))
         ot, oh, ow = g.out
         y1 = ctx.buf(("s1", "y1"), (n, ot, oh, ow, c1))
-        m_tiles, _ = ops.dwconv_tiles(g, c1, True)
+        m_tiles, _ = ops.dwconv_tiles(g, c1)
         stats = ctx.buf(("s1", "stats"), (2, c1, m_tiles))
         ops.dwconv_fwd(g, c1, c1, stem.conv.weight, ops.f32view(y1), stats, x_f32=ops.f32view(y0))
         bb = {k: ctx.buf(("s1", k), (c1,), zero=True) for k in ("scale", "shift", "mean", "invstd")}
@@ -446,7 +450,7 @@ class B200X3D(_VideoResNetBase):
         dy1 = bn_gate_act_backward(ctx, ops.f32view(y1), bb, None, None, ops.ACT_RELU, g.n, c1, out.grad_view(),
                                    stem.bn, None)
         dy0 = ctx.scratch_planes("dy", *y0.shape)
-        ops.dwconv_bwd(g, c1, c1, stem.conv.weight, dy1, ctx.grad_of(stem.conv.weight), None, x_f32=ops.f32view(y0),
+        ops.dwconv_bwd(g, c1, c1, stem.conv.weight, dy1, ctx.grad_of(stem.conv.weight), x_f32=ops.f32view(y0),
                        dx_planes=dy0)
         u["xy"].wgrad(dy0)
         return [ctx.grad_of(p) for p in params]

@@ -833,19 +833,13 @@ class DwGeom:
                                                                      self.pad))
 
 
-def _dw_desc(g: DwGeom, c: int, c_valid: int, weight: torch.Tensor, x_planes: Optional[Planes] = None,
-             x_f32: Optional[F32View] = None, in_affine=None) -> "L.DwConvDesc":
-    """``in_affine`` = (scale, shift, relu): the producer's BatchNorm (+ReLU) applied on the fly to an fp32 input."""
+def _dw_desc(g: DwGeom, c: int, c_valid: int, weight: torch.Tensor, x_f32: F32View, in_affine=None) -> "L.DwConvDesc":
+    """``in_affine`` = (scale, shift, relu): the producer's BatchNorm (+ReLU) applied on the fly to the input."""
     d = L.DwConvDesc()
     if in_affine is not None:
-        assert x_f32 is not None
         d.in_scale, d.in_shift, d.in_relu = in_affine[0].data_ptr(), in_affine[1].data_ptr(), 1 if in_affine[2] else 0
-    if x_planes is not None:
-        assert x_planes.c == c and (x_planes.n, x_planes.t, x_planes.h, x_planes.w) == (g.n, g.t, g.h, g.w)
-        d.x_hi, d.x_lo, d.x_pitch = x_planes.hi_ptr(), x_planes.lo_ptr(), x_planes.pitch
-    else:
-        assert x_f32 is not None and x_f32.c == c and x_f32.rows == g.n * g.t * g.h * g.w
-        d.x_f32, d.x_pitch = x_f32.ptr(), x_f32.pitch
+    assert x_f32.c == c and x_f32.rows == g.n * g.t * g.h * g.w
+    d.x_f32, d.x_pitch = x_f32.ptr(), x_f32.pitch
     assert weight.is_contiguous() and weight.dtype == F32 and weight.shape[0] == c_valid and weight.shape[1] == 1
     assert tuple(weight.shape[2:]) == tuple(g.k)
     d.w = weight.data_ptr()
@@ -857,9 +851,9 @@ def _dw_desc(g: DwGeom, c: int, c_valid: int, weight: torch.Tensor, x_planes: Op
     return d
 
 
-def dwconv_tiles(g: DwGeom, c: int, f32_input: bool) -> Tuple[int, int]:
+def dwconv_tiles(g: DwGeom, c: int) -> Tuple[int, int]:
     """(m_tiles, tiles_per_sample) of the forward kernel's BatchNorm partials (depends on which kernel the library
-    picks for this geometry / input format)."""
+    picks for this geometry)."""
     lib = L.load()
     d = L.DwConvDesc()
     d.n, d.t, d.h, d.w_, d.c = g.n, g.t, g.h, g.w, c
@@ -867,33 +861,24 @@ def dwconv_tiles(g: DwGeom, c: int, f32_input: bool) -> Tuple[int, int]:
     d.kt, d.kh, d.kw = g.k
     d.st, d.sh, d.sw = g.stride
     d.pt, d.ph, d.pw = g.pad
-    d.x_f32 = 1 if f32_input else None  # only its null-ness matters here
     return lib.sfb_dwconv_m_tiles(C.byref(d)), lib.sfb_dwconv_tiles_per_sample(C.byref(d))
 
 
 def dwconv_fwd(g: DwGeom, c: int, c_valid: int, weight: torch.Tensor, y: F32View, stats: Optional[torch.Tensor],
-               x_planes: Optional[Planes] = None, x_f32: Optional[F32View] = None, in_affine=None) -> None:
+               x_f32: F32View, in_affine=None) -> None:
     lib = L.load()
-    d = _dw_desc(g, c, c_valid, weight, x_planes, x_f32, in_affine)
+    d = _dw_desc(g, c, c_valid, weight, x_f32, in_affine)
     assert y.c == c
     d.y, d.y_pitch, d.stats = y.ptr(), y.pitch, _ptr(stats)
     L.check(lib.sfb_dwconv_fwd(C.byref(d), _stream()), "sfb_dwconv_fwd")
     _count()
 
 
-def dwconv_wgrad_blocks(g: DwGeom) -> int:
-    d = L.DwConvDesc()
-    d.n = g.n
-    d.ot, d.oh, d.ow = g.out
-    return L.load().sfb_dwconv_wgrad_blocks(C.byref(d))
-
-
 def dwconv_bwd(g: DwGeom, c: int, c_valid: int, weight: torch.Tensor, dy: F32View, dw: Optional[torch.Tensor],
-               wpartials: Optional[torch.Tensor], x_planes: Optional[Planes] = None,
-               x_f32: Optional[F32View] = None, dx: Optional[F32View] = None, dx_planes: Optional[Planes] = None,
+               x_f32: F32View, dx: Optional[F32View] = None, dx_planes: Optional[Planes] = None,
                dx_accumulate: bool = False, in_affine=None) -> None:
     lib = L.load()
-    d = _dw_desc(g, c, c_valid, weight, x_planes, x_f32, in_affine)
+    d = _dw_desc(g, c, c_valid, weight, x_f32, in_affine)
     d.dy, d.dy_pitch = dy.ptr(), dy.pitch
     launches = 0
     if dx is not None:
@@ -906,8 +891,7 @@ def dwconv_bwd(g: DwGeom, c: int, c_valid: int, weight: torch.Tensor, dy: F32Vie
         launches += 1
     if dw is not None:
         assert dw.is_contiguous() and dw.numel() == weight.numel()
-        d.wpartials = _ptr(wpartials)  # (only the generic planes-input kernels need the scratch)
-        launches += 2
+        launches += 2  # memset + kernel
     L.check(lib.sfb_dwconv_bwd(C.byref(d), _ptr(dw), _stream()), "sfb_dwconv_bwd")
     _count(launches)
 
@@ -979,18 +963,6 @@ def relu_bwd(dx: torch.Tensor, y: torch.Tensor) -> None:
     assert dx.is_contiguous() and y.is_contiguous() and dx.numel() == y.numel()
     L.check(L.load().sfb_relu_bwd(dx.data_ptr(), y.data_ptr(), dx.numel(), _stream()), "sfb_relu_bwd")
     _count()
-
-
-def stem_wgrad_direct(x: torch.Tensor, dy: Planes, k, stride, pad, dw: torch.Tensor) -> None:
-    """dw[8,3,kt,kh,kw] = weight gradient of the 3 -> 8 channel stem from the fp32 NCTHW clip and the dY planes."""
-    lib = L.load()
-    n, cin, t, h, w = x.shape
-    assert x.dtype == F32 and x.is_contiguous() and dw.is_contiguous() and dy.pitch == dy.c == dw.shape[0]
-    L.check(lib.sfb_stem_wgrad_direct(x.data_ptr(), n, cin, t, h, w, dy.hi_ptr(), dy.lo_ptr(), dy.c, k[0], k[1], k[2],
-                                      stride[0], stride[1], stride[2], pad[0], pad[1], pad[2], dw.data_ptr(),
-                                      _stream()), "sfb_stem_wgrad_direct")
-    _count(2)
-
 
 
 # ------------------------------------------------------------------------------------------------ token path (MViT / ViT)

@@ -322,6 +322,8 @@ STEM_CASES = [
     # n, t, h, w, cin, cout, k, stride, pad
     (2, 4, 16, 32, 3, 64, (1, 7, 7), (1, 2, 2), (0, 3, 3)),     # slow-pathway / C2D stem
     (1, 6, 20, 48, 3, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),      # fast-pathway stem
+    (2, 9, 14, 64, 3, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),      # fast-pathway stem, H not a multiple of 16 (no Toeplitz)
+    (1, 32, 28, 224, 3, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),    # fast-pathway stem, full 112-pixel output rows
     (1, 2, 12, 300, 3, 24, (1, 3, 3), (1, 2, 2), (0, 1, 1)),    # X3D conv_xy, output row (150) > one 128-pixel tile
 ]
 
@@ -522,10 +524,10 @@ def test_maxpool3d_planes(k, s, p, cuda_device):
 # ------------------------------------------------------------------------------------------------ X3D kernels
 DW_CASES = [
     # n, t, h, w, c_valid, k, stride, pad, input format
-    (2, 4, 14, 14, 54, (3, 3, 3), (1, 1, 1), (1, 1, 1), "planes"),
-    (2, 4, 14, 14, 54, (3, 3, 3), (1, 2, 2), (1, 1, 1), "planes"),
-    (3, 4, 9, 9, 216, (3, 3, 3), (1, 2, 2), (1, 1, 1), "planes"),
-    (1, 3, 7, 7, 432, (3, 3, 3), (1, 1, 1), (1, 1, 1), "planes"),
+    (2, 4, 14, 14, 54, (3, 3, 3), (1, 1, 1), (1, 1, 1), "f32+affine"),
+    (2, 4, 14, 14, 54, (3, 3, 3), (1, 2, 2), (1, 1, 1), "f32+affine"),
+    (3, 4, 9, 9, 216, (3, 3, 3), (1, 2, 2), (1, 1, 1), "f32"),
+    (1, 3, 7, 7, 432, (3, 3, 3), (1, 1, 1), (1, 1, 1), "f32"),
     (2, 6, 12, 12, 24, (5, 1, 1), (1, 1, 1), (2, 0, 0), "f32"),
     (2, 5, 13, 15, 54, (3, 3, 3), (1, 1, 1), (1, 1, 1), "f32"),
     (2, 4, 14, 18, 108, (3, 3, 3), (1, 2, 2), (1, 1, 1), "f32"),
@@ -546,9 +548,10 @@ DW_CASES = [
 
 
 @pytest.mark.parametrize("case", DW_CASES)
-def test_dwconv_forward_backward(case, cuda_device):
-    """Channelwise Conv3d (X3DTransform.b / X3DStem.conv): y, BN partial sums, dx (fp32 and planes) and dw against
-    torch's grouped conv in fp64 on the operands the kernel saw; pad channels (54 -> 56) stay exactly zero."""
+def test_dwconv_fp32_forward_backward(case, cuda_device):
+    """Channelwise Conv3d (X3DTransform.b / X3DStem.conv) on its fp32 input, with or without the fused producer
+    BatchNorm + ReLU: y, BN partial sums, dx (fp32 and planes) and dw against torch's grouped conv in fp64; pad channels
+    (54 -> 56) stay exactly zero."""
     ops = _ops()
     n, t, h, w, c, k, stride, pad, fmt = case
     dev = cuda_device
@@ -560,11 +563,7 @@ def test_dwconv_forward_backward(case, cuda_device):
     wt = (torch.randn(c, 1, *k, generator=g) / (k[0] * k[1] * k[2]) ** 0.5).to(dev)
     geom = ops.DwGeom(n, t, h, w, k, stride, pad)
     ot, oh, ow = geom.out
-    if fmt == "planes":
-        xp = make_planes(x, 3)
-        xin = dict(x_planes=xp)
-        xv = planes_value(xp, 3)
-    elif fmt == "f32":
+    if fmt == "f32":
         xin = dict(x_f32=ops.f32view(x))
         xv = x.double()
     else:  # producer BatchNorm + ReLU applied on the fly (pad channels: scale = shift = 0)
@@ -575,7 +574,7 @@ def test_dwconv_forward_backward(case, cuda_device):
         xin = dict(x_f32=ops.f32view(x), in_affine=(sc, sh, True))
         xv = torch.relu(torch.addcmul(sh, x, sc)).double()
     y = torch.full((n, ot, oh, ow, cp), float("nan"), device=dev)
-    m_tiles, tps = ops.dwconv_tiles(geom, cp, fmt != "planes")
+    m_tiles, tps = ops.dwconv_tiles(geom, cp)
     stats = torch.zeros(2, c, m_tiles, device=dev)
     ops.dwconv_fwd(geom, cp, c, wt, ops.f32view(y), stats, **xin)
     ref = F.conv3d(xv[..., :c].permute(0, 4, 1, 2, 3), wt.double(), None, stride, pad, 1, c).permute(0, 2, 3, 4, 1)
@@ -595,19 +594,18 @@ def test_dwconv_forward_backward(case, cuda_device):
     F.conv3d(xr, wr, None, stride, pad, 1, c).backward(dy[..., :c].double().permute(0, 4, 1, 2, 3))
     dx = torch.full((n, t, h, w, cp), float("nan"), device=dev)
     dw = torch.empty_like(wt)
-    wp = torch.empty(ops.dwconv_wgrad_blocks(geom) * cp * wt[0].numel(), device=dev)
-    ops.dwconv_bwd(geom, cp, c, wt, ops.f32view(dy), dw, wp, dx=ops.f32view(dx), **xin)
+    ops.dwconv_bwd(geom, cp, c, wt, ops.f32view(dy), dw, dx=ops.f32view(dx), **xin)
     assert relerr(dx[..., :c], xr.grad.permute(0, 2, 3, 4, 1)) < 1e-5
     assert (dx[..., c:] == 0).all()
     assert relerr(dw, wr.grad) < 2e-5
-    if stride == (1, 1, 1) or fmt == "planes":  # (the stride-2 register-tiled data gradient is fp32-output only)
+    if stride == (1, 1, 1):  # (the stride-2 register-tiled data gradient is fp32-output only)
         dxp = ops.alloc_planes(n, t, h, w, cp, 3, dev)
-        ops.dwconv_bwd(geom, cp, c, wt, ops.f32view(dy), None, None, dx_planes=dxp, **xin)
+        ops.dwconv_bwd(geom, cp, c, wt, ops.f32view(dy), None, dx_planes=dxp, **xin)
         assert relerr(dxp.to_float()[..., :c], xr.grad.permute(0, 2, 3, 4, 1)) < 2e-5
     # accumulate form
     base = torch.randn(n, t, h, w, cp, generator=g).to(dev)
     acc = base.clone()
-    ops.dwconv_bwd(geom, cp, c, wt, ops.f32view(dy), None, None, dx=ops.f32view(acc), dx_accumulate=True, **xin)
+    ops.dwconv_bwd(geom, cp, c, wt, ops.f32view(dy), None, dx=ops.f32view(acc), dx_accumulate=True, **xin)
     assert relerr((acc - base)[..., :c], xr.grad.permute(0, 2, 3, 4, 1)) < 1e-4
 
 
@@ -751,30 +749,3 @@ def test_conv_padded_output_channels(cuda_device):
     assert relerr(y[..., :cout], ref) < TOL[3]
     assert (y[..., cout:] == 0).all()
     assert relerr(stats[1].sum(1), (ref * ref).sum((0, 1, 2, 3))) < 1e-4
-
-
-@pytest.mark.parametrize("shape", [(1, 6, 20, 48), (2, 9, 14, 64), (1, 32, 28, 224)])
-def test_stem_wgrad_direct(shape, cuda_device):
-    """fp32 SIMT weight gradient of the fast-pathway stem (3 -> 8, 5x7x7, stride (1,2,2)) vs torch autograd in fp64:
-    exact fp32 inputs on the X side, the (hi+lo) planes on the dY side."""
-    ops = _ops()
-    dev = cuda_device
-    n, t, h, w = shape
-    k, stride, pad = (5, 7, 7), (1, 2, 2), (2, 3, 3)
-    g = torch.Generator().manual_seed(11)
-    x = torch.randn(n, 3, t, h, w, generator=g).to(dev)
-    ot, oh, ow = t, (h + 6 - 7) // 2 + 1, (w + 6 - 7) // 2 + 1
-    dy = torch.randn(n, ot, oh, ow, 8, generator=g).to(dev)
-    dyp = make_planes(dy, 3)
-    dw = torch.full((8, 3, *k), float("nan"), device=dev)
-    ops.stem_wgrad_direct(x, dyp, k, stride, pad, dw)
-    wref = torch.zeros(8, 3, *k, dtype=torch.float64, device=dev, requires_grad=True)
-    (gref,) = torch.autograd.grad(F.conv3d(x.double(), wref, stride=stride, padding=pad), wref,
-                                  planes_value(dyp, 3).permute(0, 4, 1, 2, 3))
-    assert relerr(dw, gref) < 1e-5
-    # bf16 fast mode: no lo plane
-    dyp1 = make_planes(dy, 1)
-    ops.stem_wgrad_direct(x, dyp1, k, stride, pad, dw)
-    (gref1,) = torch.autograd.grad(F.conv3d(x.double(), wref, stride=stride, padding=pad), wref,
-                                   planes_value(dyp1, 1).permute(0, 4, 1, 2, 3))
-    assert relerr(dw, gref1) < 1e-5

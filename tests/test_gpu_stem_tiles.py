@@ -4,7 +4,8 @@ saw, with the BatchNorm partials against fp64 column sums and the weight gradien
 W-shift stem (csrc/conv_stem.cu): forward tile widths 16 / 32 / 48 / 64 (cout rounded up to 16), weight gradient with
 2 or 4 folded W taps and 3 or 4 (kt, kh) pairs per CTA, including groups padded past the last pair.  Toeplitz stem
 (csrc/conv_stem8.cu): 1, 3, 4 and 5 T taps, one and several bands, fewer steps than CTAs.  The extents leave partial
-128-pixel tiles, odd T / H tails and partial last waves."""
+128-pixel tiles, odd T / H tails and partial last waves.  The engine's fast-pathway stem unit, forward and backward, at
+the 158-wide short-cycle crop of multigrid training."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -128,3 +129,47 @@ def test_stem8_tiles(case, nsplit, cuda_device):
     dwm = pre.clone()
     ops.stem8_wgrad(xp, dyp, geo, dwm, nsplit=nsplit)
     _check_wgrad(dwm, pre, xr, dyp, geo, k, stride, pad, nsplit, dev)
+
+
+@pytest.mark.parametrize("nsplit", [1, 3])
+def test_fast_stem_unit_at_crop_158(nsplit, cuda_device):
+    """The engine's fast-pathway stem unit (StemConvBN: Conv3d 3 -> 8, 5x7x7, stride (1,2,2), + train-mode BatchNorm)
+    forward and backward on a 158 x 158 clip, multigrid's short-cycle crop: 158 is not a multiple of 16, so the W-shift
+    kernels take it instead of the Toeplitz ones.  Conv output and the conv / BN parameter gradients against fp64
+    conv3d + batch_norm autograd on the fp32 clip and weights."""
+    import torch.nn as nn
+    from slowfast_b200 import ops
+    from slowfast_b200.engine import Ctx, StemConvBN
+    dev = cuda_device
+    n, t, h, w = 2, 4, 158, 158
+    k, stride, pad = (5, 7, 7), (1, 2, 2), (2, 3, 3)
+    g = torch.Generator().manual_seed(17)
+    conv = nn.Conv3d(3, 8, k, stride, pad, bias=False)
+    bn = nn.BatchNorm3d(8)
+    with torch.no_grad():
+        conv.weight.copy_(torch.randn(conv.weight.shape, generator=g) / conv.weight[0].numel() ** 0.5)
+        bn.weight.copy_(torch.rand(8, generator=g) + 0.5)
+        bn.bias.copy_(torch.randn(8, generator=g) * 0.2)
+    conv, bn = conv.to(dev), bn.to(dev)
+    ctx = Ctx(nsplit)
+    ctx.device = dev
+    assert StemConvBN.supported(conv, w)
+    unit = StemConvBN("s1.pathway1_stem", conv, bn, ctx)
+    x = torch.randn(n, 3, t, h, w, generator=g).to(dev)
+    xin = unit.pack_input(x, ("in", 1))
+    assert not unit.t8
+    y = unit.fprop(xin.planes)
+    ctx.begin_backward([conv.weight, bn.weight, bn.bias])
+    dz = torch.randn(y.shape, generator=g).to(dev)
+    unit.bwd(ops.f32view(dz), None, None)
+    torch.cuda.synchronize()
+
+    wr, gr, br = (p.detach().double().requires_grad_(True) for p in (conv.weight, bn.weight, bn.bias))
+    yr = F.conv3d(x.double(), wr, stride=stride, padding=pad)
+    F.batch_norm(yr, None, None, gr, br, training=True, eps=bn.eps).backward(dz.double().permute(0, 4, 1, 2, 3))
+    # parity: split-bf16 operands; fast: bf16 operands (clip, weights and the conv-output gradient)
+    tol = 1e-4 if nsplit == 3 else 2e-2
+    assert relerr(y, yr.detach().permute(0, 2, 3, 4, 1)) < tol
+    assert relerr(ctx.grad_of(conv.weight), wr.grad) < tol
+    assert relerr(ctx.grad_of(bn.weight), gr.grad) < tol
+    assert relerr(ctx.grad_of(bn.bias), br.grad) < tol

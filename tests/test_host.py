@@ -168,6 +168,8 @@ def test_x3d_widths_and_parameter_count():
     assert [getattr(m, f"s{i}").pathway0_res0._dim_inner for i in range(2, 6)] == [54, 108, 216, 432]
     assert [se_width(c, 0.0625) for c in (54, 108, 216, 432)] == [8, 8, 16, 32]
     assert sum(p.numel() for p in m.parameters()) == 3794322  # 3.79 M (X3D-M, Kinetics-400 head)
+    with pytest.raises(AssertionError, match="512"):   # res5's channelwise conv would be 540 wide
+        B200X3D(get_cfg("X3D_M", X3D={"WIDTH_FACTOR": 2.5}))
 
 
 MORE_YAMLS = ["Kinetics/SLOW_8x8_R50.yaml", "Kinetics/SLOW_4x16_R50.yaml", "Kinetics/I3D_8x8_R50.yaml",
@@ -208,3 +210,26 @@ def test_stem8_selection_predicate_without_a_gpu():
     assert not ok(3, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3), 32, 224, 232)      # width not a multiple of 16
     assert not ok(3, 8, (5, 3, 3), (1, 2, 2), (2, 1, 1), 32, 224, 224)      # X3D-like 3x3
     assert ops.stem8_plane_dims(8, 32, 224, 224) == (8, 64, 112, 120, 8)
+
+
+def test_dwconv_rejects_geometries_no_kernel_takes():
+    """The channelwise convolution's geometry check is host logic in the C library: the tiling query returns 0 and
+    fwd / bwd fail with a message, before any launch, for what no kernel takes (here c > 512 and a temporal stride)."""
+    import ctypes as C
+    from slowfast_b200 import lib as L
+    from slowfast_b200 import ops
+    lib = L.load()
+    ok = ops.DwGeom(2, 8, 56, 56, (3, 3, 3), (1, 1, 1), (1, 1, 1))
+    assert ops.dwconv_tiles(ok, 432)[1] > 0 and ops.dwconv_tiles(ops.DwGeom(2, 8, 56, 56, (5, 1, 1), (1, 1, 1),
+                                                                            (2, 0, 0)), 48)[1] > 0
+    for geom, c in ((ok, 520), (ops.DwGeom(2, 8, 56, 56, (3, 3, 3), (2, 1, 1), (1, 1, 1)), 432)):
+        assert ops.dwconv_tiles(geom, c) == (0, 0)
+        d = L.DwConvDesc()
+        d.n, d.t, d.h, d.w_, d.c, d.c_valid = geom.n, geom.t, geom.h, geom.w, c, c
+        d.ot, d.oh, d.ow = geom.out
+        d.kt, d.kh, d.kw = geom.k
+        d.st, d.sh, d.sw = geom.stride
+        d.pt, d.ph, d.pw = geom.pad
+        assert lib.sfb_dwconv_fwd(C.byref(d), None) != 0
+        assert b"channelwise kernels take" in lib.sfb_last_error()
+        assert lib.sfb_dwconv_bwd(C.byref(d), None, None) != 0

@@ -91,8 +91,8 @@ def test_launch_counter_matches_the_device_activities_of_one_step(family, cuda_d
     """``ops.launches()`` advances by exactly the number of device activities the library issues in one eager training
     step (forward, targets, backward).  The library's activities are its kernels - those in namespace ``sfb::`` and the
     three csrc/mvit_ops.cu defines at file scope (LIBRARY_FILE_SCOPE_KERNELS) - and its own ``cudaMemsetAsync`` /
-    ``cudaMemset2DAsync`` calls (dwpool / dwconv weight gradients, gemm_batched split-K, zero_f32, the direct stem
-    wgrad).  Memsets are told apart from any torch issues in the same step by the profiler's
+    ``cudaMemset2DAsync`` calls (dwpool / dwconv weight gradients, gemm_batched split-K, zero_f32).  Memsets are told
+    apart from any torch issues in the same step by the profiler's
     correlation of each device activity with the host op that was open when it was enqueued: torch's own memsets run
     inside an ``aten::`` op, the library's from a ctypes call that no ``aten::`` op encloses."""
     from torch.autograd import DeviceType
