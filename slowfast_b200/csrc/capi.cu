@@ -1,6 +1,6 @@
 // Small C-ABI entry points that do not belong to a kernel file.
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 #ifndef SFB_BUILD_ARCH
 #define SFB_BUILD_ARCH "unknown"

@@ -11,7 +11,7 @@
 #include <dlfcn.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 // the two NCCL enums used (nccl.h: ncclFloat = 7, ncclSum = 0, ncclAvg = 4) and entry points, resolved lazily

@@ -16,7 +16,7 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -213,13 +213,7 @@ int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out) {
     case 32: conv_direct_kernel<32><<<p.m_tiles, 128, smem, stream>>>(p); break;
     default: conv_direct_kernel<64><<<p.m_tiles, 128, smem, stream>>>(p); break;
   }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_conv_igemm (direct SIMT body) launch failed: %s", cudaGetErrorString(e));
-    *rc_out = -20;
-  } else {
-    *rc_out = 0;
-  }
+  *rc_out = launch_status("sfb_conv_igemm (direct SIMT body)");
   return 1;
 }
 

@@ -23,7 +23,7 @@
 
 #include "../../include/slowfast_b200.h"
 #include "ptx.cuh"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -337,21 +337,6 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
 
 }
 
-static int g_num_sms = 0;
-static int g_smem_optin = 0;
-
-static int device_props() {
-  if (g_num_sms) return 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) {
-    set_error("cudaGetDevice failed: no CUDA device");
-    return -1;
-  }
-  cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&g_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  return 0;
-}
-
 static int pick_ck(int c) {
   if (c % 64 == 0) return 64;
   if (c % 32 == 0) return 32;
@@ -391,9 +376,8 @@ static bool rows_regular(const sfb_conv_desc* d) {
 // (short launches, where the zero fill and the statistics pass are fixed costs), narrow inputs (C_in <= 8 may take
 // the SIMT body), overwrites of views that are not a row matrix, and statistics of accumulating launches or over
 // channels that are not a multiple of 8 (sfb_bn_split_stats).
-static int conv_ksplit(const sfb_conv_desc* d, const ConvGrid& g, bool with_stats) {
+static int conv_ksplit(const sfb_conv_desc* d, const ConvGrid& g, int P, bool with_stats) {
   const int tiles = g.m_tiles * g.n_tiles;
-  const int P = g_num_sms;
   if (P <= 0 || d->c <= 8 || 2 * tiles < P) return 1;
   if ((d->accumulate == 0 || with_stats) && !rows_regular(d)) return 1;
   if (with_stats && (d->accumulate != 0 || d->cout % 8 != 0 || d->os_w % 4 != 0)) return 1;
@@ -410,19 +394,22 @@ using namespace sfb;
 
 extern "C" int64_t sfb_conv_m_tiles(const sfb_conv_desc* d) {
   const ConvGrid g = conv_grid(d);
-  if (device_props() == 0 && conv_ksplit(d, g, true) > 1)
+  int sms = 0;
+  if (device_limits(&sms, nullptr) == 0 && conv_ksplit(d, g, sms, true) > 1)
     return sfb_bn_split_stats_tiles(g.M, g.M, 1, d->cout);  // statistics from y after the split GEMM
   return g.m_tiles;
 }
 
 extern "C" int32_t sfb_conv_ksplit(const sfb_conv_desc* d) {
-  if (device_props()) return 1;
-  return conv_ksplit(d, conv_grid(d), d->stats != nullptr);
+  int sms = 0;
+  if (device_limits(&sms, nullptr)) return 1;
+  return conv_ksplit(d, conv_grid(d), sms, d->stats != nullptr);
 }
 
 extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (device_props()) return -1;
+  int num_sms = 0, smem_optin = 0;
+  if (device_limits(&num_sms, &smem_optin)) return -1;
   if (d->nsplit != 1 && d->nsplit != 3) {
     set_error("sfb_conv_igemm: nsplit must be 1 or 3 (got %d)", d->nsplit);
     return -10;
@@ -476,7 +463,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   p.BN = g.BN;
   p.n_tiles = g.n_tiles;
   p.m_tiles = g.m_tiles;
-  p.ksplit = conv_ksplit(d, g, d->stats != nullptr);
+  p.ksplit = conv_ksplit(d, g, num_sms, d->stats != nullptr);
   p.chunk_bytes = BLOCK_M * p.CK * 2;
   p.b_bytes = p.BN * 128;
   // one A plane holds the chunks of ONE k-block, 64 K-columns (zero chunks past the last filter tap)
@@ -499,7 +486,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   p.acc_pitch = uint32_t(p.BN) + 4;  // 16-byte rows; the 4-float skew spreads the fragment stores over the banks
   const uint32_t acc_bytes = BLOCK_M * p.acc_pitch * 4;
   const uint32_t tail = acc_bytes + EPI_WARPS * EPI_STAGE_FLOATS * 4 + 2 * 4 * p.BN * 2 * 4 + 256;
-  const uint32_t budget = uint32_t(g_smem_optin) - 1024 - tail;
+  const uint32_t budget = uint32_t(smem_optin) - 1024 - tail;
   p.stages = std::min<int>(MAX_STAGES, budget / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.k_blocks * 4));
   const int ctas_per_sm = 1;  // 544 threads x up to 120 registers: one CTA fills the register file
@@ -561,7 +548,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
     }
   }
   const int units = p.m_tiles * p.n_tiles * p.ksplit;
-  const int grid = std::min(units, g_num_sms * ctas_per_sm);
+  const int grid = std::min(units, num_sms * ctas_per_sm);
   {
     typedef void (*KernelFn)(const ConvParams);
 #define SFB_CONV_FNS(S) {conv_igemm_kernel<S, 16>, conv_igemm_kernel<S, 32>, conv_igemm_kernel<S, 48>, \
@@ -572,17 +559,14 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
     static bool attr[2][BN_MAX / 16] = {};
     const int a = d->nsplit == 3 ? 1 : 0, b = p.BN / 16 - 1;
     if (!attr[a][b]) {
-      cudaFuncSetAttribute(fns[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
+      cudaFuncSetAttribute(fns[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin);
       attr[a][b] = true;
     }
     fns[a][b]<<<grid, CONV_THREADS, smem_bytes, stream>>>(p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_conv_igemm launch failed: %s (grid=%d smem=%u stages=%d BN=%d CK=%d ksplit=%d)",
-              cudaGetErrorString(e), grid, smem_bytes, p.stages, p.BN, p.CK, p.ksplit);
-    return -20;
-  }
+  if (int rc = launch_status("sfb_conv_igemm", "grid=%d smem=%u stages=%d BN=%d CK=%d ksplit=%d", grid, smem_bytes,
+                             p.stages, p.BN, p.CK, p.ksplit))
+    return rc;
   if (p.ksplit > 1 && d->stats != nullptr)  // [2][cout][sfb_conv_m_tiles(d)] partials of the finished output
     return sfb_bn_split_stats(d->out, d->os_w, p.M, d->cout, 1, p.M, d->stats, stream);
   return 0;

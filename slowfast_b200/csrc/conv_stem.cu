@@ -21,7 +21,8 @@
 
 #include "../../include/slowfast_b200.h"
 #include "ptx.cuh"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -490,80 +491,9 @@ __global__ void stem_filter_fold_kernel(const float* __restrict__ w, float* __re
     if (reverse) {
       if (valid) dw[widx] = gmat[i];
     } else {
-      const float v = valid ? w[widx] : 0.f;
-      const __nv_bfloat16 h = __float2bfloat16_rn(v);
-      hi[i] = h;
-      if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+      put_split(hi, lo, i, valid ? w[widx] : 0.f);
     }
   }
-}
-
-typedef CUresult (*EncodeTiledFnS)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFnS st_encode() {
-  static EncodeTiledFnS fn = nullptr;
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    void* f = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFnS>(f);
-  }
-  return fn;
-}
-// X'[n, t, h, w', 8] bf16, box = [1,1,1,pix,8], no swizzle
-static int make_tmap_fold(CUtensorMap* out, const void* base, int n, int t, int h, int w2, uint32_t pix) {
-  EncodeTiledFnS fn = st_encode();
-  if (!fn) {
-    set_error("cuTensorMapEncodeTiled entry point unavailable");
-    return -1;
-  }
-  cuuint64_t dims[5] = {8, (cuuint64_t)w2, (cuuint64_t)h, (cuuint64_t)t, (cuuint64_t)n};
-  cuuint64_t strides[4] = {16, 16ull * w2, 16ull * w2 * h, 16ull * w2 * h * t};
-  cuuint32_t box[5] = {8, pix, 1, 1, 1};
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled(fold 5d) failed (%d)", (int)r);
-    return -2;
-  }
-  return 0;
-}
-// dY [rows, OW, cout] bf16 (cout contiguous), box = [1][64 ow][64 co], 128B swizzle
-static int make_tmap_dy3(CUtensorMap* out, const void* base, int64_t rows, int ow, int cout) {
-  EncodeTiledFnS fn = st_encode();
-  if (!fn) {
-    set_error("cuTensorMapEncodeTiled entry point unavailable");
-    return -1;
-  }
-  cuuint64_t dims[3] = {(cuuint64_t)cout, (cuuint64_t)ow, (cuuint64_t)rows};
-  cuuint64_t strides[2] = {2ull * cout, 2ull * cout * ow};
-  cuuint32_t box[3] = {64, 64, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled(dy 3d) failed (%d)", (int)r);
-    return -2;
-  }
-  return 0;
-}
-
-static int st_sms = 0, st_smem = 0;
-static int st_props() {
-  if (st_sms) return 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) {
-    set_error("cudaGetDevice failed: no CUDA device");
-    return -1;
-  }
-  cudaDeviceGetAttribute(&st_sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&st_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  return 0;
 }
 
 static int fill_common(StemParams& p, const sfb_stem_desc* d) {
@@ -597,14 +527,9 @@ extern "C" int sfb_stem_input_fold(const float* x, int32_t n, int32_t cin, int32
   }
   const int64_t items = int64_t(n) * t * h * (w / 2);
   int64_t grid = (items + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > kGridSms * 16) grid = kGridSms * 16;
   stem_input_fold_kernel<<<int(grid), 256, 0, (cudaStream_t)stream>>>(x, n, cin, t, h, w, (bf16s*)hi, (bf16s*)lo);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem_input_fold launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem_input_fold");
 }
 
 extern "C" int sfb_stem_filter_fold(const float* w, float* dw, int32_t cout, int32_t cin, int32_t kt, int32_t kh,
@@ -612,15 +537,10 @@ extern "C" int sfb_stem_filter_fold(const float* w, float* dw, int32_t cout, int
                                     int32_t reverse, void* stream) {
   const int64_t items = int64_t(cout) * kt * kh * kwf * 8;
   int64_t grid = (items + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > kGridSms * 8) grid = kGridSms * 8;
   stem_filter_fold_kernel<<<int(grid), 256, 0, (cudaStream_t)stream>>>(w, dw, cout, cin, kt, kh, kw, pad_w, kwf,
                                                                        (bf16s*)hi, (bf16s*)lo, gmat, reverse);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem_filter_fold launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem_filter_fold");
 }
 
 extern "C" int64_t sfb_stem_m_tiles(const sfb_stem_desc* d) {
@@ -629,7 +549,8 @@ extern "C" int64_t sfb_stem_m_tiles(const sfb_stem_desc* d) {
 
 extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (st_props()) return -1;
+  int st_sms = 0, st_smem = 0;
+  if (device_limits(&st_sms, &st_smem)) return -1;
   StemParams p;
   memset(&p, 0, sizeof(p));
   int rc = fill_common(p, d);
@@ -688,17 +609,13 @@ extern "C" int sfb_stem_fprop(const sfb_stem_desc* d, void* stream_) {
     }
     fns[a][b]<<<grid, ST_FPROP_THREADS, smem_bytes, stream>>>(p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem_fprop launch failed: %s (smem=%u stages=%d)", cudaGetErrorString(e), smem_bytes, p.stages);
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem_fprop", "smem=%u stages=%d", smem_bytes, p.stages);
 }
 
 extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (st_props()) return -1;
+  int st_sms = 0, st_smem = 0;
+  if (device_limits(&st_sms, &st_smem)) return -1;
   if (d->cout > 64) {
     set_error("sfb_stem_wgrad: cout=%d > 64 not supported", d->cout);
     return -10;
@@ -753,10 +670,5 @@ extern "C" int sfb_stem_wgrad(const sfb_stem_desc* d, void* stream_) {
     }
     fns[a][b]<<<grid, ST_WGRAD_THREADS, smem_bytes, stream>>>(p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem_wgrad launch failed: %s (grid=%d smem=%u)", cudaGetErrorString(e), grid, smem_bytes);
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem_wgrad", "grid=%d smem=%u", grid, smem_bytes);
 }

@@ -32,7 +32,8 @@
 
 #include "../../include/slowfast_b200.h"
 #include "ptx.cuh"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -429,55 +430,8 @@ __global__ void stem8_filter_fold_kernel(const float* __restrict__ w, int cin, i
       const int tap = 2 * kwp + par - 1;
       if (tap >= 0 && tap < 7) v = w[(((int64_t(co) * cin + c) * kt + it) * 7 + kh) * 7 + tap];
     }
-    const __nv_bfloat16 hb = __float2bfloat16_rn(v);
-    hi[i] = hb;
-    if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(hb));
+    put_split(hi, lo, i, v);
   }
-}
-
-typedef CUresult (*EncodeTiledFn8)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn8 t8_encode() {
-  static EncodeTiledFn8 fn = nullptr;
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    void* f = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn8>(f);
-  }
-  return fn;
-}
-static int t8_tmap5(CUtensorMap* out, const void* base, const cuuint64_t dims[5], const cuuint64_t strides[4],
-                    const cuuint32_t box[5], bool swz128, const char* what) {
-  EncodeTiledFn8 fn = t8_encode();
-  if (!fn) {
-    set_error("cuTensorMapEncodeTiled entry point unavailable");
-    return -1;
-  }
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled(%s) failed (%d)", what, (int)r);
-    return -2;
-  }
-  return 0;
-}
-
-static int t8_sms = 0, t8_smem = 0;
-static int t8_props() {
-  if (t8_sms) return 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) {
-    set_error("cudaGetDevice failed: no CUDA device");
-    return -1;
-  }
-  cudaDeviceGetAttribute(&t8_sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&t8_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  return 0;
 }
 
 static bool t8_geometry_ok(const sfb_stem_desc* d) {
@@ -510,7 +464,8 @@ static int t8_xmaps(Stem8Params& p, const sfb_stem_desc* d, int np) {
   cuuint64_t strides[4] = {16ull * p.MR, row, row * (d->h / 2), row * (d->h / 2) * 2 * d->t};
   cuuint32_t box[5] = {(cuuint32_t)(8 * p.MR), 1, (cuuint32_t)T8_SLOTS, 1, 1};
   for (int pl = 0; pl < np; ++pl) {
-    int rc = t8_tmap5(&p.tmX[pl], pl ? d->x_lo : d->x_hi, dims, strides, box, false, "stem8 x");
+    int rc = encode_tiled_bf16(&p.tmX[pl], 5, pl ? d->x_lo : d->x_hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                               "stem8 x");
     if (rc) return rc;
   }
   return 0;
@@ -536,31 +491,22 @@ extern "C" int sfb_stem8_input_fold(const float* x, int32_t n, int32_t cin, int3
   const int mr = w / 16 + 1;
   const int64_t items = int64_t(n) * t * h * 8 * mr;
   int64_t grid = (items + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > kGridSms * 16) grid = kGridSms * 16;
   stem8_input_fold_kernel<<<int(grid), 256, 0, (cudaStream_t)stream>>>(x, n, cin, t, h, w, mr, (bf16t*)hi, (bf16t*)lo);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem8_input_fold launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem8_input_fold");
 }
 
 extern "C" int sfb_stem8_filter_fold(const float* w, int32_t cin, int32_t kt, void* hi, void* lo, void* stream) {
   const int zg = 7 * 12 + 8;
   const int items = kt * zg * 64;
   stem8_filter_fold_kernel<<<(items + 255) / 256, 256, 0, (cudaStream_t)stream>>>(w, cin, kt, zg, (bf16t*)hi, (bf16t*)lo);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem8_filter_fold launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem8_filter_fold");
 }
 
 extern "C" int sfb_stem8_fprop(const sfb_stem_desc* d, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (t8_props()) return -1;
+  int t8_sms = 0, t8_smem = 0;
+  if (device_limits(&t8_sms, &t8_smem)) return -1;
   Stem8Params p;
   memset(&p, 0, sizeof(p));
   int rc = t8_fill(p, d);
@@ -597,17 +543,13 @@ extern "C" int sfb_stem8_fprop(const sfb_stem_desc* d, void* stream_) {
     if (!a) { cudaFuncSetAttribute(stem8_fprop_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }
     stem8_fprop_kernel<1><<<grid, T8_FPROP_THREADS, smem_bytes, stream>>>(p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem8_fprop launch failed: %s (smem=%u)", cudaGetErrorString(e), smem_bytes);
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem8_fprop", "smem=%u", smem_bytes);
 }
 
 extern "C" int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (t8_props()) return -1;
+  int t8_sms = 0, t8_smem = 0;
+  if (device_limits(&t8_sms, &t8_smem)) return -1;
   Stem8Params p;
   memset(&p, 0, sizeof(p));
   int rc = t8_fill(p, d);
@@ -641,7 +583,8 @@ extern "C" int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream_) {
     cuuint64_t strides[4] = {128, rowb, rowb * d->out_h, rowb * d->out_h * d->out_t};
     cuuint32_t box[5] = {64, (cuuint32_t)p.MR, (cuuint32_t)T8_ROWS, 1, 1};
     for (int pl = 0; pl < np; ++pl) {
-      rc = t8_tmap5(&p.tmB[pl], pl ? d->dy_lo : d->dy_hi, dims, strides, box, true, "stem8 dy");
+      rc = encode_tiled_bf16(&p.tmB[pl], 5, pl ? d->dy_lo : d->dy_hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                             "stem8 dy");
       if (rc) return rc;
     }
   }
@@ -655,10 +598,5 @@ extern "C" int sfb_stem8_wgrad(const sfb_stem_desc* d, void* stream_) {
     if (!a) { cudaFuncSetAttribute(stem8_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, t8_smem); a = true; }
     stem8_wgrad_kernel<1><<<grid, T8_WGRAD_THREADS, smem_bytes, stream>>>(p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_stem8_wgrad launch failed: %s (grid=%d smem=%u)", cudaGetErrorString(e), grid, smem_bytes);
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_stem8_wgrad", "grid=%d smem=%u", grid, smem_bytes);
 }

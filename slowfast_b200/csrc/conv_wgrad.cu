@@ -20,7 +20,7 @@
 
 #include "../../include/slowfast_b200.h"
 #include "ptx.cuh"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -246,8 +246,6 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
   }
 }
 
-static int wg_num_sms = 0, wg_smem_optin = 0;
-
 static int pick_ck(int c) {
   if (c % 64 == 0) return 64;
   if (c % 32 == 0) return 32;
@@ -352,7 +350,7 @@ static int wgrad_check(const sfb_wgrad_desc* d) {
 }
 
 bool wgrad_direct_takes(const sfb_wgrad_desc* d);
-int wgrad_direct_try(const sfb_wgrad_desc* d, cudaStream_t stream, int* rc_out);
+int wgrad_direct_try(const sfb_wgrad_desc* d, int sms, cudaStream_t stream, int* rc_out);
 
 typedef void (*WgradKernel)(const WgradParams);
 // The shapes wgrad_plan can choose: co-rows with either row count and any BN, transposed with BN = 16 / 32 / 64 / 128.
@@ -405,15 +403,8 @@ extern "C" int sfb_conv_wgrad_plan(const sfb_wgrad_desc* d, int32_t num_sms, sfb
 
 extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!wg_num_sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) {
-      set_error("cudaGetDevice failed: no CUDA device");
-      return -1;
-    }
-    cudaDeviceGetAttribute(&wg_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaDeviceGetAttribute(&wg_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  }
+  int wg_num_sms = 0, wg_smem_optin = 0;
+  if (device_limits(&wg_num_sms, &wg_smem_optin)) return -1;
   int rc = wgrad_check(d);
   if (rc) return rc;
   if (!d->x_hi || !d->dy_hi || !d->dw || (d->nsplit == 3 && (!d->x_lo || !d->dy_lo))) {
@@ -423,7 +414,7 @@ extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
   {
     // narrow layers with many positions: fp32 SIMT body (conv_wgrad_direct.cu), same operands and dW layout
     int rc_direct = 0;
-    if (sfb::wgrad_direct_try(d, stream, &rc_direct)) return rc_direct;
+    if (sfb::wgrad_direct_try(d, wg_num_sms, stream, &rc_direct)) return rc_direct;
   }
   const sfb_wgrad_plan pl = wgrad_plan(d, wg_num_sms);
   WgradParams p;
@@ -506,11 +497,6 @@ extern "C" int sfb_conv_wgrad(const sfb_wgrad_desc* d, void* stream_) {
     configured[n_configured++] = fn;
   }
   fn<<<pl.ctas, WG_THREADS, smem_bytes, stream>>>(p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_conv_wgrad launch failed: %s (grid=%d smem=%u transposed=%d rows=%d bn=%d)", cudaGetErrorString(e),
-              pl.ctas, smem_bytes, pl.transposed, pl.tile_rows, pl.bn);
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_conv_wgrad", "grid=%d smem=%u transposed=%d rows=%d bn=%d", pl.ctas, smem_bytes,
+                       pl.transposed, pl.tile_rows, pl.bn);
 }

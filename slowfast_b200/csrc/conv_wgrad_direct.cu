@@ -18,7 +18,7 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -148,7 +148,6 @@ __global__ void __launch_bounds__(WGD_MAX_WARPS * 32, 2) conv_wgrad_direct_kerne
 }
 
 static int g_wgd_enabled = 1;
-static int g_wgd_sms = 0;
 
 void wgrad_direct_configure(int enabled) { g_wgd_enabled = enabled; }
 
@@ -163,16 +162,11 @@ bool wgrad_direct_takes(const sfb_wgrad_desc* d) {
   return int64_t(d->n) * d->d * d->h * d->w * d->c_pitch < (int64_t(1) << 31) && M * d->dy_pitch < (int64_t(1) << 31);
 }
 
-// Returns 1 and sets *rc_out when the direct kernel took the job.
-int wgrad_direct_try(const sfb_wgrad_desc* d, cudaStream_t stream, int* rc_out) {
+// Returns 1 and sets *rc_out when the direct kernel took the job; `sms` is the device's SM count.
+int wgrad_direct_try(const sfb_wgrad_desc* d, int sms, cudaStream_t stream, int* rc_out) {
   if (!wgrad_direct_takes(d)) return 0;
   const int taps = d->kt * d->kh * d->kw;
   const int jobs = taps * (d->c / 8) * (d->cout / 8);
-  if (!g_wgd_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_wgd_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
   WgdParams p;
   p.x_hi = (const __nv_bfloat16*)d->x_hi; p.x_lo = (const __nv_bfloat16*)d->x_lo; p.c_pitch = d->c_pitch;
   p.dy_hi = (const __nv_bfloat16*)d->dy_hi; p.dy_lo = (const __nv_bfloat16*)d->dy_lo; p.dy_pitch = d->dy_pitch;
@@ -194,20 +188,14 @@ int wgrad_direct_try(const sfb_wgrad_desc* d, cudaStream_t stream, int* rc_out) 
   const int wpb = p.jobs_per_block * p.slices;                       // warps per block
   const int blocks_per_sm = std::max(2, 20 / wpb);                   // 96 registers per thread: ~21 warps fit an SM
   const int gx = std::max(1, std::min((p.total_chunks + p.slices - 1) / p.slices,
-                                      (blocks_per_sm * g_wgd_sms + groups - 1) / groups));
+                                      (blocks_per_sm * sms + groups - 1) / groups));
   dim3 grid(gx, groups);
   const int threads = wpb * 32;
   if (d->nsplit == 3)
     conv_wgrad_direct_kernel<3><<<grid, threads, 0, stream>>>(p);
   else
     conv_wgrad_direct_kernel<1><<<grid, threads, 0, stream>>>(p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_conv_wgrad (direct) launch failed: %s", cudaGetErrorString(e));
-    *rc_out = -20;
-  } else {
-    *rc_out = 0;
-  }
+  *rc_out = launch_status("sfb_conv_wgrad (direct)");
   return 1;
 }
 

@@ -2,50 +2,32 @@
 // filter matrices), train-mode BatchNorm (finalize / apply+residual+ReLU / backward), ReLU+MaxPool for the stems,
 // and the classification head pieces.  All kernels view an activation as a [rows = n*t*h*w, C] matrix with a row
 // pitch (so channel slices of a wider tensor - "concat in place" - need no copies) and move 8 channels per thread
-// (16-byte bf16 / 32-byte fp32 vectors), grid-strided with a grid of a few waves of 148 SMs.
+// (16-byte bf16 / 32-byte fp32 vectors), grid-strided with a grid of a few waves of the
+// device's SMs (runtime.h's kGridSms stands in when no device answers).
 #include <cstdint>
 #include <cstring>
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
+// SM count of the device; kGridSms when there is none (the launch that follows reports that)
 static int ew_sms() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
+  int sms = kGridSms;
+  device_limits(&sms, nullptr);
   return sms;
 }
-static int ew_grid(int64_t items, int block) {
-  int64_t want = (items + block - 1) / block;
-  int64_t cap = int64_t(ew_sms()) * 8;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
-}
+static int ew_grid(int64_t items, int block) { return capped_grid(items, block, int64_t(ew_sms()) * 8); }
 // grid of the row-lane kernels (RowLanes): every thread walks ~4 rows of its channel group, at most 8 blocks per SM
 static int rowlane_grid(int64_t rows, int cg, int block) {
   const int lanes_c = cg < block ? cg : block;
   const int lanes_r = block / lanes_c;
-  int64_t want = (rows + int64_t(lanes_r) * 4 - 1) / (int64_t(lanes_r) * 4);
-  const int64_t cap = int64_t(ew_sms()) * 8;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
+  return capped_grid(rows, lanes_r * 4, int64_t(ew_sms()) * 8);
 }
-#define SFB_LAUNCH_CHECK(name)                                            \
-  do {                                                                    \
-    cudaError_t e_ = cudaGetLastError();                                  \
-    if (e_ != cudaSuccess) {                                              \
-      set_error("%s launch failed: %s", name, cudaGetErrorString(e_));    \
-      return -20;                                                         \
-    }                                                                     \
-  } while (0)
 
-struct alignas(16) bf16x8 {
-  __nv_bfloat162 v[4];
-};
 struct f32x8 {
   float4 a, b;
 };
@@ -60,36 +42,6 @@ __device__ __forceinline__ void store8(float* p, const float (&x)[8]) {
   *reinterpret_cast<float4*>(p) = make_float4(x[0], x[1], x[2], x[3]);
   *reinterpret_cast<float4*>(p + 4) = make_float4(x[4], x[5], x[6], x[7]);
 }
-// split 8 fp32 values into hi = bf16(x), lo = bf16(x - hi) and store both planes (lo may be null)
-__device__ __forceinline__ void store_split8(__nv_bfloat16* hi, __nv_bfloat16* lo, const float (&x)[8]) {
-  bf16x8 h, l;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(x[2 * i]), h1 = __float2bfloat16_rn(x[2 * i + 1]);
-    h.v[i] = __halves2bfloat162(h0, h1);
-    l.v[i] = __halves2bfloat162(__float2bfloat16_rn(x[2 * i] - __bfloat162float(h0)),
-                                __float2bfloat16_rn(x[2 * i + 1] - __bfloat162float(h1)));
-  }
-  *reinterpret_cast<bf16x8*>(hi) = h;
-  if (lo) *reinterpret_cast<bf16x8*>(lo) = l;
-}
-__device__ __forceinline__ void load_planes8(const __nv_bfloat16* hi, const __nv_bfloat16* lo, float (&x)[8]) {
-  const bf16x8 h = *reinterpret_cast<const bf16x8*>(hi);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    x[2 * i] = __bfloat162float(__low2bfloat16(h.v[i]));
-    x[2 * i + 1] = __bfloat162float(__high2bfloat16(h.v[i]));
-  }
-  if (lo) {
-    const bf16x8 l = *reinterpret_cast<const bf16x8*>(lo);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      x[2 * i] += __bfloat162float(__low2bfloat16(l.v[i]));
-      x[2 * i + 1] += __bfloat162float(__high2bfloat16(l.v[i]));
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------- packing
 __global__ void split_planes_kernel(const float* __restrict__ x, int64_t rows, int cg, int64_t x_pitch,
                                     __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int64_t o_pitch) {
@@ -145,9 +97,7 @@ __global__ void filter_pack_kernel(const __grid_constant__ FilterPackParams p) {
       const int ci = p.transpose ? r : cc;
       v = p.w[(int64_t(co) * p.cin + ci) * p.taps_total + p.tapmap[j]];
     }
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    p.hi[i] = h;
-    if (p.lo) p.lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+    put_split(p.hi, p.lo, i, v);
   }
 }
 
@@ -717,8 +667,7 @@ extern "C" int sfb_split_planes(const float* x, int64_t rows, int32_t c, int64_t
   if (items == 0) return 0;
   split_planes_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, rows, c / 8, x_pitch, (bf16*)hi,
                                                                             (bf16*)lo, o_pitch);
-  SFB_LAUNCH_CHECK("sfb_split_planes");
-  return 0;
+  return launch_status("sfb_split_planes");
 }
 
 extern "C" int sfb_input_pack(const float* x, int32_t n, int32_t c, int32_t t, int32_t h, int32_t w, int32_t c_pad,
@@ -730,8 +679,7 @@ extern "C" int sfb_input_pack(const float* x, int32_t n, int32_t c, int32_t t, i
   const int64_t thw = int64_t(t) * h * w;
   const int64_t items = int64_t(n) * thw * (c_pad / 8);
   input_pack_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, n, c, thw, c_pad, (bf16*)hi, (bf16*)lo);
-  SFB_LAUNCH_CHECK("sfb_input_pack");
-  return 0;
+  return launch_status("sfb_input_pack");
 }
 
 extern "C" int sfb_filter_pack(const float* w, int32_t cout, int32_t cin, int32_t taps_total, const int32_t* tapmap,
@@ -762,8 +710,7 @@ extern "C" int sfb_filter_pack(const float* w, int32_t cout, int32_t cin, int32_
   }
   const int64_t items = int64_t(p.rows) * ntaps * cols_pad;
   filter_pack_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_filter_pack");
-  return 0;
+  return launch_status("sfb_filter_pack");
 }
 
 extern "C" int sfb_filter_unpack_grad(const float* dwm, float* dw, int32_t cout, int32_t cin, int32_t taps,
@@ -771,8 +718,7 @@ extern "C" int sfb_filter_unpack_grad(const float* dwm, float* dw, int32_t cout,
   const int64_t items = int64_t(cout) * cin * taps;
   filter_unpack_grad_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dwm, dw, cout, cin, taps, cin_pad,
                                                                                   accumulate);
-  SFB_LAUNCH_CHECK("sfb_filter_unpack_grad");
-  return 0;
+  return launch_status("sfb_filter_unpack_grad");
 }
 
 extern "C" int sfb_bn_finalize(const float* partials, int32_t m_tiles, int32_t c, int64_t count, const float* gamma,
@@ -791,8 +737,7 @@ extern "C" int sfb_bn_finalize(const float* partials, int32_t m_tiles, int32_t c
   bn_finalize_kernel<<<c, 256, 0, (cudaStream_t)stream>>>(partials, m_tiles, c, affine_c, double(count), gamma,
                                                                        beta, running_mean, running_var, momentum, eps,
                                                                        training, scale, shift, save_mean, save_invstd);
-  SFB_LAUNCH_CHECK("sfb_bn_finalize");
-  return 0;
+  return launch_status("sfb_bn_finalize");
 }
 
 static int split_geometry_ok(const char* who, int64_t rows, int32_t splits, int64_t rows_per_clip) {
@@ -829,8 +774,7 @@ extern "C" int sfb_bn_split_stats(const float* y, int64_t y_pitch, int64_t rows,
   const int64_t blocks = rows / rows_per_clip * p.chunks;
   if (blocks == 0) return 0;
   bn_split_stats_kernel<<<unsigned(blocks), 256, 256 * 16 * sizeof(float), (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_bn_split_stats");
-  return 0;
+  return launch_status("sfb_bn_split_stats");
 }
 
 extern "C" int sfb_bn_apply(const sfb_bn_apply_desc* d, void* stream) {
@@ -849,8 +793,7 @@ extern "C" int sfb_bn_apply(const sfb_bn_apply_desc* d, void* stream) {
   const int64_t items = d->rows * (d->c / 8);
   if (items == 0) return 0;
   bn_apply_kernel<<<rowlane_grid(d->rows, d->c / 8, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_bn_apply");
-  return 0;
+  return launch_status("sfb_bn_apply");
 }
 
 static int64_t bn_bwd_slabs(int64_t rows) {
@@ -897,12 +840,12 @@ extern "C" int sfb_bn_bwd(const sfb_bn_bwd_desc* d, void* stream_) {
   r.rows = d->rows; r.c = d->c; r.partials = d->partials;
   r.splits = splits; r.rows_per_clip = d->rows_per_clip; r.blocks_per_clip = bpc;
   bn_bwd_reduce_kernel<<<nblocks, 256, 256 * 16 * sizeof(float), stream>>>(r);
-  SFB_LAUNCH_CHECK("sfb_bn_bwd(reduce)");
+  if (int rc = launch_status("sfb_bn_bwd(reduce)")) return rc;
   bn_bwd_finalize_kernel<<<d->c, 64, 0, stream>>>(d->partials, nblocks, d->c, double(d->rows / splits), d->gamma,
                                                                  d->invstd, d->dgamma, d->dbeta, d->accumulate_param_grads,
                                                                  d->training, d->coef,
                                                                  d->c_valid > 0 ? d->c_valid : d->c, splits, bpc);
-  SFB_LAUNCH_CHECK("sfb_bn_bwd(finalize)");
+  if (int rc = launch_status("sfb_bn_bwd(finalize)")) return rc;
   BnBwdApplyParams a;
   a.dout = d->dout; a.dout_pitch = d->dout_pitch;
   a.mask = (const bf16*)d->mask_hi; a.mask_pitch = d->mask_pitch;
@@ -914,8 +857,7 @@ extern "C" int sfb_bn_bwd(const sfb_bn_bwd_desc* d, void* stream_) {
   a.splits = splits; a.rows_per_clip = d->rows_per_clip;
   const int64_t items = d->rows * (d->c / 8);
   bn_bwd_apply_kernel<<<rowlane_grid(d->rows, d->c / 8, 256), 256, 0, stream>>>(a);
-  SFB_LAUNCH_CHECK("sfb_bn_bwd(apply)");
-  return 0;
+  return launch_status("sfb_bn_bwd(apply)");
 }
 
 extern "C" int sfb_bn_relu_maxpool_fwd(const sfb_pool_desc* d, void* stream) {
@@ -936,8 +878,7 @@ extern "C" int sfb_bn_relu_maxpool_fwd(const sfb_pool_desc* d, void* stream) {
   }
   const int64_t items = int64_t(d->n) * d->t * d->oh * d->ow * (d->c / 8);
   bn_relu_maxpool_fwd_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_bn_relu_maxpool_fwd");
-  return 0;
+  return launch_status("sfb_bn_relu_maxpool_fwd");
 }
 
 extern "C" int sfb_bn_relu_maxpool_bwd(const sfb_pool_desc* d, void* stream) {
@@ -952,8 +893,7 @@ extern "C" int sfb_bn_relu_maxpool_bwd(const sfb_pool_desc* d, void* stream) {
   p.argmax = d->argmax; p.dout = d->dout; p.dout_pitch = d->dout_pitch; p.dz = d->dz;
   const int64_t items = int64_t(d->n) * d->t * d->h * d->w * (d->c / 8);
   bn_relu_maxpool_bwd_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_bn_relu_maxpool_bwd");
-  return 0;
+  return launch_status("sfb_bn_relu_maxpool_bwd");
 }
 
 // ------------------------------------------------------------------------------------------- MaxPool3d on planes
@@ -1077,8 +1017,7 @@ extern "C" int sfb_maxpool3d_fwd(const sfb_pool3d_desc* d, void* stream) {
   p.kt = d->kt; p.kh = d->kh; p.kw = d->kw; p.st = d->st; p.sh = d->sh; p.sw = d->sw; p.pt = d->pt; p.ph = d->ph; p.pw = d->pw;
   const int64_t items = int64_t(d->n) * d->ot * d->oh * d->ow * (d->c / 8);
   sfb::maxpool3d_fwd_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_maxpool3d_fwd");
-  return 0;
+  return launch_status("sfb_maxpool3d_fwd");
 }
 extern "C" int sfb_maxpool3d_bwd(const sfb_pool3d_desc* d, void* stream) {
   if (d->c % 8) {
@@ -1094,8 +1033,7 @@ extern "C" int sfb_maxpool3d_bwd(const sfb_pool3d_desc* d, void* stream) {
   p.din_accumulate = d->din_accumulate;
   const int64_t items = int64_t(d->n) * d->t * d->h * d->w * (d->c / 8);
   sfb::maxpool3d_bwd_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_LAUNCH_CHECK("sfb_maxpool3d_bwd");
-  return 0;
+  return launch_status("sfb_maxpool3d_bwd");
 }
 
 // dst[rows, c] += src[rows, c] (fp32 views with row pitches): the second and later contributions to an activation
@@ -1127,6 +1065,5 @@ extern "C" int sfb_add_f32_2d(float* dst, const float* src, int64_t rows, int32_
   if (items == 0) return 0;
   sfb::add_f32_2d_kernel<<<ew_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dst, src, rows, c / 8, dst_pitch,
                                                                                src_pitch);
-  SFB_LAUNCH_CHECK("sfb_add_f32_2d");
-  return 0;
+  return launch_status("sfb_add_f32_2d");
 }

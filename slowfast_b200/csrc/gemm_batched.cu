@@ -19,7 +19,7 @@
 
 #include "../../include/slowfast_b200.h"
 #include "ptx.cuh"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -248,57 +248,14 @@ __global__ void __launch_bounds__(BG_THREADS, 1) gemm_batched_kernel(const __gri
 
 }
 
-typedef CUresult (*EncodeTiledFn3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// 3-D map over bf16 [batch][rows][cols] (cols contiguous, row pitch ld, batch stride bs), box = [1][box_rows][64]
-static int make_tmap_3d(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint64_t ld,
-                        uint64_t bs, uint32_t box_rows) {
-  static EncodeTiledFn3 fn = nullptr;
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    void* f = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess) {
-      set_error("cuTensorMapEncodeTiled entry point unavailable");
-      return -1;
-    }
-    fn = reinterpret_cast<EncodeTiledFn3>(f);
-  }
-  cuuint64_t dims[3] = {cols, rows, batch};
-  cuuint64_t strides[2] = {ld * 2, bs * 2};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled(3d) failed (%d): cols=%llu rows=%llu batch=%llu ld=%llu bs=%llu box_rows=%u", (int)r,
-              (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)batch, (unsigned long long)ld,
-              (unsigned long long)bs, box_rows);
-    return -2;
-  }
-  return 0;
-}
-
-static int bg_sms = 0, bg_smem = 0;
-
 }  // namespace sfb
 
 using namespace sfb;
 
 extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!bg_sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) {
-      set_error("cudaGetDevice failed: no CUDA device");
-      return -1;
-    }
-    cudaDeviceGetAttribute(&bg_sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaDeviceGetAttribute(&bg_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  }
+  int bg_sms = 0, bg_smem = 0;
+  if (device_limits(&bg_sms, &bg_smem)) return -1;
   if (d->nsplit != 1 && d->nsplit != 3) {
     set_error("sfb_gemm_batched: nsplit must be 1 or 3");
     return -10;
@@ -395,11 +352,5 @@ extern "C" int sfb_gemm_batched(const sfb_bgemm_desc* d, void* stream_) {
     }
     gemm_batched_kernel<1><<<grid, BG_THREADS, smem_bytes, stream>>>(p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_gemm_batched launch failed: %s (grid=%d smem=%u stages=%d BN=%d)", cudaGetErrorString(e), grid,
-              smem_bytes, p.stages, p.BN);
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_gemm_batched", "grid=%d smem=%u stages=%d BN=%d", grid, smem_bytes, p.stages, p.BN);
 }

@@ -7,18 +7,9 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
-
-#define SFB_HEAD_CHECK(name)                                             \
-  do {                                                                   \
-    cudaError_t e_ = cudaGetLastError();                                 \
-    if (e_ != cudaSuccess) {                                             \
-      set_error("%s launch failed: %s", name, cudaGetErrorString(e_));   \
-      return -20;                                                        \
-    }                                                                    \
-  } while (0)
 
 // out[n, c] = mean_{s < spatial} (hi + lo)[n, s, c]; one block per (n, 32-channel strip), 8 row-lanes
 __global__ void __launch_bounds__(256) global_avgpool_fwd_kernel(const __nv_bfloat16* __restrict__ hi,
@@ -199,10 +190,7 @@ __global__ void row_softmax_kernel(float* __restrict__ x, int rows, int cols) {
   for (int t = lane; t < cols; t += 32) r[t] = expf(r[t] - mx) * inv;
 }
 
-static int hd_grid(int64_t items, int block) {
-  int64_t want = (items + block - 1) / block;
-  return int(want < 1 ? 1 : (want > 148 * 8 ? 148 * 8 : want));
-}
+static int hd_grid(int64_t items, int block) { return capped_grid(items, block, int64_t(kGridSms) * 8); }
 
 }  // namespace sfb
 
@@ -213,16 +201,14 @@ extern "C" int sfb_global_avgpool_fwd(const void* hi, const void* lo, int64_t pi
   dim3 grid((c + 31) / 32, n);
   global_avgpool_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)hi, (const __nv_bfloat16*)lo,
                                                                    pitch, spatial, c, out, out_pitch);
-  SFB_HEAD_CHECK("sfb_global_avgpool_fwd");
-  return 0;
+  return launch_status("sfb_global_avgpool_fwd");
 }
 extern "C" int sfb_global_avgpool_bwd(const float* dpooled, int64_t dp_pitch, int32_t n, int32_t spatial, int32_t c,
                                       float* dx, int64_t dx_pitch, void* stream) {
   const int64_t items = int64_t(n) * spatial * c;
   global_avgpool_bwd_kernel<<<hd_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dpooled, dp_pitch, spatial, c, n, dx,
                                                                                   dx_pitch);
-  SFB_HEAD_CHECK("sfb_global_avgpool_bwd");
-  return 0;
+  return launch_status("sfb_global_avgpool_bwd");
 }
 extern "C" int sfb_window_avgpool_fwd(const void* hi, const void* lo, int64_t pitch, int32_t n, int32_t t, int32_t h,
                                       int32_t w, int32_t c, int32_t kt, int32_t kh, int32_t kw, float* out,
@@ -233,20 +219,18 @@ extern "C" int sfb_window_avgpool_fwd(const void* hi, const void* lo, int64_t pi
   }
   const int64_t items = int64_t(n) * (t - kt + 1) * (h - kh + 1) * (w - kw + 1) * c;
   if (items == 0) return 0;
-  const int blocks = int(std::min<int64_t>((items + 255) / 256, 148 * 8));
+  const int blocks = int(std::min<int64_t>((items + 255) / 256, kGridSms * 8));
   sfb::window_avgpool_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)hi, (const __nv_bfloat16*)lo, pitch, n, t, h, w, c, kt, kh, kw, out, out_pitch);
-  SFB_HEAD_CHECK("window_avgpool_fwd");
-  return 0;
+  return launch_status("window_avgpool_fwd");
 }
 
 extern "C" int sfb_rows_group_mean(const float* in, float* out, int32_t n, int32_t g, int32_t k, void* stream) {
   const int64_t items = int64_t(n) * k;
   if (items == 0) return 0;
-  const int blocks = int(std::min<int64_t>((items + 255) / 256, 148 * 8));
+  const int blocks = int(std::min<int64_t>((items + 255) / 256, kGridSms * 8));
   sfb::rows_group_mean_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(in, out, n, g, k);
-  SFB_HEAD_CHECK("rows_group_mean");
-  return 0;
+  return launch_status("rows_group_mean");
 }
 
 extern "C" int sfb_dropout_fwd(float* x, uint8_t* mask, int64_t nelem, float p, uint64_t seed, uint64_t* step,
@@ -256,25 +240,23 @@ extern "C" int sfb_dropout_fwd(float* x, uint8_t* mask, int64_t nelem, float p, 
     return -10;
   }
   dropout_fwd_kernel<<<hd_grid(nelem, 256), 256, 0, (cudaStream_t)stream>>>(x, mask, nelem, p, seed, step);
-  SFB_HEAD_CHECK("sfb_dropout_fwd");
+  if (int rc = launch_status("sfb_dropout_fwd")) return rc;
   if (step) {
     counter_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step);
-    SFB_HEAD_CHECK("sfb_dropout_fwd(counter)");
+    if (int rc = launch_status("sfb_dropout_fwd(counter)")) return rc;
   }
   return 0;
 }
 extern "C" int sfb_dropout_bwd(float* dx, const uint8_t* mask, int64_t nelem, float p, void* stream) {
   dropout_bwd_kernel<<<hd_grid(nelem, 256), 256, 0, (cudaStream_t)stream>>>(dx, mask, nelem, p);
-  SFB_HEAD_CHECK("sfb_dropout_bwd");
-  return 0;
+  return launch_status("sfb_dropout_bwd");
 }
 template <bool RELU>
 static int small_linear_fwd(const float* x, const float* w, const float* b, float* y, int32_t m, int32_t k, int32_t j,
                             void* stream, const char* name) {
   const int64_t threads = int64_t(m) * k * 32;
   small_linear_fwd_kernel<RELU><<<int((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, w, b, y, m, k, j);
-  SFB_HEAD_CHECK(name);
-  return 0;
+  return launch_status(name);
 }
 template <bool RELU_MASK>
 static int small_linear_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx, int32_t m,
@@ -282,12 +264,12 @@ static int small_linear_bwd(const float* dy, const float* x, const float* w, flo
   if (dw) {
     small_linear_wgrad_kernel<<<hd_grid(int64_t(k) * j, 256), 256, 0, (cudaStream_t)stream>>>(dy, x, dw, db, m, k, j,
                                                                                              accumulate);
-    SFB_HEAD_CHECK("sfb_small_linear_bwd(wgrad)");
+    if (int rc = launch_status("sfb_small_linear_bwd(wgrad)")) return rc;
   }
   if (dx) {
     small_linear_dgrad_kernel<RELU_MASK><<<hd_grid(int64_t(m) * j, 256), 256, 0, (cudaStream_t)stream>>>(dy, w, dx, m,
                                                                                                         k, j, x);
-    SFB_HEAD_CHECK("sfb_small_linear_bwd(dgrad)");
+    if (int rc = launch_status("sfb_small_linear_bwd(dgrad)")) return rc;
   }
   return 0;
 }
@@ -309,8 +291,7 @@ extern "C" int sfb_small_linear_relu_bwd(const float* dy, const float* x, const 
 }
 extern "C" int sfb_row_softmax(float* x, int32_t rows, int32_t cols, void* stream) {
   row_softmax_kernel<<<(rows * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(x, rows, cols);
-  SFB_HEAD_CHECK("sfb_row_softmax");
-  return 0;
+  return launch_status("sfb_row_softmax");
 }
 
 // Stochastic-depth scales (common.py:46-59 drop_path): out[i*b + s] = floor(keep_i + U) / keep_i per sample, from the
@@ -330,10 +311,10 @@ extern "C" int sfb_droppath_scales(float* out, const float* rates, int32_t n_rat
                                    uint64_t* step, void* stream) {
   const int n = n_rates * b;
   sfb::droppath_scales_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(out, rates, n_rates, b, seed, step);
-  SFB_HEAD_CHECK("sfb_droppath_scales");
+  if (int rc = launch_status("sfb_droppath_scales")) return rc;
   if (step) {
     sfb::counter_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step);
-    SFB_HEAD_CHECK("sfb_droppath_scales(counter)");
+    if (int rc = launch_status("sfb_droppath_scales(counter)")) return rc;
   }
   return 0;
 }

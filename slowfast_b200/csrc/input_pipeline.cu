@@ -8,7 +8,7 @@
 #include <cstdint>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -64,14 +64,9 @@ extern "C" int sfb_clip_normalize_pack(const uint8_t* frames, int32_t b, int32_t
   }
   const int64_t items = int64_t(b) * t_out * h * (w / 4);
   const int64_t want = (items + 255) / 256;
-  const int grid = int(want > 148 * 16 ? 148 * 16 : want);
+  const int grid = int(want > sfb::kGridSms * 16 ? sfb::kGridSms * 16 : want);
   sfb::clip_normalize_pack_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frames, b, t, h, w, frame_idx, t_out, mean3[0],
                                                                         mean3[1], mean3[2], std3[0], std3[1], std3[2],
                                                                         reverse_channels, out);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    sfb::set_error("sfb_clip_normalize_pack launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return sfb::launch_status("sfb_clip_normalize_pack");
 }

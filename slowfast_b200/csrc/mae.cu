@@ -12,28 +12,15 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
-
-#define SFB_MAE_CHECK(name)                                               \
-  do {                                                                    \
-    cudaError_t e_ = cudaGetLastError();                                  \
-    if (e_ != cudaSuccess) {                                              \
-      set_error("%s launch failed: %s", name, cudaGetErrorString(e_));    \
-      return -20;                                                         \
-    }                                                                     \
-  } while (0)
 
 constexpr int kMaeMaxTokens = 4096;  // noise row of one clip held in shared memory
 constexpr int kMaskThreads = 1024;
 constexpr int kMaskPer = kMaeMaxTokens / kMaskThreads;
 
-static int mae_grid(int64_t items, int block) {
-  int64_t want = (items + block - 1) / block;
-  int64_t cap = int64_t(148) * 8;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
-}
+static int mae_grid(int64_t items, int block) { return capped_grid(items, block, int64_t(kGridSms) * 8); }
 
 // ------------------------------------------------------------------------------------------- masking
 // One CTA per clip.  rank[i] = #{j : noise[j] < noise[i] or (noise[j] == noise[i] and j < i)} is the position of token i
@@ -302,8 +289,7 @@ extern "C" int sfb_mae_random_masking(const float* noise, int32_t b, int32_t l, 
   }
   mae_masking_kernel<<<b, kMaskThreads, 0, (cudaStream_t)stream>>>(noise, l, keep, ids_keep, ids_restore, mask,
                                                                     masked_rows);
-  SFB_MAE_CHECK("sfb_mae_random_masking");
-  return 0;
+  return launch_status("sfb_mae_random_masking");
 }
 
 extern "C" int sfb_tokens_assemble_keep(const float* y, const float* bias, const float* cls, const float* pos_spatial,
@@ -318,8 +304,7 @@ extern "C" int sfb_tokens_assemble_keep(const float* y, const float* bias, const
   const int64_t items = int64_t(b) * (nkeep + 1) * c;
   tokens_assemble_keep_kernel<<<mae_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(
       y, bias, cls, pos_spatial, pos_temporal, pos_class, ids_keep, b, nkeep, hw, c, x);
-  SFB_MAE_CHECK("sfb_tokens_assemble_keep");
-  return 0;
+  return launch_status("sfb_tokens_assemble_keep");
 }
 
 extern "C" int sfb_tokens_scatter_keep(const float* dx, const int32_t* ids_restore, int32_t b, int32_t nkeep, int32_t l,
@@ -327,8 +312,7 @@ extern "C" int sfb_tokens_scatter_keep(const float* dx, const int32_t* ids_resto
   const int64_t items = int64_t(b) * (l + 1) * c;
   tokens_scatter_keep_kernel<<<mae_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dx, ids_restore, b, nkeep, l, c,
                                                                                       dense);
-  SFB_MAE_CHECK("sfb_tokens_scatter_keep");
-  return 0;
+  return launch_status("sfb_tokens_scatter_keep");
 }
 
 extern "C" int sfb_decoder_assemble(const float* z, const float* bias, const float* mask_token, const float* pos,
@@ -337,8 +321,7 @@ extern "C" int sfb_decoder_assemble(const float* z, const float* bias, const flo
   const int64_t items = int64_t(b) * (l + 1) * c;
   decoder_assemble_kernel<<<mae_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(z, bias, mask_token, pos, ids_restore,
                                                                                    b, nkeep, l, c, out);
-  SFB_MAE_CHECK("sfb_decoder_assemble");
-  return 0;
+  return launch_status("sfb_decoder_assemble");
 }
 
 extern "C" int sfb_decoder_assemble_bwd(const float* dx, const int32_t* ids_keep, const int32_t* masked_rows, int32_t b,
@@ -351,31 +334,28 @@ extern "C" int sfb_decoder_assemble_bwd(const float* dx, const int32_t* ids_keep
   }
   const int64_t items = int64_t(b) * (nkeep + 1) * c;
   decoder_gather_grad_kernel<<<mae_grid(items, 256), 256, 0, stream>>>(dx, ids_keep, b, nkeep, l, c, dz);
-  SFB_MAE_CHECK("sfb_decoder_assemble_bwd(gather)");
+  if (int rc = launch_status("sfb_decoder_assemble_bwd(gather)")) return rc;
   const int64_t pitems = int64_t(l + 1) * c;
   batch_sum_kernel<<<mae_grid(pitems, 256), 256, 0, stream>>>(dx, b, pitems, dpos);
-  SFB_MAE_CHECK("sfb_decoder_assemble_bwd(pos)");
+  if (int rc = launch_status("sfb_decoder_assemble_bwd(pos)")) return rc;
   const int nrows = b * (l - nkeep);
   const int nslab = sfb_segment_slabs(1, nrows);
   indexed_rowsum_partial_kernel<<<nslab, c < 256 ? (c + 31) / 32 * 32 : 256, 0, stream>>>(dx, masked_rows, nrows, c,
                                                                                           partials);
-  SFB_MAE_CHECK("sfb_decoder_assemble_bwd(mask token)");
+  if (int rc = launch_status("sfb_decoder_assemble_bwd(mask token)")) return rc;
   slab_merge_kernel<<<(c + 127) / 128, 128, 0, stream>>>(partials, nslab, c, dmask_token);
-  SFB_MAE_CHECK("sfb_decoder_assemble_bwd(mask token merge)");
-  return 0;
+  return launch_status("sfb_decoder_assemble_bwd(mask token merge)");
 }
 
 extern "C" int sfb_rows_gather(const float* src, int64_t src_pitch, const int32_t* idx, int64_t rows, int32_t c,
                                const float* bias, float* dst, void* stream) {
   rows_gather_kernel<<<mae_grid(rows * c, 256), 256, 0, (cudaStream_t)stream>>>(src, src_pitch, idx, rows, c, bias, dst);
-  SFB_MAE_CHECK("sfb_rows_gather");
-  return 0;
+  return launch_status("sfb_rows_gather");
 }
 
 extern "C" int sfb_rows_scatter(const float* src, const int32_t* idx, int64_t rows, int32_t c, float* dst, void* stream) {
   rows_scatter_kernel<<<mae_grid(rows * c, 256), 256, 0, (cudaStream_t)stream>>>(src, idx, rows, c, dst);
-  SFB_MAE_CHECK("sfb_rows_scatter");
-  return 0;
+  return launch_status("sfb_rows_scatter");
 }
 
 extern "C" int sfb_pixel_targets(const float* x, int32_t b, int32_t ch, int32_t t, int32_t h, int32_t w,
@@ -388,6 +368,5 @@ extern "C" int sfb_pixel_targets(const float* x, int32_t b, int32_t ch, int32_t 
   if (nrows < 1) return 0;
   pixel_targets_kernel<<<mae_grid(int64_t(nrows) * 32, 256), 256, 0, (cudaStream_t)stream>>>(
       x, b, ch, t, h, w, t_stride, u, p, rows, nrows, norm, out);
-  SFB_MAE_CHECK("sfb_pixel_targets");
-  return 0;
+  return launch_status("sfb_pixel_targets");
 }

@@ -10,31 +10,14 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
 using bf = __nv_bfloat16;
 
-#define SFB_MF_CHECK(name)                                                \
-  do {                                                                    \
-    cudaError_t e_ = cudaGetLastError();                                  \
-    if (e_ != cudaSuccess) {                                              \
-      set_error("%s launch failed: %s", name, cudaGetErrorString(e_));    \
-      return -20;                                                         \
-    }                                                                     \
-  } while (0)
-
-static int mf_grid(int64_t items, int block) {
-  int64_t want = (items + block - 1) / block;
-  int64_t cap = int64_t(148) * 8;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
-}
-__device__ __forceinline__ void mf_put_split(bf* hi, bf* lo, int64_t i, float v) {
-  const bf h = __float2bfloat16_rn(v);
-  hi[i] = h;
-  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-}
+static int mf_grid(int64_t items, int block) { return capped_grid(items, block, int64_t(kGridSms) * 8); }
 
 __global__ void mask_upsample_kernel(const float* __restrict__ mask, int b, int mt, int mh, int mw, int t, int h, int w,
                                      float* __restrict__ out) {
@@ -82,7 +65,7 @@ __global__ void tokens_split_grad_masked_kernel(const float* __restrict__ dx, co
     const float g = dx[(bb * (l + 1) + n + 1) * c + ch];
     const float mm = m[bb * l + n];
     const float v = g * (1.f - mm);
-    mf_put_split(dy_hi, dy_lo, i, v);
+    put_split(dy_hi, dy_lo, i, v);
     dy_f32[i] = v;
     dxm[i] = g * mm;
   }
@@ -107,7 +90,7 @@ __global__ void rows_pad_split_kernel(const float* __restrict__ d, int b, int l,
     const int n = int(t % (l + 1));
     const int64_t bb = t / (l + 1);
     const float v = (n > 0 && ch < c) ? d[(bb * l + n - 1) * c + ch] : 0.f;
-    mf_put_split(hi, lo, i, v);
+    put_split(hi, lo, i, v);
   }
 }
 
@@ -175,36 +158,31 @@ extern "C" int sfb_mask_upsample(const float* mask, int32_t b, int32_t mt, int32
                                  int32_t w, float* out, void* stream) {
   mask_upsample_kernel<<<mf_grid(int64_t(b) * t * h * w, 256), 256, 0, (cudaStream_t)stream>>>(mask, b, mt, mh, mw, t,
                                                                                               h, w, out);
-  SFB_MF_CHECK("sfb_mask_upsample");
-  return 0;
+  return launch_status("sfb_mask_upsample");
 }
 extern "C" int sfb_tokens_assemble_masked(const float* y, const float* bias, const float* cls, const float* mask_token,
                                           const float* tokmask, int32_t b, int32_t l, int32_t c, float* x,
                                           void* stream) {
   tokens_assemble_masked_kernel<<<mf_grid(int64_t(b) * (l + 1) * c, 256), 256, 0, (cudaStream_t)stream>>>(
       y, bias, cls, mask_token, tokmask, b, l, c, x);
-  SFB_MF_CHECK("sfb_tokens_assemble_masked");
-  return 0;
+  return launch_status("sfb_tokens_assemble_masked");
 }
 extern "C" int sfb_tokens_split_grad_masked(const float* dx, const float* tokmask, int32_t b, int32_t l, int32_t c,
                                             void* dy_hi, void* dy_lo, float* dy_f32, float* dxm, void* stream) {
   tokens_split_grad_masked_kernel<<<mf_grid(int64_t(b) * l * c, 256), 256, 0, (cudaStream_t)stream>>>(
       dx, tokmask, b, l, c, (bf*)dy_hi, (bf*)dy_lo, dy_f32, dxm);
-  SFB_MF_CHECK("sfb_tokens_split_grad_masked");
-  return 0;
+  return launch_status("sfb_tokens_split_grad_masked");
 }
 extern "C" int sfb_rows_unpad_bias(const float* y, int64_t ldy, const float* bias, int32_t b, int32_t l, int32_t c,
                                    float* out, void* stream) {
   rows_unpad_bias_kernel<<<mf_grid(int64_t(b) * l * c, 256), 256, 0, (cudaStream_t)stream>>>(y, ldy, bias, b, l, c, out);
-  SFB_MF_CHECK("sfb_rows_unpad_bias");
-  return 0;
+  return launch_status("sfb_rows_unpad_bias");
 }
 extern "C" int sfb_rows_pad_split(const float* d, int32_t b, int32_t l, int32_t c, int32_t cp, void* hi, void* lo,
                                   void* stream) {
   rows_pad_split_kernel<<<mf_grid(int64_t(b) * (l + 1) * cp, 256), 256, 0, (cudaStream_t)stream>>>(d, b, l, c, cp,
                                                                                                   (bf*)hi, (bf*)lo);
-  SFB_MF_CHECK("sfb_rows_pad_split");
-  return 0;
+  return launch_status("sfb_rows_pad_split");
 }
 extern "C" int sfb_hog_targets(const float* x, int32_t b, int32_t ch, int32_t t, int32_t h, int32_t w, int32_t t_stride,
                                int32_t nbins, int32_t cell, int32_t fs, float* out, void* stream) {
@@ -215,6 +193,5 @@ extern "C" int sfb_hog_targets(const float* x, int32_t b, int32_t ch, int32_t t,
   const int64_t items = int64_t(b) * (t / t_stride) * ch * (h / cell) * (w / cell);
   hog_targets_kernel<<<mf_grid(items, 128), 128, 0, (cudaStream_t)stream>>>(x, b, ch, t, h, w, t_stride, nbins, cell, fs,
                                                                            out);
-  SFB_MF_CHECK("sfb_hog_targets");
-  return 0;
+  return launch_status("sfb_hog_targets");
 }

@@ -11,36 +11,16 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
-#define SFB_MV_CHECK(name)                                               \
-  do {                                                                   \
-    cudaError_t e_ = cudaGetLastError();                                 \
-    if (e_ != cudaSuccess) {                                             \
-      set_error("%s launch failed: %s", name, cudaGetErrorString(e_));   \
-      return -20;                                                        \
-    }                                                                    \
-  } while (0)
-
 static constexpr size_t kSoftmaxSmemMax = 160 * 1024;  // 8 warps x (keys + rel-pos bins) fp32 rows
 static int mv_grid(int64_t items, int block, int waves = 8) {
-  int64_t want = (items + block - 1) / block;
-  int64_t cap = int64_t(148) * waves;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
+  return capped_grid(items, block, int64_t(kGridSms) * waves);
 }
 
-__device__ __forceinline__ void put_split(__nv_bfloat16* hi, __nv_bfloat16* lo, int64_t i, float v) {
-  const __nv_bfloat16 h = __float2bfloat16_rn(v);
-  hi[i] = h;
-  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-}
-__device__ __forceinline__ float get_split(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int64_t i) {
-  float v = __bfloat162float(hi[i]);
-  if (lo) v += __bfloat162float(lo[i]);
-  return v;
-}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -1039,14 +1019,13 @@ extern "C" int sfb_layernorm_fwd(const float* x, int64_t x_pitch, int64_t rows, 
                                                                          (bf*)o_lo, o_f32, o_pitch, mean, rstd);
   else ln_fwd_kernel<40><<<mv_grid(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(x, x_pitch, rows, c, gamma, beta, eps, (bf*)o_hi,
                                                                          (bf*)o_lo, o_f32, o_pitch, mean, rstd);
-  SFB_MV_CHECK("sfb_layernorm_fwd");
-  return 0;
+  return launch_status("sfb_layernorm_fwd");
 }
 extern "C" int32_t sfb_rowslab_blocks(int64_t rows) {
   // one slab per 8 rows (= one row per warp of a 256-thread block) until the machine is full: the deep stages of MViT have
   // only ~1.6 k token rows, and 64-row slabs left 5/6 of the SMs idle there (ncu r2a: 25 blocks, 127 us for 14 MB)
   int64_t b = (rows + 7) / 8;
-  if (b > 148 * 2) b = 148 * 2;   // (more slabs only move the time into the partial-merge kernel: ncu r2h)
+  if (b > kGridSms * 2) b = kGridSms * 2;   // (more slabs only move the time into the partial-merge kernel: ncu r2h)
   return int32_t(b < 1 ? 1 : b);
 }
 // out_k[ch] (=|+=) sum_b partials[b][k][ch]: fp64 merge of row-slab partials, one 64-thread block per (channel, k)
@@ -1087,10 +1066,9 @@ extern "C" int sfb_layernorm_bwd(const float* dy, int64_t dy_pitch, const float*
                                                                     dx_pitch, dx_accumulate, partials);
   else ln_bwd_wide_kernel<40><<<nb, 256, 0, stream>>>(dy, dy_pitch, x, x_pitch, rows, c, gamma, mean, rstd, dx, dx_pitch,
                                                      dx_accumulate, partials);
-  SFB_MV_CHECK("sfb_layernorm_bwd");
+  if (int rc = launch_status("sfb_layernorm_bwd")) return rc;
   partial_merge2_kernel<<<dim3(c, 2), 64, 0, stream>>>(partials, nb, 2, c, dgamma, dbeta, param_accumulate);
-  SFB_MV_CHECK("sfb_layernorm_bwd(merge)");
-  return 0;
+  return launch_status("sfb_layernorm_bwd(merge)");
 }
 extern "C" int sfb_colsum(const float* src, int64_t pitch, int64_t rows, int32_t c, float* out, int32_t accumulate,
                           float* partials, void* stream_) {
@@ -1100,10 +1078,9 @@ extern "C" int sfb_colsum(const float* src, int64_t pitch, int64_t rows, int32_t
     colsum4_kernel<<<nb, 256, 0, stream>>>(src, pitch, rows, c, partials);
   else
     colsum_kernel<<<nb, 256, 0, stream>>>(src, pitch, rows, c, partials);
-  SFB_MV_CHECK("sfb_colsum");
+  if (int rc = launch_status("sfb_colsum")) return rc;
   partial_merge2_kernel<<<dim3(c, 1), 64, 0, stream>>>(partials, nb, 1, c, out, nullptr, accumulate);
-  SFB_MV_CHECK("sfb_colsum(merge)");
-  return 0;
+  return launch_status("sfb_colsum(merge)");
 }
 extern "C" int sfb_tokens_assemble(const float* y, const float* bias, const float* cls, const float* pos_spatial,
                                    const float* pos_temporal, const float* pos_class, int32_t b, int32_t l, int32_t hw,
@@ -1116,8 +1093,7 @@ extern "C" int sfb_tokens_assemble(const float* y, const float* bias, const floa
   const int64_t items = int64_t(b) * (l + 1) * c;
   tokens_assemble_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(
       y, bias, cls, pos_spatial, pos_temporal, pos_class, b, l, any ? hw : 1, c, x);
-  SFB_MV_CHECK("sfb_tokens_assemble");
-  return 0;
+  return launch_status("sfb_tokens_assemble");
 }
 extern "C" int32_t sfb_segment_slabs(int32_t groups, int32_t seg_rows) {
   // about two blocks per SM over all groups, and at least 8 rows per slab
@@ -1131,11 +1107,10 @@ static int segment_rowsum(const float* src, int c, int n_outer, int64_t outer_st
   const int threads = std::min(256, (c + 31) / 32 * 32);
   segment_rowsum_partial_kernel<<<dim3(nslab, groups), threads, 0, stream>>>(src, c, n_outer, outer_stride, group_stride,
                                                                              seg_rows, partials);
-  SFB_MV_CHECK("segment_rowsum");
+  if (int rc = launch_status("segment_rowsum")) return rc;
   segment_rowsum_merge_kernel<<<mv_grid(int64_t(groups) * c, 256), 256, 0, stream>>>(partials, nslab, groups, c, scale,
                                                                                     out);
-  SFB_MV_CHECK("segment_rowsum(merge)");
-  return 0;
+  return launch_status("segment_rowsum(merge)");
 }
 extern "C" int sfb_pos_embed_sep_bwd(const float* dx, int32_t b, int32_t t, int32_t hw, int32_t c, float* dps, float* dpt,
                                      float* dpc, float* partials, void* stream_) {
@@ -1145,7 +1120,7 @@ extern "C" int sfb_pos_embed_sep_bwd(const float* dx, int32_t b, int32_t t, int3
     return -10;
   }
   pos_sep_bwd_spatial_kernel<<<mv_grid(int64_t(hw + 1) * c, 256), 256, 0, stream>>>(dx, b, t, hw, c, dps, dpc);
-  SFB_MV_CHECK("sfb_pos_embed_sep_bwd");
+  if (int rc = launch_status("sfb_pos_embed_sep_bwd")) return rc;
   const int64_t n = 1 + int64_t(t) * hw;
   return segment_rowsum(dx + c, c, b, n, hw, hw, t, 1.f, dpt, partials, stream);
 }
@@ -1164,8 +1139,7 @@ extern "C" int sfb_token_mean_bwd(const float* dmean, int32_t b, int32_t n, int3
   }
   token_mean_bwd_kernel<1><<<mv_grid(int64_t(b) * n * c, 256), 256, 0, (cudaStream_t)stream>>>(dmean, b, n, c,
                                                                                               1.f / float(n - 1), dx);
-  SFB_MV_CHECK("sfb_token_mean_bwd");
-  return 0;
+  return launch_status("sfb_token_mean_bwd");
 }
 extern "C" int sfb_token_mean_all_fwd(const float* x, int32_t b, int32_t n, int32_t c, float* out, float* partials,
                                       void* stream) {
@@ -1182,8 +1156,7 @@ extern "C" int sfb_token_mean_all_bwd(const float* dmean, int32_t b, int32_t n, 
   }
   token_mean_bwd_kernel<0><<<mv_grid(int64_t(b) * n * c, 256), 256, 0, (cudaStream_t)stream>>>(dmean, b, n, c,
                                                                                               1.f / float(n), dx);
-  SFB_MV_CHECK("sfb_token_mean_all_bwd");
-  return 0;
+  return launch_status("sfb_token_mean_all_bwd");
 }
 extern "C" int sfb_tokens_assemble_joint(const float* y, const float* bias, const float* cls, const float* pos, int32_t b,
                                          int32_t l, int32_t c, float* x, void* stream) {
@@ -1193,8 +1166,7 @@ extern "C" int sfb_tokens_assemble_joint(const float* y, const float* bias, cons
   }
   const int64_t items = int64_t(b) * (l + (cls ? 1 : 0)) * c;
   tokens_assemble_joint_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(y, bias, cls, pos, b, l, c, x);
-  SFB_MV_CHECK("sfb_tokens_assemble_joint");
-  return 0;
+  return launch_status("sfb_tokens_assemble_joint");
 }
 extern "C" int sfb_pos_embed_joint_bwd(const float* dx, int32_t b, int32_t n, int32_t c, float* dpos, void* stream) {
   if (b < 1 || n < 1 || c < 1) {
@@ -1202,8 +1174,7 @@ extern "C" int sfb_pos_embed_joint_bwd(const float* dx, int32_t b, int32_t n, in
     return -10;
   }
   pos_joint_bwd_kernel<<<mv_grid(int64_t(n) * c, 256), 256, 0, (cudaStream_t)stream>>>(dx, b, n, c, dpos);
-  SFB_MV_CHECK("sfb_pos_embed_joint_bwd");
-  return 0;
+  return launch_status("sfb_pos_embed_joint_bwd");
 }
 extern "C" int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt, int32_t kh,
                             int32_t kw, void* hi, void* lo, void* stream) {
@@ -1216,8 +1187,7 @@ extern "C" int sfb_patchify(const float* x, int32_t b, int32_t cin, int32_t t, i
   const int64_t items = int64_t(b) * ot * oh * ow * cin * kt * kh * kw;
   patchify_kernel<false><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, b, cin, t, h, w, kt, kh, kw, ot, oh,
                                                                                 ow, nullptr, 0, (bf*)hi, (bf*)lo);
-  SFB_MV_CHECK("sfb_patchify");
-  return 0;
+  return launch_status("sfb_patchify");
 }
 extern "C" int sfb_patchify_gather(const float* x, int32_t b, int32_t cin, int32_t t, int32_t h, int32_t w, int32_t kt,
                                    int32_t kh, int32_t kw, const int32_t* keep, int32_t nkeep, void* hi, void* lo,
@@ -1233,16 +1203,14 @@ extern "C" int sfb_patchify_gather(const float* x, int32_t b, int32_t cin, int32
   const int64_t items = int64_t(b) * nkeep * cin * kt * kh * kw;
   patchify_kernel<true><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, b, cin, t, h, w, kt, kh, kw, ot, oh,
                                                                                ow, keep, nkeep, (bf*)hi, (bf*)lo);
-  SFB_MV_CHECK("sfb_patchify_gather");
-  return 0;
+  return launch_status("sfb_patchify_gather");
 }
 extern "C" int sfb_tokens_split_grad(const float* dx, int32_t b, int32_t l, int32_t c, void* dy_hi, void* dy_lo,
                                      float* dy_f32, void* stream) {
   const int64_t items = int64_t(b) * l * c;
   tokens_split_grad_kernel<<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dx, b, l, c, (bf*)dy_hi, (bf*)dy_lo,
                                                                                   dy_f32);
-  SFB_MV_CHECK("sfb_tokens_split_grad");
-  return 0;
+  return launch_status("sfb_tokens_split_grad");
 }
 
 // ring kernels of x3d_ops.cu (shared-memory frame ring, every input byte crosses HBM once) for the stride-1 3x3x3 pools
@@ -1298,8 +1266,7 @@ extern "C" int sfb_dwpool_fwd(const sfb_dwpool_desc* d, void* stream) {
       if (rc) return rc;
       const int n = d->b * d->heads * d->hd;
       dwpool_cls_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(p, 0);
-      SFB_MV_CHECK("sfb_dwpool_fwd(cls)");
-      return 0;
+      return launch_status("sfb_dwpool_fwd(cls)");
     }
   }
   const int64_t items = int64_t(d->b) * d->heads * (int64_t(d->ot) * d->oh * d->ow + (d->no_cls ? 0 : 1)) * (d->hd / 4);
@@ -1307,13 +1274,12 @@ extern "C" int sfb_dwpool_fwd(const sfb_dwpool_desc* d, void* stream) {
     dwpool_fwd_kernel<0><<<mv_grid(items, 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
   else
     dwpool_fwd_kernel<1><<<mv_grid(items, 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_MV_CHECK("sfb_dwpool_fwd");
-  return 0;
+  return launch_status("sfb_dwpool_fwd");
 }
 extern "C" int32_t sfb_dwpool_wgrad_blocks(const sfb_dwpool_desc* d) {
   int64_t total = int64_t(d->b) * d->heads * d->ot * d->oh * d->ow;
   int64_t nb = (total + 15) / 16;
-  if (nb > 148 * 4) nb = 148 * 4;
+  if (nb > kGridSms * 4) nb = kGridSms * 4;
   return int32_t(nb < 1 ? 1 : nb);
 }
 __global__ void dwpool_wmerge_kernel(const float* __restrict__ partials, int nblocks, int n, float* __restrict__ out,
@@ -1339,7 +1305,7 @@ extern "C" int sfb_dwpool_bwd(const sfb_dwpool_desc* d, float* dw, int32_t dw_ac
       if (rc) return rc;
       const int n = d->b * d->heads * d->hd;
       dwpool_cls_kernel<<<(n + 255) / 256, 256, 0, stream>>>(p, 1);
-      SFB_MV_CHECK("sfb_dwpool_bwd(cls)");
+      if (int rc = launch_status("sfb_dwpool_bwd(cls)")) return rc;
       if (dw) {
         if (!dw_accumulate) cudaMemsetAsync(dw, 0, size_t(d->hd) * 27 * sizeof(float), stream);
         rc = dw3_run_strided(1, d->src + d->src_pitch + d->src_c0, d->src_pitch, (L + 1) * d->src_pitch, d->hd,
@@ -1364,7 +1330,7 @@ extern "C" int sfb_dwpool_bwd(const sfb_dwpool_desc* d, float* dw, int32_t dw_ac
     else
       dwpool_bwd_data_kernel<0><<<mv_grid(items, 256, 16), 256, 0, stream>>>(p);
   }
-  SFB_MV_CHECK("sfb_dwpool_bwd(data)");
+  if (int rc = launch_status("sfb_dwpool_bwd(data)")) return rc;
   if (d->has_pool && dw) {
     const int nb = sfb_dwpool_wgrad_blocks(d);
     if (d->hd > 256 || d->kt > 3 || d->kh > 3 || d->kw > 3) {
@@ -1379,7 +1345,7 @@ extern "C" int sfb_dwpool_bwd(const sfb_dwpool_desc* d, float* dw, int32_t dw_ac
       dwpool_bwd_weight_kernel<1><<<nb, pl * d->hd, size_t(pl) * d->hd * 27 * sizeof(float), stream>>>(p);
     else
       dwpool_bwd_weight_kernel<0><<<nb, pl * d->hd, size_t(pl) * d->hd * 27 * sizeof(float), stream>>>(p);
-    SFB_MV_CHECK("sfb_dwpool_bwd(weight)");
+    if (int rc = launch_status("sfb_dwpool_bwd(weight)")) return rc;
   }
   return 0;
 }
@@ -1428,8 +1394,7 @@ extern "C" int sfb_softmax_relpos_fwd(const sfb_softmax_desc* d, void* stream) {
     return -10;
   }
   softmax_dispatch<false>(d, p, rows, smem, (cudaStream_t)stream);
-  SFB_MV_CHECK("sfb_softmax_relpos_fwd");
-  return 0;
+  return launch_status("sfb_softmax_relpos_fwd");
 }
 extern "C" int sfb_softmax_relpos_bwd(const sfb_softmax_desc* d, void* stream) {
   SoftmaxParams p;
@@ -1441,68 +1406,59 @@ extern "C" int sfb_softmax_relpos_bwd(const sfb_softmax_desc* d, void* stream) {
     return -10;
   }
   softmax_dispatch<true>(d, p, rows, smem, (cudaStream_t)stream);
-  SFB_MV_CHECK("sfb_softmax_relpos_bwd");
-  return 0;
+  return launch_status("sfb_softmax_relpos_bwd");
 }
 extern "C" int sfb_attn_merge(const float* o, const void* q_hi, const void* q_lo, int32_t b, int32_t h, int32_t n,
                               int32_t hd, int32_t residual, void* m_hi, void* m_lo, void* stream) {
   const int64_t items = int64_t(b) * n * h * hd;
   attn_merge_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(o, (const bf*)q_hi, (const bf*)q_lo, b, h, n,
                                                                              hd, residual, (bf*)m_hi, (bf*)m_lo);
-  SFB_MV_CHECK("sfb_attn_merge");
-  return 0;
+  return launch_status("sfb_attn_merge");
 }
 extern "C" int sfb_attn_merge_nocls(const float* o, const void* q_hi, const void* q_lo, int32_t b, int32_t h, int32_t n,
                                     int32_t hd, int32_t residual, void* m_hi, void* m_lo, void* stream) {
   const int64_t items = int64_t(b) * n * h * hd;
   attn_merge_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(o, (const bf*)q_hi, (const bf*)q_lo, b, h, n,
                                                                              hd, residual, (bf*)m_hi, (bf*)m_lo);
-  SFB_MV_CHECK("sfb_attn_merge_nocls");
-  return 0;
+  return launch_status("sfb_attn_merge_nocls");
 }
 extern "C" int sfb_attn_split_grad(const float* dm, int32_t b, int32_t h, int32_t n, int32_t hd, int32_t residual,
                                    void* do_hi, void* do_lo, float* dq, void* stream) {
   const int64_t items = int64_t(b) * h * n * hd;
   attn_split_grad_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dm, b, h, n, hd, residual,
                                                                                    (bf*)do_hi, (bf*)do_lo, dq);
-  SFB_MV_CHECK("sfb_attn_split_grad");
-  return 0;
+  return launch_status("sfb_attn_split_grad");
 }
 extern "C" int sfb_attn_split_grad_nocls(const float* dm, int32_t b, int32_t h, int32_t n, int32_t hd, int32_t residual,
                                          void* do_hi, void* do_lo, float* dq, void* stream) {
   const int64_t items = int64_t(b) * h * n * hd;
   attn_split_grad_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(dm, b, h, n, hd, residual,
                                                                                    (bf*)do_hi, (bf*)do_lo, dq);
-  SFB_MV_CHECK("sfb_attn_split_grad_nocls");
-  return 0;
+  return launch_status("sfb_attn_split_grad_nocls");
 }
 extern "C" int sfb_residual_add(const float* a, const float* a_bias, const float* y, const float* y_bias,
                                 const float* scale, int64_t rows, int32_t c, int64_t rows_per_sample, float* out,
                                 void* stream) {
   residual_add_kernel<<<mv_grid(rows * c, 256), 256, 0, (cudaStream_t)stream>>>(a, a_bias, y, y_bias, scale, rows, c,
                                                                                 rows_per_sample, out);
-  SFB_MV_CHECK("sfb_residual_add");
-  return 0;
+  return launch_status("sfb_residual_add");
 }
 extern "C" int sfb_bias_gelu(const float* y, const float* bias, int64_t rows, int32_t c, void* hi, void* lo,
                              void* stream) {
   bias_gelu_kernel<<<mv_grid(rows * c, 256), 256, 0, (cudaStream_t)stream>>>(y, bias, rows, c, (bf*)hi, (bf*)lo);
-  SFB_MV_CHECK("sfb_bias_gelu");
-  return 0;
+  return launch_status("sfb_bias_gelu");
 }
 extern "C" int sfb_bias_gelu_bwd(const float* dh, const float* y, const float* bias, int64_t rows, int32_t c, void* hi,
                                  void* lo, float* dpre, void* stream) {
   bias_gelu_bwd_kernel<<<mv_grid(rows * c, 256), 256, 0, (cudaStream_t)stream>>>(dh, y, bias, rows, c, (bf*)hi, (bf*)lo,
                                                                                  dpre);
-  SFB_MV_CHECK("sfb_bias_gelu_bwd");
-  return 0;
+  return launch_status("sfb_bias_gelu_bwd");
 }
 extern "C" int sfb_scale_split(const float* src, const float* scale, int64_t rows, int32_t c, int64_t rows_per_sample,
                                void* hi, void* lo, float* f32, void* stream) {
   scale_split_kernel<<<mv_grid(rows * c, 256), 256, 0, (cudaStream_t)stream>>>(src, scale, rows, c, rows_per_sample,
                                                                                (bf*)hi, (bf*)lo, f32);
-  SFB_MV_CHECK("sfb_scale_split");
-  return 0;
+  return launch_status("sfb_scale_split");
 }
 static void fill_tp(TokPoolParams& p, const sfb_tokpool_desc* d) {
   memset(&p, 0, sizeof(p));
@@ -1520,8 +1476,7 @@ extern "C" int sfb_token_maxpool_fwd(const sfb_tokpool_desc* d, void* stream) {
     token_maxpool_fwd_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
   else
     token_maxpool_fwd_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_MV_CHECK("sfb_token_maxpool_fwd");
-  return 0;
+  return launch_status("sfb_token_maxpool_fwd");
 }
 extern "C" int sfb_token_maxpool_bwd(const sfb_tokpool_desc* d, void* stream) {
   TokPoolParams p;
@@ -1531,6 +1486,5 @@ extern "C" int sfb_token_maxpool_bwd(const sfb_tokpool_desc* d, void* stream) {
     token_maxpool_bwd_kernel<0><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
   else
     token_maxpool_bwd_kernel<1><<<mv_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_MV_CHECK("sfb_token_maxpool_bwd");
-  return 0;
+  return launch_status("sfb_token_maxpool_bwd");
 }

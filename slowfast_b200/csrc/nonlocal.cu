@@ -7,28 +7,18 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
 typedef __nv_bfloat16 nl_bf;
 
+// 8 blocks per SM of the device (of kGridSms when there is none: the launch that follows reports it)
 static int nl_grid(int64_t items, int block) {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  int64_t want = (items + block - 1) / block;
-  const int64_t cap = int64_t(sms) * 8;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
-}
-
-__device__ __forceinline__ void nl_put_split(nl_bf* hi, nl_bf* lo, int64_t i, float v) {
-  const nl_bf h = __float2bfloat16_rn(v);
-  hi[i] = h;
-  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+  int sms = kGridSms;
+  device_limits(&sms, nullptr);
+  return capped_grid(items, block, int64_t(sms) * 8);
 }
 
 // out[r, j] = x[r, j] + bias[j] for j < c, 0 for c <= j < c_out; one thread per 8 output columns of a row
@@ -45,7 +35,7 @@ __global__ void bias_split_kernel(const float* __restrict__ x, int64_t rows, int
     for (int e = 0; e < 8; ++e) {
       const int j = j0 + e;
       const float v = j < c ? xr[j] + (bias ? bias[j] : 0.f) : 0.f;
-      nl_put_split(hi, lo, r * o_pitch + j, v);
+      put_split(hi, lo, r * o_pitch + j, v);
     }
   }
 }
@@ -96,12 +86,7 @@ extern "C" int sfb_bias_split(const float* x, int64_t rows, int32_t c, int64_t x
   if (items == 0) return 0;
   bias_split_kernel<<<nl_grid(items, 256), 256, 0, (cudaStream_t)stream>>>(x, rows, c, x_pitch, bias, (nl_bf*)hi,
                                                                            (nl_bf*)lo, o_pitch, c_out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_bias_split launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_bias_split");
 }
 
 extern "C" int sfb_bn_conv_bias(const float* bias, int32_t c, float momentum, int32_t training, float* running_mean,
@@ -113,12 +98,7 @@ extern "C" int sfb_bn_conv_bias(const float* bias, int32_t c, float momentum, in
   if (!training) splits = 1;  // eval uses the single BN's statistics
   bn_conv_bias_kernel<<<(c + 255) / 256, 256, 0, (cudaStream_t)stream>>>(bias, c, momentum, training, running_mean, scale,
                                                                          shift, save_mean, splits > 1 ? splits : 1);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_bn_conv_bias launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_bn_conv_bias");
 }
 
 extern "C" int sfb_planes_to_f32(const void* hi, const void* lo, int64_t rows, int32_t c, int64_t pitch, float* out,
@@ -127,10 +107,5 @@ extern "C" int sfb_planes_to_f32(const void* hi, const void* lo, int64_t rows, i
   if (items == 0) return 0;
   planes_to_f32_kernel<<<nl_grid(items, 256), 256, 0, (cudaStream_t)stream>>>((const nl_bf*)hi, (const nl_bf*)lo, rows, c,
                                                                                pitch, out, out_pitch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sfb_planes_to_f32 launch failed: %s", cudaGetErrorString(e));
-    return -20;
-  }
-  return 0;
+  return launch_status("sfb_planes_to_f32");
 }

@@ -18,7 +18,7 @@
 #include <cstdint>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "runtime.h"
 
 namespace sfb {
 
@@ -133,18 +133,9 @@ __global__ void __launch_bounds__(OPT_THREADS) momentum_update_kernel(const Mome
     c.key[i] = __fadd_rn(__fmul_rn(c.query[i], c1), __fmul_rn(c.key[i], c2));
 }
 
-#define SFB_OPT_CHECK(name)                                              \
-  do {                                                                   \
-    cudaError_t e_ = cudaGetLastError();                                 \
-    if (e_ != cudaSuccess) {                                             \
-      sfb::set_error("%s launch failed: %s", name, cudaGetErrorString(e_)); \
-      return -20;                                                        \
-    }                                                                    \
-  } while (0)
-
 }  // namespace sfb
 
-extern "C" int32_t sfb_flat_sumsq_blocks(void) { return 148 * 4; }
+extern "C" int32_t sfb_flat_sumsq_blocks(void) { return sfb::kGridSms * 4; }
 
 extern "C" int sfb_flat_sumsq(const float* flat, int64_t n, double* partials, float max_norm, float inv_scale,
                               float* out3, void* stream) {
@@ -154,10 +145,9 @@ extern "C" int sfb_flat_sumsq(const float* flat, int64_t n, double* partials, fl
   }
   const int nb = sfb_flat_sumsq_blocks();
   sfb::flat_sumsq_partial_kernel<<<nb, sfb::OPT_THREADS, 0, (cudaStream_t)stream>>>(flat, n, partials);
-  SFB_OPT_CHECK("flat_sumsq_partial");
+  if (int rc = sfb::launch_status("flat_sumsq_partial")) return rc;
   sfb::flat_sumsq_final_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(partials, nb, max_norm, inv_scale, out3);
-  SFB_OPT_CHECK("flat_sumsq_final");
-  return 0;
+  return sfb::launch_status("flat_sumsq_final");
 }
 
 extern "C" int32_t sfb_opt_chunk_size(void) { return int32_t(sizeof(sfb::OptChunk)); }
@@ -169,8 +159,7 @@ extern "C" int sfb_flat_sgd(const void* chunks, int32_t n_chunks, const float* g
   sfb::flat_update_kernel<false><<<n_chunks, sfb::OPT_THREADS, 0, (cudaStream_t)stream>>>(
       (const sfb::OptChunk*)chunks, grad, momentum_buf, nullptr, group_lr, group_wd, gscale, momentum, dampening,
       nesterov, first_step, 0.f, 0.f, 0.f, 1.f, 1.f);
-  SFB_OPT_CHECK("flat_sgd");
-  return 0;
+  return sfb::launch_status("flat_sgd");
 }
 
 extern "C" int sfb_flat_adamw(const void* chunks, int32_t n_chunks, const float* grad, float* exp_avg, float* exp_avg_sq,
@@ -182,8 +171,7 @@ extern "C" int sfb_flat_adamw(const void* chunks, int32_t n_chunks, const float*
   sfb::flat_update_kernel<true><<<n_chunks, sfb::OPT_THREADS, 0, (cudaStream_t)stream>>>(
       (const sfb::OptChunk*)chunks, grad, exp_avg, exp_avg_sq, group_lr, group_wd, gscale, 0.f, 0.f, 0, 0, beta1, beta2,
       eps, float(bc1), float(sqrt(bc2)));
-  SFB_OPT_CHECK("flat_adamw");
-  return 0;
+  return sfb::launch_status("flat_adamw");
 }
 
 extern "C" int32_t sfb_momentum_chunk_size(void) { return int32_t(sizeof(sfb::MomentumChunk)); }
@@ -192,6 +180,5 @@ extern "C" int sfb_momentum_update(const void* chunks, int32_t n_chunks, float c
   if (n_chunks <= 0) return 0;
   sfb::momentum_update_kernel<<<n_chunks, sfb::OPT_THREADS, 0, (cudaStream_t)stream>>>(
       (const sfb::MomentumChunk*)chunks, c1, c2);
-  SFB_OPT_CHECK("momentum_update");
-  return 0;
+  return sfb::launch_status("momentum_update");
 }

@@ -15,47 +15,15 @@
 #include <cuda_bf16.h>
 
 #include "../../include/slowfast_b200.h"
-#include "tmap.h"
+#include "planes.cuh"
+#include "runtime.h"
 
 namespace sfb {
 
 using bf = __nv_bfloat16;
 
-#define SFB_X3_CHECK(name)                                                \
-  do {                                                                    \
-    cudaError_t e_ = cudaGetLastError();                                  \
-    if (e_ != cudaSuccess) {                                              \
-      set_error("%s launch failed: %s", name, cudaGetErrorString(e_));    \
-      return -20;                                                         \
-    }                                                                     \
-  } while (0)
-
 static int x3_grid(int64_t items, int block, int waves = 8) {
-  int64_t want = (items + block - 1) / block;
-  int64_t cap = int64_t(148) * waves;
-  return int(want < 1 ? 1 : (want > cap ? cap : want));
-}
-
-__device__ __forceinline__ uint32_t pack_bf2(float a, float b) {
-  const __nv_bfloat162 t = __halves2bfloat162(__float2bfloat16_rn(a), __float2bfloat16_rn(b));
-  return *reinterpret_cast<const uint32_t*>(&t);
-}
-__device__ __forceinline__ void store_planes4(bf* hi, bf* lo, int64_t off, float4 v) {
-  const bf h0 = __float2bfloat16_rn(v.x), h1 = __float2bfloat16_rn(v.y), h2 = __float2bfloat16_rn(v.z),
-           h3 = __float2bfloat16_rn(v.w);
-  uint2 h;
-  {
-    const __nv_bfloat162 a = __halves2bfloat162(h0, h1), b = __halves2bfloat162(h2, h3);
-    h.x = *reinterpret_cast<const uint32_t*>(&a);
-    h.y = *reinterpret_cast<const uint32_t*>(&b);
-  }
-  *reinterpret_cast<uint2*>(hi + off) = h;
-  if (lo) {
-    uint2 l;
-    l.x = pack_bf2(v.x - __bfloat162float(h0), v.y - __bfloat162float(h1));
-    l.y = pack_bf2(v.z - __bfloat162float(h2), v.w - __bfloat162float(h3));
-    *reinterpret_cast<uint2*>(lo + off) = l;
-  }
+  return capped_grid(items, block, int64_t(kGridSms) * waves);
 }
 
 // ============================================================================================ channelwise conv, v2
@@ -1015,7 +983,7 @@ __global__ void relu_bwd_kernel(float* dx, const float* y, int64_t n) {
 
 // ------------------------------------------------------------------------------------------------ host helpers
 static int dw_tiles_per_sample(int n, int64_t P) {
-  int64_t want = (int64_t(148) * 8 + n - 1) / n;  // ~8 tiles per SM over the whole batch
+  int64_t want = (int64_t(kGridSms) * 8 + n - 1) / n;  // ~8 tiles per SM over the whole batch
   int64_t maxt = (P + 63) / 64;                   // at least 64 positions per tile
   if (want > maxt) want = maxt;
   return int(want < 1 ? 1 : want);
@@ -1089,7 +1057,7 @@ static void dw2_fwd_tiling(int n, int ot, int oh, int ow, int c, int cfg, Dw2Par
   p.mt_w = (ow + kDw2Tile[cfg][2] - 1) / kDw2Tile[cfg][2];
   p.MT = p.mt_t * p.mt_h * p.mt_w;
   const int sp = dw2_sp(c);
-  int want = (148 * 8 + n - 1) / n;
+  int want = (kGridSms * 8 + n - 1) / n;
   const int maxt = (p.MT + sp - 1) / sp;
   if (want > maxt) want = maxt;
   if (want < 1) want = 1;
@@ -1109,7 +1077,7 @@ static void dw2_block_split(Dw2Params& p, int c, int* blocks) {
   const int sp = dw2_sp(c);
   p.total_mts = int64_t(p.n) * p.MT;
   int64_t nb = (p.total_mts + sp - 1) / sp;
-  if (nb > 148 * 4) nb = 148 * 4;
+  if (nb > kGridSms * 4) nb = kGridSms * 4;
   if (nb < 1) nb = 1;
   p.mts_per_block = (p.total_mts + nb - 1) / nb;
   *blocks = int((p.total_mts + p.mts_per_block - 1) / p.mts_per_block);
@@ -1126,7 +1094,7 @@ static int dw3_tile(int t, int h, int w, int ot, int oh, int ow, int kt, int kh,
     // measured (profiles/r2_dw_ring_probe.md): the conv wants >= 1 block per SM before the 4x smaller tile pays off; the
     // weight gradient (one atomic per channel, tap and block) keeps the big tile down to half a block per SM
     const int64_t blocks14 = int64_t(h / 14) * (w / 14) * ((c + DW3_CB - 1) / DW3_CB) * samples;
-    return blocks14 >= (wgrad ? 64 : 148) ? 14 : 7;
+    return blocks14 >= (wgrad ? 64 : kGridSms) ? 14 : 7;
   }
   if (h % 7 == 0 && w % 7 == 0) return 7;
   return 0;
@@ -1174,8 +1142,7 @@ static int dw3_launch(int tile, bool wgrad, Dw2Params& p, cudaStream_t st, int s
     if (wgrad) dw3_wgrad_kernel<7, 7, 1><<<grid, 224, dw3_smem<7, 1>(true), st>>>(p);
     else dw3_conv_kernel<7, 7, 1><<<grid, 224, dw3_smem<7, 1>(false), st>>>(p);
   }
-  SFB_X3_CHECK("sfb_dwconv (v3 ring kernel)");
-  return 0;
+  return launch_status("sfb_dwconv (v3 ring kernel)");
 }
 
 // stride (1,2,2) eligibility: 3x3x3, padding 1, even input extents, output extents multiples of 7
@@ -1220,8 +1187,7 @@ static int dw2_launch_conv(int cfg, const Dw2Params& p, int threads, size_t smem
   if (cfg == 0) dw2_conv_kernel<3, 3, 3, 1, 1, 2, 4><<<p.m_tiles, threads, smem, st>>>(p);
   else if (cfg == 1) dw2_conv_kernel<3, 3, 3, 2, 1, 1, 4><<<p.m_tiles, threads, smem, st>>>(p);
   else dw2_conv_kernel<5, 1, 1, 1, 4, 1, 1><<<p.m_tiles, threads, smem, st>>>(p);
-  SFB_X3_CHECK("sfb_dwconv (v2 conv)");
-  return 0;
+  return launch_status("sfb_dwconv (v2 conv)");
 }
 static int dw2_launch_wgrad(int cfg, const Dw2Params& p, int blocks, int threads, size_t smem, cudaStream_t st) {
   static bool attr = false;
@@ -1234,8 +1200,7 @@ static int dw2_launch_wgrad(int cfg, const Dw2Params& p, int blocks, int threads
   if (cfg == 0) dw2_wgrad_kernel<3, 3, 3, 1, 1, 2, 4><<<blocks, threads, smem, st>>>(p);
   else if (cfg == 1) dw2_wgrad_kernel<3, 3, 3, 2, 1, 1, 4><<<blocks, threads, smem, st>>>(p);
   else dw2_wgrad_kernel<5, 1, 1, 1, 4, 1, 1><<<blocks, threads, smem, st>>>(p);
-  SFB_X3_CHECK("sfb_dwconv (v2 wgrad)");
-  return 0;
+  return launch_status("sfb_dwconv (v2 wgrad)");
 }
 
 }  // namespace sfb
@@ -1327,7 +1292,7 @@ extern "C" int sfb_dwconv_bwd(const sfb_dwconv_desc* d, float* dw, void* stream)
       int blocks = 1;
       dw2_block_split(q, d->c, &blocks);
       dw2_dgrad_s2_kernel<<<blocks, threads, 0, st>>>(q);
-      SFB_X3_CHECK("sfb_dwconv_bwd (v2 stride-2 data)");
+      if (int rc = launch_status("sfb_dwconv_bwd (v2 stride-2 data)")) return rc;
     } else {
       // stride 1: dx = correlation of dy with the mirrored filter, padding K-1-p; "input" = dy, "output" = dx
       q.flip = 1;
@@ -1351,8 +1316,7 @@ extern "C" int sfb_bnact_fwd(const sfb_bnact_desc* d, void* stream) {
   BnActParams p;
   bnact_fill(p, d);
   bnact_fwd_kernel<<<x3_grid(d->rows * (d->c / 4), 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_bnact_fwd");
-  return 0;
+  return launch_status("sfb_bnact_fwd");
 }
 extern "C" int32_t sfb_bnact_tiles_per_sample(int64_t rows, int64_t rows_per_sample) {
   return dw_tiles_per_sample(int(rows / rows_per_sample), rows_per_sample);
@@ -1365,40 +1329,34 @@ extern "C" int sfb_bnact_bwd_reduce(const sfb_bnact_desc* d, void* stream) {
   const int PL = 256 / (d->c / 4);
   bnact_bwd_reduce_kernel<<<n * p.tiles_per_sample, 256, size_t(PL) * 2 * d->c * sizeof(float),
                             (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_bnact_bwd_reduce");
-  return 0;
+  return launch_status("sfb_bnact_bwd_reduce");
 }
 extern "C" int sfb_bnact_bwd_apply(const sfb_bnact_desc* d, void* stream) {
   if (int rc = bnact_check(d, "sfb_bnact_bwd_apply")) return rc;
   BnActParams p;
   bnact_fill(p, d);
   bnact_bwd_apply_kernel<<<x3_grid(d->rows * (d->c / 4), 256, 16), 256, 0, (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_bnact_bwd_apply");
-  return 0;
+  return launch_status("sfb_bnact_bwd_apply");
 }
 extern "C" int sfb_se_fwd(const sfb_se_desc* d, void* stream) {
   SeParams p;
   se_fill(p, d);
   se_fwd_kernel<<<d->n, 256, size_t(d->c_pad + d->f) * sizeof(float), (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_se_fwd");
-  return 0;
+  return launch_status("sfb_se_fwd");
 }
 extern "C" int sfb_se_bwd(const sfb_se_desc* d, void* stream) {
   SeParams p;
   se_fill(p, d);
   se_bwd_sample_kernel<<<d->n, 256, size_t(d->c_pad + d->f) * sizeof(float), (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_se_bwd(sample)");
+  if (int rc = launch_status("sfb_se_bwd(sample)")) return rc;
   se_bwd_channel_kernel<<<(d->c_pad + 63) / 64, 64, 0, (cudaStream_t)stream>>>(p);
-  SFB_X3_CHECK("sfb_se_bwd(channel)");
-  return 0;
+  return launch_status("sfb_se_bwd(channel)");
 }
 extern "C" int sfb_relu_fwd(float* x, int64_t n, void* stream) {
   relu_fwd_kernel<<<x3_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(x, n);
-  SFB_X3_CHECK("sfb_relu_fwd");
-  return 0;
+  return launch_status("sfb_relu_fwd");
 }
 extern "C" int sfb_relu_bwd(float* dx, const float* y, int64_t n, void* stream) {
   relu_bwd_kernel<<<x3_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(dx, y, n);
-  SFB_X3_CHECK("sfb_relu_bwd");
-  return 0;
+  return launch_status("sfb_relu_bwd");
 }
