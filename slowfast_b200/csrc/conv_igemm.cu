@@ -11,12 +11,15 @@
 //   issued back to back (a runtime width switch makes ptxas serialise them).
 // * Split-K (conv_ksplit): a grid that fills too little of its last wave gives each tile to s CTAs, each over a slice
 //   of the k-blocks; the partial tiles meet in the output with red.global.add.
-// * Persistent CTAs, warp-specialised: warps 0..7 = two MMA warpgroups (rows 0..63 / 64..127 of the tile),
-//   warp 8 = TMA producer, warps 9..16 = epilogue.  The MMA warpgroups hand a finished tile to the epilogue through a
-//   shared-memory accumulator tile and go on with the main loop of the next one.
-// * Epilogue: accumulator tile -> coalesced fp32 stores through an arbitrary (n,t,h,w)-strided
-//   output view (channel-slice "concat in place", strided dgrad scatter), optional accumulate, and per-tile
-//   per-channel (sum, sum^2) partials for train-mode BatchNorm ([2][cout][m_tiles]).
+// * Persistent ping-pong CTAs, warp-specialised: warpgroup 0 is the TMA producer (one elected lane issues the loads),
+//   warpgroups 1 and 2 are consumers.  A consumer owns whole 128 x BN tiles (two m64 row blocks in its registers) and
+//   the CTA's work units alternate between the two.  An ordered pair of named barriers lets one consumer issue its
+//   main loop while the other runs its epilogue, so no shared-memory accumulator tile is needed and all of shared
+//   memory but the BatchNorm scratch goes to the operand ring.
+// * Epilogue from the wgmma fragments: each warp passes its rows through a 1 KB staging block (store_fragment), so every
+//   fp32 store instruction writes whole 128-byte lines.  Stores go through an arbitrary (n,t,h,w)-strided output view
+//   (channel-slice "concat in place", strided dgrad scatter), with optional accumulate, and per-tile per-channel
+//   (sum, sum^2) partials for train-mode BatchNorm ([2][cout][m_tiles]).
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -29,15 +32,19 @@ namespace sfb {
 
 constexpr int BLOCK_M = 128;
 constexpr int MAX_STAGES = 8;
-constexpr int EPI_WARPS = 8;                     // two per 32-row quarter of the tile: the pair splits the tile's 16-column chunks
-constexpr int EPI_STAGE_FLOATS = 64;             // per epilogue warp: 32 row offsets (int64)
-constexpr int MMA_WARPS = 8;                     // two warpgroups of 64 tile rows
-constexpr int PRODUCER_WARP = MMA_WARPS;
-constexpr int EPI_WARP0 = MMA_WARPS + 1;
-constexpr int CONV_THREADS = 32 * (MMA_WARPS + 1 + EPI_WARPS);
-constexpr int BN_MAX = 128;                      // accumulator columns per tile: 64 registers per MMA thread
+constexpr int CONV_THREADS = 384;                // warpgroup 0: producer; warpgroups 1, 2: MMA + epilogue consumers
+constexpr int PRODUCER_REGS = 40;                // 128 x (40 + 2 x 232) registers fit the 64 K register file
+constexpr int CONSUMER_REGS = 232;
+constexpr int BAR_ORDER = 1;                     // named barrier 1 + c: consumer c may issue its main loop
+constexpr int BAR_EPI = 3;                       // named barrier 3 + c: consumer c's epilogue (row table, partials)
+constexpr int BN_MAX = 128;                      // accumulator columns per tile: 128 registers per consumer thread
 constexpr int BLOCK_K = 64;                      // K columns per k-block (pipeline stage)
 constexpr int KSTEPS = BLOCK_K / 16;             // wgmma k16 steps per k-block
+constexpr long long kNoRow = INT64_MIN;          // epilogue row table: tile row past M
+// per consumer: the tile's row table, then 4 warps' 8 x 32 fp32 staging blocks, which the [4][BN][2] BatchNorm
+// partials reuse once the tile is stored
+constexpr uint32_t EPI_SCRATCH = BLOCK_M * 8 + 4 * 8 * 32 * 4;
+static_assert(4 * BN_MAX * 2 * 4 <= 4 * 8 * 32 * 4, "BatchNorm partials fit the staging blocks");
 
 struct ConvParams {
   CUtensorMap tmA[2];
@@ -55,12 +62,10 @@ struct ConvParams {
   uint32_t stage_bytes, chunk_bytes, b_bytes, a_total_bytes, a_plane_bytes;
   uint32_t a_layout, a_sbo, a_lbo;
   uint32_t a_kstep[KSTEPS];  // start of k-step ks's A columns in the stage, in 16-byte units
-  uint32_t acc_pitch;  // floats per row of the shared-memory accumulator tile
-  uint32_t off_acc, off_staging, off_red, off_bars;
+  uint32_t off_epi, off_bars;
   float* out;
   long long os_n, os_z, os_p, os_q;
   int accumulate;
-  int epi_coalesced;
   float* stats;
 };
 
@@ -72,28 +77,84 @@ __device__ __forceinline__ int k_block_begin(const ConvParams& p, int kpart) {
 // csrc/conv_direct.cu: fp32 SIMT body for narrow layers (C_in <= 8); returns 1 when it handled the call
 int conv_direct_try(const sfb_conv_desc* d, cudaStream_t stream, int* rc_out);
 
+// Stores a consumer's 128 x BN accumulator fragment (layout in the kernel's epilogue).  Each warp passes its rows through
+// a 1 KB staging block, 8 rows x 32 columns at a time, so that every store instruction writes whole 128-byte lines:
+// lane l writes float4 columns 4 (l % 8) .. +3 of rows l / 8 and l / 8 + 4.  The block's 8-column groups are XOR-swizzled
+// by the row, so the fragment writes and the row reads are both conflict-free.  MODE 0 overwrites, 1 adds to the
+// destination, 2 adds with red.global.add.  roff: the tile's row table (kNoRow: not stored); columns from ncols on are
+// not stored.
+template <int BN, int MODE>
+__device__ __forceinline__ void store_fragment(const float (&d)[2][BN / 2], float* stage, const long long* roff,
+                                               float* out, int ncols) {
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int g = lane >> 2, cq = 2 * (lane & 3);  // fragment: row g (+8 h), columns 8 jn + cq, +1
+  const int rr = lane >> 3, c4 = 4 * (lane & 7);   // read-back: rows rr and rr + 4, columns c4 .. c4 + 3
+#pragma unroll
+  for (int rb = 0; rb < 2; ++rb) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int cg = 0; cg < (BN + 31) / 32; ++cg) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int jn = 4 * cg + jj;
+          if (jn < BN / 8)
+            *reinterpret_cast<float2*>(stage + g * 32 + ((8 * jj + cq) ^ (8 * (g & 3)))) =
+                make_float2(d[rb][4 * jn + 2 * h], d[rb][4 * jn + 2 * h + 1]);
+        }
+        __syncwarp();
+        float4 v[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) v[k] = *reinterpret_cast<const float4*>(stage + (rr + 4 * k) * 32 + (c4 ^ (8 * rr)));
+        __syncwarp();
+        const int col = 32 * cg + c4;
+        if (col >= ncols) continue;
+        float4* dst[2];
+        bool ok[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const long long o = roff[64 * rb + 16 * warp + 8 * h + rr + 4 * k];
+          ok[k] = o != kNoRow;
+          dst[k] = reinterpret_cast<float4*>(out + (ok[k] ? o + col : 0));
+        }
+        if (MODE == 1) {
+          float4 o[2];
+#pragma unroll
+          for (int k = 0; k < 2; ++k)
+            if (ok[k]) o[k] = *dst[k];
+#pragma unroll
+          for (int k = 0; k < 2; ++k)
+            if (ok[k]) *dst[k] = make_float4(v[k].x + o[k].x, v[k].y + o[k].y, v[k].z + o[k].z, v[k].w + o[k].w);
+        } else {
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            if (!ok[k]) continue;
+            if (MODE == 2)
+              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst[k]), "f"(v[k].x), "f"(v[k].y),
+                           "f"(v[k].z), "f"(v[k].w) : "memory");
+            else
+              *dst[k] = v[k];
+          }
+        }
+      }
+    }
+  }
+}
+
 template <int NSPLIT, int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
   static_assert(BN % 16 == 0 && BN <= BN_MAX, "tile width: a multiple of 16 up to BN_MAX");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bars);
   uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tfull = empty + MAX_STAGES;
-  uint64_t* tempty = tfull + 1;
-  float* acc_tile = reinterpret_cast<float*>(smem + p.off_acc);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 32 * MMA_WARPS);
+      mbar_init(&empty[s], 128);  // the 128 threads of the consumer that read the stage
     }
-    mbar_init(tfull, 32 * MMA_WARPS);
-    mbar_init(tempty, EPI_WARPS);
     fence_mbar_init();
     fence_proxy_async_smem();
   }
@@ -102,9 +163,11 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
   // A work unit is one output tile and one of its p.ksplit slices of k-blocks; a tile's slices are consecutive units.
   const int total_units = p.m_tiles * p.n_tiles * p.ksplit;
 
-  if (warp == PRODUCER_WARP) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+  if (threadIdx.x < 128) {
+    // ------------------------------------------------------------------ TMA producer (warp 0; warps 1..3 idle)
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x >= 32) return;
+    if (threadIdx.x == 0) {
       tma_prefetch_desc(&p.tmA[0]);
       tma_prefetch_desc(&p.tmB[0]);
       if (NSPLIT == 3) {
@@ -175,166 +238,142 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_igemm_kernel(const __gri
         }
       }
     }
-  } else if (warp < MMA_WARPS) {
-    // ------------------------------------------------------------------ MMA warpgroups
-    // Every k-block is KSTEPS k16 steps (the producer pads the last one with zero chunks) and the tile width is the
-    // template's BN, so the k-block's 3 x KSTEPS wgmmas are straight-line code issued back to back.
-    const int g = warp >> 2;  // tile rows 64g .. 64g+63: 8 core-matrix row groups (SBO apart) further into the A tile
-    const uint32_t a_row_off = uint32_t(g) * 8u * p.a_sbo;
-    float d[BN / 2];
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++it) {
-      const int kpart = unit % p.ksplit;
-      const int kb0 = k_block_begin(p, kpart), kb1 = k_block_begin(p, kpart + 1);
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
-      int held = -1;  // stage whose MMAs may still be reading shared memory
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers (warpgroups 1, 2)
+  // The CTA's j-th unit belongs to consumer j & 1.  Consumer c issues the main loop of unit j after the other consumer
+  // has issued that of unit j - 1 (named barrier BAR_ORDER + c), so one consumer's epilogue overlaps the other's MMAs.
+  // Every k-block is KSTEPS k16 steps (the producer pads the last one with zero chunks) and the tile width is the
+  // template's BN, so the k-block's wgmmas are straight-line code issued back to back.
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int c = (threadIdx.x >> 7) - 1;
+  const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+  const uint32_t a_rb = (8u * p.a_sbo) >> 4;  // row block 1 = 8 core-matrix row groups (SBO apart) into the A tile
+  float d[2][BN / 2];                         // rows 0..63 / 64..127 of the tile
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int j = 0, unit = blockIdx.x; unit < total_units; ++j, unit += gridDim.x) {
+    const int tile = unit / p.ksplit, kpart = unit - tile * p.ksplit;
+    const int kb0 = k_block_begin(p, kpart), kb1 = k_block_begin(p, kpart + 1);
+    if ((j & 1) != c) {  // the other consumer's unit: step over its stages
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full[stage], phase);
-        wgmma_fence();
-        // descriptors of k-step 0; a later k-step adds its offset to the start-address field (16-byte units)
-        const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + a_row_off;
-        const uint32_t b_base = smem_u32(smem + size_t(stage) * p.stage_bytes) + p.a_total_bytes;
-        const uint64_t a_hi0 = make_smem_desc(a_base, p.a_lbo, p.a_sbo, p.a_layout);
-        const uint64_t b_hi0 = make_smem_desc(b_base, 16, 1024, 2);
-#pragma unroll
-        for (int ks = 0; ks < KSTEPS; ++ks) {
-          const uint64_t a_hi = a_hi0 + p.a_kstep[ks];
-          const uint64_t b_hi = b_hi0 + uint64_t(ks * 2);  // 32 bytes = 16 bf16 of the 128-byte swizzled rows
-          if (NSPLIT == 3) {
-            const uint64_t a_lo = a_hi + (p.a_plane_bytes >> 4);
-            const uint64_t b_lo = b_hi + (p.b_bytes >> 4);
-            wgmma_m64n<BN>(d, a_lo, b_hi);
-            wgmma_m64n<BN>(d, a_hi, b_lo);
-          }
-          wgmma_m64n<BN>(d, a_hi, b_hi);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage can be refilled
-        if (held >= 0) mbar_arrive(&empty[held]);
-        held = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
-      wgmma_wait<0>();
-      mbar_arrive(&empty[held]);
-      mbar_wait(tempty, (it & 1) ^ 1);  // the epilogue has read the previous tile
-      acc_store<BN>(d, BN, acc_tile + size_t(g) * 64 * p.acc_pitch, int(p.acc_pitch));
-      mbar_arrive(tfull);
+      continue;
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue (8 warps: 2 per 32-row quarter)
-    // The two warps of a quarter take the even / odd 16-column chunks of the tile.  Per chunk: 8 rows x 64 bytes per store
-    // instruction (full 32-byte sectors) read straight from the accumulator tile, and the BatchNorm column sums come out
-    // of the same reads.  accumulate = 2 adds with red.global.add (one add per element, no dependent load).
-    const int ew = warp - EPI_WARP0;
-    const int q = ew & 3;
-    const int half = ew >> 2;
-    long long* roff_s = reinterpret_cast<long long*>(reinterpret_cast<float*>(smem + p.off_staging) + ew * EPI_STAGE_FLOATS);
-    float* red = reinterpret_cast<float*>(smem + p.off_red);  // [2][4][BN][2]
-    const int sub = lane >> 2, cq = lane & 3;   // row within a group of 8, 16-byte piece of the chunk's 64-byte row
-    constexpr int nchunks = BN >> 4;
-    const float* qtile = acc_tile + size_t(q) * 32 * p.acc_pitch;
-    int it = 0;
-    for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x, ++it) {
-      const int tile = unit / p.ksplit;
-      const int acc = it & 1;
-      const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
-      const int ncol0 = nt * BN;
-      const int row = mt * BLOCK_M + q * 32 + lane;
-      const bool rvalid = row < p.M;
-      long long roff = 0;
-      if (rvalid) {
-        int t = row;
-        const int oq_ = t % p.oq;
-        t /= p.oq;
-        const int op_ = t % p.op;
-        t /= p.op;
-        const int oz_ = t % p.oz;
-        const int on_ = t / p.oz;
-        roff = on_ * p.os_n + oz_ * p.os_z + op_ * p.os_p + oq_ * p.os_q;
-      }
-      const uint32_t rmask = __ballot_sync(0xffffffffu, rvalid);
-      float* red_w = red + ((size_t(acc) * 4 + q) * BN) * 2;
-      roff_s[lane] = roff;
-      __syncwarp();
-      long long ro[4];
+    if (j > 0) named_bar_sync(BAR_ORDER + c, 256);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) ro[k] = roff_s[k * 8 + sub];
+    for (int i = 0; i < BN / 2; ++i) d[0][i] = d[1][i] = 0.f;
+    int held = -1;  // stage whose MMAs may still be reading shared memory
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full[stage], phase);
+      wgmma_fence();
+      // descriptors of k-step 0; a later k-step adds its offset to the start-address field (16-byte units)
+      const uint32_t a_base = smem_u32(smem + size_t(stage) * p.stage_bytes);
+      const uint32_t b_base = a_base + p.a_total_bytes;
+      const uint64_t a_hi0 = make_smem_desc(a_base, p.a_lbo, p.a_sbo, p.a_layout);
+      const uint64_t b_hi0 = make_smem_desc(b_base, 16, 1024, 2);
+#pragma unroll
+      for (int ks = 0; ks < KSTEPS; ++ks) {
+        const uint64_t a_hi = a_hi0 + p.a_kstep[ks];
+        const uint64_t b_hi = b_hi0 + uint64_t(ks * 2);  // 32 bytes = 16 bf16 of the 128-byte swizzled rows
+        // consecutive wgmmas alternate between the two row blocks' accumulators
+        if (NSPLIT == 3) {
+          const uint64_t a_lo = a_hi + (p.a_plane_bytes >> 4);
+          const uint64_t b_lo = b_hi + (p.b_bytes >> 4);
+          wgmma_m64n<BN>(d[0], a_lo, b_hi);
+          wgmma_m64n<BN>(d[1], a_lo + a_rb, b_hi);
+          wgmma_m64n<BN>(d[0], a_hi, b_lo);
+          wgmma_m64n<BN>(d[1], a_hi + a_rb, b_lo);
+        }
+        wgmma_m64n<BN>(d[0], a_hi, b_hi);
+        wgmma_m64n<BN>(d[1], a_hi + a_rb, b_hi);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage can be refilled
+      if (held >= 0) mbar_arrive(&empty[held]);
+      held = stage;
+      if (++stage == p.stages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    if (unit + int(gridDim.x) < total_units) named_bar_arrive(BAR_ORDER + (c ^ 1), 256);  // unit j + 1 may start
 
-      mbar_wait(tfull, it & 1);
-      for (int ch = half; ch < nchunks; ch += 2) {
-        const int c0 = ch * 16;
-        const int limit = min(BN, p.Ntot - ncol0) - c0;      // valid columns of this chunk (a multiple of 4)
-        const bool cvalid = cq * 4 < limit;
-        float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int r = k * 8 + sub;
-          const float4 y = *reinterpret_cast<const float4*>(qtile + size_t(r) * p.acc_pitch + c0 + cq * 4);
-          s4[0] += y.x; s4[1] += y.y; s4[2] += y.z; s4[3] += y.w;
-          q4[0] = fmaf(y.x, y.x, q4[0]); q4[1] = fmaf(y.y, y.y, q4[1]);
-          q4[2] = fmaf(y.z, y.z, q4[2]); q4[3] = fmaf(y.w, y.w, q4[3]);
-          if (((rmask >> r) & 1u) && cvalid) {
-            float4* dst = reinterpret_cast<float4*>(p.out + ro[k] + ncol0 + c0 + cq * 4);
-            if (p.accumulate == 2) {
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(y.x), "f"(y.y), "f"(y.z), "f"(y.w)
-                           : "memory");
-            } else if (p.accumulate) {
-              const float4 o = *dst;
-              *dst = make_float4(y.x + o.x, y.y + o.y, y.z + o.z, y.w + o.w);
-            } else {
-              *dst = y;
-            }
-          }
-        }
-        if (p.stats != nullptr) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-#pragma unroll
-            for (int o = 4; o <= 16; o <<= 1) {
-              s4[i] += __shfl_xor_sync(0xffffffffu, s4[i], o);
-              q4[i] += __shfl_xor_sync(0xffffffffu, q4[i], o);
-            }
-          }
-          if (sub == 0) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int cl = c0 + cq * 4 + i;
-              red_w[cl * 2 + 0] = s4[i];
-              red_w[cl * 2 + 1] = q4[i];
-            }
-          }
-        }
+    // ------------------------------------------------------------------ epilogue
+    // While the last MMAs run, each thread computes one row's offset through the (n,t,h,w) strides into the consumer's
+    // row table (kNoRow: a row >= M; it holds zeros, as TMA zero-fills its A row, and is not stored).
+    const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+    const int ncol0 = nt * BN;
+    uint8_t* epi = smem + p.off_epi + size_t(c) * EPI_SCRATCH;  // row table, then staging blocks / BatchNorm partials
+    long long* roff_s = reinterpret_cast<long long*>(epi);
+    {
+      int r = mt * BLOCK_M + t;
+      long long off = kNoRow;
+      if (r < p.M) {
+        const int oq_ = r % p.oq;
+        r /= p.oq;
+        const int op_ = r % p.op;
+        r /= p.op;
+        const int oz_ = r % p.oz;
+        const int on_ = r / p.oz;
+        off = on_ * p.os_n + oz_ * p.os_z + op_ * p.os_p + oq_ * p.os_q;
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);  // this warp is done with the accumulator tile
-      if (p.stats != nullptr) {
-        named_bar_sync(1, 32 * EPI_WARPS);
-        // the four quarter partials of this tile are in red[acc]; spread the column reduction over the epilogue warps
-        const float* rb = red + size_t(acc) * 4 * BN * 2;
-        for (int cl = ew * 32 + lane; cl < BN; cl += 32 * EPI_WARPS) {
-          const int col = ncol0 + cl;
-          if (col < p.Ntot) {
-            float s = 0.f, s2 = 0.f;
+      roff_s[t] = off;
+    }
+    named_bar_sync(BAR_EPI + c, 128);
+    // Thread (warp, lane) holds rows 16 warp + lane/4 (+8) of each row block and columns 8 jn + 2 (lane % 4) (+1):
+    // d[rb][4 jn + 2 h + e] is row 64 rb + 8 h + 16 warp + lane/4, column 8 jn + 2 (lane % 4) + e.
+    const int cq = 2 * (lane & 3);
+    // whole groups of 4 columns up to cout are stored, as the split-K zero fill assumes
+    const int ncols = min(BN, ((p.Ntot + 3) & ~3) - ncol0);
+    float* stage_w = reinterpret_cast<float*>(epi + BLOCK_M * 8) + warp * 256;
+    wgmma_wait<0>();
+    mbar_arrive(&empty[held]);
+    if (p.accumulate == 2) store_fragment<BN, 2>(d, stage_w, roff_s, p.out + ncol0, ncols);
+    else if (p.accumulate == 1) store_fragment<BN, 1>(d, stage_w, roff_s, p.out + ncol0, ncols);
+    else store_fragment<BN, 0>(d, stage_w, roff_s, p.out + ncol0, ncols);
+    if (p.stats != nullptr) {
+      // per-thread sums over its 4 rows, then over the 8 row lanes of the warp, then over the 4 warps in shared memory
+      float* red = reinterpret_cast<float*>(epi + BLOCK_M * 8);  // [warp][BN][sum, sum^2], over the staging blocks
+      named_bar_sync(BAR_EPI + c, 128);  // every warp is done with its staging block
 #pragma unroll
-            for (int w = 0; w < 4; ++w) {
-              s += rb[(size_t(w) * BN + cl) * 2 + 0];
-              s2 += rb[(size_t(w) * BN + cl) * 2 + 1];
-            }
-            // [2][cout][m_tiles]: tile axis contiguous for the finalize kernel's per-channel reduction
-            p.stats[size_t(col) * p.m_tiles + mt] = s;
-            p.stats[(size_t(p.Ntot) + col) * p.m_tiles + mt] = s2;
+      for (int jn = 0; jn < BN / 8; ++jn) {
+        float s[2], q[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float a0 = d[0][4 * jn + e], a1 = d[0][4 * jn + 2 + e], a2 = d[1][4 * jn + e], a3 = d[1][4 * jn + 2 + e];
+          s[e] = (a0 + a1) + (a2 + a3);
+          q[e] = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, a3 * a3)));
+#pragma unroll
+          for (int o = 4; o <= 16; o <<= 1) {
+            s[e] += __shfl_xor_sync(0xffffffffu, s[e], o);
+            q[e] += __shfl_xor_sync(0xffffffffu, q[e], o);
           }
         }
+        if (lane < 4)
+          *reinterpret_cast<float4*>(red + (size_t(warp) * BN + 8 * jn + cq) * 2) = make_float4(s[0], q[0], s[1], q[1]);
       }
+      named_bar_sync(BAR_EPI + c, 128);
+      const int col = ncol0 + t;
+      if (t < BN && col < p.Ntot) {
+        float s = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+          s += red[(size_t(w) * BN + t) * 2 + 0];
+          s2 += red[(size_t(w) * BN + t) * 2 + 1];
+        }
+        // [2][cout][m_tiles]: tile axis contiguous for the finalize kernel's per-channel reduction
+        p.stats[size_t(col) * p.m_tiles + mt] = s;
+        p.stats[(size_t(p.Ntot) + col) * p.m_tiles + mt] = s2;
+      }
+      named_bar_sync(BAR_EPI + c, 128);  // the scratch is free for this consumer's next tile
     }
   }
-
 }
 
 static int pick_ck(int c) {
@@ -483,21 +522,18 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
                                     : uint32_t(ks * 2) * p.chunk_bytes;  // CK = 8: two chunks, LBO apart
     p.a_kstep[ks] = off >> 4;
   }
-  p.acc_pitch = uint32_t(p.BN) + 4;  // 16-byte rows; the 4-float skew spreads the fragment stores over the banks
-  const uint32_t acc_bytes = BLOCK_M * p.acc_pitch * 4;
-  const uint32_t tail = acc_bytes + EPI_WARPS * EPI_STAGE_FLOATS * 4 + 2 * 4 * p.BN * 2 * 4 + 256;
-  const uint32_t budget = uint32_t(smem_optin) - 1024 - tail;
+  // all of shared memory but the barriers and the consumers' epilogue scratch goes to the operand ring
+  const uint32_t epi_bytes = 2u * EPI_SCRATCH;
+  const uint32_t budget = uint32_t(smem_optin) - 1024 - epi_bytes - 256;
   p.stages = std::min<int>(MAX_STAGES, budget / p.stage_bytes);
   p.stages = std::min(p.stages, std::max(2, p.k_blocks * 4));
-  const int ctas_per_sm = 1;  // 544 threads x up to 120 registers: one CTA fills the register file
+  const int ctas_per_sm = 1;  // 384 threads at 40 / 232 / 232 registers: one CTA fills the register file
   if (p.stages < 2) {
     set_error("sfb_conv_igemm: not enough shared memory for 2 pipeline stages (stage=%u B)", p.stage_bytes);
     return -11;
   }
-  p.off_acc = p.stages * p.stage_bytes;
-  p.off_staging = p.off_acc + acc_bytes;
-  p.off_red = p.off_staging + EPI_WARPS * EPI_STAGE_FLOATS * 4;
-  p.off_bars = p.off_red + 2 * 4 * p.BN * 2 * 4;
+  p.off_epi = p.stages * p.stage_bytes;
+  p.off_bars = p.off_epi + epi_bytes;
   const uint32_t smem_bytes = p.off_bars + 256 + 1024;
   p.out = d->out;
   p.os_n = d->os_n;
@@ -506,7 +542,6 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   p.os_q = d->os_w;
   // split-K: the slices add into the output (zero-filled first by an overwrite) and the statistics come from y afterwards
   p.accumulate = p.ksplit > 1 ? 2 : d->accumulate;
-  p.epi_coalesced = 1;
   p.stats = p.ksplit > 1 ? nullptr : d->stats;
 
   // ---- tensor maps
@@ -540,7 +575,7 @@ extern "C" int sfb_conv_igemm(const sfb_conv_desc* d, void* stream_) {
   }
 
   if (p.ksplit > 1 && d->accumulate == 0) {
-    // the epilogue writes whole float4 groups: columns [cout, cout rounded up to 4) take zeros too
+    // the epilogue writes whole groups of 4 columns: columns [cout, cout rounded up to 4) take zeros too
     const size_t width = size_t((d->cout + 3) & ~3) * sizeof(float);
     if (cudaMemset2DAsync(d->out, size_t(d->os_w) * sizeof(float), 0, width, size_t(p.M), stream) != cudaSuccess) {
       set_error("sfb_conv_igemm: zero fill of the split-K output failed: %s", cudaGetErrorString(cudaGetLastError()));

@@ -150,5 +150,21 @@ __device__ __forceinline__ void acc_ld_x16(const float* src, uint32_t (&v)[16]) 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// signal a named barrier without waiting on it (nthreads counts the arriving and the waiting threads)
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// ----------------------------------------------------------------------------- register reallocation
+// Lower / raise the calling warpgroup's per-thread register limit (all 128 threads execute it).  N is a multiple of 8
+// in [24, 256]; a raise waits until other warpgroups of the CTA have released enough registers.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 }  // namespace sfb
