@@ -455,6 +455,9 @@ int sfb_small_linear_relu_fwd(const float* x, const float* w, const float* b, fl
 int sfb_small_linear_relu_bwd(const float* dy, const float* x, const float* w, float* dw, float* db, float* dx,
                               int32_t m, int32_t k, int32_t j, int32_t accumulate, void* stream);
 int sfb_row_softmax(float* x, int32_t rows, int32_t cols, void* stream);
+/* MODEL.HEAD_ACT sigmoid (head_helper.py:279-280 / :339-340 ResNetBasicHead, :454-455 / :483-484 X3DHead, :538-539 /
+ * :555-556 TransformerBasicHead): x = 1 / (1 + exp(-x)) in place over the rows x cols fp32 matrix, in eval mode. */
+int sfb_row_sigmoid(float* x, int32_t rows, int32_t cols, void* stream);
 /* Stochastic depth (common.py:46-59): out[i*b + s] = floor(keep_i + U)/keep_i for n_rates drop rates and b samples. */
 int sfb_droppath_scales(float* out, const float* rates, int32_t n_rates, int32_t b, uint64_t seed, uint64_t* step,
                         void* stream);

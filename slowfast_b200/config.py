@@ -56,7 +56,7 @@ _DEFAULTS = {
     "MODEL": {
         "ARCH": "slowfast", "MODEL_NAME": "SlowFast", "NUM_CLASSES": 400, "LOSS_FUNC": "cross_entropy",
         "DROPOUT_RATE": 0.5, "DROPCONNECT_RATE": 0.0, "FC_INIT_STD": 0.01, "HEAD_ACT": "softmax",
-        "ACT_CHECKPOINT": False, "DETACH_FINAL_FC": False,
+        "ACT_CHECKPOINT": False, "DETACH_FINAL_FC": False, "FROZEN_BN": False,
     },
     "SLOWFAST": {"BETA_INV": 8, "ALPHA": 8, "FUSION_CONV_CHANNEL_RATIO": 2, "FUSION_KERNEL_SZ": 5},
     "DATA": {"NUM_FRAMES": 8, "TRAIN_CROP_SIZE": 224, "TEST_CROP_SIZE": 256, "INPUT_CHANNEL_NUM": [3, 3],

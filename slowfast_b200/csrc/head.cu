@@ -1,5 +1,5 @@
 // Classification-head pieces (head_helper.py:305-350 ResNetBasicHead / :547-563 TransformerBasicHead):
-// global average pool over (T,H,W), dropout, the small Linear (M = batch rows) and the eval-mode softmax.
+// global average pool over (T,H,W), dropout, the small Linear (M = batch rows) and the eval-mode softmax / sigmoid.
 // These are tiny next to the backbone (a few MFLOP); they are plain SIMT kernels so that the whole model path
 // stays inside this library and on the caller's stream.
 #include <algorithm>
@@ -189,6 +189,15 @@ __global__ void row_softmax_kernel(float* __restrict__ x, int rows, int cols) {
   const float inv = 1.f / s;
   for (int t = lane; t < cols; t += 32) r[t] = expf(r[t] - mx) * inv;
 }
+// elementwise logistic sigmoid in place (eval-mode multi-label head activation); exp of -|x| only, so no overflow
+// for large |x|: 1 / (1 + e^-x) for x >= 0, e^x / (1 + e^x) below
+__global__ void row_sigmoid_kernel(float* __restrict__ x, int64_t nelem) {
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < nelem; i += int64_t(gridDim.x) * blockDim.x) {
+    const float v = x[i];
+    const float e = expf(-fabsf(v));
+    x[i] = v >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+  }
+}
 
 static int hd_grid(int64_t items, int block) { return capped_grid(items, block, int64_t(kGridSms) * 8); }
 
@@ -292,6 +301,12 @@ extern "C" int sfb_small_linear_relu_bwd(const float* dy, const float* x, const 
 extern "C" int sfb_row_softmax(float* x, int32_t rows, int32_t cols, void* stream) {
   row_softmax_kernel<<<(rows * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(x, rows, cols);
   return launch_status("sfb_row_softmax");
+}
+extern "C" int sfb_row_sigmoid(float* x, int32_t rows, int32_t cols, void* stream) {
+  const int64_t nelem = int64_t(rows) * cols;
+  if (nelem == 0) return 0;
+  row_sigmoid_kernel<<<hd_grid(nelem, 256), 256, 0, (cudaStream_t)stream>>>(x, nelem);
+  return launch_status("sfb_row_sigmoid");
 }
 
 // Stochastic-depth scales (common.py:46-59 drop_path): out[i*b + s] = floor(keep_i + U) / keep_i per sample, from the

@@ -171,6 +171,11 @@ class Ctx:
     def grad_of(self, p: nn.Parameter) -> torch.Tensor:
         return self.grad_slots[id(p)]
 
+    def grads(self, params: Sequence[nn.Parameter]) -> List[Optional[torch.Tensor]]:
+        """Every parameter's gradient slot; None for a parameter this backward writes none for (not in the list
+        ``begin_backward`` took)."""
+        return [self.grad_slots.get(id(p)) for p in params]
+
 
 FLAT_ALIGN = 64  # fp32 elements: every gradient slot of the flat bucket starts on a 256-byte boundary
 
@@ -206,6 +211,13 @@ def allreduce_flat_gradients(flat: torch.Tensor, params: Sequence[nn.Parameter],
             p.grad = flat[off:off + n].view_as(p)
 
 
+def check_head_act(act_func: str) -> None:
+    """MODEL.HEAD_ACT of a classification head: the eval-mode softmax / sigmoid, or none; anything else is rejected."""
+    if act_func not in ops.HEAD_ACTS:
+        raise NotImplementedError(f"head activation {act_func!r} is not on the engine path (MODEL.HEAD_ACT takes "
+                                  f"softmax, sigmoid or none)")
+
+
 def _t3(v) -> Tuple[int, int, int]:
     return tuple(int(x) for x in v)
 
@@ -222,7 +234,11 @@ class ConvBN:
 
     ``bn`` may be a sub-batch BN container (subbn.py): gamma / beta are the container's; a training pass takes its
     statistics per split (``bn_split_stats``) into ``split_bn`` and emits [S][C] coefficient tables, which every
-    apply / backward kernel indexes by the split of the row's clip (``split_kw``); eval is the plain path on ``bn``."""
+    apply / backward kernel indexes by the split of the row's clip (``split_kw``); eval is the plain path on ``bn``.
+
+    The BN runs on batch statistics (and updates its running buffers) iff the model AND its own module are in training
+    mode (``bn_mode``): ``misc.frozen_bn_stats`` (MODEL.FROZEN_BN) puts BN modules in eval inside a training model, and
+    such a unit takes the running statistics forward and backward while its conv still trains."""
 
     def __init__(self, name: str, conv: nn.Conv3d, bn: Optional[nn.Module], ctx: Ctx):
         assert conv.groups == 1 and _t3(conv.dilation) == (1, 1, 1), \
@@ -235,6 +251,7 @@ class ConvBN:
         assert not self.sub or (bn.affine and conv.out_channels % 8 == 0), \
             f"{name}: sub-batch BN needs an affine container and a multiple of 8 channels"
         self.splits, self.rows_per_clip = 1, 0
+        self.bn_train = False
         self.k, self.stride, self.pad = _t3(conv.kernel_size), _t3(conv.stride), _t3(conv.padding)
         self.cin, self.cout = conv.in_channels, conv.out_channels
         self.cin_pad = ops.pad8(self.cin)
@@ -257,6 +274,14 @@ class ConvBN:
             return self.bn
         return self.bn.split_bn if training else self.bn.bn
 
+    def _set_bn_mode(self) -> None:
+        """The BN mode of this forward (and of the backward that follows it): see ``bn_mode``."""
+        self.bn_train = self.bn is not None and bn_mode(self.ctx, self.bn)
+        if self.sub and self.ctx.training and not (self.bn.training and self.bn.split_bn.training and
+                                                   self.bn.bn.training):
+            raise NotImplementedError(f"{self.name}: MODEL.FROZEN_BN (a sub-batch BN, or one of its inner BNs, in eval "
+                                      f"mode inside a training model) is not on the engine path")
+
     @property
     def split_kw(self) -> dict:
         """Split geometry of the last forward, for the kernels that apply this unit's coefficients."""
@@ -275,12 +300,12 @@ class ConvBN:
         self.shift = ctx.buf((self.name, "shift"), (s * cp,), zero=zero)
         self.mean = ctx.buf((self.name, "mean"), (s * cp,), zero=zero)
         self.invstd = ctx.buf((self.name, "invstd"), (s * cp,), zero=zero)
-        sbn = self._stats_bn(ctx.training)
+        sbn = self._stats_bn(self.bn_train)
         momentum = sbn.momentum if sbn.momentum is not None else 0.1
         ops.bn_finalize(stats, m_tiles, s * c, rows // s, bn.weight, bn.bias, sbn.running_mean, sbn.running_var,
-                        momentum, sbn.eps, ctx.training, self.scale, self.shift, self.mean, self.invstd, affine_c=c)
+                        momentum, sbn.eps, self.bn_train, self.scale, self.shift, self.mean, self.invstd, affine_c=c)
         if self.bias is not None:
-            ops.bn_conv_bias(self.bias, c, momentum, ctx.training, sbn.running_mean, self.scale, self.shift, self.mean,
+            ops.bn_conv_bias(self.bias, c, momentum, self.bn_train, sbn.running_mean, self.scale, self.shift, self.mean,
                              splits=s)
 
     def fprop(self, x: Planes) -> torch.Tensor:
@@ -297,11 +322,11 @@ class ConvBN:
         y = ctx.buf((self.name, "y"), (x.n, ot, oh, ow, cp))
         strides = (ot * oh * ow * cp, oh * ow * cp, ow * cp, cp)
         m_tiles = ops.conv_stats_tiles(x, fm, geom, y, strides, nsplit=ctx.nsplit)
-        self.splits = self.bn.num_splits if (self.sub and ctx.training) else 1
+        self._set_bn_mode()
+        self.splits = self.bn.num_splits if (self.sub and self.bn_train) else 1
         self.rows_per_clip = ot * oh * ow
         # (sub-batch BN: the epilogue's 128-row tiles cross clips, so the statistics are a separate pass)
-        stats = ctx.buf((self.name, "stats"), (2, c, m_tiles)) \
-            if (ctx.training and self.bn is not None and self.splits == 1) else None
+        stats = ctx.buf((self.name, "stats"), (2, c, m_tiles)) if (self.bn_train and self.splits == 1) else None
         # (the epilogue stores whole float4 groups: columns [c, cp) receive the zero accumulators of filter rows
         # the TMA box reads out of bounds)
         ops.conv_igemm(x, fm, geom, y, strides, stats=stats, nsplit=ctx.nsplit)
@@ -323,7 +348,7 @@ class ConvBN:
         partials, coef = self._bwd_scratch(n * ot * oh * ow, c)
         bn = self.bn
         ops.bn_bwd(dout, mask, ops.f32view(self.y), self.mean, self.invstd, bn.weight, ctx.grad_of(bn.weight),
-                   ctx.grad_of(bn.bias), dy, partials, coef, training=ctx.training, dres=dres,
+                   ctx.grad_of(bn.bias), dy, partials, coef, training=self.bn_train, dres=dres,
                    dres_accumulate=dres_accumulate, c_valid=self.cout,
                    mask_affine=(self.scale, self.shift) if mask_from_y else None, **self.split_kw)
         if self.bias is not None:
@@ -410,8 +435,9 @@ class StemConvBN(ConvBN):
     def fprop(self, x: Planes) -> torch.Tensor:
         ctx, g = self.ctx, self.g
         c = self.cout
-        self.splits = self.bn.num_splits if (self.sub and ctx.training) else 1
-        want_stats = ctx.training and self.splits == 1  # (sub-batch BN: statistics in a separate pass)
+        self._set_bn_mode()
+        self.splits = self.bn.num_splits if (self.sub and self.bn_train) else 1
+        want_stats = self.bn_train and self.splits == 1  # (sub-batch BN: statistics in a separate pass)
         if self.t8:
             n, t, h, w = x.n, x.t // 2, x.h * 2, (x.w // 8 - 1) * 16
             ot, oh, ow = g.out_dims(t, h, w)
@@ -503,7 +529,7 @@ class GraphedProgram:
             # gradient accumulation (zero_grad(set_to_none=False), or .grad re-pointed at the bucket by
             # allreduce_flat_gradients): a live .grad must never alias the static slot the replay overwrites
             for p, g in zip(self.params, self.static_grads):
-                if p.grad is not None and p.grad.data_ptr() == g.data_ptr():
+                if g is not None and p.grad is not None and p.grad.data_ptr() == g.data_ptr():
                     p.grad = p.grad.clone()
         self.static_dout.copy_(dout)
         self.bwd_graph.replay()
@@ -524,15 +550,42 @@ def pointer_signature(model, params) -> int:
     return hash(tuple(ptrs))
 
 
-def bn_momentum_signature(model) -> Tuple:
+def _bn_list(model) -> List[nn.Module]:
     bns = model.__dict__.get("_bn_list")
     if bns is None:
         bns = [m for m in model.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)]
         object.__setattr__(model, "_bn_list", bns)
+    return bns
+
+
+def bn_momentum_signature(model) -> Tuple:
+    bns = _bn_list(model)
     if not bns or not model.training:
         return ()
     first = bns[0].momentum
     return (first,) if all(b.momentum == first for b in bns) else tuple(b.momentum for b in bns)
+
+
+def bn_mode(ctx: Ctx, bn: nn.Module) -> bool:
+    """True: this BN normalises with batch statistics and updates its running buffers (model and module both in
+    training mode); False: it applies its running statistics, in eval and under MODEL.FROZEN_BN alike."""
+    return ctx.training and bn.training
+
+
+def bn_mode_signature(model) -> Tuple:
+    """Indices of the BatchNorm modules in eval mode inside a training model (MODEL.FROZEN_BN freezes them all,
+    a hand-frozen subset some): a captured program bakes each BN's mode into its kernel arguments."""
+    if not model.training:
+        return ()
+    return tuple(i for i, b in enumerate(_bn_list(model)) if not b.training)
+
+
+def program_key(model, needs_grad: bool, inputs: Sequence[torch.Tensor]) -> Tuple:
+    """Arena / CUDA-graph key of one forward: mode, grad mode, input signature, BN momenta and BN modes."""
+    # BatchNorm momentum is a by-value kernel argument (baked into a captured program): precise-BN (fvcore
+    # update_bn_stats, tools/train_net.py:425-446) temporarily sets it to 1.0, so it is part of the signature
+    return (model.training, needs_grad, tuple((tuple(x.shape), x.dtype) for x in inputs), bn_momentum_signature(model),
+            bn_mode_signature(model))
 
 
 class ModelFunction(torch.autograd.Function):
@@ -546,9 +599,7 @@ class ModelFunction(torch.autograd.Function):
         fctx.prog = None
         # (grad mode is always off inside Function.forward; needs_input_grad says whether a backward can follow)
         needs_grad = any(fctx.needs_input_grad)
-        # BatchNorm momentum is a by-value kernel argument (baked into a captured program): precise-BN (fvcore
-        # update_bn_stats, tools/train_net.py:425-446) temporarily sets it to 1.0, so it is part of the signature
-        key = (model.training, needs_grad, tuple((tuple(x.shape), x.dtype) for x in inputs), bn_momentum_signature(model))
+        key = program_key(model, needs_grad, inputs)
         arena = model.ctx.use_arena(key)
         arena.generation += 1
         gen = getattr(model, "_fwd_generation", 0) + 1
@@ -595,6 +646,7 @@ class ModelFunction(torch.autograd.Function):
         if getattr(model, "flat_grad_only", False):
             # the caller consumes ctx.flat_grad directly (slowfast_b200.optim.FlatOptimizer): no param.grad copies
             return (None, None) + (None,) * (fctx.n_inputs + len(grads))
+        # (None: a parameter in front of MODEL.DETACH_FINAL_FC's detach, whose .grad stays None as in the reference)
         return (None, None) + (None,) * fctx.n_inputs + tuple(grads)
 
 
@@ -606,7 +658,8 @@ class Namespace(nn.Module):
 
 
 def bump_num_batches_tracked(bns: List[nn.BatchNorm3d]) -> None:
-    """torch's BatchNorm increments num_batches_tracked once per training forward (one fused op for all BNs)."""
-    ts = [b.num_batches_tracked for b in bns if b.num_batches_tracked is not None]
+    """torch's BatchNorm increments num_batches_tracked once per training forward of a BN in training mode (one fused
+    op for all BNs); a frozen BN (module in eval) keeps its count."""
+    ts = [b.num_batches_tracked for b in bns if b.num_batches_tracked is not None and b.training]
     if ts:
         torch._foreach_add_(ts, 1)

@@ -339,6 +339,7 @@ _SIGNATURES = [
     ("sfb_small_linear_relu_bwd", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_row_softmax", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    ("sfb_row_sigmoid", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     ("sfb_droppath_scales", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
     ("sfb_dwconv_m_tiles", C.c_int32, [C.POINTER(DwConvDesc)]),
     ("sfb_dwconv_tiles_per_sample", C.c_int32, [C.POINTER(DwConvDesc)]),

@@ -30,7 +30,7 @@ import torch.nn as nn
 from .. import lib as L
 from .. import ops
 from ..config import nsplit_of
-from ..engine import Ctx, ModelFunction, Namespace
+from ..engine import Ctx, ModelFunction, Namespace, check_head_act
 from ..ops import F32, Planes
 
 BF16 = torch.bfloat16
@@ -161,14 +161,19 @@ class PatchEmbedModule(Namespace):
 
 
 class TransformerHeadModule(Namespace):
-    def __init__(self, dim_in, num_classes, dropout_rate, act_func):
+    """TransformerBasicHead container: dropout, projection.  ``detach_final_fc`` (MODEL.DETACH_FINAL_FC,
+    head_helper.py:550-551): the features are detached after the dropout, so the backward runs the projection only."""
+
+    def __init__(self, dim_in, num_classes, dropout_rate, act_func, detach_final_fc=False):
         super().__init__()
+        check_head_act(act_func)
         if dropout_rate > 0.0:
             self.dropout = nn.Dropout(dropout_rate)
         self.projection = nn.Linear(dim_in, num_classes, bias=True)  # the reference constructs it twice (:515,:517)
         self.projection = nn.Linear(dim_in, num_classes, bias=True)
         self.dropout_rate = dropout_rate
         self.act_func = act_func
+        self.detach_final_fc = bool(detach_final_fc)
 
 
 class B200MViT(nn.Module):
@@ -222,7 +227,8 @@ class B200MViT(nn.Module):
                                            mv.REL_POS_ZERO_INIT, mv.DIM_MUL_IN_ATT))
         embed = self.specs[-1]["dim_out"]
         self.norm = nn.LayerNorm(embed, eps=1e-6)
-        self.head = TransformerHeadModule(embed, self.num_classes, cfg.MODEL.DROPOUT_RATE, cfg.MODEL.HEAD_ACT)
+        self.head = TransformerHeadModule(embed, self.num_classes, cfg.MODEL.DROPOUT_RATE, cfg.MODEL.HEAD_ACT,
+                                          cfg.MODEL.DETACH_FINAL_FC)
         if self.use_abs_pos and self.sep_pos_embed:  # drawn after the head and before cls_token, as the reference does
             nn.init.trunc_normal_(self.pos_embed_spatial, std=0.02)  # (:1057-1077)
             nn.init.trunc_normal_(self.pos_embed_temporal, std=0.02)
@@ -317,10 +323,18 @@ class B200MViT(nn.Module):
         params = [p for p in self.parameters()]
         return ModelFunction.apply(self, 1, *x, *params)
 
+    def grad_params(self) -> List[nn.Parameter]:
+        """The parameters the backward writes gradients for, in flat-bucket order: all of them, or the head's
+        projection under MODEL.DETACH_FINAL_FC."""
+        head = getattr(self, "head", None)  # (the MAE / MaskFeat pre-training models replace the head)
+        if getattr(head, "detach_final_fc", False):
+            return [head.projection.weight, head.projection.bias]
+        return list(self.parameters())
+
     def allreduce_gradients(self, group=None) -> None:
         from ..engine import allreduce_flat_gradients
         assert self.ctx.flat_grad is not None, "call after backward()"
-        allreduce_flat_gradients(self.ctx.flat_grad, list(self.parameters()), group,
+        allreduce_flat_gradients(self.ctx.flat_grad, self.grad_params(), group,
                                  repoint=not getattr(self, "flat_grad_only", False))
 
     # ================================================================================== helpers
@@ -515,14 +529,14 @@ class B200MViT(nn.Module):
             ops.dropout_fwd(feat, mask, head.dropout_rate, self._seed + 17, self._drop_counter)
         logits = torch.empty((B, self.num_classes), dtype=F32, device=ctx.device)
         ops.small_linear_fwd(feat, head.projection.weight, head.projection.bias, logits)
-        if not ctx.training and head.act_func == "softmax":
-            ops.row_softmax(logits)
+        if not ctx.training:
+            ops.head_act(logits, head.act_func)
         self._saved["final"] = (cur, ln_in, ln_pitch, fmean, frstd, feat, mask)
         return logits
 
-    def _final_backward(self, dlogits: torch.Tensor) -> torch.Tensor:
+    def _final_backward(self, dlogits: torch.Tensor) -> Optional[torch.Tensor]:
         """Returns the gradient w.r.t. the block stack output [B, Nf, Cf] (zero except the cls rows, or zero on the cls
-        rows under USE_MEAN_POOLING)."""
+        rows under USE_MEAN_POOLING); None under MODEL.DETACH_FINAL_FC."""
         ctx = self.ctx
         sv = self._saved
         B = sv["B"]
@@ -531,6 +545,9 @@ class B200MViT(nn.Module):
         head = self.head
         dfeat = ctx.buf(("head.dfeat",), (B, Cf))
         proj = head.projection
+        if head.detach_final_fc:  # nothing before the detach has a gradient
+            ops.small_linear_bwd(dlogits, feat, proj.weight, ctx.grad_of(proj.weight), ctx.grad_of(proj.bias), None)
+            return None
         ops.small_linear_bwd(dlogits, feat, proj.weight, ctx.grad_of(proj.weight), ctx.grad_of(proj.bias), dfeat)
         if mask is not None:
             ops.dropout_bwd(dfeat, mask, head.dropout_rate)
@@ -684,10 +701,12 @@ class B200MViT(nn.Module):
     def _engine_backward(self, dlogits: torch.Tensor):
         ctx = self.ctx
         params = [p for p in self.parameters()]
-        ctx.begin_backward(params)
+        ctx.begin_backward(self.grad_params())
         sv = self._saved
         B = sv["B"]
         dx = self._final_backward(dlogits)
+        if dx is None:
+            return ctx.grads(params)
         which = "a"
         for i in range(len(self.blocks) - 1, -1, -1):
             which = "b" if which == "a" else "a"

@@ -22,7 +22,8 @@ import torch.nn as nn
 
 from .. import ops
 from ..config import nsplit_of
-from ..engine import Act, ConvBN, Ctx, ModelFunction, Namespace, StemConvBN, bump_num_batches_tracked
+from ..engine import (Act, ConvBN, Ctx, ModelFunction, Namespace, StemConvBN, bump_num_batches_tracked,
+                      check_head_act)
 from ..ops import F32, Planes
 from ..subbn import is_sub_bn, norm_factory, num_splits_of
 
@@ -403,9 +404,12 @@ def _check_contrastive_head(contrastive) -> int:
 
 class BasicHeadModule(Namespace):
     """ResNetBasicHead container: projection (+ inert pools / dropout / act).  ``contrastive`` (cfg.CONTRASTIVE)
-    selects the MLPHead projection when NUM_MLP_LAYERS > 1."""
+    selects the MLPHead projection when NUM_MLP_LAYERS > 1.  ``detach_final_fc`` (MODEL.DETACH_FINAL_FC, linear
+    evaluation, head_helper.py:319-320): the pooled features are detached after the dropout, so the backward runs the
+    projection's Linear layers only."""
 
-    def __init__(self, dim_in, num_classes, dropout_rate, act_func, pool_size=None, contrastive=None):
+    def __init__(self, dim_in, num_classes, dropout_rate, act_func, pool_size=None, contrastive=None,
+                 detach_final_fc=False):
         super().__init__()
         mlp_layers = _check_contrastive_head(contrastive)
         # AvgPool3d(pool_size, stride=1) per pathway (None = adaptive 1x1x1, video_model_builder.py:398-416)
@@ -418,10 +422,10 @@ class BasicHeadModule(Namespace):
             self.projection = nn.Linear(sum(dim_in), num_classes, bias=True)
         else:
             self.projection = MLPHeadModule(sum(dim_in), num_classes, int(contrastive.MLP_DIM), mlp_layers)
-        if act_func not in ("softmax", "none"):
-            raise NotImplementedError(f"head activation {act_func!r} is not on the engine path")
+        check_head_act(act_func)
         self.act_func = act_func
         self.dropout_rate = dropout_rate
+        self.detach_final_fc = bool(detach_final_fc)
         self.dim_in = list(dim_in)
 
     def linears(self) -> List[nn.Linear]:
@@ -477,6 +481,9 @@ class _VideoResNetBase(nn.Module):
         # BN.NORM_TYPE: batchnorm or sub_batchnorm (multigrid's long cycle); norm_factory rejects the others
         self._norm = norm_factory(cfg)
         self._bn_splits = num_splits_of(cfg)
+        if cfg.MODEL.FROZEN_BN and cfg.BN.NORM_TYPE == "sub_batchnorm":
+            raise NotImplementedError("MODEL.FROZEN_BN with BN.NORM_TYPE sub_batchnorm (frozen sub-batch BN statistics) "
+                                      "is not on the engine path")
         assert cfg.RESNET.TRANS_FUNC == "bottleneck_transform"
         assert cfg.RESNET.NUM_GROUPS == 1
         assert not cfg.DETECTION.ENABLE, "RoI head is out of scope"
@@ -503,13 +510,21 @@ class _VideoResNetBase(nn.Module):
         skip = {id(m.bn) for m in self.modules() if is_sub_bn(m)}
         return [m for m in self._all_bns() if id(m) not in skip]
 
+    def grad_params(self) -> List[nn.Parameter]:
+        """The parameters the backward writes gradients for, in flat-bucket order: all of them, or the head's Linear
+        layers under MODEL.DETACH_FINAL_FC."""
+        head = getattr(self, "head", None)
+        if getattr(head, "detach_final_fc", False):
+            return [p for lin in head.linears() for p in (lin.weight, lin.bias)]
+        return list(self.parameters())
+
     def allreduce_gradients(self, group=None) -> None:
         """Data-parallel exchange step (SURVEY.md §8e): ONE NCCL all-reduce (average) over the flat gradient
         bucket the last backward filled; ``param.grad`` is re-pointed at the bucket slices where autograd made a
         private copy.  (Under the reference's build_model the DDP wrapper does its own bucketing instead.)"""
         from ..engine import allreduce_flat_gradients
         assert self.ctx.flat_grad is not None, "call after backward()"
-        allreduce_flat_gradients(self.ctx.flat_grad, list(self.parameters()), group,
+        allreduce_flat_gradients(self.ctx.flat_grad, self.grad_params(), group,
                                  repoint=not getattr(self, "flat_grad_only", False))
 
     # ------------------------------------------------------------------ helpers
@@ -562,8 +577,7 @@ class _VideoResNetBase(nn.Module):
                 ops.window_avgpool_fwd(f.planes, ps, pooled, col)
                 col += f.c
             proj = self._head_mlp_forward(pooled, ("head.proj.win",))[-1]
-            if head.act_func == "softmax":
-                ops.row_softmax(proj)
+            ops.head_act(proj, head.act_func)
             logits = torch.empty((n, proj.shape[1]), dtype=torch.float32, device=ctx.device)
             ops.rows_group_mean(proj, logits, g)
             self._head_saved = None
@@ -582,8 +596,8 @@ class _VideoResNetBase(nn.Module):
             ops.dropout_fwd(pooled, self._drop_mask, p, self._drop_seed, self._drop_counter)
         acts = self._head_mlp_forward(pooled, None)
         logits = acts[-1]
-        if not ctx.training and head.act_func == "softmax":
-            ops.row_softmax(logits)
+        if not ctx.training:
+            ops.head_act(logits, head.act_func)
         self._head_saved = (feats, acts[:-1])
         return logits
 
@@ -605,15 +619,22 @@ class _VideoResNetBase(nn.Module):
             acts.append(y)
         return acts
 
-    def _head_backward(self, dlogits: torch.Tensor) -> None:
+    def _head_backward(self, dlogits: torch.Tensor) -> bool:
+        """The head's backward into the feature gradients; False under MODEL.DETACH_FINAL_FC, where it stops at the
+        projection's first Linear and nothing before the detach has a gradient."""
         ctx, head = self.ctx, self.head
         feats, acts = self._head_saved
         dy = dlogits
         for i in reversed(range(len(acts))):
             lin, x = head.linears()[i], acts[i]
-            dx = ctx.buf(("head.dpooled",) if i == 0 else ("head.dmlp", i), x.shape)
+            if i == 0 and head.detach_final_fc:
+                dx = None
+            else:
+                dx = ctx.buf(("head.dpooled",) if i == 0 else ("head.dmlp", i), x.shape)
             ops.small_linear_bwd(dy, x, lin.weight, ctx.grad_of(lin.weight), ctx.grad_of(lin.bias), dx, relu_mask=i > 0)
             dy = dx
+        if head.detach_final_fc:
+            return False
         dpooled = dy
         if self._drop_mask is not None:
             ops.dropout_bwd(dpooled, self._drop_mask, head.dropout_rate)
@@ -624,6 +645,7 @@ class _VideoResNetBase(nn.Module):
             ops.global_avgpool_bwd(dpooled, col, nn_, t * h * w, f.c, f.grad_view())
             f.s.grad_written = True
             col += f.c
+        return True
 
 
 class B200SlowFast(_VideoResNetBase):
@@ -676,7 +698,8 @@ class B200SlowFast(_VideoResNetBase):
         pools = None if cfg.MULTIGRID.SHORT_CYCLE or cfg.MODEL.MODEL_NAME == "ContrastiveModel" else [[cfg.DATA.NUM_FRAMES // alpha, crop32, crop32],
                                                          [cfg.DATA.NUM_FRAMES, crop32, crop32]]
         self.head = BasicHeadModule([wpg * 32, wpg * 32 // beta_inv], cfg.MODEL.NUM_CLASSES, cfg.MODEL.DROPOUT_RATE,
-                                    cfg.MODEL.HEAD_ACT, pool_size=pools, contrastive=cfg.get("CONTRASTIVE"))
+                                    cfg.MODEL.HEAD_ACT, pool_size=pools, contrastive=cfg.get("CONTRASTIVE"),
+                                    detach_final_fc=cfg.MODEL.DETACH_FINAL_FC)
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN,
                             cfg.RESNET.ZERO_INIT_FINAL_CONV)
         self._ratio = ratio
@@ -765,9 +788,10 @@ class B200SlowFast(_VideoResNetBase):
     def _engine_backward(self, dlogits: torch.Tensor):
         ctx = self.ctx
         params = [p for p in self.parameters()]
-        ctx.begin_backward(params)
+        ctx.begin_backward(self.grad_params())
         u = self._engine_units()
-        self._head_backward(dlogits)
+        if not self._head_backward(dlogits):
+            return ctx.grads(params)
         for i in range(5, 1, -1):
             stage: StageModule = getattr(self, f"s{i}")
             if i < 5:

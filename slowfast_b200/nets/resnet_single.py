@@ -54,7 +54,8 @@ class B200ResNet(_VideoResNetBase):
         p1 = self._pool1
         pools = None if cfg.MULTIGRID.SHORT_CYCLE or cfg.MODEL.MODEL_NAME == "ContrastiveModel" else [[cfg.DATA.NUM_FRAMES // p1[0], crop32 // p1[1], crop32 // p1[2]]]
         self.head = BasicHeadModule([wpg * 32], cfg.MODEL.NUM_CLASSES, cfg.MODEL.DROPOUT_RATE, cfg.MODEL.HEAD_ACT,
-                                    pool_size=pools, contrastive=cfg.get("CONTRASTIVE"))
+                                    pool_size=pools, contrastive=cfg.get("CONTRASTIVE"),
+                                    detach_final_fc=cfg.MODEL.DETACH_FINAL_FC)
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN,
                             cfg.RESNET.ZERO_INIT_FINAL_CONV)
         self._init_graph_state()
@@ -112,9 +113,10 @@ class B200ResNet(_VideoResNetBase):
     def _engine_backward(self, dlogits: torch.Tensor):
         ctx = self.ctx
         params = [p for p in self.parameters()]
-        ctx.begin_backward(params)
+        ctx.begin_backward(self.grad_params())
         u = self._engine_units()
-        self._head_backward(dlogits)
+        if not self._head_backward(dlogits):
+            return ctx.grads(params)
         for i in range(5, 1, -1):
             if i == 2 and self._pool_saved is not None:
                 src, pooled, argmax, k = self._pool_saved

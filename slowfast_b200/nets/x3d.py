@@ -28,7 +28,7 @@ import torch.nn as nn
 from .. import lib as L
 from .. import ops
 from ..config import nsplit_of
-from ..engine import Act, ConvBN, Ctx, Namespace, bump_num_batches_tracked
+from ..engine import Act, ConvBN, Ctx, Namespace, bn_mode, bump_num_batches_tracked, check_head_act
 from ..ops import F32
 from .resnet import STAGE_DEPTH, _conv, _VideoResNetBase, init_resnet_weights
 
@@ -149,7 +149,7 @@ class X3DBlockModule(Namespace):
         bb = {k: ctx.buf((nm, "b." + k), (cp,), zero=True) for k in ("scale", "shift", "mean", "invstd")}
         bn = b2.b_bn
         ops.bn_finalize(stats, m_tiles, c, n * rps, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                        bn.momentum if bn.momentum is not None else 0.1, bn.eps, ctx.training, bb["scale"],
+                        bn.momentum if bn.momentum is not None else 0.1, bn.eps, bn_mode(ctx, bn), bb["scale"],
                         bb["shift"], bb["mean"], bb["invstd"])
         # ---- SE gate
         gate = None
@@ -223,7 +223,7 @@ def bn_gate_act_backward(ctx: Ctx, y: ops.F32View, bb, gate, sed: Optional["L.Se
     d.coef = coef.data_ptr()
     d.gamma, d.beta = bn.weight.data_ptr(), bn.bias.data_ptr()
     d.dgamma, d.dbeta = ctx.grad_of(bn.weight).data_ptr(), ctx.grad_of(bn.bias).data_ptr()
-    d.training = 1 if ctx.training else 0
+    d.training = 1 if bn_mode(ctx, bn) else 0
     davg = None
     if se is not None:
         f = se.fc1.out_channels
@@ -274,8 +274,7 @@ class X3DHeadModule(Namespace):
         if dropout_rate > 0.0:
             self.dropout = nn.Dropout(dropout_rate)
         self.projection = nn.Linear(dim_out, num_classes, bias=True)
-        if act_func not in ("softmax", "none"):
-            raise NotImplementedError(f"head activation {act_func!r} is not on the engine path")
+        check_head_act(act_func)
         self.act_func = act_func
         self.dropout_rate = dropout_rate
 
@@ -372,7 +371,7 @@ class B200X3D(_VideoResNetBase):
         bb = {k: ctx.buf(("s1", k), (c1,), zero=True) for k in ("scale", "shift", "mean", "invstd")}
         bn = stem.bn
         ops.bn_finalize(stats, m_tiles, c1, n * ot * oh * ow, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                        bn.momentum if bn.momentum is not None else 0.1, bn.eps, ctx.training, bb["scale"],
+                        bn.momentum if bn.momentum is not None else 0.1, bn.eps, bn_mode(ctx, bn), bb["scale"],
                         bb["shift"], bb["mean"], bb["invstd"])
         cur = Act(ctx.storage(("s1", "out"), n, ot, oh, ow, c1))
         ops.bnact_fwd(ops.f32view(y1), bb["scale"], bb["shift"], None, ops.ACT_RELU, ot * oh * ow, cur.planes)
@@ -414,8 +413,8 @@ class B200X3D(_VideoResNetBase):
             ops.dropout_fwd(l5, self._drop_mask, p, self._drop_seed, self._drop_counter)
         logits = torch.empty((n, head.projection.out_features), dtype=torch.float32, device=ctx.device)
         ops.small_linear_fwd(l5, head.projection.weight, head.projection.bias, logits)
-        if not ctx.training and head.act_func == "softmax":
-            ops.row_softmax(logits)
+        if not ctx.training:
+            ops.head_act(logits, head.act_func)
         self._head_saved = (feat, x5, pooled, l5)
         return logits
 

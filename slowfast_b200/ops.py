@@ -540,6 +540,25 @@ def row_softmax(x: torch.Tensor) -> None:
     _count()
 
 
+def row_sigmoid(x: torch.Tensor) -> None:
+    lib = L.load()
+    L.check(lib.sfb_row_sigmoid(x.data_ptr(), x.shape[0], x.shape[1], _stream()), "sfb_row_sigmoid")
+    _count()
+
+
+HEAD_ACTS = ("softmax", "sigmoid", "none")
+
+
+def head_act(x: torch.Tensor, act_func: str) -> None:
+    """The eval-mode activation of a classification head (MODEL.HEAD_ACT) in place on the [rows, classes] output."""
+    if act_func == "softmax":
+        row_softmax(x)
+    elif act_func == "sigmoid":
+        row_sigmoid(x)
+    else:
+        assert act_func == "none", act_func
+
+
 # ------------------------------------------------------------------------------------------------ stem (W-shift)
 @dataclass
 class StemGeom:

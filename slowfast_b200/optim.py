@@ -66,12 +66,15 @@ class FlatOptimizer:
         self.momentum, self.dampening, self.nesterov = float(momentum), float(dampening), bool(nesterov)
         self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
         self.clip = float(clip_grad_l2norm)
-        params = list(model.parameters())
+        # the bucket holds the parameters the backward writes (all of them, or the head under MODEL.DETACH_FINAL_FC);
+        # the others keep their values, momentum and weight decay included, as torch SGD leaves a None .grad
+        params = model.grad_params() if hasattr(model, "grad_params") else list(model.parameters())
+        written = {id(p) for p in params}
         if groups is None:
             groups = [dict(params=[p for p in params if p.requires_grad], weight_decay=weight_decay)]
         self.param_groups = []
         for g in groups:
-            self.param_groups.append(dict(params=list(g["params"]), lr=float(g.get("lr", lr)),
+            self.param_groups.append(dict(params=[p for p in g["params"] if id(p) in written], lr=float(g.get("lr", lr)),
                                           weight_decay=float(g.get("weight_decay", weight_decay)),
                                           layer_decay=float(g.get("layer_decay", 1.0))))
         self._params = params
