@@ -11,6 +11,7 @@ Building blocks:
   * ``ConvBN``           - conv (wgmma implicit GEMM) + train/eval BatchNorm statistics; backward = BN backward,
                            wgrad, dgrad (strided dgrad via ``conv_plan``).
   * ``Ctx``              - per-model buffer cache, scratch, flat gradient buffer, launch bookkeeping.
+  * ``EngineModel``      - the base class of every engine network: what ``ModelFunction`` drives.
 """
 from __future__ import annotations
 
@@ -20,6 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .config import nsplit_of
 from .conv_plan import dgrad_out_view, dgrad_plan
 from .ops import F32, F32View, Planes
 from .subbn import is_sub_bn
@@ -538,11 +540,10 @@ class GraphedProgram:
         return self.static_grads
 
 
-def pointer_signature(model, params) -> int:
+def pointer_signature(model: "EngineModel", params) -> int:
     """Hash of the device pointers a captured program bakes in: every parameter and every BatchNorm buffer."""
-    bn_momentum_signature(model)  # (fills the BN module cache)
     ptrs = [p.data_ptr() for p in params]
-    for b in model.__dict__["_bn_list"]:
+    for b in model._all_bns():
         if b.running_mean is not None:
             ptrs.append(b.running_mean.data_ptr())
             ptrs.append(b.running_var.data_ptr())
@@ -550,16 +551,8 @@ def pointer_signature(model, params) -> int:
     return hash(tuple(ptrs))
 
 
-def _bn_list(model) -> List[nn.Module]:
-    bns = model.__dict__.get("_bn_list")
-    if bns is None:
-        bns = [m for m in model.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)]
-        object.__setattr__(model, "_bn_list", bns)
-    return bns
-
-
-def bn_momentum_signature(model) -> Tuple:
-    bns = _bn_list(model)
+def bn_momentum_signature(model: "EngineModel") -> Tuple:
+    bns = model._all_bns()
     if not bns or not model.training:
         return ()
     first = bns[0].momentum
@@ -572,15 +565,15 @@ def bn_mode(ctx: Ctx, bn: nn.Module) -> bool:
     return ctx.training and bn.training
 
 
-def bn_mode_signature(model) -> Tuple:
+def bn_mode_signature(model: "EngineModel") -> Tuple:
     """Indices of the BatchNorm modules in eval mode inside a training model (MODEL.FROZEN_BN freezes them all,
     a hand-frozen subset some): a captured program bakes each BN's mode into its kernel arguments."""
     if not model.training:
         return ()
-    return tuple(i for i, b in enumerate(_bn_list(model)) if not b.training)
+    return tuple(i for i, b in enumerate(model._all_bns()) if not b.training)
 
 
-def program_key(model, needs_grad: bool, inputs: Sequence[torch.Tensor]) -> Tuple:
+def program_key(model: "EngineModel", needs_grad: bool, inputs: Sequence[torch.Tensor]) -> Tuple:
     """Arena / CUDA-graph key of one forward: mode, grad mode, input signature, BN momenta and BN modes."""
     # BatchNorm momentum is a by-value kernel argument (baked into a captured program): precise-BN (fvcore
     # update_bn_stats, tools/train_net.py:425-446) temporarily sets it to 1.0, so it is part of the signature
@@ -602,10 +595,9 @@ class ModelFunction(torch.autograd.Function):
         key = program_key(model, needs_grad, inputs)
         arena = model.ctx.use_arena(key)
         arena.generation += 1
-        gen = getattr(model, "_fwd_generation", 0) + 1
-        object.__setattr__(model, "_fwd_generation", gen)
-        fctx.key, fctx.arena, fctx.arena_gen, fctx.model_gen = key, arena, arena.generation, gen
-        if getattr(model, "cuda_graphs", False) and inputs[0].is_cuda:
+        model._fwd_generation += 1
+        fctx.key, fctx.arena, fctx.arena_gen, fctx.model_gen = key, arena, arena.generation, model._fwd_generation
+        if model.cuda_graphs and inputs[0].is_cuda:
             prog = model._graphs.get(key)
             sig = pointer_signature(model, tensors[n_inputs:])
             if prog is not None and prog.ptr_sig != sig:
@@ -637,17 +629,123 @@ class ModelFunction(torch.autograd.Function):
         if fctx.prog is not None:
             grads = fctx.prog.run_backward(dout)
         else:
-            if getattr(model, "_fwd_generation", 0) != fctx.model_gen:
+            if model._fwd_generation != fctx.model_gen:
                 raise RuntimeError(
                     "slowfast_b200: another forward ran between this (eager) forward and its backward; the saved "
                     "activations are per model - run backward first, or enable cfg.B200.CUDA_GRAPH")
             model.ctx.use_arena(fctx.key)
             grads = model._engine_backward(dout)
-        if getattr(model, "flat_grad_only", False):
+        if model.flat_grad_only:
             # the caller consumes ctx.flat_grad directly (slowfast_b200.optim.FlatOptimizer): no param.grad copies
             return (None, None) + (None,) * (fctx.n_inputs + len(grads))
         # (None: a parameter in front of MODEL.DETACH_FINAL_FC's detach, whose .grad stays None as in the reference)
         return (None, None) + (None,) * fctx.n_inputs + tuple(grads)
+
+
+class EngineModel(nn.Module):
+    """What every engine network provides to ``ModelFunction`` and ``GraphedProgram``.
+
+    A subclass calls ``super().__init__(cfg)`` before it registers any module, and supplies
+      * ``forward``: its own input handling, then ``self._run(inputs)`` with the list of input tensors;
+      * ``_forward_program(inputs)``: the forward kernels, returning the output tensor autograd receives;
+      * ``_backward_program(dout)``: the backward kernels, writing the gradient of every ``grad_params()`` entry into
+        its slot ``ctx.grad_of(p)``; under MODEL.DETACH_FINAL_FC it stops at the detach;
+      * a module ``head`` with ``detach_final_fc`` and, when that is set, ``params_after_detach()`` (the pre-training
+        models, which have no classification head, have no ``head``).
+
+    The base holds the rest:
+      * ``ctx``: the execution context (``Ctx``) at cfg.B200.NSPLIT;
+      * ``cuda_graphs``: capture each input signature's programs as CUDA graphs after ``graph_warmup`` eager calls
+        (cfg.B200.CUDA_GRAPH; a config without a B200 section, such as the reference's own, keeps the default on);
+      * ``flat_grad_only``: autograd receives no parameter gradients, the caller reads ``ctx.flat_grad`` itself
+        (``optim.FlatOptimizer``);
+      * ``_seed``: cfg.RNG_SEED, the seed of the device-side dropout / stochastic-depth draws;
+      * the BatchNorm registry behind the program key and the ``num_batches_tracked`` updates;
+      * the flat gradient bucket (``grad_params``) and its data-parallel exchange (``allreduce_gradients``).
+    The base registers no parameter, buffer or submodule and draws no random numbers, so a subclass's ``state_dict``
+    and initial values stay the reference's."""
+
+    cuda_graphs = True
+    graph_warmup = 2
+    flat_grad_only = False
+
+    def __init__(self, cfg):
+        super().__init__()
+        self.cfg = cfg
+        self.ctx = Ctx(nsplit_of(cfg))
+        b200 = getattr(cfg, "B200", None)
+        if b200 is not None and "CUDA_GRAPH" in b200:
+            self.cuda_graphs = bool(b200["CUDA_GRAPH"])
+        self._graphs: Dict[Tuple, GraphedProgram] = {}
+        self._graph_seen: Dict[Tuple, int] = {}
+        self._fwd_generation = 0
+        self._seed = int(getattr(cfg, "RNG_SEED", 0))
+        self._drop_counter: Optional[torch.Tensor] = None
+        self._bns: Optional[Tuple[List[nn.Module], List[nn.Module]]] = None
+
+    def _run(self, inputs: Sequence[torch.Tensor]) -> torch.Tensor:
+        return ModelFunction.apply(self, len(inputs), *inputs, *self.parameters())
+
+    def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
+        ctx = self.ctx
+        ctx.device = inputs[0].device
+        ctx.training = self.training
+        if ctx.device.type != "cuda":
+            raise ops.L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
+        out = self._forward_program(inputs)
+        if ctx.training:
+            # torch's BatchNorm increments num_batches_tracked once per training forward of a BN in training mode (one
+            # fused op for all BNs); a frozen BN (module in eval) keeps its count
+            ts = [b.num_batches_tracked for b in self._train_bns() if b.num_batches_tracked is not None and b.training]
+            if ts:
+                torch._foreach_add_(ts, 1)
+        return out
+
+    def _engine_backward(self, dout: torch.Tensor) -> List[Optional[torch.Tensor]]:
+        params = list(self.parameters())
+        self.ctx.begin_backward(self.grad_params())
+        self._backward_program(dout)
+        return self.ctx.grads(params)
+
+    def grad_params(self) -> List[nn.Parameter]:
+        """The parameters the backward writes gradients for, in flat-bucket order: all of them, or the head's
+        parameters behind MODEL.DETACH_FINAL_FC's detach."""
+        head = getattr(self, "head", None)
+        if head is not None and head.detach_final_fc:
+            return head.params_after_detach()
+        return list(self.parameters())
+
+    def allreduce_gradients(self, group=None) -> None:
+        """Data-parallel exchange step (SURVEY.md §8e): ONE NCCL all-reduce (average) over the flat gradient
+        bucket the last backward filled; ``param.grad`` is re-pointed at the bucket slices where autograd made a
+        private copy.  (Under the reference's build_model the DDP wrapper does its own bucketing instead.)"""
+        assert self.ctx.flat_grad is not None, "call after backward()"
+        allreduce_flat_gradients(self.ctx.flat_grad, self.grad_params(), group, repoint=not self.flat_grad_only)
+
+    def _bn_registry(self) -> Tuple[List[nn.Module], List[nn.Module]]:
+        if self._bns is None:
+            mods = list(self.modules())
+            eval_only = {id(m.bn) for m in mods if is_sub_bn(m)}
+            bns = [m for m in mods if isinstance(m, nn.modules.batchnorm._BatchNorm)]
+            self._bns = (bns, [b for b in bns if id(b) not in eval_only])
+        return self._bns
+
+    def _all_bns(self) -> List[nn.Module]:
+        """Every BatchNorm module in module order, both BNs of a sub-batch BN included (fvcore's precise-BN sees them
+        all too): their momenta, modes and buffer pointers are part of a captured program's key."""
+        return self._bn_registry()[0]
+
+    def _train_bns(self) -> List[nn.Module]:
+        """The BNs a training forward runs: a sub-batch BN runs its split_bn only, never its eval ``bn``."""
+        return self._bn_registry()[1]
+
+    def _head_drop_counter(self) -> torch.Tensor:
+        """The head dropout's device-side step counter: one per model, so that the captured programs of every input
+        signature advance the same draw.  Created at zero on the device of the forward, not in ``__init__``: a plain
+        tensor attribute does not follow ``module.to()``."""
+        if self._drop_counter is None or self._drop_counter.device != self.ctx.device:
+            self._drop_counter = torch.zeros(1, dtype=torch.int64, device=self.ctx.device)
+        return self._drop_counter
 
 
 class Namespace(nn.Module):
@@ -655,11 +753,3 @@ class Namespace(nn.Module):
 
     def forward(self, *a, **k):  # pragma: no cover - containers are never called
         raise RuntimeError("engine containers hold parameters only; call the top-level model")
-
-
-def bump_num_batches_tracked(bns: List[nn.BatchNorm3d]) -> None:
-    """torch's BatchNorm increments num_batches_tracked once per training forward of a BN in training mode (one fused
-    op for all BNs); a frozen BN (module in eval) keeps its count."""
-    ts = [b.num_batches_tracked for b in bns if b.num_batches_tracked is not None and b.training]
-    if ts:
-        torch._foreach_add_(ts, 1)

@@ -32,7 +32,7 @@ import torch.nn as nn
 
 from .. import lib as L
 from .. import ops
-from ..engine import ModelFunction, Namespace
+from ..engine import Namespace
 from ..ops import F32
 from .maskfeat import MSSeparateHeadModule, calc_mvit_feature_geometry
 from .mvit import B200MViT, BlockModule, _is_pool, block_specs
@@ -139,8 +139,7 @@ class B200MAE(B200MViT):
         assert not return_all
         frames = x[0]
         noise = torch.rand(frames.shape[0], self.n_tokens, device=frames.device)  # masked.py:298
-        params = [p for p in self.parameters()]
-        pred = ModelFunction.apply(self, 2, frames, noise, *params)
+        pred = self._run([frames, noise])
         B = frames.shape[0]
         rows = self.ctx.buf(("mae.rows",), (B * (self.n_tokens - self.len_keep),), I32)
         return [pred], [(self.pixel_targets(frames, rows), 1.0)]
@@ -157,13 +156,9 @@ class B200MAE(B200MViT):
         return out
 
     # ------------------------------------------------------------------------------------------ forward program
-    def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
+    def _forward_program(self, inputs: List[torch.Tensor]) -> torch.Tensor:
         ctx = self.ctx
         x, noise = inputs
-        ctx.device = x.device
-        ctx.training = self.training
-        if x.device.type != "cuda":
-            raise L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         B, cin, t, h, w = x.shape
         Lt, K = self.n_tokens, self.len_keep
         M = Lt - K
@@ -227,10 +222,8 @@ class B200MAE(B200MViT):
         return pred
 
     # ------------------------------------------------------------------------------------------ backward program
-    def _engine_backward(self, dpred: torch.Tensor):
+    def _backward_program(self, dpred: torch.Tensor) -> None:
         ctx = self.ctx
-        params = [p for p in self.parameters()]
-        ctx.begin_backward(params)
         sv = self._saved
         B = sv["B"]
         Lt, K = self.n_tokens, self.len_keep
@@ -290,4 +283,3 @@ class B200MAE(B200MViT):
         gw = ctx.grad_of(pe.weight).view(E, xr.c)
         ops.zero_f32(ops.f32view(gw))
         ops.conv_wgrad(xr, dyp, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 0), (xr.t, xr.h, xr.w)), gw, nsplit=ctx.nsplit)
-        return [ctx.grad_of(p) for p in params]

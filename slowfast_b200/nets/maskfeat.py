@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from .. import lib as L
 from .. import ops
-from ..engine import ModelFunction, Namespace
+from ..engine import Namespace
 from ..ops import BF16, F32, Planes
 from .mvit import B200MViT
 
@@ -136,8 +136,7 @@ class B200MaskMViT(B200MViT):
         # multiscale boolean masks (masked.py:165-176): nearest resize of the cube mask to each feature map
         output_masks = [F.interpolate(float_mask, size=self.feat_size[d][-1]).flatten(1).to(torch.bool)
                         for d in self.pretrain_depth]
-        params = [p for p in self.parameters()]
-        pred_all = ModelFunction.apply(self, 2, frames, float_mask, *params)  # [B, L, classes], every token
+        pred_all = self._run([frames, float_mask])  # [B, L, classes], every token
         labels_all = self.hog_targets(frames)
         preds, labels = [], []
         for m in output_masks:

@@ -27,10 +27,8 @@ from typing import List, Optional
 import torch
 import torch.nn as nn
 
-from .. import lib as L
 from .. import ops
-from ..config import nsplit_of
-from ..engine import Ctx, ModelFunction, Namespace, check_head_act
+from ..engine import EngineModel, Namespace, check_head_act
 from ..ops import F32, Planes
 
 BF16 = torch.bfloat16
@@ -175,15 +173,16 @@ class TransformerHeadModule(Namespace):
         self.act_func = act_func
         self.detach_final_fc = bool(detach_final_fc)
 
+    def params_after_detach(self) -> List[nn.Parameter]:
+        """The parameters behind the detach: the projection's weight and bias."""
+        return [self.projection.weight, self.projection.bias]
 
-class B200MViT(nn.Module):
+
+class B200MViT(EngineModel):
     """MViTv2 on the engine (drop-in for the reference's registered ``MViT``)."""
 
-    cuda_graphs = True
-    graph_warmup = 2
-
     def __init__(self, cfg):
-        super().__init__()
+        super().__init__(cfg)
         mv = cfg.MVIT
         assert cfg.DATA.TRAIN_CROP_SIZE == cfg.DATA.TEST_CROP_SIZE
         assert mv.MODE == "conv" and not mv.POOL_FIRST
@@ -192,8 +191,6 @@ class B200MViT(nn.Module):
         assert float(mv.LAYER_SCALE_INIT_VALUE) == 0.0
         self._reject_unsupported(cfg)
         self.specs = block_specs(cfg)
-        self.cfg = cfg
-        self.ctx = Ctx(nsplit_of(cfg))
         self.patch_2d = bool(mv.PATCH_2D)
         self.patch_stride = ([1] if self.patch_2d else []) + list(mv.PATCH_STRIDE)
         self.T = cfg.DATA.NUM_FRAMES // self.patch_stride[0]
@@ -242,12 +239,6 @@ class B200MViT(nn.Module):
         self.head.projection.bias.data.mul_(mv.HEAD_INIT_SCALE)
         depth = mv.DEPTH
         self.drop_rates = [x.item() for x in torch.linspace(0, float(mv.DROPPATH_RATE), depth)]
-        object.__setattr__(self, "_graphs", {})
-        object.__setattr__(self, "_graph_seen", {})
-        b200 = getattr(cfg, "B200", None)
-        if b200 is not None and "CUDA_GRAPH" in b200:
-            self.cuda_graphs = bool(b200["CUDA_GRAPH"])
-        self._seed = int(getattr(cfg, "RNG_SEED", 0))
         object.__setattr__(self, "_saved", None)
 
     @staticmethod
@@ -320,22 +311,7 @@ class B200MViT(nn.Module):
         if self.patch_2d and x[0].dim() != 4:
             raise ValueError(f"MVIT.PATCH_2D takes images [B, C, H, W]; got a {x[0].dim()}-D input of shape "
                              f"{tuple(x[0].shape)}")
-        params = [p for p in self.parameters()]
-        return ModelFunction.apply(self, 1, *x, *params)
-
-    def grad_params(self) -> List[nn.Parameter]:
-        """The parameters the backward writes gradients for, in flat-bucket order: all of them, or the head's
-        projection under MODEL.DETACH_FINAL_FC."""
-        head = getattr(self, "head", None)  # (the MAE / MaskFeat pre-training models replace the head)
-        if getattr(head, "detach_final_fc", False):
-            return [head.projection.weight, head.projection.bias]
-        return list(self.parameters())
-
-    def allreduce_gradients(self, group=None) -> None:
-        from ..engine import allreduce_flat_gradients
-        assert self.ctx.flat_grad is not None, "call after backward()"
-        allreduce_flat_gradients(self.ctx.flat_grad, self.grad_params(), group,
-                                 repoint=not getattr(self, "flat_grad_only", False))
+        return self._run(x)
 
     # ================================================================================== helpers
     def _lin_fwd(self, key, lin: nn.Linear, x: Planes) -> torch.Tensor:
@@ -397,15 +373,11 @@ class B200MViT(nn.Module):
                           ctx.grad_of(ln.bias), part, dx_accumulate=dx_acc, param_accumulate=param_acc)
 
     # ================================================================================== forward program
-    def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
+    def _forward_program(self, inputs: List[torch.Tensor]) -> torch.Tensor:
         ctx = self.ctx
         x = inputs[0]
         if self.patch_2d:
             x = x.unsqueeze(2)  # [B, C, H, W] -> [B, C, 1, H, W]: the same memory as a one-frame clip
-        ctx.device = x.device
-        ctx.training = self.training
-        if x.device.type != "cuda":
-            raise L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         B = x.shape[0]
         pe = self.patch_embed.proj
         # ---- patch embedding: clip -> [B, L, 96] (+bias, cls) -------------------------------------------------
@@ -524,9 +496,7 @@ class B200MViT(nn.Module):
             feat = ctx.buf(("head.feat",), (B, Cf))
             feat.copy_(cls_n)
             mask = ctx.buf(("head.mask",), (B, Cf), torch.uint8)
-            if getattr(self, "_drop_counter", None) is None or self._drop_counter.device != ctx.device:
-                object.__setattr__(self, "_drop_counter", torch.zeros(1, dtype=torch.int64, device=ctx.device))
-            ops.dropout_fwd(feat, mask, head.dropout_rate, self._seed + 17, self._drop_counter)
+            ops.dropout_fwd(feat, mask, head.dropout_rate, self._seed + 17, self._head_drop_counter())
         logits = torch.empty((B, self.num_classes), dtype=F32, device=ctx.device)
         ops.small_linear_fwd(feat, head.projection.weight, head.projection.bias, logits)
         if not ctx.training:
@@ -698,15 +668,13 @@ class B200MViT(nn.Module):
         return x2, list(q_thw), sv
 
     # ================================================================================== backward program
-    def _engine_backward(self, dlogits: torch.Tensor):
+    def _backward_program(self, dlogits: torch.Tensor) -> None:
         ctx = self.ctx
-        params = [p for p in self.parameters()]
-        ctx.begin_backward(self.grad_params())
         sv = self._saved
         B = sv["B"]
         dx = self._final_backward(dlogits)
         if dx is None:
-            return ctx.grads(params)
+            return
         which = "a"
         for i in range(len(self.blocks) - 1, -1, -1):
             which = "b" if which == "a" else "a"
@@ -732,13 +700,12 @@ class B200MViT(nn.Module):
             ops.zero_f32(ops.f32view(gw))
             ops.conv_wgrad(xr, dyp, ops.ConvGeom((1, 1, 1), (1, 1, 1), (0, 0, 0), (xr.t, xr.h, xr.w)), gw,
                            nsplit=ctx.nsplit)
-            return [ctx.grad_of(p) for p in params]
+            return
         taps = math.prod(pe.kernel_size)
         dwm = ctx.scratch("pe.dwm", E * taps * 8, F32).view(E, taps * 8)
         ops.zero_f32(ops.f32view(dwm))
         ops.conv_wgrad(sv["xin"], Planes(dyp.hi, dyp.lo, B, T, H, W, E, 0), sv["geom"], dwm, nsplit=ctx.nsplit)
         ops.filter_unpack_grad(dwm, ctx.grad_of(pe.weight), 8, accumulate=False)
-        return [ctx.grad_of(p) for p in params]
 
     def _block_backward(self, i, blk: BlockModule, spec, sv, dx2: torch.Tensor, B, which: str) -> torch.Tensor:
         """dx2: gradient w.r.t. the block output [B, Nq, A] (clobbered).  Returns the gradient w.r.t. the block input."""

@@ -21,11 +21,9 @@ import torch
 import torch.nn as nn
 
 from .. import ops
-from ..config import nsplit_of
-from ..engine import (Act, ConvBN, Ctx, ModelFunction, Namespace, StemConvBN, bump_num_batches_tracked,
-                      check_head_act)
+from ..engine import Act, ConvBN, Ctx, EngineModel, Namespace, StemConvBN, check_head_act
 from ..ops import F32, Planes
-from ..subbn import is_sub_bn, norm_factory, num_splits_of
+from ..subbn import norm_factory, num_splits_of
 
 # depth -> blocks per stage (video_model_builder.py:38)
 STAGE_DEPTH = {18: (2, 2, 2, 2), 50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
@@ -434,6 +432,10 @@ class BasicHeadModule(Namespace):
             return [self.projection]
         return [m for m in self.projection.projection if isinstance(m, nn.Linear)]
 
+    def params_after_detach(self) -> List[nn.Parameter]:
+        """The parameters behind the detach: every Linear layer's weight and bias."""
+        return [p for lin in self.linears() for p in (lin.weight, lin.bias)]
+
 
 def init_resnet_weights(model: nn.Module, fc_init_std, zero_init_final_bn, zero_init_final_conv) -> None:
     """ResNet-style initialisation, same draws in the same module order as the reference
@@ -461,21 +463,12 @@ def init_resnet_weights(model: nn.Module, fc_init_std, zero_init_final_bn, zero_
                 m.bias.data.zero_()
 
 
-class _VideoResNetBase(nn.Module):
-    """Shared engine driver of the ResNet-family models."""
+class _VideoResNetBase(EngineModel):
+    """Config checks, stem, head and MLP of the ResNet-family models."""
 
     num_pathways = 1
-    # CUDA-graph execution of the forward / backward programs (set False to run every launch eagerly)
-    cuda_graphs = True
-    graph_warmup = 2
-    # W-shift stem kernels (csrc/conv_stem.cu); False = generic im2col path (kept for A/B checks)
-    wshift_stem = True
     # splits of the training batch (BN.NUM_SPLITS under sub_batchnorm; set by _check_cfg)
     _bn_splits = 1
-
-    def _init_graph_state(self):
-        object.__setattr__(self, "_graphs", {})
-        object.__setattr__(self, "_graph_seen", {})
 
     def _check_cfg(self, cfg):
         # BN.NORM_TYPE: batchnorm or sub_batchnorm (multigrid's long cycle); norm_factory rejects the others
@@ -488,7 +481,6 @@ class _VideoResNetBase(nn.Module):
         assert cfg.RESNET.NUM_GROUPS == 1
         assert not cfg.DETECTION.ENABLE, "RoI head is out of scope"
         assert all(d == 1 for st in cfg.RESNET.SPATIAL_DILATIONS for d in st)
-        assert float(cfg.MODEL.DROPCONNECT_RATE) == 0.0 or True  # drop-connect is a no-op in the reference (§3.3)
 
     # ------------------------------------------------------------------ public nn.Module API
     def forward(self, x, bboxes=None):
@@ -498,34 +490,7 @@ class _VideoResNetBase(nn.Module):
         if self.training and self._bn_splits > 1 and x[0].shape[0] % self._bn_splits:
             raise ValueError(f"sub_batchnorm: BN.NUM_SPLITS {self._bn_splits} does not divide the batch size "
                              f"{x[0].shape[0]} (every split takes batch / NUM_SPLITS clips)")
-        params = [p for p in self.parameters()]
-        return ModelFunction.apply(self, len(x), *x, *params)
-
-    def _all_bns(self):
-        """Every nn.BatchNorm3d, both BNs of a sub-batch BN included (fvcore's precise-BN sees them all too)."""
-        return [m for m in self.modules() if isinstance(m, nn.BatchNorm3d)]
-
-    def _train_bns(self):
-        """The BNs a training forward runs: a sub-batch BN runs its split_bn only, never its eval ``bn``."""
-        skip = {id(m.bn) for m in self.modules() if is_sub_bn(m)}
-        return [m for m in self._all_bns() if id(m) not in skip]
-
-    def grad_params(self) -> List[nn.Parameter]:
-        """The parameters the backward writes gradients for, in flat-bucket order: all of them, or the head's Linear
-        layers under MODEL.DETACH_FINAL_FC."""
-        head = getattr(self, "head", None)
-        if getattr(head, "detach_final_fc", False):
-            return [p for lin in head.linears() for p in (lin.weight, lin.bias)]
-        return list(self.parameters())
-
-    def allreduce_gradients(self, group=None) -> None:
-        """Data-parallel exchange step (SURVEY.md §8e): ONE NCCL all-reduce (average) over the flat gradient
-        bucket the last backward filled; ``param.grad`` is re-pointed at the bucket slices where autograd made a
-        private copy.  (Under the reference's build_model the DDP wrapper does its own bucketing instead.)"""
-        from ..engine import allreduce_flat_gradients
-        assert self.ctx.flat_grad is not None, "call after backward()"
-        allreduce_flat_gradients(self.ctx.flat_grad, self.grad_params(), group,
-                                 repoint=not getattr(self, "flat_grad_only", False))
+        return self._run(x)
 
     # ------------------------------------------------------------------ helpers
     def _stem_forward(self, p: int, x: torch.Tensor, stem: StemModule, unit: ConvBN, out: Act) -> None:
@@ -591,9 +556,7 @@ class _VideoResNetBase(nn.Module):
         self._drop_mask = None
         if ctx.training and p > 0.0:
             self._drop_mask = ctx.buf(("head.mask",), (n, dim), torch.uint8)
-            if getattr(self, "_drop_counter", None) is None or self._drop_counter.device != ctx.device:
-                self._drop_counter = torch.zeros(1, dtype=torch.int64, device=ctx.device)
-            ops.dropout_fwd(pooled, self._drop_mask, p, self._drop_seed, self._drop_counter)
+            ops.dropout_fwd(pooled, self._drop_mask, p, self._seed, self._head_drop_counter())
         acts = self._head_mlp_forward(pooled, None)
         logits = acts[-1]
         if not ctx.training:
@@ -654,10 +617,8 @@ class B200SlowFast(_VideoResNetBase):
     num_pathways = 2
 
     def __init__(self, cfg):
-        super().__init__()
-        self.cfg = cfg
+        super().__init__(cfg)
         self._check_cfg(cfg)
-        self.ctx = Ctx(nsplit_of(cfg))
         ctx = self.ctx
         d2, d3, d4, d5 = STAGE_DEPTH[cfg.RESNET.DEPTH]
         wpg = cfg.RESNET.WIDTH_PER_GROUP
@@ -703,13 +664,7 @@ class B200SlowFast(_VideoResNetBase):
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN,
                             cfg.RESNET.ZERO_INIT_FINAL_CONV)
         self._ratio = ratio
-        self._init_graph_state()
-        b200 = getattr(cfg, "B200", None)
-        if b200 is not None and "CUDA_GRAPH" in b200:
-            self.cuda_graphs = bool(b200["CUDA_GRAPH"])
         self._stem_saved = {}
-        self._drop_seed = int(getattr(cfg, "RNG_SEED", 0))
-        self._drop_step = 0
         object.__setattr__(self, "_units", None)
 
     def _engine_units(self):
@@ -718,7 +673,7 @@ class B200SlowFast(_VideoResNetBase):
             crop = int(self.cfg.DATA.TRAIN_CROP_SIZE)
             u = {}
             for p, stem in enumerate((self.s1.pathway0_stem, self.s1.pathway1_stem)):
-                cls = StemConvBN if (self.wshift_stem and StemConvBN.supported(stem.conv, crop)) else ConvBN
+                cls = StemConvBN if StemConvBN.supported(stem.conv, crop) else ConvBN
                 u[f"stem{p}"] = cls(f"s1.p{p}", stem.conv, stem.bn, ctx)
             for i in range(1, 5):
                 f = getattr(self, f"s{i}_fuse")
@@ -727,12 +682,8 @@ class B200SlowFast(_VideoResNetBase):
         return self._units
 
     # ------------------------------------------------------------------ forward program
-    def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
+    def _forward_program(self, inputs: List[torch.Tensor]) -> torch.Tensor:
         ctx = self.ctx
-        ctx.device = inputs[0].device
-        ctx.training = self.training
-        if inputs[0].device.type != "cuda":
-            raise ops.L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         u = self._engine_units()
         xs, xf = inputs
         n = xs.shape[0]
@@ -773,10 +724,7 @@ class B200SlowFast(_VideoResNetBase):
                 self._fuse_forward(i, fast, slow.slice(cs, slow.c - cs))
             trace.append((slow, fast, cs))
         self._trace = trace
-        if ctx.training:
-            bump_num_batches_tracked(self._train_bns())
-        out = self._head_forward([slow, fast])
-        return out
+        return self._head_forward([slow, fast])
 
     def _fuse_forward(self, i: int, fast: Act, out: Act) -> None:
         unit = self._engine_units()[f"fuse{i}"]
@@ -785,13 +733,10 @@ class B200SlowFast(_VideoResNetBase):
         self.__dict__.setdefault("_fuse_saved", {})[i] = (fast, out)
 
     # ------------------------------------------------------------------ backward program
-    def _engine_backward(self, dlogits: torch.Tensor):
-        ctx = self.ctx
-        params = [p for p in self.parameters()]
-        ctx.begin_backward(self.grad_params())
+    def _backward_program(self, dlogits: torch.Tensor) -> None:
         u = self._engine_units()
         if not self._head_backward(dlogits):
-            return ctx.grads(params)
+            return
         for i in range(5, 1, -1):
             stage: StageModule = getattr(self, f"s{i}")
             if i < 5:
@@ -804,4 +749,3 @@ class B200SlowFast(_VideoResNetBase):
         u["fuse1"].bwd(out.grad_view(), out.planes, fast)
         self._stem_backward(0, u["stem0"])
         self._stem_backward(1, u["stem1"])
-        return [ctx.grad_of(p) for p in params]

@@ -11,8 +11,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops
-from ..config import nsplit_of
-from ..engine import Act, ConvBN, Ctx, Namespace, StemConvBN, bump_num_batches_tracked
+from ..engine import Act, ConvBN, Namespace, StemConvBN
 from .resnet import (POOL1, STAGE_DEPTH, TEMPORAL_KERNELS, BasicHeadModule, StageModule, StemModule,
                      _VideoResNetBase, init_resnet_weights)
 
@@ -21,11 +20,9 @@ class B200ResNet(_VideoResNetBase):
     num_pathways = 1
 
     def __init__(self, cfg):
-        super().__init__()
-        self.cfg = cfg
+        super().__init__(cfg)
         self._check_cfg(cfg)
         assert cfg.MODEL.ARCH in POOL1 and len(POOL1[cfg.MODEL.ARCH]) == 1, cfg.MODEL.ARCH
-        self.ctx = Ctx(nsplit_of(cfg))
         ctx = self.ctx
         d2, d3, d4, d5 = STAGE_DEPTH[cfg.RESNET.DEPTH]
         wpg = cfg.RESNET.WIDTH_PER_GROUP
@@ -58,28 +55,19 @@ class B200ResNet(_VideoResNetBase):
                                     detach_final_fc=cfg.MODEL.DETACH_FINAL_FC)
         init_resnet_weights(self, cfg.MODEL.FC_INIT_STD, cfg.RESNET.ZERO_INIT_FINAL_BN,
                             cfg.RESNET.ZERO_INIT_FINAL_CONV)
-        self._init_graph_state()
-        b200 = getattr(cfg, "B200", None)
-        if b200 is not None and "CUDA_GRAPH" in b200:
-            self.cuda_graphs = bool(b200["CUDA_GRAPH"])
         self._stem_saved = {}
-        self._drop_seed = int(getattr(cfg, "RNG_SEED", 0))
         object.__setattr__(self, "_units", None)
 
     def _engine_units(self):
         if self._units is None:
             stem = self.s1.pathway0_stem
             crop = int(self.cfg.DATA.TRAIN_CROP_SIZE)
-            cls = StemConvBN if (self.wshift_stem and StemConvBN.supported(stem.conv, crop)) else ConvBN
+            cls = StemConvBN if StemConvBN.supported(stem.conv, crop) else ConvBN
             object.__setattr__(self, "_units", {"stem0": cls("s1.p0", stem.conv, stem.bn, self.ctx)})
         return self._units
 
-    def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
+    def _forward_program(self, inputs: List[torch.Tensor]) -> torch.Tensor:
         ctx = self.ctx
-        ctx.device = inputs[0].device
-        ctx.training = self.training
-        if inputs[0].device.type != "cuda":
-            raise ops.L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         u = self._engine_units()
         (x,) = inputs
         n = x.shape[0]
@@ -105,18 +93,12 @@ class B200ResNet(_VideoResNetBase):
                 ops.maxpool3d_fwd(cur.planes, pooled.planes, argmax, k, k, (0, 0, 0))
                 self._pool_saved = (cur, pooled, argmax, k)
                 cur = pooled
-        if ctx.training:
-            bump_num_batches_tracked(self._train_bns())
-        out = self._head_forward([cur])
-        return out
+        return self._head_forward([cur])
 
-    def _engine_backward(self, dlogits: torch.Tensor):
-        ctx = self.ctx
-        params = [p for p in self.parameters()]
-        ctx.begin_backward(self.grad_params())
+    def _backward_program(self, dlogits: torch.Tensor) -> None:
         u = self._engine_units()
         if not self._head_backward(dlogits):
-            return ctx.grads(params)
+            return
         for i in range(5, 1, -1):
             if i == 2 and self._pool_saved is not None:
                 src, pooled, argmax, k = self._pool_saved
@@ -128,4 +110,3 @@ class B200ResNet(_VideoResNetBase):
             for bi in reversed(range(stage.num_blocks[0])):
                 stage.run_block_backward(0, bi)
         self._stem_backward(0, u["stem0"])
-        return [ctx.grad_of(p) for p in params]

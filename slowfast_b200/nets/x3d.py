@@ -27,8 +27,7 @@ import torch.nn as nn
 
 from .. import lib as L
 from .. import ops
-from ..config import nsplit_of
-from ..engine import Act, ConvBN, Ctx, Namespace, bn_mode, bump_num_batches_tracked, check_head_act
+from ..engine import Act, ConvBN, Ctx, Namespace, bn_mode, check_head_act
 from ..ops import F32
 from .resnet import STAGE_DEPTH, _conv, _VideoResNetBase, init_resnet_weights
 
@@ -274,6 +273,7 @@ class X3DHeadModule(Namespace):
         if dropout_rate > 0.0:
             self.dropout = nn.Dropout(dropout_rate)
         self.projection = nn.Linear(dim_out, num_classes, bias=True)
+        self.detach_final_fc = False  # (X3DHead has no MODEL.DETACH_FINAL_FC switch)
         check_head_act(act_func)
         self.act_func = act_func
         self.dropout_rate = dropout_rate
@@ -285,15 +285,13 @@ class B200X3D(_VideoResNetBase):
     num_pathways = 1
 
     def __init__(self, cfg):
-        super().__init__()
-        self.cfg = cfg
+        super().__init__(cfg)
         assert cfg.BN.NORM_TYPE == "batchnorm", "only BN.NORM_TYPE=batchnorm is on the engine path"
         assert cfg.RESNET.TRANS_FUNC == "x3d_transform" and cfg.MODEL.ARCH == "x3d"
         assert cfg.X3D.CHANNELWISE_3x3x3, "X3D with dense 3x3x3 convolutions is not on the engine path"
         assert not cfg.DETECTION.ENABLE
         assert float(cfg.MODEL.DROPCONNECT_RATE) == 0.0, "drop-connect is not on the engine path (0.0 in X3D yamls)"
         assert all(len(l) == 0 for st in cfg.NONLOCAL.LOCATION for l in st)
-        self.ctx = Ctx(nsplit_of(cfg))
         ctx = self.ctx
         exp_stage = 2.0
         dim_c1 = cfg.X3D.DIM_C1
@@ -328,12 +326,6 @@ class B200X3D(_VideoResNetBase):
         for m in self.modules():  # c2_msra_fill zeroes conv biases (the SE FCs)
             if isinstance(m, nn.Conv3d) and m.bias is not None:
                 nn.init.constant_(m.bias, 0)
-        self._init_graph_state()
-        b200 = getattr(cfg, "B200", None)
-        if b200 is not None and "CUDA_GRAPH" in b200:
-            self.cuda_graphs = bool(b200["CUDA_GRAPH"])
-        self._drop_seed = int(getattr(cfg, "RNG_SEED", 0))
-        self._drop_counter = None
         object.__setattr__(self, "_units", None)
 
     def _engine_units(self):
@@ -345,12 +337,8 @@ class B200X3D(_VideoResNetBase):
         return self._units
 
     # ------------------------------------------------------------------ forward program
-    def _engine_forward(self, inputs: List[torch.Tensor]) -> torch.Tensor:
+    def _forward_program(self, inputs: List[torch.Tensor]) -> torch.Tensor:
         ctx = self.ctx
-        ctx.device = inputs[0].device
-        ctx.training = self.training
-        if inputs[0].device.type != "cuda":
-            raise L.NativeLibraryError("slowfast_b200 runs on CUDA devices only (no CPU fallback)")
         u = self._engine_units()
         (x,) = inputs
         n, _, t, h, w = x.shape
@@ -383,10 +371,7 @@ class B200X3D(_VideoResNetBase):
                 out = Act(ctx.storage((f"s{i}", bi), n, tt, hh, ww, blk._dim_out))
                 blk.run_forward(cur, out)
                 cur = out
-        if ctx.training:
-            bump_num_batches_tracked(self._all_bns())
-        out = self._x3d_head_forward(cur)
-        return out
+        return self._x3d_head_forward(cur)
 
     def _x3d_head_forward(self, feat: Act) -> torch.Tensor:
         ctx, head, u = self.ctx, self.head, self._engine_units()
@@ -408,9 +393,7 @@ class B200X3D(_VideoResNetBase):
         self._drop_mask = None
         if ctx.training and p > 0.0:
             self._drop_mask = ctx.buf(("head", "mask"), (n, co), torch.uint8)
-            if self._drop_counter is None or self._drop_counter.device != ctx.device:
-                self._drop_counter = torch.zeros(1, dtype=torch.int64, device=ctx.device)
-            ops.dropout_fwd(l5, self._drop_mask, p, self._drop_seed, self._drop_counter)
+            ops.dropout_fwd(l5, self._drop_mask, p, self._seed, self._head_drop_counter())
         logits = torch.empty((n, head.projection.out_features), dtype=torch.float32, device=ctx.device)
         ops.small_linear_fwd(l5, head.projection.weight, head.projection.bias, logits)
         if not ctx.training:
@@ -419,10 +402,8 @@ class B200X3D(_VideoResNetBase):
         return logits
 
     # ------------------------------------------------------------------ backward program
-    def _engine_backward(self, dlogits: torch.Tensor):
+    def _backward_program(self, dlogits: torch.Tensor) -> None:
         ctx = self.ctx
-        params = [p for p in self.parameters()]
-        ctx.begin_backward(params)
         u, head = self._engine_units(), self.head
         feat, x5, pooled, l5 = self._head_saved
         n, co = l5.shape
@@ -452,7 +433,6 @@ class B200X3D(_VideoResNetBase):
         ops.dwconv_bwd(g, c1, c1, stem.conv.weight, dy1, ctx.grad_of(stem.conv.weight), x_f32=ops.f32view(y0),
                        dx_planes=dy0)
         u["xy"].wgrad(dy0)
-        return [ctx.grad_of(p) for p in params]
 
 
 def head_pool_size(cfg):
